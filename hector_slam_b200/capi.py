@@ -34,6 +34,7 @@ EXPORTED = [
     "hsb_match_batch_submit", "hsb_match_batch_ranges_submit", "hsb_match_batch_cloud_submit", "hsb_match_batch_wait",
     "hsb_alloc_pinned", "hsb_free_pinned", "hsb_measure_h2d_gbs", "hsb_get_dirty_rects", "hsb_pack_dirty_device", "hsb_unpack_dirty_device", "hsb_get_replication_overflows", "hsb_get_mirror_dirty_rect", "hsb_download_level_rect", "hsb_download_occupancy_rect",
     "hsb_get_d2h_bytes", "hsb_covariance_batch", "hsb_get_map_origin", "hsb_get_dist_batch", "hsb_set_cloud_format", "hsb_cloud_to_points", "hsb_match_batch_cloud", "hsb_match_batch_cloud_device",
+    "hsb_get_match_record_floats", "hsb_match_data_record", "hsb_match_batch_record_device",
 ]
 
 
@@ -104,6 +105,9 @@ def load_library() -> C.CDLL:
     sig("hsb_match_data", i, vp, vp, vp, i, vp, vp, vp)
     sig("hsb_match_batch", i, vp, i, vp, vp, vp, i, vp, vp)
     sig("hsb_match_batch_device", i, vp, i, vp, vp, vp, i, i, vp, vp, vp)
+    sig("hsb_get_match_record_floats", i, vp)
+    sig("hsb_match_data_record", i, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_match_batch_record_device", i, vp, i, vp, vp, vp, i, i, vp, vp, vp, vp)
     sig("hsb_hessian_derivs", i, vp, i, vp, vp, i, vp, vp)
     sig("hsb_update_by_scan", i, vp, vp, i, vp, vp)
     sig("hsb_update_level_by_scan", i, vp, i, vp, i, vp, vp)
@@ -328,16 +332,96 @@ class MapRepB200:
         self._check(self.lib.hsb_world_coords_pose(self.h, level, m.ctypes.data, out.ctypes.data))
         return out
 
-    def matchData(self, begin_estimate_world, points_xy, cov_inout=None, origo=None):
-        """-> (pose (3,), cov (3,3)).  cov_inout is returned untouched for an empty scan."""
+    def matchData(self, begin_estimate_world, points_xy, cov_inout=None, origo=None, record: bool = False):
+        """-> (pose (3,), cov (3,3)), or with record=True (pose, cov, record) where record is split_record() of the
+        scan's per-evaluation record.  cov_inout is returned untouched for an empty scan."""
         hint = _f32(begin_estimate_world, 3)
         pts = _f32(points_xy).reshape(-1, 2)
         pose = np.zeros(3, np.float32)
         cov = np.zeros(9, np.float32) if cov_inout is None else _f32(cov_inout).reshape(9).copy()
         og = None if origo is None else _f32(origo, 2)
-        self._check(self.lib.hsb_match_data(self.h, hint.ctypes.data, pts.ctypes.data if pts.size else None,
-                                            pts.shape[0], _ptr(og), pose.ctypes.data, cov.ctypes.data))
-        return pose, cov.reshape(3, 3)
+        args = (self.h, hint.ctypes.data, pts.ctypes.data if pts.size else None, pts.shape[0], _ptr(og), pose.ctypes.data,
+                cov.ctypes.data)
+        if not record:
+            self._check(self.lib.hsb_match_data(*args))
+            return pose, cov.reshape(3, 3)
+        rec = np.zeros(self.record_floats, np.float32)
+        self._check(self.lib.hsb_match_data_record(*args, rec.ctypes.data))
+        return pose, cov.reshape(3, 3), self.split_record(rec)
+
+    match_data = matchData
+
+    # -- per-evaluation record (include/hector_slam_b200.h, hsb_get_match_record_floats) -------------
+    @property
+    def record_floats(self) -> int:
+        """R: floats of one scan's record"""
+        r = int(self.lib.hsb_get_match_record_floats(self.h))
+        if r < 0:
+            self._check(r)
+        return r
+
+    def level_evals(self) -> list[int]:
+        """Gauss-Newton evaluations per level, level 0 first (maxIterations + 1, the defaults 5 / 3 for a zero entry)"""
+        out = []
+        for l in range(self.levels):
+            mi = int(self.cfg.max_iterations[l]) or (5 if l == 0 else 3)
+            out.append(max(mi, 0) + 1)
+        return out
+
+    def split_record(self, rec) -> list[dict]:
+        """(..., R) float32 records -> one dict per level, INDEXED BY LEVEL (0 = finest):
+        start (..., 3) world pose the level starts from, H (..., E, 3, 3), dTr (..., E, 3), est (..., E, 3) the
+        estimate after each evaluation's step in the level's map cells."""
+        rec = np.asarray(rec, np.float32)
+        assert rec.shape[-1] == self.record_floats, (rec.shape, self.record_floats)
+        lead = rec.shape[:-1]
+        evals = self.level_evals()
+        out = [None] * self.levels
+        off = 0
+        for l in range(self.levels - 1, -1, -1):
+            E = evals[l]
+            start = rec[..., off:off + 3]
+            ev = rec[..., off + 3:off + 3 + 15 * E].reshape(lead + (E, 15))
+            out[l] = dict(start=start.copy(), H=ev[..., :9].reshape(lead + (E, 3, 3)).copy(), dTr=ev[..., 9:12].copy(),
+                          est=ev[..., 12:15].copy())
+            off += 3 + 15 * E
+        return out
+
+    def match_batch_record_device(self, B: int, d_hints: int, d_points: int, d_offsets: int | None, n_shared: int,
+                                  max_points_per_scan: int, d_out_poses: int, d_out_cov: int | None, d_record: int,
+                                  stream: int = 0):
+        """match_batch_device plus the records: d_record holds B x record_floats float32 (device); asynchronous."""
+        self._check(self.lib.hsb_match_batch_record_device(self.h, int(B), d_hints, d_points, d_offsets, int(n_shared),
+                                                           int(max_points_per_scan), d_out_poses, d_out_cov, d_record,
+                                                           stream))
+
+    def match_batch_record(self, hints, points_xy, offsets=None):
+        """A batch with records through the device entry point (torch allocates the device buffers).
+        -> (poses (B, 3), cov (B, 3, 3), records: split_record() of the (B, R) array, raw (B, R) array)"""
+        import torch
+
+        hints = _f32(hints).reshape(-1, 3)
+        pts = _f32(points_xy).reshape(-1, 2)
+        B = hints.shape[0]
+        dev = torch.device("cuda", self.device)
+        d_h = torch.from_numpy(hints).to(dev)
+        d_p = torch.from_numpy(pts if pts.size else np.zeros((1, 2), np.float32)).to(dev)
+        if offsets is None:
+            d_o, n_shared, max_n = None, pts.shape[0], pts.shape[0]
+        else:
+            offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+            d_o = torch.from_numpy(offsets).to(dev)
+            n_shared, max_n = 0, int(np.diff(offsets).max()) if B else 0
+        poses = torch.zeros((B, 3), dtype=torch.float32, device=dev)
+        cov = torch.zeros((B, 9), dtype=torch.float32, device=dev)
+        rec = torch.zeros((B, self.record_floats), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream().cuda_stream
+            self.match_batch_record_device(B, d_h.data_ptr(), d_p.data_ptr(), None if d_o is None else d_o.data_ptr(),
+                                           n_shared, max_n, poses.data_ptr(), cov.data_ptr(), rec.data_ptr(), stream)
+            torch.cuda.current_stream().synchronize()
+        raw = rec.cpu().numpy()
+        return poses.cpu().numpy(), cov.cpu().numpy().reshape(B, 3, 3), self.split_record(raw), raw
 
     def updateByScan(self, points_xy, robot_pose_world, origo=None):
         pts = _f32(points_xy).reshape(-1, 2)

@@ -98,6 +98,7 @@ struct hsb_handle {
   int tune_warps_per_scan = 0, tune_scans_per_block = 0, tune_stage_smem = 1, tune_chunk = 0, tune_unroll = 0, tune_packed = 0, tune_seq = 0, tune_partial = 1, tune_prefetch = 0, tune_trace = 0, tune_pace = 0, tune_pdl = 1, tune_auto_group = 1, tune_stagger = 0;
   DevBuf d_trace;
   DevBuf d_best;   // arg-max accumulator of hsb_best_hypothesis_device
+  DevBuf d_record; // per-evaluation record of hsb_match_data_record
   bool map_write_pending = false;   // a nowait SLAM step's map write may still be running on `stream`
   unsigned step_seq = 0;   // sequence number of the fused SLAM steps (host polling, hsb_slam_update_nowait)
   int trace_scans = 0;
@@ -449,6 +450,11 @@ void fill_match_params(const hsb_handle* h, HsbMatchParams& P) {
   memset(&P, 0, sizeof(P));
   P.levels = h->levels;
   for (int l = 0; l < h->levels; ++l) fill_level_dev(h, l, P.lv[l]);
+  int off = 0;   // the record holds the levels coarsest first
+  for (int l = h->levels - 1; l >= 0; --l) {
+    P.lv[l].rec_off = off;
+    off += 3 + 15 * P.lv[l].evals;
+  }
 }
 
 int destroy_level(hsb_handle* h, Level& L) {
@@ -668,7 +674,7 @@ int hsb_destroy(hsb_handle* h) {
   cudaDeviceSynchronize();
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
-                    &h->d_beam_cs, &h->d_ranges, &h->d_occ, &h->d_trace, &h->d_best,
+                    &h->d_beam_cs, &h->d_ranges, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
                     &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_cloud1};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
@@ -814,9 +820,19 @@ int hsb_world_coords_pose(const hsb_handle* h, int level, const float map[3], fl
 
 // ---- matching ----------------------------------------------------------------------------------
 
+// R of HsbMatchParams::record: floats of one scan's per-evaluation record
+static int record_floats(const hsb_handle* h) {
+  int r = 0;
+  for (int l = 0; l < h->levels; ++l) r += 3 + 15 * h->lv[l].evals;
+  return r;
+}
+
+int hsb_get_match_record_floats(const hsb_handle* h) { return h ? record_floats(h) : HSB_ERR_INVALID_ARG; }
+
 static int match_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets, int n_shared,
                         int max_points_per_scan, float* d_out_poses, float* d_out_cov, float* gate_state, const float* gate_in,
-                        float* gate_out_host, cudaStream_t stream, unsigned* seq_host = nullptr, unsigned seq_value = 0) {
+                        float* gate_out_host, cudaStream_t stream, unsigned* seq_host = nullptr, unsigned seq_value = 0,
+                        float* d_record = nullptr) {
   if (!h || B < 0 || !d_hints || !d_out_poses) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   if (!d_offsets && n_shared < 0) return fail(h, HSB_ERR_INVALID_ARG, "shared-scan mode needs n_shared >= 0");
@@ -836,6 +852,8 @@ static int match_device(hsb_handle* h, int B, const float* d_hints, const float*
   P.gate_out_host = gate_out_host;
   P.seq_host = seq_host;
   P.seq_value = seq_value;
+  P.record = d_record;
+  P.record_floats = record_floats(h);
   int max_n = d_offsets ? max_points_per_scan : n_shared;
   if (max_n < 0) max_n = 0;
   return launch_match(h, P, max_n, stream);
@@ -847,8 +865,16 @@ int hsb_match_batch_device(hsb_handle* h, int B, const float* d_hints, const flo
                       nullptr, (cudaStream_t)stream);
 }
 
-int hsb_match_data(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2], float out_pose[3],
-                   float cov_inout[9]) {
+int hsb_match_batch_record_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets,
+                                  int n_shared, int max_points_per_scan, float* d_out_poses, float* d_out_cov, float* d_record,
+                                  void* stream) {
+  if (!d_record) return HSB_ERR_INVALID_ARG;
+  return match_device(h, B, d_hints, d_pts, d_offsets, n_shared, max_points_per_scan, d_out_poses, d_out_cov, nullptr, nullptr,
+                      nullptr, (cudaStream_t)stream, nullptr, 0, d_record);
+}
+
+static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2], float out_pose[3],
+                           float cov_inout[9], float* record_out) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
   DeviceGuard guard(h->device);
   // MapRepMultiMap::matchData fills dataContainers[] from this scan (MapRepMultiMap.h:127) whenever
@@ -865,6 +891,12 @@ int hsb_match_data(hsb_handle* h, const float hint[3], const float* pts, int n, 
   const bool host_out = h->tune_host_out != 0;
   float* o_pose = host_out ? h->h_pin_dev + 4 : d_s + 4;
   float* o_cov = host_out ? h->h_pin_dev + 8 : d_s + 8;
+  const int R = record_floats(h);
+  float* d_rec = nullptr;
+  if (record_out) {
+    if ((s = ensure(h, h->d_record, (size_t)R * sizeof(float))) != HSB_OK) return s;
+    d_rec = static_cast<float*>(h->d_record.p);
+  }
   if (inline_scan_applies(h, n)) {
     // ... and the scan goes in with the launch itself: no host-to-device copy operation either; the kernel leaves
     // the endpoints in d_last_pts for hsb_update_by_scan's coarse levels
@@ -873,17 +905,32 @@ int hsb_match_data(hsb_handle* h, const float hint[3], const float* pts, int n, 
     fill_match_params(h, P);
     P.out_poses = o_pose;
     P.out_cov = o_cov;
+    P.record = d_rec;
+    P.record_floats = R;
     s = launch_match_inline(h, P, hint, 3, pts, n, scan_points(h->d_last_pts), st);
   } else {
     if ((s = upload_scan(h, h->d_last_pts, hint, 3, pts, n, st)) != HSB_OK) return s;   // header [0..2] = hint
-    s = hsb_match_batch_device(h, 1, scan_header(h->d_last_pts), scan_points(h->d_last_pts), nullptr, n, n, o_pose, o_cov, st);
+    s = match_device(h, 1, scan_header(h->d_last_pts), scan_points(h->d_last_pts), nullptr, n, n, o_pose, o_cov, nullptr,
+                     nullptr, nullptr, st, nullptr, 0, d_rec);
   }
   if (s != HSB_OK) return s;
   if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 4, d_s + 4, 13 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (record_out) HSB_CUDA(h, cudaMemcpyAsync(record_out, d_rec, (size_t)R * sizeof(float), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
   memcpy(out_pose, h->h_pin + 4, 3 * sizeof(float));
   if (cov_inout && n > 0) memcpy(cov_inout, h->h_pin + 8, 9 * sizeof(float));
   return HSB_OK;
+}
+
+int hsb_match_data(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2], float out_pose[3],
+                   float cov_inout[9]) {
+  return match_data_impl(h, hint, pts, n, origo, out_pose, cov_inout, nullptr);
+}
+
+int hsb_match_data_record(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
+                          float out_pose[3], float cov_inout[9], float* record_out) {
+  if (!record_out) return HSB_ERR_INVALID_ARG;
+  return match_data_impl(h, hint, pts, n, origo, out_pose, cov_inout, record_out);
 }
 
 int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const float* pts, int n, float H_out[9],

@@ -19,6 +19,7 @@ struct HsbLevelDev {
   float wtm[6];              // world_T_map  m[2][3] row-major
   int evals;                 // maxIterations + 1 (ScanMatcher.h:74,94)
   float pt_scale;            // 2^-level (MapRepMultiMap.h:127)
+  int rec_off;               // where this level's part of a scan's per-evaluation record starts (HsbMatchParams::record)
 };
 
 struct HsbMatchParams {
@@ -65,6 +66,15 @@ struct HsbMatchParams {
   int prefetch;             // != 0: L2 bulk prefetch of the part of a scan that is read from global memory
   // diagnostics (hsb_set_tuning "trace"): per scan 8 x u64 = {start, after coarsest level, ..., end (slot 1+levels), -, smid (slot 7)}
   unsigned long long* trace;
+  // per-evaluation record (hsb_match_data_record / hsb_match_batch_record_device), nullptr = none.  Scan b owns
+  // record[b * record_floats ..], record_floats = R = sum over levels of (3 + 15 * evals).  Per level, coarsest first:
+  //   [3]  the world pose the level starts from (ScanMatcher::matchData's beginEstimateWorld)
+  //   then for every evaluation e = 0 .. evals-1, 15 floats:
+  //   [9]  H row-major, [3] dTr, [3] the estimate after e's step in the level's map cells, angle not normalised
+  //        (equal to the estimate before it when the H(0,0) != 0 && H(1,1) != 0 gate skipped the step)
+  // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.
+  float* record;
+  int record_floats;
 };
 
 struct HsbUpdateLevelDev {

@@ -860,11 +860,19 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     float wx = hint[0], wy = hint[1], wpsi = hint[2];
     Acc last;
     acc_zero(last);
+    // per-evaluation record (hsb_internal.h HsbMatchParams::record): thread 0 stores what the group holds anyway.  The
+    // address is formed from the kernel parameters at each store (level offsets precomputed on the host), so that the
+    // evaluation loop carries no extra live register for it
+    const bool recording = P.record && t == 0;
     if (n > 0) {
       for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
         const HsbLevelDev& L = P.lv[lvl];
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
+        if (recording) {
+          float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off;
+          rec[0] = wx; rec[1] = wy; rec[2] = wpsi;
+        }
         affine_apply_exact(L.mtw, wx, wy, ex, ey);  // ScanMatcher.h:70 getMapCoordsPose
         for (int e = 0; e < L.evals; ++e) {          // ScanMatcher.h:74 + :94-97
           // OccGridMapUtil.h:70-71 and Rotation2Df (:351): sinf/cosf exactly as glibc evaluates them
@@ -938,11 +946,25 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
             ey = __fadd_rn(ey, d1);
             epsi = __fadd_rn(epsi, d2);
           }
+          if (recording) {
+            float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off + 3 + 15 * e;
+            rec[0] = a.h00; rec[1] = a.h01; rec[2] = a.h02;
+            rec[3] = a.h01; rec[4] = a.h11; rec[5] = a.h12;
+            rec[6] = a.h02; rec[7] = a.h12; rec[8] = a.h22;
+            rec[9] = a.d0;  rec[10] = a.d1; rec[11] = a.d2;
+            rec[12] = ex;   rec[13] = ey;   rec[14] = epsi;
+          }
         }
         epsi = normalize_angle(epsi);                 // ScanMatcher.h:170
         affine_apply_exact(L.wtm, ex, ey, wx, wy);    // :186 getWorldCoordsPose
         wpsi = epsi;
         if (HSB_DIAG && P.trace && t == 0) P.trace[8 * (size_t)scan + (P.levels - lvl)] = global_timer_ns();
+      }
+    } else if (recording) {   // nothing evaluated: every level starts from the hint, the evaluation slots are zero
+      for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
+        float* rec = P.record + (size_t)scan * P.record_floats + P.lv[lvl].rec_off;
+        rec[0] = wx; rec[1] = wy; rec[2] = wpsi;
+        for (int i = 3; i < 3 + 15 * P.lv[lvl].evals; ++i) rec[i] = 0.0f;
       }
     }
     if (pace && n <= 0) {   // nothing evaluated: account for the evaluations the others wait for

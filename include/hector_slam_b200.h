@@ -132,6 +132,32 @@ int hsb_match_batch_device(hsb_handle* h, int B, const float* d_hints_world, con
                            const int* d_offsets, int n_shared, int max_points_per_scan, float* d_out_poses_world,
                            float* d_out_cov, void* stream);
 
+/* ---- the match, evaluation by evaluation ---------------------------------------------------------*/
+/* What ScanMatcher::matchData (matcher/ScanMatcher.h:54-190) shows its DrawInterface and HectorDebugInfoInterface,
+ * and a little more: every Gauss-Newton evaluation of every level, written by the match kernel from the values it
+ * already holds (results are bit-identical with and without the record).  One scan's record is R floats,
+ *   R = sum over levels l of (3 + 15 * (maxIterations_l + 1))          (hsb_get_match_record_floats)
+ * and holds, per level, COARSEST FIRST:
+ *   [3]   the world pose the level starts from (matchData's beginEstimateWorld);
+ *   then for each evaluation e = 0 .. maxIterations_l, 15 floats:
+ *   [9]   H, row-major (getCompleteHessianDerivs at the estimate before e's step),
+ *   [3]   dTr,
+ *   [3]   the estimate after e's step, in the level's map cells, angle not normalised (equal to the estimate before
+ *         it when the H(0,0) != 0 && H(1,1) != 0 gate skipped the step).
+ * Evaluation 0 is the one before the loop (ScanMatcher.h:74); the hooks report evaluations 1 .. maxIterations.
+ * The last estimate of level 0, normalised and converted to world coordinates, is the returned pose, and its H is
+ * the covariance.  An empty scan writes the level start poses (all equal to the hint) and zeros in every
+ * evaluation slot. */
+int hsb_get_match_record_floats(const hsb_handle* h);
+/* hsb_match_data plus the record of that scan into `record_out` (host, R floats).  Same "last match" containers,
+ * same latency paths (tuning keys host_out, inline_scan); the record costs one extra device-to-host copy. */
+int hsb_match_data_record(hsb_handle* h, const float begin_estimate_world[3], const float* points_xy, int n,
+                          const float origo[2], float out_pose_world[3], float cov_inout[9], float* record_out);
+/* hsb_match_batch_device plus the records of all scans: d_record (device) receives B x R floats, scan b at b * R. */
+int hsb_match_batch_record_device(hsb_handle* h, int B, const float* d_hints_world, const float* d_points_xy,
+                                  const int* d_offsets, int n_shared, int max_points_per_scan, float* d_out_poses_world,
+                                  float* d_out_cov, float* d_record, void* stream);
+
 /* ---- raw laser ranges in (the step before the path: scan -> DataContainer) ---------------------*/
 /* The sensor_msgs/LaserScan fields HectorMappingRos::rosLaserScanToDataContainer reads
  * (hector_mapping/src/HectorMappingRos.cpp:483-507).  Setting a format builds the per-beam
