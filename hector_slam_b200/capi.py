@@ -35,6 +35,7 @@ EXPORTED = [
     "hsb_alloc_pinned", "hsb_free_pinned", "hsb_measure_h2d_gbs", "hsb_get_dirty_rects", "hsb_pack_dirty_device", "hsb_unpack_dirty_device", "hsb_get_replication_overflows", "hsb_get_mirror_dirty_rect", "hsb_download_level_rect", "hsb_download_occupancy_rect",
     "hsb_get_d2h_bytes", "hsb_covariance_batch", "hsb_get_map_origin", "hsb_get_dist_batch", "hsb_set_cloud_format", "hsb_cloud_to_points", "hsb_match_batch_cloud", "hsb_match_batch_cloud_device",
     "hsb_get_match_record_floats", "hsb_match_data_record", "hsb_match_batch_record_device",
+    "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update",
 ]
 
 
@@ -167,6 +168,9 @@ def load_library() -> C.CDLL:
     sig("hsb_get_last_launch_shape", i, vp, vp)
     sig("hsb_pack_rect_device", i, vp, i, vp, vp, vp)
     sig("hsb_unpack_rect_device", i, vp, i, vp, vp, vp)
+    sig("hsb_group_create", i, vp, i, C.POINTER(vp))
+    sig("hsb_group_destroy", i, vp)
+    sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
     _lib = L
     return L
 
@@ -795,3 +799,60 @@ class MapRepB200:
 
     def refresh_level(self, level: int, stream: int = 0):
         self._check(self.lib.hsb_refresh_level(self.h, level, stream))
+
+
+class SlamGroup:
+    """HectorSlamProcessor::update for several MapRepB200 handles — one SLAM session, one map each — in one device pass
+    (hsb_group_slam_update).  Each session's results and its handle's state equal a slam_update() on that handle bit for
+    bit.  The group does not own the handles: close() it before closing any of them."""
+
+    def __init__(self, reps):
+        self.lib = load_library()
+        self.reps = list(reps)
+        self.M = len(self.reps)
+        arr = (C.c_void_p * max(1, self.M))(*[None if r is None else r.h for r in self.reps])
+        g = C.c_void_p()
+        st = self.lib.hsb_group_create(C.cast(arr, C.c_void_p), self.M, C.byref(g))
+        if st != 0:
+            raise HsbError(st, (self.lib.hsb_last_error(None) or b"").decode())
+        self.g = g
+
+    def _check(self, st: int):
+        if st != 0:
+            raise HsbError(st, (self.lib.hsb_last_error(self.reps[0].h) or b"").decode())
+
+    def slam_update(self, hints, scans, origo=None, map_without_matching=None, nowait: bool = False, cov_inout=None):
+        """scans: M (n_s, 2) endpoint arrays, or a tuple (points (N, 2), offsets (M + 1,)).  hints (M, 3), origo (M, 2),
+        map_without_matching (M,) bools.  -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool); a cov entry keeps its
+        cov_inout value (zeros if None) where the session matched nothing."""
+        M = self.M
+        h = _f32(hints).reshape(M, 3)
+        if isinstance(scans, tuple):
+            pts = _f32(scans[0]).reshape(-1, 2)
+            offsets = np.ascontiguousarray(scans[1], dtype=np.int32)
+        else:
+            scans = [_f32(s).reshape(-1, 2) for s in scans]
+            assert len(scans) == M, (len(scans), M)
+            offsets = np.zeros(M + 1, np.int32)
+            offsets[1:] = np.cumsum([s.shape[0] for s in scans])
+            pts = np.concatenate(scans) if offsets[-1] else np.zeros((0, 2), np.float32)
+        og = None if origo is None else _f32(origo).reshape(M, 2)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
+        poses = np.zeros((M, 3), np.float32)
+        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
+        upd = np.zeros(M, np.int32)
+        self._check(self.lib.hsb_group_slam_update(self.g, h.ctypes.data, pts.ctypes.data if pts.size else None,
+                                                   offsets.ctypes.data, _ptr(og), _ptr(mwm), int(bool(nowait)),
+                                                   poses.ctypes.data, cov.ctypes.data, upd.ctypes.data))
+        return poses, cov.reshape(M, 3, 3), upd.astype(bool)
+
+    def close(self):
+        if getattr(self, "g", None):
+            self.lib.hsb_group_destroy(self.g)
+            self.g = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -100,6 +100,11 @@ struct hsb_handle {
   DevBuf d_best;   // arg-max accumulator of hsb_best_hypothesis_device
   DevBuf d_record; // per-evaluation record of hsb_match_data_record
   bool map_write_pending = false;   // a nowait SLAM step's map write may still be running on `stream`
+  // group steps (hsb_group_slam_update) run on the group's stream: the event of the last nowait step this handle took
+  // part in, which the handle's stream waits on before its next own operation (HandleScope) ...
+  cudaEvent_t group_ev = nullptr;
+  // ... and whether the handle may have queued work of its own since its last group step, which that step then waits for
+  bool queued = false;
   unsigned step_seq = 0;   // sequence number of the fused SLAM steps (host polling, hsb_slam_update_nowait)
   int trace_scans = 0;
   int last_shape[6] = {0, 0, 0, 0, 0, 0};  // W, G, U, staged points per scan (0 = none), grid, resident CTAs / SM
@@ -139,6 +144,23 @@ struct DeviceGuard {
   }
   ~DeviceGuard() {
     if (prev >= 0) cudaSetDevice(prev);
+  }
+};
+
+// Every entry point that works on a handle's streams opens one of these: it selects the handle's device and orders the
+// handle's stream behind the last nowait group step the handle took part in.  A group step records ONE event instead of
+// making each member's streams wait on it; a member waits here, lazily, before its next own operation (and a member that
+// takes only group steps never waits).  It also notes that the handle may now have work of its own queued, which its
+// next group step orders itself behind.
+struct HandleScope {
+  DeviceGuard dev;
+  explicit HandleScope(hsb_handle* h) : dev(h->device) {
+    if (h->group_ev) {
+      // (a failure here is the context's: the next CUDA call of the entry point reports it)
+      cudaStreamWaitEvent(h->stream, h->group_ev, 0);
+      h->group_ev = nullptr;
+    }
+    h->queued = true;
   }
 };
 
@@ -238,12 +260,12 @@ void fill_level_dev(const hsb_handle* h, int l, HsbLevelDev& d) {
 }
 
 // ---- match launch -----------------------------------------------------------------------------
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false>
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false>
 int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int Gr,
                    const hsb::InlineScan<INL>& S = hsb::InlineScan<INL>()) {
   if (Gr <= 0 || Gr > G) Gr = G;   // groups per CTA actually launched (a G-group kernel runs with fewer: see launch_match)
   const size_t header = hsb::MatchSmem<W, G>::kHeaderBytes;
-  auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL>;
+  auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL, GRP>;
   constexpr size_t kMaxDyn = 232448;   // dynamic shared memory one CTA may ask for (227 KB)
   constexpr int gt = W * 32;           // threads per scan
   int cap = 0;
@@ -502,7 +524,7 @@ int hsb_get_last_launch_shape(const hsb_handle* h, int out[6]) {
 
 int hsb_get_last_update_device_ms(hsb_handle* h, float* ms) {
   if (!h || !ms) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HSB_CUDA(h, cudaEventSynchronize(h->ev_time[1]));
   HSB_CUDA(h, cudaEventElapsedTime(ms, h->ev_time[0], h->ev_time[1]));
   return HSB_OK;
@@ -510,7 +532,7 @@ int hsb_get_last_update_device_ms(hsb_handle* h, float* ms) {
 
 int hsb_read_trace(hsb_handle* h, uint64_t* out, int max_scans) {
   if (!h || !out || max_scans < 0) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   const int n = std::min(max_scans, h->trace_scans);
   if (n > 0) HSB_CUDA(h, cudaMemcpy(out, h->d_trace.p, (size_t)n * 64, cudaMemcpyDeviceToHost));
   return n;
@@ -544,7 +566,7 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
   h->cfg = *cfg;
   h->device = cfg->device;
   h->levels = cfg->levels;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int status = HSB_OK;
   auto bail = [&](int code) {
     g_create_error = h->err;
@@ -670,7 +692,7 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
 
 int hsb_destroy(hsb_handle* h) {
   if (!h) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   cudaDeviceSynchronize();
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
@@ -743,7 +765,7 @@ static int reset_gate(hsb_handle* h) {
 
 int hsb_reset(hsb_handle* h) {
   if (!h) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   for (int l = 0; l < h->levels; ++l) {
     int s = clear_level(h, l, h->stream);
     if (s != HSB_OK) return s;
@@ -837,7 +859,7 @@ static int match_device(hsb_handle* h, int B, const float* d_hints, const float*
   if (B == 0) return HSB_OK;
   if (!d_offsets && n_shared < 0) return fail(h, HSB_ERR_INVALID_ARG, "shared-scan mode needs n_shared >= 0");
   if (!d_pts && (d_offsets || n_shared > 0)) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HsbMatchParams P;
   fill_match_params(h, P);
   P.B = B;
@@ -876,7 +898,7 @@ int hsb_match_batch_record_device(hsb_handle* h, int B, const float* d_hints, co
 static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2], float out_pose[3],
                            float cov_inout[9], float* record_out) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   // MapRepMultiMap::matchData fills dataContainers[] from this scan (MapRepMultiMap.h:127) whenever
   // there is a coarse level; hsb_update_by_scan reuses it for the coarse levels (:143).
   int s = ensure(h, h->d_scratch, 64 * sizeof(float));
@@ -937,7 +959,7 @@ int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const 
                        float dTr_out[3]) {
   if (!h || level < 0 || level >= h->levels || !pose_map || n < 0 || (n > 0 && !pts) || !H_out || !dTr_out)
     return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
@@ -965,7 +987,7 @@ int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const 
 
 int hsb_set_scan_format(hsb_handle* h, const hsb_scan_format* fmt) {
   if (!h || !fmt || fmt->n_beams < 1 || fmt->n_beams > (1 << 20)) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s = ensure(h, h->d_beam_cs, (size_t)fmt->n_beams * 8);
   if (s != HSB_OK) return s;
   std::vector<float> tab((size_t)fmt->n_beams * 2);
@@ -995,7 +1017,7 @@ static void fill_range_params(const hsb_handle* h, HsbMatchParams& P, const floa
 int hsb_scan_to_points(hsb_handle* h, const float* ranges, float* out_xy, int* out_n) {
   if (!h || !ranges || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
   if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   const int nb = h->fmt.n_beams;
   int s;
   if ((s = ensure(h, h->d_ranges, (size_t)nb * 4)) != HSB_OK) return s;
@@ -1024,7 +1046,7 @@ int hsb_match_batch_ranges_device(hsb_handle* h, int B, const float* d_hints, co
   if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
   if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
   if (B == 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HsbMatchParams P;
   fill_match_params(h, P);
   P.B = B;
@@ -1063,7 +1085,7 @@ static void fill_cloud_params(const hsb_handle* h, HsbMatchParams& P, const floa
 int hsb_cloud_to_points(hsb_handle* h, const float* points_xyz, int n, float* out_xy, int* out_n, float out_origo[2]) {
   if (!h || n < 0 || (n > 0 && !points_xyz) || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
   if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   if ((s = ensure(h, h->d_cloud, (size_t)(n > 0 ? n : 1) * 12)) != HSB_OK) return s;
   if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
@@ -1099,7 +1121,7 @@ int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, con
   if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
   if (B == 0) return HSB_OK;
   if (!d_points_xyz && max_points_per_scan > 0) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HsbMatchParams P;
   fill_match_params(h, P);
   P.B = B;
@@ -1270,7 +1292,7 @@ int hsb_match_batch_submit(hsb_handle* h, int B, const float* hints, const float
     if (ticket) *ticket = -1;
     return HSB_OK;
   }
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HostBatch hb;
   hb.kind = IN_ENDPOINTS;
   hb.B = B;
@@ -1297,7 +1319,7 @@ int hsb_match_batch_ranges_submit(hsb_handle* h, int B, const float* hints, cons
     if (ticket) *ticket = -1;
     return HSB_OK;
   }
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HostBatch hb;
   hb.kind = IN_RANGES;
   hb.B = B;
@@ -1321,7 +1343,7 @@ int hsb_match_batch_cloud_submit(hsb_handle* h, int B, const float* hints, const
     if (ticket) *ticket = -1;
     return HSB_OK;
   }
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HostBatch hb;
   hb.kind = IN_CLOUD;
   hb.B = B;
@@ -1342,13 +1364,13 @@ int hsb_match_batch_cloud(hsb_handle* h, int B, const float* hints, const float*
 int hsb_match_batch_wait(hsb_handle* h, int ticket) {
   if (!h || ticket < -1 || ticket > 1) return HSB_ERR_INVALID_ARG;
   if (ticket < 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   return wait_set(h, ticket);
 }
 
 int hsb_measure_h2d_gbs(hsb_handle* h, const void* host, size_t bytes, int reps, float* out_gbs) {
   if (!h || !host || !bytes || reps < 1 || !out_gbs) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s = ensure(h, h->d_occ, bytes);
   if (s != HSB_OK) return s;
   cudaStream_t st = h->stream;
@@ -1430,10 +1452,11 @@ static int run_update(hsb_handle* h, HsbUpdateParams& P, int max_n) {
   return HSB_OK;
 }
 
-static int next_stamp_base(hsb_handle* h, int level, uint32_t* base) {
+// `st`: the stream the map write goes to (the handle's, or a group's)
+static int next_stamp_base(hsb_handle* h, int level, uint32_t* base, cudaStream_t st) {
   Level& L = h->lv[level];
   if (L.stamp_base > 0xfffffff0u - 8u) {  // wrap guard: forget old stamps
-    HSB_CUDA(h, cudaMemsetAsync(L.stamp, 0, (size_t)L.sx * L.sy * sizeof(uint32_t), h->stream));
+    HSB_CUDA(h, cudaMemsetAsync(L.stamp, 0, (size_t)L.sx * L.sy * sizeof(uint32_t), st));
     L.stamp_base = 0;
   }
   *base = L.stamp_base;
@@ -1490,7 +1513,7 @@ static int enqueue_update_by_scan(hsb_handle* h, const float2* d_pts0, int n, co
     // an empty container still advances the stamps in the reference (OccGridMapBase.h:164-167); no-op here
     d.active = d.n > 0;
     if (d.active) {
-      if ((s = next_stamp_base(h, l, &d.stamp_base)) != HSB_OK) return s;
+      if ((s = next_stamp_base(h, l, &d.stamp_base, h->stream)) != HSB_OK) return s;
       if (d.n > max_n) max_n = d.n;
     }
   }
@@ -1499,7 +1522,7 @@ static int enqueue_update_by_scan(hsb_handle* h, const float2* d_pts0, int n, co
 
 int hsb_update_by_scan(hsb_handle* h, const float* pts, int n, const float origo[2], const float pose[3]) {
   if (!h || !pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   cudaStream_t st = h->stream;
   if ((s = upload_scan(h, h->d_upd_pts, nullptr, 0, pts, n, st)) != HSB_OK) return s;
@@ -1523,7 +1546,7 @@ int hsb_set_map_update_min_angle_diff(hsb_handle* h, float min_angle) {
 static int slam_update_impl(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
                             int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated, bool wait_map) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
@@ -1620,7 +1643,7 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
                           int* out_kept) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
   if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
@@ -1726,7 +1749,7 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
 
 int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
   if (!h || !pose) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s = ensure(h, h->d_gate, 4 * sizeof(float));
   if (s != HSB_OK) return s;
   memcpy(h->h_pin + 56, pose, 3 * sizeof(float));
@@ -1737,7 +1760,7 @@ int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
 
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]) {
   if (!h || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   if (!h->d_gate.p) {
     int s = reset_gate(h);
     if (s != HSB_OK) return s;
@@ -1750,7 +1773,7 @@ int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]) {
 
 int hsb_update_level_by_scan(hsb_handle* h, int level, const float* pts, int n, const float origo[2], const float pose[3]) {
   if (!h || level < 0 || level >= h->levels || !pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   cudaStream_t st = h->stream;
   if ((s = upload_scan(h, h->d_upd_pts, nullptr, 0, pts, n, st)) != HSB_OK) return s;
@@ -1768,7 +1791,7 @@ int hsb_update_level_by_scan(hsb_handle* h, int level, const float* pts, int n, 
   d.origo_x = origo ? origo[0] : 0.f;
   d.origo_y = origo ? origo[1] : 0.f;
   d.active = n > 0;
-  if (d.active && (s = next_stamp_base(h, level, &d.stamp_base)) != HSB_OK) return s;
+  if (d.active && (s = next_stamp_base(h, level, &d.stamp_base, h->stream)) != HSB_OK) return s;
   if ((s = run_update(h, P, n)) != HSB_OK) return s;
   HSB_CUDA(h, cudaStreamSynchronize(st));
   return HSB_OK;
@@ -1776,7 +1799,7 @@ int hsb_update_level_by_scan(hsb_handle* h, int level, const float* pts, int n, 
 
 int hsb_on_map_updated(hsb_handle* h) {
   if (!h) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
   h->map_write_pending = false;
   return HSB_OK;
@@ -1786,7 +1809,7 @@ int hsb_on_map_updated(hsb_handle* h) {
 
 int hsb_upload_level(hsb_handle* h, int level, const float* logodds_host) {
   if (!h || level < 0 || level >= h->levels || !logodds_host) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   HSB_CUDA(h, cudaMemcpyAsync(L.logodds, logodds_host, (size_t)L.sx * L.sy * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   int s = refresh_level(h, level, h->stream);
@@ -1798,7 +1821,7 @@ int hsb_upload_level(hsb_handle* h, int level, const float* logodds_host) {
 
 int hsb_download_level(hsb_handle* h, int level, float* out) {
   if (!h || level < 0 || level >= h->levels || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   HSB_CUDA(h, cudaMemcpyAsync(out, L.logodds, (size_t)L.sx * L.sy * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -1808,7 +1831,7 @@ int hsb_download_level(hsb_handle* h, int level, float* out) {
 
 int hsb_download_level_rect(hsb_handle* h, int level, const int rect[4], float* out) {
   if (!h || level < 0 || level >= h->levels || !rect || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s = check_rect(h, L, rect);
   if (s != HSB_OK) return s;
@@ -1822,7 +1845,7 @@ int hsb_download_level_rect(hsb_handle* h, int level, const int rect[4], float* 
 
 int hsb_download_occupancy_rect(hsb_handle* h, int level, const int rect[4], int8_t* out) {
   if (!h || level < 0 || level >= h->levels || !rect || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s = check_rect(h, L, rect);
   if (s != HSB_OK) return s;
@@ -1843,7 +1866,7 @@ uint64_t hsb_get_d2h_bytes(const hsb_handle* h) { return h ? h->d2h_bytes : 0; }
 
 int hsb_download_prob(hsb_handle* h, int level, float* out) {
   if (!h || level < 0 || level >= h->levels || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   if (L.arr) {  // read what the texture path sees
     HSB_CUDA(h, cudaMemcpy2DFromArrayAsync(out, (size_t)L.sx * sizeof(float), L.arr, 0, 0, (size_t)L.sx * sizeof(float), L.sy,
@@ -1857,7 +1880,7 @@ int hsb_download_prob(hsb_handle* h, int level, float* out) {
 
 int hsb_download_occupancy(hsb_handle* h, int level, int8_t* out) {
   if (!h || level < 0 || level >= h->levels || !out) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   const size_t n = (size_t)L.sx * L.sy;
   int s = ensure(h, h->d_occ, n);
@@ -1897,7 +1920,7 @@ int hsb_likelihood_batch_device(hsb_handle* h, int level, int B, const float* d_
   if (!d_offsets && n_shared < 0) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   if (!d_points_xy && (d_offsets || n_shared > 0)) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   return likelihood_device(h, level, B, d_poses_world, reinterpret_cast<const float2*>(d_points_xy), d_offsets, n_shared,
                            d_out_likelihood, (cudaStream_t)stream);
 }
@@ -1907,7 +1930,7 @@ int hsb_best_hypothesis_device(hsb_handle* h, int level, int B, const float* d_p
   if (!h || level < 0 || level >= h->levels || B < 0 || !d_best4 || (B > 0 && !d_poses_world)) return HSB_ERR_INVALID_ARG;
   if (!d_offsets && n_shared < 0) return HSB_ERR_INVALID_ARG;
   if (B > 0 && !d_points_xy && (d_offsets || n_shared > 0)) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int s;
   if (!h->d_best.p) {
     if ((s = ensure(h, h->d_best, sizeof(unsigned long long))) != HSB_OK) return s;
@@ -1927,7 +1950,7 @@ int hsb_likelihood_batch(hsb_handle* h, int level, int B, const float* poses, co
                          int n_shared, float* out) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !poses || !out) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   size_t total = offsets ? (size_t)offsets[B] : (size_t)(n_shared > 0 ? n_shared : 0);
   if (total > 0 && !pts) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
   int s;
@@ -1953,7 +1976,7 @@ int hsb_covariance_batch(hsb_handle* h, int level, int B, const float* poses, co
                          float* out_cov_map, float* out_cov_world) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !poses || (!out_cov_map && !out_cov_world)) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   size_t total = offsets ? (size_t)offsets[B] : (size_t)(n_shared > 0 ? n_shared : 0);
   if (total > 0 && !pts) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
   int s;
@@ -1989,7 +2012,7 @@ int hsb_covariance_batch(hsb_handle* h, int level, int B, const float* poses, co
 
 static int get_dirty(hsb_handle* h, int level, int which, int rect[4], int reset) {
   if (!h || level < 0 || level >= h->levels || !rect) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int* src = L.dirty + 4 * which;
   int* pin = reinterpret_cast<int*>(h->h_pin + 60);
@@ -2008,7 +2031,7 @@ int hsb_get_mirror_dirty_rect(hsb_handle* h, int level, int rect[4], int reset) 
 // All levels' replication rectangles with one copy and one synchronize (levels x 4 ints).
 int hsb_get_dirty_rects(hsb_handle* h, int* rects, int reset) {
   if (!h || !rects) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int all[HSB_MAX_LEVELS * 8];
   HSB_CUDA(h, cudaMemcpyAsync(all, h->d_dirty_all, sizeof(all), cudaMemcpyDeviceToHost, h->stream));
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -2049,7 +2072,7 @@ static int order_after(hsb_handle* h, cudaStream_t user, bool all_streams) {
 
 int hsb_pack_rect_device(hsb_handle* h, int level, const int rect[4], float* d_buf, void* stream) {
   if (!h || level < 0 || level >= h->levels || !rect || !d_buf) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s = check_rect(h, L, rect);
   if (s != HSB_OK) return s;
@@ -2065,7 +2088,7 @@ int hsb_pack_rect_device(hsb_handle* h, int level, const int rect[4], float* d_b
 
 int hsb_unpack_rect_device(hsb_handle* h, int level, const int rect[4], const float* d_buf, void* stream) {
   if (!h || level < 0 || level >= h->levels || !rect || !d_buf) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s = check_rect(h, L, rect);
   if (s != HSB_OK) return s;
@@ -2099,7 +2122,7 @@ static void fill_tile_params(hsb_handle* h, HsbTileParams& T, float* d_buf, size
 
 int hsb_pack_dirty_device(hsb_handle* h, float* d_buf, size_t capacity_bytes, int reset, void* stream) {
   if (!h || !d_buf || capacity_bytes < HSB_TILE_HEADER_WORDS * 4) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HsbTileParams T;
   fill_tile_params(h, T, d_buf, capacity_bytes);
   T.reset = reset;
@@ -2114,7 +2137,7 @@ int hsb_pack_dirty_device(hsb_handle* h, float* d_buf, size_t capacity_bytes, in
 
 int hsb_unpack_dirty_device(hsb_handle* h, const float* d_buf, size_t capacity_bytes, void* stream) {
   if (!h || !d_buf || capacity_bytes < HSB_TILE_HEADER_WORDS * 4) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   HsbTileParams T;
   fill_tile_params(h, T, const_cast<float*>(d_buf), capacity_bytes);
   int s;
@@ -2127,7 +2150,7 @@ int hsb_unpack_dirty_device(hsb_handle* h, const float* d_buf, size_t capacity_b
 
 int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset) {
   if (!h || !count) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   int* d = h->d_dirty_all + HSB_MAX_LEVELS * 8;
   HSB_CUDA(h, cudaDeviceSynchronize());
   HSB_CUDA(h, cudaMemcpy(count, d, sizeof(int), cudaMemcpyDeviceToHost));
@@ -2139,7 +2162,7 @@ int hsb_raycast_batch(hsb_handle* h, int level, int B, const int* begin_cells, c
                       int* out_hit) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !begin_cells || !end_cells || !out_dist) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s;
   if ((s = ensure(h, h->d_pts, (size_t)B * 16 + 16)) != HSB_OK) return s;      // begin | end
@@ -2177,7 +2200,7 @@ int hsb_get_dist_batch(hsb_handle* h, int level, int B, const float* begin_world
                        float* out_hit_world, int* out_found) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !begin_world || !end_world || !out_dist) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   Level& L = h->lv[level];
   int s;
   if ((s = ensure(h, h->d_pts, (size_t)B * 16 + 16)) != HSB_OK) return s;      // begin | end
@@ -2212,8 +2235,324 @@ void* hsb_level_logodds_device_ptr(hsb_handle* h, int level) {
 
 int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
   if (!h || level < 0 || level >= h->levels) return HSB_ERR_INVALID_ARG;
-  DeviceGuard guard(h->device);
+  HandleScope guard(h);
   return refresh_level(h, level, (cudaStream_t)stream);
+}
+
+}  // extern "C"
+
+// ---- group SLAM step: HectorSlamProcessor::update for M handles in one device pass ----------------------------------
+// One host-to-device copy (hints, thresholds, offsets, per-session descriptors, all scans) and three launches on the
+// group's stream, whatever M is: the match kernel with one 8-warp CTA per session (the shape hsb_slam_update uses, so
+// every session's pose, Hessian and gate decision are the single call's bits) and the gate of each session in its
+// epilogue, then mark and apply over (session, level).  The per-step handle state the single call keeps on the host
+// (stamp bases, writer slots, the last match's container size and origo) is advanced here exactly as it advances there.
+
+struct hsb_group {
+  std::vector<hsb_handle*> m;      // the members, in session order
+  int device = 0;
+  int levels = 0;
+  cudaStream_t stream = nullptr;   // every step of the group runs here
+  cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
+  HsbLevelDev* d_lv = nullptr;     // M x levels match-kernel level descriptors (a handle's planes never move)
+  float* d_res = nullptr;          // M x 4 (pose, write flag) for the map writer, then the finished-session counter
+  float* h_res = nullptr;          // mapped pinned: M x 4 (pose, flag), M x 9 Hessian, the sequence number
+  float* h_res_dev = nullptr;      // device alias of h_res
+  char* h_stage = nullptr;         // pinned staging of the step's host-to-device copy
+  size_t h_stage_bytes = 0;
+  DevBuf d_stage;
+  unsigned seq = 0;
+};
+
+namespace {
+
+// hsb_group_create's errors: hsb_last_error(NULL), and hsb_last_error(handles[0]) when that is a handle
+int group_fail(hsb_handle* h, int code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  g_create_error = buf;
+  if (h) h->err = buf;
+  return code;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_group_destroy(hsb_group* g) {
+  if (!g) return HSB_OK;
+  DeviceGuard guard(g->device);
+  if (g->stream) cudaStreamSynchronize(g->stream);
+  for (hsb_handle* h : g->m)
+    if (h->group_ev == g->ev) h->group_ev = nullptr;   // the step it would wait for is complete
+  if (g->d_lv) cudaFree(g->d_lv);
+  if (g->d_res) cudaFree(g->d_res);
+  if (g->d_stage.p) cudaFree(g->d_stage.p);
+  if (g->h_res) cudaFreeHost(g->h_res);
+  if (g->h_stage) cudaFreeHost(g->h_stage);
+  if (g->ev) cudaEventDestroy(g->ev);
+  if (g->stream) cudaStreamDestroy(g->stream);
+  delete g;
+  return HSB_OK;
+}
+
+int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
+  if (!out) return group_fail(nullptr, HSB_ERR_INVALID_ARG, "hsb_group_create: out is NULL");
+  *out = nullptr;
+  hsb_handle* h0 = (handles && M > 0) ? handles[0] : nullptr;
+  if (!handles || M < 1) return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: a group needs M >= 1 handles (M = %d)", M);
+  for (int s = 0; s < M; ++s)
+    if (!handles[s]) return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: handle %d is NULL", s);
+  {
+    std::vector<hsb_handle*> sorted(handles, handles + M);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+      return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: a handle is listed twice");
+  }
+  for (int s = 1; s < M; ++s) {
+    const hsb_handle* h = handles[s];
+    if (h->device != h0->device)
+      return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: handle %d is on device %d, handle 0 on device %d", s,
+                        h->device, h0->device);
+    bool same = h->levels == h0->levels && h->cfg.map_size_x == h0->cfg.map_size_x &&
+                h->cfg.map_size_y == h0->cfg.map_size_y && h->cfg.map_resolution == h0->cfg.map_resolution &&
+                h->cfg.start_x == h0->cfg.start_x && h->cfg.start_y == h0->cfg.start_y && h->gather_mode == h0->gather_mode;
+    for (int l = 0; same && l < h0->levels; ++l) same = h->lv[l].evals == h0->lv[l].evals;
+    if (!same)
+      return group_fail(h0, HSB_ERR_INVALID_ARG,
+                        "hsb_group_create: handle %d differs from handle 0 in levels, map size, resolution, start, "
+                        "max_iterations or gather mode", s);
+  }
+  DeviceGuard guard(h0->device);
+  hsb_group* g = new (std::nothrow) hsb_group();
+  if (!g) return group_fail(h0, HSB_ERR_OUT_OF_MEMORY, "hsb_group_create: out of host memory");
+  g->m.assign(handles, handles + M);
+  g->device = h0->device;
+  g->levels = h0->levels;
+#define HSB_GROUP_CUDA(expr)                                                                                 \
+  do {                                                                                                       \
+    cudaError_t _e = (expr);                                                                                 \
+    if (_e != cudaSuccess) {                                                                                 \
+      const int _code = _e == cudaErrorMemoryAllocation ? HSB_ERR_OUT_OF_MEMORY : HSB_ERR_CUDA;              \
+      group_fail(h0, _code, "hsb_group_create: %s failed: %s", #expr, cudaGetErrorString(_e));               \
+      hsb_group_destroy(g);                                                                                  \
+      return _code;                                                                                          \
+    }                                                                                                        \
+  } while (0)
+  // the gate state a member's first SLAM step would create (lastMapUpdatePose = FLT_MAX, HectorSlamProcessor.h:117)
+  for (hsb_handle* h : g->m) {
+    if (h->d_gate.p) continue;
+    HandleScope scope(h);
+    const int s = reset_gate(h);
+    if (s != HSB_OK) {
+      group_fail(h0, s, "hsb_group_create: %s", h->err.c_str());
+      hsb_group_destroy(g);
+      return s;
+    }
+    HSB_GROUP_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  HSB_GROUP_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
+  HSB_GROUP_CUDA(cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming));
+  {
+    std::vector<HsbLevelDev> lv((size_t)M * g->levels);
+    memset(lv.data(), 0, lv.size() * sizeof(HsbLevelDev));
+    for (int s = 0; s < M; ++s)
+      for (int l = 0; l < g->levels; ++l) fill_level_dev(g->m[s], l, lv[(size_t)s * g->levels + l]);
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_lv, lv.size() * sizeof(HsbLevelDev)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_lv, lv.data(), lv.size() * sizeof(HsbLevelDev), cudaMemcpyHostToDevice));
+  }
+  HSB_GROUP_CUDA(cudaMalloc(&g->d_res, ((size_t)M * 4 + 4) * sizeof(float)));
+  HSB_GROUP_CUDA(cudaMemset(g->d_res, 0, ((size_t)M * 4 + 4) * sizeof(float)));
+  HSB_GROUP_CUDA(cudaHostAlloc(&g->h_res, ((size_t)M * 13 + 4) * sizeof(float), cudaHostAllocMapped));
+  memset(g->h_res, 0, ((size_t)M * 13 + 4) * sizeof(float));
+  HSB_GROUP_CUDA(cudaHostGetDevicePointer(&g->h_res_dev, g->h_res, 0));
+#undef HSB_GROUP_CUDA
+  *out = g;
+  return HSB_OK;
+}
+
+int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_xy, const int* offsets, const float* origo,
+                          const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  hsb_handle* h0 = g->m[0];
+  const int M = (int)g->m.size(), levels = g->levels;
+  if (!hints || !offsets || !out_poses)
+    return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: hints, offsets and out_poses must not be NULL");
+  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: offsets[0] is %d, must be 0", offsets[0]);
+  int max_n = 0;
+  for (int k = 0; k < M; ++k) {
+    const int n = offsets[k + 1] - offsets[k];
+    if (n < 0)
+      return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: offsets decrease at session %d (%d -> %d)", k, offsets[k],
+                  offsets[k + 1]);
+    max_n = std::max(max_n, n);
+  }
+  const int total = offsets[M];
+  if (total > 0 && !points_xy) return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: points_xy is NULL");
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  int s;
+  // not before the work the members queued themselves, nor before a pending step of another group they belong to
+  for (hsb_handle* h : g->m) {
+    if (h->group_ev && h->group_ev != g->ev) HSB_CUDA(h0, cudaStreamWaitEvent(st, h->group_ev, 0));
+    if (h->queued) {
+      if ((s = order_before(h, st, true)) != HSB_OK) return s;
+      h->queued = false;
+    }
+  }
+
+  // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments | scans
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t o_gin = al((size_t)M * 12), o_off = al(o_gin + (size_t)M * 12), o_sess = al(o_off + (size_t)(M + 1) * 4);
+  const size_t o_upd = al(o_sess + (size_t)M * sizeof(HsbGroupSessionDev));
+  const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_pts = al(o_lo + (size_t)M * 8);
+  const size_t bytes = o_pts + (size_t)total * 8;
+  if (bytes > g->h_stage_bytes) {
+    if (g->h_stage) cudaFreeHost(g->h_stage);
+    g->h_stage = nullptr;
+    g->h_stage_bytes = 0;
+    const size_t cap = bytes < (64u << 10) ? (64u << 10) : bytes + bytes / 2;
+    HSB_CUDA(h0, cudaMallocHost(reinterpret_cast<void**>(&g->h_stage), cap));
+    g->h_stage_bytes = cap;
+  }
+  if ((s = ensure(h0, g->d_stage, bytes)) != HSB_OK) return s;
+  char* hs = g->h_stage;
+  const char* ds = static_cast<const char*>(g->d_stage.p);
+  float* s_gin = reinterpret_cast<float*>(hs + o_gin);
+  HsbGroupSessionDev* s_sess = reinterpret_cast<HsbGroupSessionDev*>(hs + o_sess);
+  HsbUpdateLevelDev* s_upd = reinterpret_cast<HsbUpdateLevelDev*>(hs + o_upd);
+  float2* s_lo = reinterpret_cast<float2*>(hs + o_lo);
+  const float2* d_pts = reinterpret_cast<const float2*>(ds + o_pts);
+  memcpy(hs, hints, (size_t)M * 12);
+  memcpy(hs + o_off, offsets, (size_t)(M + 1) * 4);
+  if (total > 0) memcpy(hs + o_pts, points_xy, (size_t)total * 8);
+  int max_upd = 0;
+  for (int k = 0; k < M; ++k) {
+    hsb_handle* h = g->m[k];
+    const int n = offsets[k + 1] - offsets[k];
+    const bool matched = !(map_without_matching && map_without_matching[k]);
+    const float ox = origo ? origo[2 * k] : 0.f, oy = origo ? origo[2 * k + 1] : 0.f;
+    s_gin[3 * k] = h->min_dist;
+    s_gin[3 * k + 1] = h->min_angle;
+    s_gin[3 * k + 2] = matched ? 0.f : 1.f;
+    s_lo[k] = make_float2(h->log_odds_free, h->log_odds_occ);
+    s_sess[k].gate_state = static_cast<float*>(h->d_gate.p);
+    s_sess[k].last_pts = nullptr;
+    if (matched) {   // this scan becomes the last match's container (without matching the old one stays, :77-81)
+      if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
+      s_sess[k].last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
+      h->last_n = n;
+      h->last_origo[0] = ox;
+      h->last_origo[1] = oy;
+    }
+    // MapRepMultiMap::updateByScan: level 0 from this scan, the coarse levels from the last match's container (:143)
+    for (int l = 0; l < levels; ++l) {
+      HsbUpdateLevelDev& d = s_upd[(size_t)k * levels + l];
+      fill_update_level(h, l, d);
+      d.pt_scale = (float)(1.0 / pow(2.0, (double)l));
+      if (l == 0 || matched) {
+        d.pts = d_pts + offsets[k];
+        d.n = n;
+        d.origo_x = ox;
+        d.origo_y = oy;
+      } else {
+        d.pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+        d.n = h->last_n;
+        d.origo_x = h->last_origo[0];
+        d.origo_y = h->last_origo[1];
+      }
+      d.active = d.n > 0;
+      if (d.active) {
+        if ((s = next_stamp_base(h, l, &d.stamp_base, st)) != HSB_OK) return s;
+        max_upd = std::max(max_upd, d.n);
+      }
+    }
+  }
+  HSB_CUDA(h0, cudaMemcpyAsync(g->d_stage.p, hs, bytes, cudaMemcpyHostToDevice, st));
+
+  // K1: match + gate, one session per CTA; the last session to finish publishes the step's sequence number
+  HsbMatchParams P;
+  fill_match_params(h0, P);
+  P.B = M;
+  P.hints = reinterpret_cast<const float*>(ds);
+  P.pts = d_pts;
+  P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.out_poses = g->d_res;
+  P.out_cov = g->h_res_dev + 4 * (size_t)M;
+  P.gate_in = reinterpret_cast<const float*>(ds + o_gin);
+  P.gate_out_host = g->h_res_dev;
+  P.seq_host = reinterpret_cast<unsigned*>(g->h_res_dev + 13 * (size_t)M);
+  P.seq_value = ++g->seq;
+  P.group_lv = g->d_lv;
+  P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
+  P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
+  s = h0->gather_mode == HSB_GATHER_TEX ? launch_match_t<8, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
+                                        : launch_match_t<8, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
+  if (s != HSB_OK) return s;
+
+  // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
+  // one-wave grids are shared out among the sessions
+  HsbGroupUpdateParams U;
+  U.lv = reinterpret_cast<const HsbUpdateLevelDev*>(ds + o_upd);
+  U.log_odds = reinterpret_cast<const float2*>(ds + o_lo);
+  U.res = g->d_res;
+  U.levels = levels;
+  constexpr int TEAM = 2;
+  const int slots = M * levels;
+  const int blocks = std::max(1, std::min((max_upd * TEAM + 7) / 8, (h0->sm_count * 6 + slots - 1) / slots));
+  static int apply_ctas_per_sm = 0;
+  if (!apply_ctas_per_sm) {
+    int nb = 0;
+    HSB_CUDA(h0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hsb::update_apply_group_kernel, 256, 0));
+    apply_ctas_per_sm = nb > 0 ? nb : 4;
+  }
+  const int sweep = std::max(1, (h0->sm_count * apply_ctas_per_sm + slots - 1) / slots);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(256);
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cfg.gridDim = dim3(blocks, levels, M);
+  HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_mark_group_kernel<TEAM>, U));
+  cfg.gridDim = dim3(sweep, levels, M);
+  HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_apply_group_kernel, U));
+  h0->launches += 2;
+  HSB_CUDA(h0, cudaGetLastError());
+  HSB_CUDA(h0, cudaEventRecord(g->ev, st));
+  for (hsb_handle* h : g->m) {   // every later operation of a member waits for this step (HandleScope)
+    h->group_ev = nowait ? g->ev : nullptr;
+    h->map_write_pending = nowait != 0;
+  }
+
+  if (nowait) {   // return when every pose has arrived; the map writes continue on the group's stream
+    volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(g->h_res + 13 * (size_t)M);
+    unsigned spins = 0;
+    while (*seq != P.seq_value) {
+      if ((++spins & 0xfffu) == 0) {
+        cudaError_t e = cudaStreamQuery(st);
+        if (e != cudaSuccess && e != cudaErrorNotReady) return fail(h0, HSB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
+        if (e == cudaSuccess && *seq != P.seq_value) return fail(h0, HSB_ERR_CUDA, "group step finished without publishing its poses");
+      }
+    }
+    __sync_synchronize();
+  } else {
+    HSB_CUDA(h0, cudaStreamSynchronize(st));   // :93 onMapUpdated for every member
+  }
+  for (int k = 0; k < M; ++k) {
+    const float* r = g->h_res + 4 * (size_t)k;
+    memcpy(out_poses + 3 * (size_t)k, r, 3 * sizeof(float));
+    if (map_updated) map_updated[k] = r[3] != 0.f;
+    const bool matched = !(map_without_matching && map_without_matching[k]);
+    if (cov_inout && matched && offsets[k + 1] > offsets[k])
+      memcpy(cov_inout + 9 * (size_t)k, g->h_res + 4 * (size_t)M + 9 * (size_t)k, 9 * sizeof(float));
+  }
+  return HSB_OK;
 }
 
 }  // extern "C"

@@ -22,6 +22,12 @@ struct HsbLevelDev {
   int rec_off;               // where this level's part of a scan's per-evaluation record starts (HsbMatchParams::record)
 };
 
+// One session of a group SLAM step (hsb_group_slam_update): the member handle's state the match kernel touches.
+struct HsbGroupSessionDev {
+  float* gate_state;   // the member's lastMapUpdatePose[3] and write flag (hsb_handle::d_gate)
+  float2* last_pts;    // the member's "containers of the last match": a matched scan's endpoints are copied here
+};
+
 struct HsbMatchParams {
   HsbLevelDev lv[HSB_MAX_LEVELS];
   int levels;
@@ -75,6 +81,14 @@ struct HsbMatchParams {
   // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.
   float* record;
   int record_floats;
+  // group SLAM step (match_kernel<..., GRP = true>): scan b is session b of the group.  Its level descriptors are
+  // group_lv[b * levels ..] (built once per group) instead of lv[], its gate thresholds and map_without_matching flag
+  // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
+  // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done
+  // counts the sessions that have finished: the last one publishes seq_value to seq_host.
+  const HsbLevelDev* group_lv;
+  const HsbGroupSessionDev* group_sess;
+  unsigned* group_done;
 };
 
 struct HsbUpdateLevelDev {
@@ -128,6 +142,15 @@ struct HsbUpdateParams {
   float log_odds_free, log_odds_occ;
   const float* pose_dev;     // if set, the pose is read from device memory (fused SLAM step) instead of pose_world
   const float* gate_flag;    // if set, *gate_flag == 0 turns the launch into a no-op (slam_gate_kernel in update_kernel.cuh)
+};
+
+// Map write of a group SLAM step (update_mark_group_kernel / update_apply_group_kernel): blockIdx.z = session,
+// blockIdx.y = level.  Everything per session lives in device memory, uploaded with the step's scans.
+struct HsbGroupUpdateParams {
+  const HsbUpdateLevelDev* lv;   // sessions x levels, session-major
+  const float2* log_odds;        // per session: the member's (free, occupied) log-odds increments
+  const float* res;              // per session 4 floats: the step's pose and write flag (the match kernel's gate)
+  int levels;
 };
 
 #endif

@@ -708,7 +708,16 @@ struct MatchBounds {
   static constexpr int kMinBlocks = (W == 1 && 28 % G == 0) ? 28 / G : 1;
 };
 
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false>
+// Level descriptors of scan `scan`: the kernel parameters' (one map for the whole batch), or — group SLAM step, every
+// session steps its own map — the session's row of the group's device array.
+template <bool GRP>
+__device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P, int scan, int lvl) {
+  if constexpr (GRP) return P.group_lv[(size_t)scan * P.levels + lvl];
+  else return P.lv[lvl];
+}
+
+// GRP: the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv.
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false>
 __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -732,7 +741,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
 
   // fused SLAM step: let the map writer's CTAs (launched with programmatic stream serialisation, update_kernel.cuh)
   // become resident on the idle SMs while this single-scan match runs; they wait for this grid's completion
-  if (P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (GRP || P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (t == 0) mbar_init(mbar, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   // Pacing (G > 1, P.pace_slack > 0).  The per-scan timeline (tuning key trace) shows that the warps of an SM do NOT
@@ -773,6 +782,9 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     } else {
       beg = 0;
       n = P.n_shared;
+    }
+    if constexpr (GRP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
+      if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;
     }
     const float2* __restrict__ gpts = P.pts + beg;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
@@ -866,7 +878,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     const bool recording = P.record && t == 0;
     if (n > 0) {
       for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
-        const HsbLevelDev& L = P.lv[lvl];
+        const HsbLevelDev& L = level_desc<GRP>(P, scan, lvl);
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
         if (recording) {
@@ -976,7 +988,11 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       P.trace[8 * (size_t)scan + 6] = warp_id();
       P.trace[8 * (size_t)scan + 7] = sm_id();
     }
-    if (t == 0 && P.gate_state) {
+    if (GRP && t == 0) {
+      // group SLAM step: the session's gate, against its own handle's state and thresholds
+      slam_gate(P.group_sess[scan].gate_state, P.gate_in + 3 * scan, wx, wy, wpsi, P.out_poses + 4 * scan,
+                P.gate_out_host + 4 * scan);
+    } else if (t == 0 && P.gate_state) {
       // fused SLAM step (one scan): the map-update gate runs in the match kernel's epilogue — no separate launch
       const float* gate_in;
       if constexpr (INL) gate_in = S.header + 3;
@@ -997,9 +1013,24 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
         c[6] = last.h02; c[7] = last.h12; c[8] = last.h22;
       }
     }
-    if (t == 0 && P.seq_host) {   // fused SLAM step: results are in mapped host memory — tell the polling host
+    if (GRP && t == 0) {
+      // group SLAM step: the LAST session to finish publishes the sequence number — every session's results (each made
+      // visible system-wide before its count) are then in host memory
+      __threadfence_system();
+      if (atomicAdd(P.group_done, 1u) == (unsigned)P.B - 1u) {
+        *P.group_done = 0u;   // re-armed for the next step, which is stream-ordered behind this grid
+        __threadfence_system();
+        *reinterpret_cast<volatile unsigned*>(P.seq_host) = P.seq_value;
+      }
+    } else if (t == 0 && P.seq_host) {   // fused SLAM step: results are in mapped host memory — tell the polling host
       __threadfence_system();
       *reinterpret_cast<volatile unsigned*>(P.seq_host) = P.seq_value;
+    }
+    if constexpr (GRP) {
+      // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
+      // its later map writes without matching read it (after the pose is out: only the map writers wait for this)
+      float2* keep = P.group_sess[scan].last_pts;
+      for (int i = t; i < n; i += GT) keep[i] = gpts[i];
     }
     if (cap > 0) group_sync<W>(g);  // everyone done with spts before the next bulk copy lands
   }

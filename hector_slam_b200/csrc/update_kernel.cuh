@@ -268,16 +268,16 @@ __device__ __forceinline__ bool beam_end(const HsbUpdateLevelDev& L, const BeamF
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// One level of one scan's mark phase (blockIdx.x / gridDim.x stride over the beams); gate_flag / pose_dev as in
+// HsbUpdateParams, pose_world the pose when pose_dev is null.
 template <int TEAM>
-__global__ void __launch_bounds__(256) update_mark_kernel(const __grid_constant__ HsbUpdateParams P) {
-  pdl_launch_dependents();   // the apply kernel's CTAs may take the free slots now; they wait for this grid to finish
-  pdl_wait();
-  const HsbUpdateLevelDev& L = P.lv[blockIdx.y];
+__device__ __forceinline__ void mark_level(const HsbUpdateLevelDev& L, const float* gate_flag, const float* pose_dev,
+                                           const float* pose_world) {
   if (!L.active) return;
   // gate flag, pose and beam count in ONE L2 round trip (independent loads, issued before the first dependent branch)
   // (plain loads: every thread reads these words, they have to hit L1)
-  const float flag = P.gate_flag ? *P.gate_flag : 1.0f;
-  const float* pw = P.pose_dev ? P.pose_dev : P.pose_world;
+  const float flag = gate_flag ? *gate_flag : 1.0f;
+  const float* pw = pose_dev ? pose_dev : pose_world;
   const float wx = pw[0], wy = pw[1], wpsi = pw[2];
   const int n_dev = L.n_dev ? *L.n_dev : L.n;
   if (flag == 0.0f) return;
@@ -373,6 +373,23 @@ __global__ void __launch_bounds__(256) update_mark_kernel(const __grid_constant_
   }
 }
 
+template <int TEAM>
+__global__ void __launch_bounds__(256) update_mark_kernel(const __grid_constant__ HsbUpdateParams P) {
+  pdl_launch_dependents();   // the apply kernel's CTAs may take the free slots now; they wait for this grid to finish
+  pdl_wait();
+  mark_level<TEAM>(P.lv[blockIdx.y], P.gate_flag, P.pose_dev, P.pose_world);
+}
+
+// Group SLAM step: the mark phase of every session's every level in one launch (blockIdx.z = session, blockIdx.y =
+// level); each session's pose and write flag come from the group match kernel's gate.
+template <int TEAM>
+__global__ void __launch_bounds__(256) update_mark_group_kernel(const __grid_constant__ HsbGroupUpdateParams P) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const float* res = P.res + 4 * blockIdx.z;
+  mark_level<TEAM>(P.lv[(size_t)blockIdx.z * P.levels + blockIdx.y], res + 3, res, res);
+}
+
 // APPLY: every marked cell lies in the bounding box of the start cell and the end cells, which the mark phase left in
 // the scan's scratch slot, so the apply phase is a coalesced sweep of that box over the stamp plane (uint4 loads, four
 // in flight per thread; a scalar variant for levels whose rows are not 16-byte multiples): stamp == base+1 -> l += lf,
@@ -397,9 +414,8 @@ __device__ __forceinline__ void apply_cell(const HsbUpdateLevelDev& L, unsigned 
   }
 }
 
-__global__ void __launch_bounds__(256) update_apply_kernel(const __grid_constant__ HsbUpdateParams P) {
-  pdl_wait();
-  const HsbUpdateLevelDev& L = P.lv[blockIdx.y];
+// One level of one scan's apply phase (blockIdx.x / gridDim.x sweep the box); lf / lo the log-odds increments.
+__device__ __forceinline__ void apply_level(const HsbUpdateLevelDev& L, const float* gate_flag, float lf, float lo) {
   if (!L.active) return;
   const int* cur = L.scratch + 8 * L.slot;
   if (blockIdx.x == 0 && threadIdx.x == 0) {   // the other slot is the next scan's: clear it (nobody reads it now)
@@ -409,7 +425,7 @@ __global__ void __launch_bounds__(256) update_apply_kernel(const __grid_constant
   }
   // gate flag and box in ONE round trip (independent loads, issued before the first dependent branch; plain loads:
   // every thread of the grid reads these words, they have to hit L1 — ld.cg here hot-spots one L2 sector)
-  const float flag = P.gate_flag ? *P.gate_flag : 1.0f;
+  const float flag = gate_flag ? *gate_flag : 1.0f;
   const int bx0 = cur[1], by0 = cur[2], bx1 = cur[3], by1 = cur[4];
   if (flag == 0.0f) return;
   if (bx1 < bx0) return;                       // nothing was marked (pose outside the map, every beam dropped)
@@ -419,7 +435,6 @@ __global__ void __launch_bounds__(256) update_apply_kernel(const __grid_constant
     atomicMax(L.dirty + 2, bx1); atomicMax(L.dirty + 6, bx1);
     atomicMax(L.dirty + 3, by1); atomicMax(L.dirty + 7, by1);
   }
-  const float lf = P.log_odds_free, lo = P.log_odds_occ;
   const unsigned nthreads = gridDim.x * blockDim.x, tid = blockIdx.x * blockDim.x + threadIdx.x;
   const unsigned rows = (unsigned)(by1 - by0 + 1);
   constexpr int U = 4;
@@ -457,6 +472,19 @@ __global__ void __launch_bounds__(256) update_apply_kernel(const __grid_constant
       apply_cell(L, off, __ldcg(L.stamp + off), lf, lo);
     }
   }
+}
+
+__global__ void __launch_bounds__(256) update_apply_kernel(const __grid_constant__ HsbUpdateParams P) {
+  pdl_wait();
+  apply_level(P.lv[blockIdx.y], P.gate_flag, P.log_odds_free, P.log_odds_occ);
+}
+
+// Group SLAM step: every session's every level (blockIdx.z = session, blockIdx.y = level) with that member's
+// increments; one owner per cell as above (a session writes only its own member's planes).
+__global__ void __launch_bounds__(256) update_apply_group_kernel(const __grid_constant__ HsbGroupUpdateParams P) {
+  pdl_wait();
+  const float2 lo = P.log_odds[blockIdx.z];
+  apply_level(P.lv[(size_t)blockIdx.z * P.levels + blockIdx.y], P.res + 4 * blockIdx.z + 3, lo.x, lo.y);
 }
 
 // Dirty-rectangle transport: pack the log-odds of rect = {x0, y0, x1, y1} (inclusive) row by row

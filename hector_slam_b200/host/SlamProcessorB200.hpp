@@ -11,8 +11,10 @@
 
 #include <cfloat>
 #include <cmath>
+#include <cstring>
 #include <stdexcept>
 #include <string>
+#include <vector>
 
 #include "hector_slam_b200.h"
 
@@ -27,7 +29,7 @@ class SlamProcessor {
   // HectorSlamProcessor.h:54
   SlamProcessor(float mapResolution, int mapSizeX, int mapSizeY, float startX, float startY, int multi_res_size,
                 int device = 0)
-      : h_(0) {
+      : h_(0), group_(0), groupOwner_(0) {
     hsb_config cfg = hsb_config();
     cfg.map_resolution = mapResolution;
     cfg.map_size_x = mapSizeX;
@@ -42,7 +44,11 @@ class SlamProcessor {
     setMapUpdateMinAngleDiff(0.13f * 1.0f);  // :63
     for (int i = 0; i < 9; ++i) lastScanMatchCov_[i] = 0.f;
   }
-  ~SlamProcessor() { hsb_destroy(h_); }
+  ~SlamProcessor() {
+    if (groupOwner_) groupOwner_->dropGroup();   // a group goes before its handles
+    dropGroup();
+    hsb_destroy(h_);
+  }
   SlamProcessor(const SlamProcessor&) = delete;
   SlamProcessor& operator=(const SlamProcessor&) = delete;
 
@@ -57,6 +63,33 @@ class SlamProcessor {
     check(hsb_slam_update(h_, hint, points_xy, n, origo, map_without_matching ? 1 : 0, out, lastScanMatchCov_, &updated));
     lastScanMatchPose_ = Pose{out[0], out[1], out[2]};  // :83
     if (updated) lastMapUpdatePose_ = lastScanMatchPose_;  // :94
+  }
+
+  // update() for M processors at once — M robots, each with its own map — in one device pass (hsb_group_slam_update):
+  // processor s takes the scan points_xy[offsets[s] .. offsets[s+1]) with origo[2s..] (origo may be null), the hint
+  // poseHintsWorld[s] and map_without_matching[s] (may be null).  Every processor ends exactly as its own update() would
+  // have left it.  The group is kept by ps[0] for as long as the same processors are stepped together in the same order.
+  static void updateMany(SlamProcessor* const* ps, int M, const float* points_xy, const int* offsets, const float* origo,
+                         const Pose* poseHintsWorld, const int* map_without_matching = 0) {
+    if (!ps || M < 1 || !ps[0]) throw std::invalid_argument("hector_slam_b200: updateMany needs M >= 1 processors");
+    SlamProcessor& owner = *ps[0];
+    hsb_group* g = owner.groupFor(ps, M);
+    std::vector<float> hints(3 * (size_t)M), poses(3 * (size_t)M), cov(9 * (size_t)M);
+    std::vector<int> updated(M);
+    for (int s = 0; s < M; ++s) {
+      hints[3 * s] = poseHintsWorld[s].x;
+      hints[3 * s + 1] = poseHintsWorld[s].y;
+      hints[3 * s + 2] = poseHintsWorld[s].psi;
+      std::memcpy(&cov[9 * s], ps[s]->lastScanMatchCov_, sizeof(ps[s]->lastScanMatchCov_));   // untouched where unmatched
+    }
+    owner.check(hsb_group_slam_update(g, hints.data(), points_xy, offsets, origo, map_without_matching, 0, poses.data(),
+                                      cov.data(), updated.data()));
+    for (int s = 0; s < M; ++s) {
+      SlamProcessor& p = *ps[s];
+      p.lastScanMatchPose_ = Pose{poses[3 * s], poses[3 * s + 1], poses[3 * s + 2]};  // :83
+      if (updated[s]) p.lastMapUpdatePose_ = p.lastScanMatchPose_;                    // :94
+      std::memcpy(p.lastScanMatchCov_, &cov[9 * s], sizeof(p.lastScanMatchCov_));
+    }
   }
 
   // The same step with the control flow on the host (two C-ABI calls and a round trip in between), as the
@@ -124,7 +157,39 @@ class SlamProcessor {
   void check(int st) const {
     if (st != HSB_OK) throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(h_));
   }
+  // the cached group of updateMany: rebuilt only when the member list changes.  A processor belongs to at most one
+  // cached group (its groupOwner_), so that destroying any member destroys that group first.
+  hsb_group* groupFor(SlamProcessor* const* ps, int M) {
+    bool same = group_ && (int)groupMembers_.size() == M;
+    for (int s = 0; same && s < M; ++s) same = groupMembers_[s] == ps[s];
+    if (same) return group_;
+    dropGroup();
+    std::vector<hsb_handle*> hs(M);
+    for (int s = 0; s < M; ++s) {
+      if (!ps[s]) throw std::invalid_argument("hector_slam_b200: updateMany: processor is null");
+      if (ps[s]->groupOwner_) ps[s]->groupOwner_->dropGroup();
+      hs[s] = ps[s]->h_;
+    }
+    hsb_group* g = 0;
+    if (hsb_group_create(hs.data(), M, &g) != HSB_OK)
+      throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(0));
+    group_ = g;
+    groupMembers_.assign(ps, ps + M);
+    for (int s = 0; s < M; ++s) ps[s]->groupOwner_ = this;
+    return group_;
+  }
+  void dropGroup() {
+    if (!group_) return;
+    hsb_group_destroy(group_);
+    group_ = 0;
+    for (size_t s = 0; s < groupMembers_.size(); ++s)
+      if (groupMembers_[s]->groupOwner_ == this) groupMembers_[s]->groupOwner_ = 0;
+    groupMembers_.clear();
+  }
   hsb_handle* h_;
+  hsb_group* group_;                           // updateMany's group, when this processor is its ps[0]
+  std::vector<SlamProcessor*> groupMembers_;
+  SlamProcessor* groupOwner_;                  // the processor whose cached group contains this one
   Pose lastMapUpdatePose_, lastScanMatchPose_;
   float lastScanMatchCov_[9];
   float minDist_, minAngle_;

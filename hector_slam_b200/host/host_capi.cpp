@@ -3,6 +3,7 @@
 #include "SlamProcessorB200.hpp"
 
 #include <cstring>
+#include <vector>
 
 extern "C" {
 
@@ -28,6 +29,30 @@ int hsbp_update(void* p, const float* pts, int n, const float* origo, const floa
   out_pose[1] = q.y;
   out_pose[2] = q.psi;
   if (out_cov) std::memcpy(out_cov, s->getLastScanMatchCovariance(), 9 * sizeof(float));
+  return 0;
+}
+int hsbp_update_many(void* const* ps, int M, const float* pts, const int* offsets, const float* origo, const float* hints,
+                     const int* map_without_matching) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) {
+    procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+    poses[s] = hsb200::Pose{hints[3 * s], hints[3 * s + 1], hints[3 * s + 2]};
+  }
+  try {
+    hsb200::SlamProcessor::updateMany(procs.data(), M, pts, offsets, origo, poses.data(), map_without_matching);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
+  hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
+  const hsb200::Pose& q = s->getLastScanMatchPose();
+  out_pose[0] = q.x;
+  out_pose[1] = q.y;
+  out_pose[2] = q.psi;
+  std::memcpy(out_cov, s->getLastScanMatchCovariance(), 9 * sizeof(float));
   return 0;
 }
 int hsbp_reset(void* p) {

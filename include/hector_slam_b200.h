@@ -290,6 +290,33 @@ int hsb_slam_update_nowait(hsb_handle* h, const float pose_hint_world[3], const 
 int hsb_slam_update_cloud(hsb_handle* h, const float pose_hint_world[3], const float* points_xyz, int n,
                           const double* transform, int map_without_matching, int nowait, float out_pose_world[3],
                           float cov_inout[9], int* map_updated, int* out_kept);
+/* ---- many SLAM sessions in one device pass ------------------------------------------------------*/
+/* N robots that each build their own map are N independent HectorSlamProcessors, i.e. N handles.  A group steps
+ * them together: one host-to-device copy and three kernel launches per step whatever the number of members, instead
+ * of N single steps in series.  (The batch matchers above serve many scans against ONE shared map.)
+ * A group of existing handles stepped together.  The group does not own the handles.  Destroy the group before any of
+ * its handles.  Members must have the same geometry: levels, map_size_x/y, map_resolution, start_x/y, the resolved
+ * max_iterations of every level and the resolved gather mode, and sit on one device; update factors and the two gate
+ * thresholds are per handle and may differ.  A handle may belong to several groups.  Errors of hsb_group_create:
+ * hsb_last_error(NULL) and hsb_last_error(handles[0]); of the other two calls: hsb_last_error(handles[0]). */
+typedef struct hsb_group hsb_group;
+int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out);
+int hsb_group_destroy(hsb_group* g);
+/* HectorSlamProcessor::update for every member at once. Session s is handles[s] with hint hints[3s..], the scan
+ * points_xy[offsets[s] .. offsets[s+1]) (level-0 cells, DataContainer layout), origo[2s..] (NULL = 0,0) and
+ * map_without_matching[s] (NULL = all 0). Host buffers. out_poses M x 3. cov_inout M x 9 (may be NULL; an entry is
+ * left untouched where the single call leaves it untouched). map_updated M (may be NULL). nowait != 0: return once all
+ * M poses have arrived, as hsb_slam_update_nowait does.
+ * Every member is left in exactly the state hsb_slam_update with the same inputs would have left it in (gate pose,
+ * last match's containers, stamps, both dirty rectangles, the pending map write after nowait), and each session's
+ * results are bit-identical to that call's, so group steps, single steps and every other call may be mixed freely on a
+ * member.  Ordering: a group step runs after everything already queued on its members' streams; every later call on a
+ * member runs after the group step (hsb_on_map_updated(member) is the completion point after nowait), and "_device"
+ * calls on caller streams are ordered as after hsb_slam_update_nowait.  The step runs on the group's own stream; its
+ * kernel launches are counted on handles[0] (hsb_get_launch_count), three per step. */
+int hsb_group_slam_update(hsb_group* g, const float* hints_world, const float* points_xy, const int* offsets,
+                          const float* origo, const int* map_without_matching, int nowait,
+                          float* out_poses_world, float* cov_inout, int* map_updated);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
