@@ -35,7 +35,7 @@ EXPORTED = [
     "hsb_alloc_pinned", "hsb_free_pinned", "hsb_measure_h2d_gbs", "hsb_get_dirty_rects", "hsb_pack_dirty_device", "hsb_unpack_dirty_device", "hsb_get_replication_overflows", "hsb_get_mirror_dirty_rect", "hsb_download_level_rect", "hsb_download_occupancy_rect",
     "hsb_get_d2h_bytes", "hsb_covariance_batch", "hsb_get_map_origin", "hsb_get_dist_batch", "hsb_set_cloud_format", "hsb_cloud_to_points", "hsb_match_batch_cloud", "hsb_match_batch_cloud_device",
     "hsb_get_match_record_floats", "hsb_match_data_record", "hsb_match_batch_record_device",
-    "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update",
+    "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update", "hsb_group_slam_update_cloud",
 ]
 
 
@@ -171,6 +171,7 @@ def load_library() -> C.CDLL:
     sig("hsb_group_create", i, vp, i, C.POINTER(vp))
     sig("hsb_group_destroy", i, vp)
     sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
+    sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -827,15 +828,7 @@ class SlamGroup:
         cov_inout value (zeros if None) where the session matched nothing."""
         M = self.M
         h = _f32(hints).reshape(M, 3)
-        if isinstance(scans, tuple):
-            pts = _f32(scans[0]).reshape(-1, 2)
-            offsets = np.ascontiguousarray(scans[1], dtype=np.int32)
-        else:
-            scans = [_f32(s).reshape(-1, 2) for s in scans]
-            assert len(scans) == M, (len(scans), M)
-            offsets = np.zeros(M + 1, np.int32)
-            offsets[1:] = np.cumsum([s.shape[0] for s in scans])
-            pts = np.concatenate(scans) if offsets[-1] else np.zeros((0, 2), np.float32)
+        pts, offsets = self._pack(scans, 2)
         og = None if origo is None else _f32(origo).reshape(M, 2)
         mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
         poses = np.zeros((M, 3), np.float32)
@@ -845,6 +838,37 @@ class SlamGroup:
                                                    offsets.ctypes.data, _ptr(og), _ptr(mwm), int(bool(nowait)),
                                                    poses.ctypes.data, cov.ctypes.data, upd.ctypes.data))
         return poses, cov.reshape(M, 3, 3), upd.astype(bool)
+
+    def slam_update_cloud(self, hints, clouds, transforms=None, map_without_matching=None, nowait: bool = False,
+                          cov_inout=None):
+        """The same step from the node's default input (hsb_group_slam_update_cloud): clouds are M (n_s, 3) Point32
+        arrays in the laser frame, or a tuple (points (N, 3), offsets (M + 1,)); transforms (M, 12) float64 laser
+        transforms, None = each member's cloud format.  Each member converts with its own cloud format's thresholds.
+        -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
+        M = self.M
+        h = _f32(hints).reshape(M, 3)
+        pts, offsets = self._pack(clouds, 3)
+        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(M, 12)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
+        poses = np.zeros((M, 3), np.float32)
+        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
+        upd = np.zeros(M, np.int32)
+        kept = np.zeros(M, np.int32)
+        self._check(self.lib.hsb_group_slam_update_cloud(self.g, h.ctypes.data, pts.ctypes.data if pts.size else None,
+                                                         offsets.ctypes.data, _ptr(T), _ptr(mwm), int(bool(nowait)),
+                                                         poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
+                                                         kept.ctypes.data))
+        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+
+    def _pack(self, scans, width):
+        """M per-session arrays (n_s, width), or a tuple (points (N, width), offsets (M + 1,)) -> (points, offsets)."""
+        if isinstance(scans, tuple):
+            return _f32(scans[0]).reshape(-1, width), np.ascontiguousarray(scans[1], dtype=np.int32)
+        scans = [_f32(s).reshape(-1, width) for s in scans]
+        assert len(scans) == self.M, (len(scans), self.M)
+        offsets = np.zeros(self.M + 1, np.int32)
+        offsets[1:] = np.cumsum([s.shape[0] for s in scans])
+        return (np.concatenate(scans) if offsets[-1] else np.zeros((0, width), np.float32)), offsets
 
     def close(self):
         if getattr(self, "g", None):

@@ -260,17 +260,32 @@ void fill_level_dev(const hsb_handle* h, int l, HsbLevelDev& d) {
 }
 
 // ---- match launch -----------------------------------------------------------------------------
+constexpr size_t kMaxDynSmem = 232448;   // dynamic shared memory one CTA may ask for (227 KB)
+
+// shared-memory slots that stage a whole scan of n points: n + head padding, even
+inline int whole_scan_slots(int n) { return ((n + 1) + 1) & ~1; }
+
+// whether Gr groups of the <W, G> match kernel can each stage `cap` slots in one CTA
+template <int W, int G>
+bool staging_fits(int cap, int Gr) {
+  return hsb::MatchSmem<W, G>::kHeaderBytes + (size_t)Gr * cap * 8 <= kMaxDynSmem;
+}
+
+int fail_fused_too_long(hsb_handle* h, int max_n) {
+  return fail(h, HSB_ERR_UNSUPPORTED, "scan too long for the fused conversion (%d points)", max_n);
+}
+
 template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false>
 int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int Gr,
                    const hsb::InlineScan<INL>& S = hsb::InlineScan<INL>()) {
   if (Gr <= 0 || Gr > G) Gr = G;   // groups per CTA actually launched (a G-group kernel runs with fewer: see launch_match)
   const size_t header = hsb::MatchSmem<W, G>::kHeaderBytes;
   auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL, GRP>;
-  constexpr size_t kMaxDyn = 232448;   // dynamic shared memory one CTA may ask for (227 KB)
+  constexpr size_t kMaxDyn = kMaxDynSmem;
   constexpr int gt = W * 32;           // threads per scan
   int cap = 0;
   const bool fused = P.ranges || P.cloud || INL;   // conversion / inline scan: the whole scan must be staged
-  if (h->tune_stage_smem || fused) cap = ((max_n + 1) + 1) & ~1;  // n + head padding, even
+  if (h->tune_stage_smem || fused) cap = whole_scan_slots(max_n);
   // resident CTAs per SM for a given dynamic shared-memory size: block, thread, register and
   // shared-memory limits (1 KB per CTA is reserved by the driver)
   static int regs = 0;
@@ -294,8 +309,8 @@ int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st,
     return pts >= 4 * gt ? pts + 2 : 0;
   };
   const bool may_split = h->tune_partial && !PACK && !fused;   // a staged PREFIX is allowed
-  if (cap > 0 && header + (size_t)Gr * cap * 8 > kMaxDyn) {        // the CTA's scans do not fit whole
-    if (fused) return fail(h, HSB_ERR_UNSUPPORTED, "scan too long for the fused conversion (%d points)", max_n);
+  if (cap > 0 && !staging_fits<W, G>(cap, Gr)) {        // the CTA's scans do not fit whole
+    if (fused) return fail_fused_too_long(h, max_n);
     cap = may_split ? cap_for(1) : 0;
   }
   if (cap > 0 && !fused && h->tune_stage_smem == 1) {
@@ -1082,6 +1097,15 @@ static void fill_cloud_params(const hsb_handle* h, HsbMatchParams& P, const floa
   P.out_origo = d_origo;
 }
 
+// The container's origo of a cloud with laser transform T (HectorMappingRos.cpp:516-517):
+// Vector2f(laserPos.x(), laserPos.y()) * scaleToMap, host fp32 without contraction
+static void cloud_origo(const hsb_handle* h, const double* T, float out[2]) {
+  volatile float ox = (float)T[3], oy = (float)T[7];
+  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
+  out[0] = sx;
+  out[1] = sy;
+}
+
 int hsb_cloud_to_points(hsb_handle* h, const float* points_xyz, int n, float* out_xy, int* out_n, float out_origo[2]) {
   if (!h || n < 0 || (n > 0 && !points_xyz) || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
   if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
@@ -1105,12 +1129,7 @@ int hsb_cloud_to_points(hsb_handle* h, const float* points_xyz, int n, float* ou
   const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
   if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
   *out_n = kept;
-  if (out_origo) {   // HectorMappingRos.cpp:516-517: Vector2f(laserPos.x(), laserPos.y()) * scaleToMap (host fp32, no contraction)
-    volatile float ox = (float)h->cfmt.laser_transform[3], oy = (float)h->cfmt.laser_transform[7];
-    volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
-    out_origo[0] = sx;
-    out_origo[1] = sy;
-  }
+  if (out_origo) cloud_origo(h, h->cfmt.laser_transform, out_origo);
   return HSB_OK;
 }
 
@@ -1679,10 +1698,9 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
   float* d_s = static_cast<float*>(h->d_scratch.p);
   float* d_gate = static_cast<float*>(h->d_gate.p);
   int* d_n = reinterpret_cast<int*>(d_s + 40);
-  // the container's origo (HectorMappingRos.cpp:516-517) is known on the host: Vector2f(laserPos) * scaleToMap in fp32
-  volatile float ox = (float)T[3], oy = (float)T[7];
-  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
-  const float origo[2] = {sx, sy};
+  // the container's origo is known on the host
+  float origo[2];
+  cloud_origo(h, T, origo);
   const bool host_out = true;   // results always travel through mapped host memory here
   const bool poll = nowait != 0;
   volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
@@ -2255,8 +2273,11 @@ struct hsb_group {
   cudaStream_t stream = nullptr;   // every step of the group runs here
   cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
   HsbLevelDev* d_lv = nullptr;     // M x levels match-kernel level descriptors (a handle's planes never move)
-  float* d_res = nullptr;          // M x 4 (pose, write flag) for the map writer, then the finished-session counter
-  float* h_res = nullptr;          // mapped pinned: M x 4 (pose, flag), M x 9 Hessian, the sequence number
+  // M x 4 (pose, write flag) for the map writer, the finished-session counter (4 words), then M kept-endpoint counts of a
+  // cloud step (ints, the map writer's n_dev)
+  float* d_res = nullptr;
+  // mapped pinned: M x 4 (pose, flag), M x 9 Hessian, the sequence number (4 words), M kept-endpoint counts (ints)
+  float* h_res = nullptr;
   float* h_res_dev = nullptr;      // device alias of h_res
   char* h_stage = nullptr;         // pinned staging of the step's host-to-device copy
   size_t h_stage_bytes = 0;
@@ -2364,34 +2385,65 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
     HSB_GROUP_CUDA(cudaMalloc(&g->d_lv, lv.size() * sizeof(HsbLevelDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_lv, lv.data(), lv.size() * sizeof(HsbLevelDev), cudaMemcpyHostToDevice));
   }
-  HSB_GROUP_CUDA(cudaMalloc(&g->d_res, ((size_t)M * 4 + 4) * sizeof(float)));
-  HSB_GROUP_CUDA(cudaMemset(g->d_res, 0, ((size_t)M * 4 + 4) * sizeof(float)));
-  HSB_GROUP_CUDA(cudaHostAlloc(&g->h_res, ((size_t)M * 13 + 4) * sizeof(float), cudaHostAllocMapped));
-  memset(g->h_res, 0, ((size_t)M * 13 + 4) * sizeof(float));
+  HSB_GROUP_CUDA(cudaMalloc(&g->d_res, ((size_t)M * 5 + 4) * sizeof(float)));
+  HSB_GROUP_CUDA(cudaMemset(g->d_res, 0, ((size_t)M * 5 + 4) * sizeof(float)));
+  HSB_GROUP_CUDA(cudaHostAlloc(&g->h_res, ((size_t)M * 14 + 4) * sizeof(float), cudaHostAllocMapped));
+  memset(g->h_res, 0, ((size_t)M * 14 + 4) * sizeof(float));
   HSB_GROUP_CUDA(cudaHostGetDevicePointer(&g->h_res_dev, g->h_res, 0));
 #undef HSB_GROUP_CUDA
   *out = g;
   return HSB_OK;
 }
 
-int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_xy, const int* offsets, const float* origo,
-                          const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {
-  if (!g) return HSB_ERR_INVALID_ARG;
+}  // extern "C"
+
+namespace {
+
+// What a group step's sessions bring: level-0 endpoints (hsb_group_slam_update) or the node's projected point clouds
+// (hsb_group_slam_update_cloud, converted in the match kernel's staging step as hsb_slam_update_cloud converts them).
+enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD };
+struct GroupInput {
+  GroupInputKind kind;
+  const char* fn;              // the entry point, for the error messages
+  const float* hints;          // M x 3
+  const float* pts;            // endpoints: xy pairs; cloud: Point32 triples
+  const int* offsets;          // M + 1, in points
+  const float* origo;          // endpoints: M x 2 (NULL = 0, 0)
+  const double* transforms;    // cloud: M x 12 (NULL = every member's hsb_set_cloud_format transform)
+};
+
+// warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
+constexpr int kGroupW = 8;
+
+// One group step of either input kind.  Everything that can reject the step is checked before any member's state moves.
+int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matching, int nowait, float* out_poses,
+               float* cov_inout, int* map_updated, int* out_kept) {
   hsb_handle* h0 = g->m[0];
   const int M = (int)g->m.size(), levels = g->levels;
-  if (!hints || !offsets || !out_poses)
-    return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: hints, offsets and out_poses must not be NULL");
-  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: offsets[0] is %d, must be 0", offsets[0]);
+  const bool cloud = in.kind == GROUP_CLOUD;
+  const int* offsets = in.offsets;
+  if (!in.hints || !offsets || !out_poses)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
+  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", in.fn, offsets[0]);
   int max_n = 0;
   for (int k = 0; k < M; ++k) {
     const int n = offsets[k + 1] - offsets[k];
     if (n < 0)
-      return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: offsets decrease at session %d (%d -> %d)", k, offsets[k],
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets decrease at session %d (%d -> %d)", in.fn, k, offsets[k],
                   offsets[k + 1]);
     max_n = std::max(max_n, n);
   }
   const int total = offsets[M];
-  if (total > 0 && !points_xy) return fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_slam_update: points_xy is NULL");
+  if (total > 0 && !in.pts)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : "points_xy");
+  if (cloud) {
+    for (int k = 0; k < M; ++k)
+      if (!g->m[k]->cfmt_set)
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_cloud_format has not been called on its handle",
+                    in.fn, k);
+    // every cloud is converted whole into shared memory: the launcher's limit for the group kernel's shape
+    if (!staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
+  }
   DeviceGuard guard(g->device);
   cudaStream_t st = g->stream;
   int s;
@@ -2404,12 +2456,15 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
     }
   }
 
-  // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments | scans
+  // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments |
+  // laser transforms (cloud) | scans
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
   const size_t o_gin = al((size_t)M * 12), o_off = al(o_gin + (size_t)M * 12), o_sess = al(o_off + (size_t)(M + 1) * 4);
   const size_t o_upd = al(o_sess + (size_t)M * sizeof(HsbGroupSessionDev));
-  const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_pts = al(o_lo + (size_t)M * 8);
-  const size_t bytes = o_pts + (size_t)total * 8;
+  const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_tf = al(o_lo + (size_t)M * 8);
+  const size_t o_pts = al(o_tf + (cloud ? (size_t)M * 12 * sizeof(double) : 0));
+  const size_t pt_bytes = cloud ? 12 : 8;
+  const size_t bytes = o_pts + (size_t)total * pt_bytes;
   if (bytes > g->h_stage_bytes) {
     if (g->h_stage) cudaFreeHost(g->h_stage);
     g->h_stage = nullptr;
@@ -2425,28 +2480,59 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
   HsbGroupSessionDev* s_sess = reinterpret_cast<HsbGroupSessionDev*>(hs + o_sess);
   HsbUpdateLevelDev* s_upd = reinterpret_cast<HsbUpdateLevelDev*>(hs + o_upd);
   float2* s_lo = reinterpret_cast<float2*>(hs + o_lo);
-  const float2* d_pts = reinterpret_cast<const float2*>(ds + o_pts);
-  memcpy(hs, hints, (size_t)M * 12);
+  double* s_tf = reinterpret_cast<double*>(hs + o_tf);
+  const char* d_in = ds + o_pts;
+  memcpy(hs, in.hints, (size_t)M * 12);
   memcpy(hs + o_off, offsets, (size_t)(M + 1) * 4);
-  if (total > 0) memcpy(hs + o_pts, points_xy, (size_t)total * 8);
+  if (total > 0) memcpy(hs + o_pts, in.pts, (size_t)total * pt_bytes);
+  // a cloud session's kept-endpoint count: in device memory for the map writer, in mapped host memory for the host
+  int* kept_dev = reinterpret_cast<int*>(g->d_res + 4 * (size_t)M + 4);
+  int* kept_mapped = reinterpret_cast<int*>(g->h_res_dev + 13 * (size_t)M + 4);
   int max_upd = 0;
   for (int k = 0; k < M; ++k) {
     hsb_handle* h = g->m[k];
-    const int n = offsets[k + 1] - offsets[k];
+    const int n = offsets[k + 1] - offsets[k];   // a cloud's size: an upper bound of the endpoints it keeps
     const bool matched = !(map_without_matching && map_without_matching[k]);
-    const float ox = origo ? origo[2 * k] : 0.f, oy = origo ? origo[2 * k + 1] : 0.f;
+    float og[2] = {0.f, 0.f};
+    if (cloud) {
+      const double* T = in.transforms ? in.transforms + 12 * (size_t)k : h->cfmt.laser_transform;
+      memcpy(s_tf + 12 * (size_t)k, T, 12 * sizeof(double));
+      cloud_origo(h, T, og);
+    } else if (in.origo) {
+      og[0] = in.origo[2 * k];
+      og[1] = in.origo[2 * k + 1];
+    }
     s_gin[3 * k] = h->min_dist;
     s_gin[3 * k + 1] = h->min_angle;
     s_gin[3 * k + 2] = matched ? 0.f : 1.f;
     s_lo[k] = make_float2(h->log_odds_free, h->log_odds_occ);
-    s_sess[k].gate_state = static_cast<float*>(h->d_gate.p);
-    s_sess[k].last_pts = nullptr;
+    HsbGroupSessionDev& ss = s_sess[k];
+    memset(&ss, 0, sizeof(ss));
+    ss.gate_state = static_cast<float*>(h->d_gate.p);
     if (matched) {   // this scan becomes the last match's container (without matching the old one stays, :77-81)
       if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
-      s_sess[k].last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
+      if (!cloud) ss.last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
       h->last_n = n;
-      h->last_origo[0] = ox;
-      h->last_origo[1] = oy;
+      h->last_origo[0] = og[0];
+      h->last_origo[1] = og[1];
+    }
+    // where level 0 reads this scan, and (cloud) where the writer finds its endpoint count
+    const float2* pts0 = nullptr;
+    const int* n_dev = nullptr;
+    if (cloud) {   // converted into the buffer hsb_slam_update_cloud converts into
+      DevBuf& pbuf = matched ? h->d_last_pts : h->d_upd_pts;
+      if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
+      ss.cloud_pts = reinterpret_cast<float2*>(scan_points(pbuf));
+      ss.kept = kept_dev + k;
+      ss.kept_host = kept_mapped + k;
+      ss.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
+      ss.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
+      ss.z_min = h->cfmt.laser_z_min_value;
+      ss.z_max = h->cfmt.laser_z_max_value;
+      pts0 = ss.cloud_pts;
+      n_dev = kept_dev + k;
+    } else {
+      pts0 = reinterpret_cast<const float2*>(d_in) + offsets[k];
     }
     // MapRepMultiMap::updateByScan: level 0 from this scan, the coarse levels from the last match's container (:143)
     for (int l = 0; l < levels; ++l) {
@@ -2454,10 +2540,11 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
       fill_update_level(h, l, d);
       d.pt_scale = (float)(1.0 / pow(2.0, (double)l));
       if (l == 0 || matched) {
-        d.pts = d_pts + offsets[k];
+        d.pts = pts0;
         d.n = n;
-        d.origo_x = ox;
-        d.origo_y = oy;
+        d.n_dev = n_dev;
+        d.origo_x = og[0];
+        d.origo_y = og[1];
       } else {
         d.pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
         d.n = h->last_n;
@@ -2473,13 +2560,18 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
   }
   HSB_CUDA(h0, cudaMemcpyAsync(g->d_stage.p, hs, bytes, cudaMemcpyHostToDevice, st));
 
-  // K1: match + gate, one session per CTA; the last session to finish publishes the step's sequence number
+  // K1: (conversion +) match + gate, one session per CTA; the last session to finish publishes the step's sequence number
   HsbMatchParams P;
   fill_match_params(h0, P);
   P.B = M;
   P.hints = reinterpret_cast<const float*>(ds);
-  P.pts = d_pts;
-  P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  if (cloud) {   // (the kernel takes the thresholds from the session descriptors, not from h0's format)
+    fill_cloud_params(h0, P, reinterpret_cast<const float*>(d_in), reinterpret_cast<const int*>(ds + o_off),
+                      reinterpret_cast<const double*>(ds + o_tf), nullptr);
+  } else {
+    P.pts = reinterpret_cast<const float2*>(d_in);
+    P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  }
   P.out_poses = g->d_res;
   P.out_cov = g->h_res_dev + 4 * (size_t)M;
   P.gate_in = reinterpret_cast<const float*>(ds + o_gin);
@@ -2489,12 +2581,13 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
   P.group_lv = g->d_lv;
   P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
-  s = h0->gather_mode == HSB_GATHER_TEX ? launch_match_t<8, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
-                                        : launch_match_t<8, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
+  s = h0->gather_mode == HSB_GATHER_TEX
+          ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
+          : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
   if (s != HSB_OK) return s;
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
-  // one-wave grids are shared out among the sessions
+  // one-wave grids are shared out among the sessions (a cloud's size bounds its endpoints: the grids are sized by it)
   HsbGroupUpdateParams U;
   U.lv = reinterpret_cast<const HsbUpdateLevelDev*>(ds + o_upd);
   U.log_odds = reinterpret_cast<const float2*>(ds + o_lo);
@@ -2544,15 +2637,40 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
   } else {
     HSB_CUDA(h0, cudaStreamSynchronize(st));   // :93 onMapUpdated for every member
   }
+  const int* kept_host = reinterpret_cast<const int*>(g->h_res + 13 * (size_t)M + 4);
   for (int k = 0; k < M; ++k) {
     const float* r = g->h_res + 4 * (size_t)k;
     memcpy(out_poses + 3 * (size_t)k, r, 3 * sizeof(float));
     if (map_updated) map_updated[k] = r[3] != 0.f;
     const bool matched = !(map_without_matching && map_without_matching[k]);
-    if (cov_inout && matched && offsets[k + 1] > offsets[k])
+    const int n = cloud ? kept_host[k] : offsets[k + 1] - offsets[k];   // the endpoints the session had
+    if (cloud) {
+      if (out_kept) out_kept[k] = n;
+      if (matched) g->m[k]->last_n = n;   // the last match's container holds exactly these (as hsb_slam_update_cloud)
+    }
+    if (cov_inout && matched && n > 0)
       memcpy(cov_inout + 9 * (size_t)k, g->h_res + 4 * (size_t)M + 9 * (size_t)k, 9 * sizeof(float));
   }
   return HSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_xy, const int* offsets, const float* origo,
+                          const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {GROUP_ENDPOINTS, "hsb_group_slam_update", hints, points_xy, offsets, origo, nullptr};
+  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, nullptr);
+}
+
+int hsb_group_slam_update_cloud(hsb_group* g, const float* hints, const float* points_xyz, const int* offsets,
+                                const double* transforms, const int* map_without_matching, int nowait, float* out_poses,
+                                float* cov_inout, int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {GROUP_CLOUD, "hsb_group_slam_update_cloud", hints, points_xyz, offsets, nullptr, transforms};
+  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 
 }  // extern "C"

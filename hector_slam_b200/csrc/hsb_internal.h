@@ -22,10 +22,18 @@ struct HsbLevelDev {
   int rec_off;               // where this level's part of a scan's per-evaluation record starts (HsbMatchParams::record)
 };
 
-// One session of a group SLAM step (hsb_group_slam_update): the member handle's state the match kernel touches.
+// One session of a group SLAM step (hsb_group_slam_update / _cloud): the member handle's state the match kernel touches.
 struct HsbGroupSessionDev {
   float* gate_state;   // the member's lastMapUpdatePose[3] and write flag (hsb_handle::d_gate)
   float2* last_pts;    // the member's "containers of the last match": a matched scan's endpoints are copied here
+  // point-cloud input (HsbMatchParams::cloud set): the converted endpoints go to cloud_pts (the member's last-match
+  // container when the session matches, its update-scan buffer when not), their number to kept (device memory, the map
+  // writer's n_dev) and to kept_host (the group's mapped host block, before the step's sequence number is published);
+  // the conversion thresholds are the member's hsb_set_cloud_format values at step time
+  float2* cloud_pts;
+  int* kept;
+  int* kept_host;
+  float sqr_min_dist, sqr_max_dist, z_min, z_max;
 };
 
 struct HsbMatchParams {
@@ -85,7 +93,9 @@ struct HsbMatchParams {
   // group_lv[b * levels ..] (built once per group) instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done
-  // counts the sessions that have finished: the last one publishes seq_value to seq_host.
+  // counts the sessions that have finished: the last one publishes seq_value to seq_host.  With cloud input a session
+  // reads its thresholds from group_sess[b] (sqr_min_dist .. z_max above are unused) and a set map_without_matching flag
+  // still converts the cloud for the map writer: only the match is skipped.
   const HsbLevelDev* group_lv;
   const HsbGroupSessionDev* group_sess;
   unsigned* group_done;

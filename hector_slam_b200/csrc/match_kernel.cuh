@@ -784,7 +784,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       n = P.n_shared;
     }
     if constexpr (GRP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
-      if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;
+      if (!P.cloud && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a cloud is converted first, below)
     }
     const float2* __restrict__ gpts = P.pts + beg;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
@@ -810,8 +810,16 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       staged = true;
     } else if (P.cloud) {
       const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
-      n = stage_from_cloud<W>(P.cloud + 3 * (size_t)beg, n, T, P.sqr_min_dist, P.sqr_max_dist, P.z_min, P.z_max,
-                              P.scale_to_map, spts, warp_cnt, g, w, lane);
+      float min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
+      if constexpr (GRP) {   // group SLAM step: every session converts with its own member's format
+        const HsbGroupSessionDev& SS = P.group_sess[scan];
+        min2 = SS.sqr_min_dist;
+        max2 = SS.sqr_max_dist;
+        zmin = SS.z_min;
+        zmax = SS.z_max;
+      }
+      n = stage_from_cloud<W>(P.cloud + 3 * (size_t)beg, n, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt, g,
+                              w, lane);
       if (P.out_origo && t == 0) {   // dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
         P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], P.scale_to_map);
         P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], P.scale_to_map);
@@ -822,6 +830,17 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
           *P.out_n = n;
           if (P.out_n_host) *P.out_n_host = n;
         }
+      }
+      if constexpr (GRP) {
+        // group SLAM step: the session's endpoints and their number go to its member for the map writer (and, matched,
+        // become its last-match container); the count reaches host memory before the step's sequence number (below)
+        const HsbGroupSessionDev& SS = P.group_sess[scan];
+        for (int i = t; i < n; i += GT) SS.cloud_pts[i] = spts[i];
+        if (t == 0) {
+          *SS.kept = n;
+          *SS.kept_host = n;
+        }
+        if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // map_without_matching: converted for the writer, not matched
       }
       ns = n;
       staged = true;
@@ -1028,9 +1047,12 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     }
     if constexpr (GRP) {
       // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
-      // its later map writes without matching read it (after the pose is out: only the map writers wait for this)
-      float2* keep = P.group_sess[scan].last_pts;
-      for (int i = t; i < n; i += GT) keep[i] = gpts[i];
+      // its later map writes without matching read it (after the pose is out: only the map writers wait for this).
+      // A converted cloud is already there (cloud_pts, above).
+      if (!P.cloud) {
+        float2* keep = P.group_sess[scan].last_pts;
+        for (int i = t; i < n; i += GT) keep[i] = gpts[i];
+      }
     }
     if (cap > 0) group_sync<W>(g);  // everyone done with spts before the next bulk copy lands
   }

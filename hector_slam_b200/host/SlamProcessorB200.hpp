@@ -71,26 +71,43 @@ class SlamProcessor {
   // have left it.  The group is kept by ps[0] for as long as the same processors are stepped together in the same order.
   static void updateMany(SlamProcessor* const* ps, int M, const float* points_xy, const int* offsets, const float* origo,
                          const Pose* poseHintsWorld, const int* map_without_matching = 0) {
-    if (!ps || M < 1 || !ps[0]) throw std::invalid_argument("hector_slam_b200: updateMany needs M >= 1 processors");
-    SlamProcessor& owner = *ps[0];
-    hsb_group* g = owner.groupFor(ps, M);
-    std::vector<float> hints(3 * (size_t)M), poses(3 * (size_t)M), cov(9 * (size_t)M);
-    std::vector<int> updated(M);
-    for (int s = 0; s < M; ++s) {
-      hints[3 * s] = poseHintsWorld[s].x;
-      hints[3 * s + 1] = poseHintsWorld[s].y;
-      hints[3 * s + 2] = poseHintsWorld[s].psi;
-      std::memcpy(&cov[9 * s], ps[s]->lastScanMatchCov_, sizeof(ps[s]->lastScanMatchCov_));   // untouched where unmatched
-    }
-    owner.check(hsb_group_slam_update(g, hints.data(), points_xy, offsets, origo, map_without_matching, 0, poses.data(),
-                                      cov.data(), updated.data()));
-    for (int s = 0; s < M; ++s) {
-      SlamProcessor& p = *ps[s];
-      p.lastScanMatchPose_ = Pose{poses[3 * s], poses[3 * s + 1], poses[3 * s + 2]};  // :83
-      if (updated[s]) p.lastMapUpdatePose_ = p.lastScanMatchPose_;                    // :94
-      std::memcpy(p.lastScanMatchCov_, &cov[9 * s], sizeof(p.lastScanMatchCov_));
-    }
+    stepMany(ps, M, poseHintsWorld, "updateMany", [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+      return hsb_group_slam_update(g, hints, points_xy, offsets, origo, map_without_matching, 0, poses, cov, updated);
+    });
   }
+
+  // The node's default input (use_tf_scan_transformation, HectorMappingRos.cpp:283, 509-542): update() from the projected
+  // point cloud of a scan, converted on the device (hsb_slam_update_cloud).  points_xyz: n Point32 triples in the laser
+  // frame; transform: the scan's tf laser transform (12 doubles, rows of [R | t]), null = the cloud format's.  Returns
+  // the number of endpoints the conversion kept.
+  int updateCloud(const float* points_xyz, int n, const double* transform, const Pose& poseHintWorld,
+                  bool map_without_matching = false) {
+    const float hint[3] = {poseHintWorld.x, poseHintWorld.y, poseHintWorld.psi};
+    float out[3];
+    int updated = 0, kept = 0;
+    check(hsb_slam_update_cloud(h_, hint, points_xyz, n, transform, map_without_matching ? 1 : 0, 0, out, lastScanMatchCov_,
+                                &updated, &kept));
+    lastScanMatchPose_ = Pose{out[0], out[1], out[2]};  // :83
+    if (updated) lastMapUpdatePose_ = lastScanMatchPose_;  // :94
+    return kept;
+  }
+
+  // updateCloud() for M processors in one device pass (hsb_group_slam_update_cloud): processor s takes the cloud
+  // points_xyz[3*offsets[s] .. 3*offsets[s+1]) with transforms[12s..] (transforms may be null: each processor's cloud
+  // format), the hint poseHintsWorld[s] and map_without_matching[s] (may be null); kept (M ints, may be null) receives
+  // each conversion's endpoint count.  Same group cache and end state as updateMany.
+  static void updateManyCloud(SlamProcessor* const* ps, int M, const float* points_xyz, const int* offsets,
+                              const double* transforms, const Pose* poseHintsWorld, const int* map_without_matching = 0,
+                              int* kept = 0) {
+    stepMany(ps, M, poseHintsWorld, "updateManyCloud",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_cloud(g, hints, points_xyz, offsets, transforms, map_without_matching, 0,
+                                                  poses, cov, updated, kept);
+             });
+  }
+
+  // the cloud format of updateCloud / updateManyCloud (the node's laser transform and filter parameters)
+  void setCloudFormat(const hsb_cloud_format& fmt) { check(hsb_set_cloud_format(h_, &fmt)); }
 
   // The same step with the control flow on the host (two C-ABI calls and a round trip in between), as the
   // reference's own HectorSlamProcessor drives MapRepB200; kept for comparison and tests.
@@ -156,6 +173,30 @@ class SlamProcessor {
  private:
   void check(int st) const {
     if (st != HSB_OK) throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(h_));
+  }
+  // One group step for M processors: `step(group, hints, poses, cov, updated)` makes the C-ABI call; the processors'
+  // poses and covariances are kept as update() keeps them.
+  template <class Step>
+  static void stepMany(SlamProcessor* const* ps, int M, const Pose* poseHintsWorld, const char* what, Step step) {
+    if (!ps || M < 1 || !ps[0])
+      throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs M >= 1 processors");
+    SlamProcessor& owner = *ps[0];
+    hsb_group* g = owner.groupFor(ps, M);
+    std::vector<float> hints(3 * (size_t)M), poses(3 * (size_t)M), cov(9 * (size_t)M);
+    std::vector<int> updated(M);
+    for (int s = 0; s < M; ++s) {
+      hints[3 * s] = poseHintsWorld[s].x;
+      hints[3 * s + 1] = poseHintsWorld[s].y;
+      hints[3 * s + 2] = poseHintsWorld[s].psi;
+      std::memcpy(&cov[9 * s], ps[s]->lastScanMatchCov_, sizeof(ps[s]->lastScanMatchCov_));   // untouched where unmatched
+    }
+    owner.check(step(g, hints.data(), poses.data(), cov.data(), updated.data()));
+    for (int s = 0; s < M; ++s) {
+      SlamProcessor& p = *ps[s];
+      p.lastScanMatchPose_ = Pose{poses[3 * s], poses[3 * s + 1], poses[3 * s + 2]};  // :83
+      if (updated[s]) p.lastMapUpdatePose_ = p.lastScanMatchPose_;                    // :94
+      std::memcpy(p.lastScanMatchCov_, &cov[9 * s], sizeof(p.lastScanMatchCov_));
+    }
   }
   // the cached group of updateMany: rebuilt only when the member list changes.  A processor belongs to at most one
   // cached group (its groupOwner_), so that destroying any member destroys that group first.

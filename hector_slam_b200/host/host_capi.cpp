@@ -46,6 +46,48 @@ int hsbp_update_many(void* const* ps, int M, const float* pts, const int* offset
   }
   return 0;
 }
+int hsbp_set_cloud_format(void* p, const double transform[12], float sqr_min_dist, float sqr_max_dist, float z_min,
+                          float z_max) {
+  hsb_cloud_format fmt;
+  std::memcpy(fmt.laser_transform, transform, sizeof(fmt.laser_transform));
+  fmt.sqr_laser_min_dist = sqr_min_dist;
+  fmt.sqr_laser_max_dist = sqr_max_dist;
+  fmt.laser_z_min_value = z_min;
+  fmt.laser_z_max_value = z_max;
+  try {
+    static_cast<hsb200::SlamProcessor*>(p)->setCloudFormat(fmt);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_cloud(void* p, const float* points_xyz, int n, const double* transform, const float hint[3],
+                      int map_without_matching, int* out_kept) {
+  try {
+    const int kept = static_cast<hsb200::SlamProcessor*>(p)->updateCloud(
+        points_xyz, n, transform, hsb200::Pose{hint[0], hint[1], hint[2]}, map_without_matching != 0);
+    if (out_kept) *out_kept = kept;
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_many_cloud(void* const* ps, int M, const float* points_xyz, const int* offsets, const double* transforms,
+                           const float* hints, const int* map_without_matching, int* out_kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) {
+    procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+    poses[s] = hsb200::Pose{hints[3 * s], hints[3 * s + 1], hints[3 * s + 2]};
+  }
+  try {
+    hsb200::SlamProcessor::updateManyCloud(procs.data(), M, points_xyz, offsets, transforms, poses.data(),
+                                           map_without_matching, out_kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

@@ -298,7 +298,7 @@ int hsb_slam_update_cloud(hsb_handle* h, const float pose_hint_world[3], const f
  * its handles.  Members must have the same geometry: levels, map_size_x/y, map_resolution, start_x/y, the resolved
  * max_iterations of every level and the resolved gather mode, and sit on one device; update factors and the two gate
  * thresholds are per handle and may differ.  A handle may belong to several groups.  Errors of hsb_group_create:
- * hsb_last_error(NULL) and hsb_last_error(handles[0]); of the other two calls: hsb_last_error(handles[0]). */
+ * hsb_last_error(NULL) and hsb_last_error(handles[0]); of the other group calls: hsb_last_error(handles[0]). */
 typedef struct hsb_group hsb_group;
 int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out);
 int hsb_group_destroy(hsb_group* g);
@@ -317,6 +317,23 @@ int hsb_group_destroy(hsb_group* g);
 int hsb_group_slam_update(hsb_group* g, const float* hints_world, const float* points_xy, const int* offsets,
                           const float* origo, const int* map_without_matching, int nowait,
                           float* out_poses_world, float* cov_inout, int* map_updated);
+/* The same group step from the node's DEFAULT input: hsb_slam_update_cloud for every member at once.  Session s takes
+ * the Point32 triples points_xyz[3*offsets[s] .. 3*offsets[s+1]) and the laser transform transforms[12s..] (12 doubles,
+ * rows of [R | t]; transforms == NULL: every member's hsb_set_cloud_format transform).  Each session converts with its
+ * own member's format thresholds (sqr_laser_min/max_dist, laser_z_min/max_value) as they are at the call, so robots
+ * may differ in laser mount and filter settings.  out_kept (M ints, may be NULL) = the endpoints each conversion kept;
+ * hints, map_without_matching, nowait, cov_inout and map_updated as in hsb_group_slam_update.  The conversion runs in
+ * the group's match kernel (still one host-to-device copy and three launches per step; a map_without_matching session
+ * is converted for the map writer and not matched, and its endpoints do not replace the last match's container).
+ * Every session's pose, covariance, gate decision and kept count are bit-identical to hsb_slam_update_cloud on its
+ * handle with the same inputs, and every member is left in the state that call leaves (gate pose, last match's
+ * container and origo = laser position * scaleToMap, stamps, both dirty rectangles, the pending map write after
+ * nowait); ordering as in hsb_group_slam_update.  Rejected before any member changes: a member without a cloud format
+ * (HSB_ERR_INVALID_ARG, the message names the session), bad offsets (HSB_ERR_INVALID_ARG), a cloud longer than the
+ * fused conversion can stage (HSB_ERR_UNSUPPORTED, the limit of hsb_slam_update_cloud). */
+int hsb_group_slam_update_cloud(hsb_group* g, const float* hints_world, const float* points_xyz, const int* offsets,
+                                const double* transforms, const int* map_without_matching, int nowait,
+                                float* out_poses_world, float* cov_inout, int* map_updated, int* out_kept);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
