@@ -36,6 +36,7 @@ EXPORTED = [
     "hsb_get_d2h_bytes", "hsb_covariance_batch", "hsb_get_map_origin", "hsb_get_dist_batch", "hsb_set_cloud_format", "hsb_cloud_to_points", "hsb_match_batch_cloud", "hsb_match_batch_cloud_device",
     "hsb_get_match_record_floats", "hsb_match_data_record", "hsb_match_batch_record_device",
     "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update", "hsb_group_slam_update_cloud",
+    "hsb_slam_update_ranges", "hsb_group_slam_update_ranges",
 ]
 
 
@@ -118,6 +119,7 @@ def load_library() -> C.CDLL:
     sig("hsb_slam_update", i, vp, vp, vp, i, vp, i, vp, vp, vp)
     sig("hsb_slam_update_nowait", i, vp, vp, vp, i, vp, i, vp, vp, vp)
     sig("hsb_slam_update_cloud", i, vp, vp, vp, i, vp, i, i, vp, vp, vp, vp)
+    sig("hsb_slam_update_ranges", i, vp, vp, vp, i, i, i, vp, vp, vp, vp)
     sig("hsb_get_last_map_update_pose", i, vp, vp)
     sig("hsb_set_last_map_update_pose", i, vp, vp)
     sig("hsb_upload_level", i, vp, i, vp)
@@ -172,6 +174,7 @@ def load_library() -> C.CDLL:
     sig("hsb_group_destroy", i, vp)
     sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
     sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_slam_update_ranges", i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -474,6 +477,20 @@ class MapRepB200:
         self._check(self.lib.hsb_slam_update_cloud(self.h, hint.ctypes.data, pts.ctypes.data if pts.size else None,
                                                    pts.shape[0], _ptr(T), int(bool(map_without_matching)), int(bool(nowait)),
                                                    pose.ctypes.data, cov.ctypes.data, C.addressof(upd), C.addressof(kept)))
+        return pose, cov.reshape(3, 3), bool(upd.value), int(kept.value)
+
+    def slam_update_ranges(self, pose_hint_world, ranges, map_without_matching: bool = False, nowait: bool = False,
+                           cov_inout=None):
+        """scanCallback's branch without the laser tf in one call: raw ranges in the scan format (set_scan_format) ->
+        endpoints (fused), match, gate, map write.  -> (pose (3,), cov (3,3), map_updated: bool, kept endpoints: int)"""
+        hint = _f32(pose_hint_world, 3)
+        r = _f32(ranges).reshape(-1)
+        pose = np.zeros(3, np.float32)
+        cov = np.zeros(9, np.float32) if cov_inout is None else _f32(cov_inout).reshape(9).copy()
+        upd, kept = C.c_int(0), C.c_int(0)
+        self._check(self.lib.hsb_slam_update_ranges(self.h, hint.ctypes.data, r.ctypes.data, r.size,
+                                                    int(bool(map_without_matching)), int(bool(nowait)), pose.ctypes.data,
+                                                    cov.ctypes.data, C.addressof(upd), C.addressof(kept)))
         return pose, cov.reshape(3, 3), bool(upd.value), int(kept.value)
 
     def last_map_update_pose(self) -> np.ndarray:
@@ -858,6 +875,24 @@ class SlamGroup:
                                                          offsets.ctypes.data, _ptr(T), _ptr(mwm), int(bool(nowait)),
                                                          poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
                                                          kept.ctypes.data))
+        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+
+    def slam_update_ranges(self, hints, ranges_list, map_without_matching=None, nowait: bool = False, cov_inout=None):
+        """The same step from raw LaserScan ranges (hsb_group_slam_update_ranges): ranges_list is M (n_beams_s,) arrays,
+        or a tuple (ranges (N,), offsets (M + 1,)).  Each member converts with its own scan format.
+        -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
+        M = self.M
+        h = _f32(hints).reshape(M, 3)
+        r, offsets = self._pack(ranges_list, 1)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
+        poses = np.zeros((M, 3), np.float32)
+        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
+        upd = np.zeros(M, np.int32)
+        kept = np.zeros(M, np.int32)
+        self._check(self.lib.hsb_group_slam_update_ranges(self.g, h.ctypes.data, r.ctypes.data if r.size else None,
+                                                          offsets.ctypes.data, _ptr(mwm), int(bool(nowait)),
+                                                          poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
+                                                          kept.ctypes.data))
         return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
 
     def _pack(self, scans, width):

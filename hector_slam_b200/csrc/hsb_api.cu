@@ -75,7 +75,8 @@ struct hsb_handle {
   bool fmt_set = false;
   hsb_cloud_format cfmt = hsb_cloud_format();
   bool cfmt_set = false;
-  DevBuf d_cloud, d_cloud_off, d_cloud_tf, d_origo, d_cloud1;
+  DevBuf d_cloud, d_cloud_off, d_cloud_tf, d_origo;
+  DevBuf d_fused_in;   // the fused single SLAM steps' upload: header, (laser transform,) cloud or ranges
   int last_n = 0;
   float last_origo[2] = {0.f, 0.f};
   // pinned host scratch
@@ -712,7 +713,7 @@ int hsb_destroy(hsb_handle* h) {
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
                     &h->d_beam_cs, &h->d_ranges, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
-                    &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_cloud1};
+                    &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_fused_in};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int k = 0; k < 2; ++k) {
@@ -1019,13 +1020,18 @@ int hsb_set_scan_format(hsb_handle* h, const hsb_scan_format* fmt) {
   return HSB_OK;
 }
 
+// :493 maxRangeForContainer = range_max - 0.1, host fp32
+static float range_max_c(const hsb_scan_format& f) {
+  volatile float mx = f.range_max - 0.1f;
+  return mx;
+}
+
 static void fill_range_params(const hsb_handle* h, HsbMatchParams& P, const float* d_ranges) {
   P.ranges = d_ranges;
   P.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
   P.n_beams = h->fmt.n_beams;
   P.range_min = h->fmt.range_min;
-  volatile float mx = h->fmt.range_max - 0.1f;  // :493 maxRangeForContainer
-  P.range_max_c = mx;
+  P.range_max_c = range_max_c(h->fmt);
   P.scale_to_map = h->lv[0].scale;
 }
 
@@ -1652,26 +1658,32 @@ int hsb_slam_update_nowait(hsb_handle* h, const float hint[3], const float* pts,
   return slam_update_impl(h, hint, pts, n, origo, map_without_matching, out_pose, cov_inout, map_updated, false);
 }
 
-// HectorMappingRos::scanCallback's default branch in one call: rosPointCloudToDataContainer (HectorMappingRos.cpp:283,
-// 509-542) + HectorSlamProcessor::update (:297 / HectorSlamProcessor.h:71-113).  The cloud is converted by the match
-// kernel's staging step; the converted endpoints, which the map writer needs too, are written out by the same kernel and
-// their number stays on the device (the writer reads it there), so no host round trip appears between conversion, match,
-// gate and map write.
-int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* points_xyz, int n, const double* transform,
-                          int map_without_matching, int nowait, float out_pose[3], float cov_inout[9], int* map_updated,
-                          int* out_kept) {
-  if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
+// What a fused single SLAM step converts on the device: a Point32 cloud in the laser frame with its laser transform
+// (hsb_slam_update_cloud), or a LaserScan's raw ranges in the handle's scan format (hsb_slam_update_ranges).
+struct FusedScan {
+  bool ranges;
+  const float* data;    // cloud: n (x, y, z) triples; ranges: n ranges
+  int n;                // cloud: points; ranges: the scan format's n_beams
+  const double* T;      // cloud: the laser transform (12 doubles)
+};
+
+// HectorMappingRos::scanCallback's conversion + HectorSlamProcessor::update (:297 / HectorSlamProcessor.h:71-113) as
+// one step.  The scan is converted by the match kernel's staging step; the converted endpoints, which the map writer
+// needs too, are written out by the same kernel and their number stays on the device (the writer reads it there), so no
+// host round trip appears between conversion, match, gate and map write.  Without matching the stand-alone conversion
+// kernel converts the scan and the gate runs alone.
+static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& in, int map_without_matching, int nowait,
+                           float out_pose[3], float cov_inout[9], int* map_updated, int* out_kept) {
   HandleScope guard(h);
   int s;
+  const int n = in.n;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
-  const double* T = transform ? transform : h->cfmt.laser_transform;
   // staging layout (floats): [0..15] header: hint, thresholds, force, [8] = 0, [9] = n (cloud offsets, as ints);
-  // [16..39] the laser transform (12 doubles); [40..] the cloud
-  const size_t kHdr = 16, kTf = 24;
-  const size_t bytes = (kHdr + kTf + (size_t)n * 3) * sizeof(float);
-  if ((s = ensure(h, h->d_cloud1, bytes + 16)) != HSB_OK) return s;
+  // cloud: [16..39] the laser transform (12 doubles), [40..] the cloud; ranges: [16..] the ranges
+  const size_t kHdr = 16, kTf = in.ranges ? 0 : 24, per_pt = in.ranges ? 1 : 3;
+  const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
+  if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
   if (bytes > h->h_stage_bytes) {
     if (h->h_stage) cudaFreeHost(h->h_stage);
     h->h_stage = nullptr;
@@ -1686,22 +1698,22 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
   hs[3] = h->min_dist; hs[4] = h->min_angle; hs[5] = map_without_matching ? 1.f : 0.f;
   reinterpret_cast<int*>(hs)[8] = 0;
   reinterpret_cast<int*>(hs)[9] = n;
-  memcpy(hs + kHdr, T, 12 * sizeof(double));
-  if (n > 0) memcpy(hs + kHdr + kTf, points_xyz, (size_t)n * 12);
+  if (!in.ranges) memcpy(hs + kHdr, in.T, 12 * sizeof(double));
+  if (n > 0) memcpy(hs + kHdr + kTf, in.data, (size_t)n * per_pt * sizeof(float));
   cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud1.p, hs, bytes, cudaMemcpyHostToDevice, st));
-  float* d_c = static_cast<float*>(h->d_cloud1.p);
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
+  float* d_c = static_cast<float*>(h->d_fused_in.p);
   const float* d_hdr = d_c;
   const int* d_offs = reinterpret_cast<const int*>(d_c) + 8;
   const double* d_tf = reinterpret_cast<const double*>(d_c + kHdr);
-  const float* d_xyz = d_c + kHdr + kTf;
+  const float* d_in = d_c + kHdr + kTf;
   float* d_s = static_cast<float*>(h->d_scratch.p);
   float* d_gate = static_cast<float*>(h->d_gate.p);
   int* d_n = reinterpret_cast<int*>(d_s + 40);
-  // the container's origo is known on the host
-  float origo[2];
-  cloud_origo(h, T, origo);
-  const bool host_out = true;   // results always travel through mapped host memory here
+  // the container's origo is known on the host: zero for a LaserScan (HectorMappingRos.cpp:491)
+  float origo[2] = {0.f, 0.f};
+  if (!in.ranges) cloud_origo(h, in.T, origo);
+  // results always travel through mapped host memory here
   const bool poll = nowait != 0;
   volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
   unsigned* seq_dev = reinterpret_cast<unsigned*>(h->h_pin_dev + 22);
@@ -1711,7 +1723,6 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
   DevBuf& pbuf = map_without_matching ? h->d_upd_pts : h->d_last_pts;
   if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
   float2* d_pts_out = reinterpret_cast<float2*>(scan_points(pbuf));
-  (void)host_out;
   if (!map_without_matching) {
     HsbMatchParams P;
     fill_match_params(h, P);
@@ -1719,7 +1730,8 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
     P.hints = d_hdr;
     P.out_poses = d_s + 8;
     P.out_cov = h->h_pin_dev + 12;
-    fill_cloud_params(h, P, d_xyz, d_offs, d_tf, nullptr);
+    if (in.ranges) fill_range_params(h, P, d_in);
+    else fill_cloud_params(h, P, d_in, d_offs, d_tf, nullptr);
     P.out_pts = d_pts_out;
     P.out_n = d_n;
     P.out_n_host = kept_dev;
@@ -1733,8 +1745,13 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
     h->last_origo[0] = origo[0];
     h->last_origo[1] = origo[1];
   } else {
-    hsb::cloud_to_points_kernel<<<1, 256, 0, st>>>(d_xyz, n, d_tf, h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist,
-                                                   h->cfmt.laser_z_min_value, h->cfmt.laser_z_max_value, h->lv[0].scale, d_pts_out, d_n);
+    if (in.ranges)
+      hsb::scan_to_points_kernel<<<1, 256, 0, st>>>(d_in, static_cast<const float2*>(h->d_beam_cs.p), n, h->fmt.range_min,
+                                                    range_max_c(h->fmt), h->lv[0].scale, d_pts_out, d_n);
+    else
+      hsb::cloud_to_points_kernel<<<1, 256, 0, st>>>(d_in, n, d_tf, h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist,
+                                                     h->cfmt.laser_z_min_value, h->cfmt.laser_z_max_value, h->lv[0].scale,
+                                                     d_pts_out, d_n);
     hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, h->h_pin_dev + 8, nullptr, 0);
     hsb::publish_int_kernel<<<1, 32, 0, st>>>(d_n, kept_dev, poll ? seq_dev : nullptr, seq_value);
     h->launches += 3;
@@ -1763,6 +1780,30 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
   if (cov_inout && kept > 0 && !map_without_matching) memcpy(cov_inout, h->h_pin + 12, 9 * sizeof(float));
   if (out_kept) *out_kept = kept;
   return HSB_OK;
+}
+
+// HectorMappingRos::scanCallback's default branch in one call: rosPointCloudToDataContainer (HectorMappingRos.cpp:283,
+// 509-542) + HectorSlamProcessor::update (:297)
+int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* points_xyz, int n, const double* transform,
+                          int map_without_matching, int nowait, float out_pose[3], float cov_inout[9], int* map_updated,
+                          int* out_kept) {
+  if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
+  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
+  const FusedScan in = {false, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
+  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
+}
+
+// ... and its branch without the laser tf (use_tf_scan_transformation = false, :248-254): rosLaserScanToDataContainer
+// (:483-507) + HectorSlamProcessor::update with the last match as the start estimate
+int hsb_slam_update_ranges(hsb_handle* h, const float hint[3], const float* ranges, int n, int map_without_matching,
+                           int nowait, float out_pose[3], float cov_inout[9], int* map_updated, int* out_kept) {
+  if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
+  if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
+  if (n != h->fmt.n_beams)
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_slam_update_ranges: n is %d, the scan format has %d beams", n,
+                h->fmt.n_beams);
+  const FusedScan in = {true, ranges, n, nullptr};
+  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
 int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
@@ -2274,7 +2315,7 @@ struct hsb_group {
   cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
   HsbLevelDev* d_lv = nullptr;     // M x levels match-kernel level descriptors (a handle's planes never move)
   // M x 4 (pose, write flag) for the map writer, the finished-session counter (4 words), then M kept-endpoint counts of a
-  // cloud step (ints, the map writer's n_dev)
+  // cloud or ranges step (ints, the map writer's n_dev)
   float* d_res = nullptr;
   // mapped pinned: M x 4 (pose, flag), M x 9 Hessian, the sequence number (4 words), M kept-endpoint counts (ints)
   float* h_res = nullptr;
@@ -2399,15 +2440,16 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
 
 namespace {
 
-// What a group step's sessions bring: level-0 endpoints (hsb_group_slam_update) or the node's projected point clouds
-// (hsb_group_slam_update_cloud, converted in the match kernel's staging step as hsb_slam_update_cloud converts them).
-enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD };
+// What a group step's sessions bring: level-0 endpoints (hsb_group_slam_update), the node's projected point clouds
+// (hsb_group_slam_update_cloud) or raw LaserScan ranges (hsb_group_slam_update_ranges).  Clouds and ranges are
+// converted in the match kernel's staging step as hsb_slam_update_cloud / hsb_slam_update_ranges convert them.
+enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD, GROUP_RANGES };
 struct GroupInput {
   GroupInputKind kind;
   const char* fn;              // the entry point, for the error messages
   const float* hints;          // M x 3
-  const float* pts;            // endpoints: xy pairs; cloud: Point32 triples
-  const int* offsets;          // M + 1, in points
+  const float* pts;            // endpoints: xy pairs; cloud: Point32 triples; ranges: one float per beam
+  const int* offsets;          // M + 1, in points (ranges: in beams)
   const float* origo;          // endpoints: M x 2 (NULL = 0, 0)
   const double* transforms;    // cloud: M x 12 (NULL = every member's hsb_set_cloud_format transform)
 };
@@ -2415,12 +2457,13 @@ struct GroupInput {
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
 constexpr int kGroupW = 8;
 
-// One group step of either input kind.  Everything that can reject the step is checked before any member's state moves.
+// One group step of any input kind.  Everything that can reject the step is checked before any member's state moves.
 int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matching, int nowait, float* out_poses,
                float* cov_inout, int* map_updated, int* out_kept) {
   hsb_handle* h0 = g->m[0];
   const int M = (int)g->m.size(), levels = g->levels;
-  const bool cloud = in.kind == GROUP_CLOUD;
+  const bool cloud = in.kind == GROUP_CLOUD, ranges = in.kind == GROUP_RANGES;
+  const bool conv = cloud || ranges;   // converted on the device: the kept count decides what the session had
   const int* offsets = in.offsets;
   if (!in.hints || !offsets || !out_poses)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
@@ -2435,15 +2478,26 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   }
   const int total = offsets[M];
   if (total > 0 && !in.pts)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : "points_xy");
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : ranges ? "ranges" : "points_xy");
   if (cloud) {
     for (int k = 0; k < M; ++k)
       if (!g->m[k]->cfmt_set)
         return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_cloud_format has not been called on its handle",
                     in.fn, k);
-    // every cloud is converted whole into shared memory: the launcher's limit for the group kernel's shape
-    if (!staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
   }
+  if (ranges) {
+    for (int k = 0; k < M; ++k) {
+      const hsb_handle* h = g->m[k];
+      if (!h->fmt_set)
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_scan_format has not been called on its handle",
+                    in.fn, k);
+      if (offsets[k + 1] - offsets[k] != h->fmt.n_beams)
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d has %d ranges, its scan format has %d beams", in.fn, k,
+                    offsets[k + 1] - offsets[k], h->fmt.n_beams);
+    }
+  }
+  // every scan is converted whole into shared memory: the launcher's limit for the group kernel's shape
+  if (conv && !staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
   DeviceGuard guard(g->device);
   cudaStream_t st = g->stream;
   int s;
@@ -2463,7 +2517,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   const size_t o_upd = al(o_sess + (size_t)M * sizeof(HsbGroupSessionDev));
   const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_tf = al(o_lo + (size_t)M * 8);
   const size_t o_pts = al(o_tf + (cloud ? (size_t)M * 12 * sizeof(double) : 0));
-  const size_t pt_bytes = cloud ? 12 : 8;
+  const size_t pt_bytes = cloud ? 12 : ranges ? 4 : 8;
   const size_t bytes = o_pts + (size_t)total * pt_bytes;
   if (bytes > g->h_stage_bytes) {
     if (g->h_stage) cudaFreeHost(g->h_stage);
@@ -2485,20 +2539,20 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   memcpy(hs, in.hints, (size_t)M * 12);
   memcpy(hs + o_off, offsets, (size_t)(M + 1) * 4);
   if (total > 0) memcpy(hs + o_pts, in.pts, (size_t)total * pt_bytes);
-  // a cloud session's kept-endpoint count: in device memory for the map writer, in mapped host memory for the host
+  // a converted session's kept-endpoint count: in device memory for the map writer, in mapped host memory for the host
   int* kept_dev = reinterpret_cast<int*>(g->d_res + 4 * (size_t)M + 4);
   int* kept_mapped = reinterpret_cast<int*>(g->h_res_dev + 13 * (size_t)M + 4);
   int max_upd = 0;
   for (int k = 0; k < M; ++k) {
     hsb_handle* h = g->m[k];
-    const int n = offsets[k + 1] - offsets[k];   // a cloud's size: an upper bound of the endpoints it keeps
+    const int n = offsets[k + 1] - offsets[k];   // a cloud's size / a scan's beams: an upper bound of the endpoints kept
     const bool matched = !(map_without_matching && map_without_matching[k]);
     float og[2] = {0.f, 0.f};
     if (cloud) {
       const double* T = in.transforms ? in.transforms + 12 * (size_t)k : h->cfmt.laser_transform;
       memcpy(s_tf + 12 * (size_t)k, T, 12 * sizeof(double));
       cloud_origo(h, T, og);
-    } else if (in.origo) {
+    } else if (in.origo) {   // (a LaserScan's origo is zero, HectorMappingRos.cpp:491)
       og[0] = in.origo[2 * k];
       og[1] = in.origo[2 * k + 1];
     }
@@ -2511,25 +2565,32 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     ss.gate_state = static_cast<float*>(h->d_gate.p);
     if (matched) {   // this scan becomes the last match's container (without matching the old one stays, :77-81)
       if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
-      if (!cloud) ss.last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
+      if (!conv) ss.last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
       h->last_n = n;
       h->last_origo[0] = og[0];
       h->last_origo[1] = og[1];
     }
-    // where level 0 reads this scan, and (cloud) where the writer finds its endpoint count
+    // where level 0 reads this scan, and (converted) where the writer finds its endpoint count
     const float2* pts0 = nullptr;
     const int* n_dev = nullptr;
-    if (cloud) {   // converted into the buffer hsb_slam_update_cloud converts into
+    if (conv) {   // converted into the buffer the single fused step converts into
       DevBuf& pbuf = matched ? h->d_last_pts : h->d_upd_pts;
       if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
-      ss.cloud_pts = reinterpret_cast<float2*>(scan_points(pbuf));
+      ss.conv_pts = reinterpret_cast<float2*>(scan_points(pbuf));
       ss.kept = kept_dev + k;
       ss.kept_host = kept_mapped + k;
-      ss.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
-      ss.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
-      ss.z_min = h->cfmt.laser_z_min_value;
-      ss.z_max = h->cfmt.laser_z_max_value;
-      pts0 = ss.cloud_pts;
+      if (cloud) {
+        ss.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
+        ss.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
+        ss.z_min = h->cfmt.laser_z_min_value;
+        ss.z_max = h->cfmt.laser_z_max_value;
+      } else {
+        ss.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
+        ss.n_beams = h->fmt.n_beams;
+        ss.range_min = h->fmt.range_min;
+        ss.range_max_c = range_max_c(h->fmt);
+      }
+      pts0 = ss.conv_pts;
       n_dev = kept_dev + k;
     } else {
       pts0 = reinterpret_cast<const float2*>(d_in) + offsets[k];
@@ -2568,6 +2629,9 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   if (cloud) {   // (the kernel takes the thresholds from the session descriptors, not from h0's format)
     fill_cloud_params(h0, P, reinterpret_cast<const float*>(d_in), reinterpret_cast<const int*>(ds + o_off),
                       reinterpret_cast<const double*>(ds + o_tf), nullptr);
+  } else if (ranges) {   // (likewise the scan format; the offsets locate each session's ranges)
+    fill_range_params(h0, P, reinterpret_cast<const float*>(d_in));
+    P.offsets = reinterpret_cast<const int*>(ds + o_off);
   } else {
     P.pts = reinterpret_cast<const float2*>(d_in);
     P.offsets = reinterpret_cast<const int*>(ds + o_off);
@@ -2587,7 +2651,8 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   if (s != HSB_OK) return s;
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
-  // one-wave grids are shared out among the sessions (a cloud's size bounds its endpoints: the grids are sized by it)
+  // one-wave grids are shared out among the sessions (a cloud's size or a scan's beam count bounds its endpoints: the
+  // grids are sized by it)
   HsbGroupUpdateParams U;
   U.lv = reinterpret_cast<const HsbUpdateLevelDev*>(ds + o_upd);
   U.log_odds = reinterpret_cast<const float2*>(ds + o_lo);
@@ -2643,10 +2708,10 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     memcpy(out_poses + 3 * (size_t)k, r, 3 * sizeof(float));
     if (map_updated) map_updated[k] = r[3] != 0.f;
     const bool matched = !(map_without_matching && map_without_matching[k]);
-    const int n = cloud ? kept_host[k] : offsets[k + 1] - offsets[k];   // the endpoints the session had
-    if (cloud) {
+    const int n = conv ? kept_host[k] : offsets[k + 1] - offsets[k];   // the endpoints the session had
+    if (conv) {
       if (out_kept) out_kept[k] = n;
-      if (matched) g->m[k]->last_n = n;   // the last match's container holds exactly these (as hsb_slam_update_cloud)
+      if (matched) g->m[k]->last_n = n;   // the last match's container holds exactly these (as the single fused step)
     }
     if (cov_inout && matched && n > 0)
       memcpy(cov_inout + 9 * (size_t)k, g->h_res + 4 * (size_t)M + 9 * (size_t)k, 9 * sizeof(float));
@@ -2670,6 +2735,14 @@ int hsb_group_slam_update_cloud(hsb_group* g, const float* hints, const float* p
                                 float* cov_inout, int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {GROUP_CLOUD, "hsb_group_slam_update_cloud", hints, points_xyz, offsets, nullptr, transforms};
+  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+}
+
+int hsb_group_slam_update_ranges(hsb_group* g, const float* hints, const float* ranges, const int* offsets,
+                                 const int* map_without_matching, int nowait, float* out_poses, float* cov_inout,
+                                 int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {GROUP_RANGES, "hsb_group_slam_update_ranges", hints, ranges, offsets, nullptr, nullptr};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 

@@ -22,18 +22,24 @@ struct HsbLevelDev {
   int rec_off;               // where this level's part of a scan's per-evaluation record starts (HsbMatchParams::record)
 };
 
-// One session of a group SLAM step (hsb_group_slam_update / _cloud): the member handle's state the match kernel touches.
+// One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges): the member handle's state the match
+// kernel touches.
 struct HsbGroupSessionDev {
   float* gate_state;   // the member's lastMapUpdatePose[3] and write flag (hsb_handle::d_gate)
   float2* last_pts;    // the member's "containers of the last match": a matched scan's endpoints are copied here
-  // point-cloud input (HsbMatchParams::cloud set): the converted endpoints go to cloud_pts (the member's last-match
-  // container when the session matches, its update-scan buffer when not), their number to kept (device memory, the map
-  // writer's n_dev) and to kept_host (the group's mapped host block, before the step's sequence number is published);
-  // the conversion thresholds are the member's hsb_set_cloud_format values at step time
-  float2* cloud_pts;
+  // converted input (HsbMatchParams::cloud or ::ranges set): the converted endpoints go to conv_pts (the member's
+  // last-match container when the session matches, its update-scan buffer when not), their number to kept (device
+  // memory, the map writer's n_dev) and to kept_host (the group's mapped host block, before the step's sequence number
+  // is published)
+  float2* conv_pts;
   int* kept;
   int* kept_host;
+  // point clouds: the member's hsb_set_cloud_format thresholds at step time
   float sqr_min_dist, sqr_max_dist, z_min, z_max;
+  // raw ranges: the member's hsb_set_scan_format at step time — its (cos, sin) table, beam count and range window
+  const float2* beam_cs;
+  int n_beams;
+  float range_min, range_max_c;
 };
 
 struct HsbMatchParams {
@@ -63,8 +69,8 @@ struct HsbMatchParams {
   double cloud_tf0[12];
   float sqr_min_dist, sqr_max_dist, z_min, z_max;
   float* out_origo;         // B x 2 (may be null): dataContainer origo = laser position * scaleToMap
-  // fused single-scan SLAM step from a point cloud (B == 1): the converted endpoints are also written out for the map
-  // writer, their number goes to device memory (out_n) and to mapped host memory (out_n_host)
+  // fused single-scan SLAM step from a point cloud or raw ranges (B == 1): the converted endpoints are also written out
+  // for the map writer, their number goes to device memory (out_n) and to mapped host memory (out_n_host)
   float2* out_pts;
   int* out_n;
   int* out_n_host;
@@ -94,8 +100,10 @@ struct HsbMatchParams {
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done
   // counts the sessions that have finished: the last one publishes seq_value to seq_host.  With cloud input a session
-  // reads its thresholds from group_sess[b] (sqr_min_dist .. z_max above are unused) and a set map_without_matching flag
-  // still converts the cloud for the map writer: only the match is skipped.
+  // reads its thresholds from group_sess[b] (sqr_min_dist .. z_max above are unused); with ranges input its ranges are
+  // ranges[offsets[b] .. offsets[b+1]) and its format comes from group_sess[b] (beam_cs .. range_max_c above are
+  // unused).  Either way a set map_without_matching flag still converts the scan for the map writer: only the match is
+  // skipped.
   const HsbLevelDev* group_lv;
   const HsbGroupSessionDev* group_sess;
   unsigned* group_done;

@@ -784,7 +784,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       n = P.n_shared;
     }
     if constexpr (GRP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
-      if (!P.cloud && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a cloud is converted first, below)
+      if (!P.cloud && !P.ranges && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a conversion runs first, below)
     }
     const float2* __restrict__ gpts = P.pts + beg;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
@@ -802,27 +802,38 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       group_sync<W>(g);
       ns = n;
       staged = true;
-    } else if (P.ranges) {
-      // raw ranges in: convert + compact straight into shared memory (host guarantees cap >= n_beams)
-      n = stage_from_ranges<W>(P.ranges + (size_t)scan * P.n_beams, P.beam_cs, P.n_beams, P.range_min, P.range_max_c,
-                               P.scale_to_map, spts, warp_cnt, g, w, lane);
-      ns = n;
-      staged = true;
-    } else if (P.cloud) {
-      const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
-      float min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
-      if constexpr (GRP) {   // group SLAM step: every session converts with its own member's format
-        const HsbGroupSessionDev& SS = P.group_sess[scan];
-        min2 = SS.sqr_min_dist;
-        max2 = SS.sqr_max_dist;
-        zmin = SS.z_min;
-        zmax = SS.z_max;
-      }
-      n = stage_from_cloud<W>(P.cloud + 3 * (size_t)beg, n, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt, g,
-                              w, lane);
-      if (P.out_origo && t == 0) {   // dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
-        P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], P.scale_to_map);
-        P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], P.scale_to_map);
+    } else if (P.ranges || P.cloud) {
+      // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
+      if (P.ranges) {   // raw ranges
+        const float* r = P.ranges + (size_t)scan * P.n_beams;
+        const float2* cs = P.beam_cs;
+        int nb = P.n_beams;
+        float rmin = P.range_min, rmaxc = P.range_max_c;
+        if constexpr (GRP) {   // group SLAM step: every session converts its own slice with its own member's format
+          const HsbGroupSessionDev& SS = P.group_sess[scan];
+          r = P.ranges + beg;
+          cs = SS.beam_cs;
+          nb = SS.n_beams;
+          rmin = SS.range_min;
+          rmaxc = SS.range_max_c;
+        }
+        n = stage_from_ranges<W>(r, cs, nb, rmin, rmaxc, P.scale_to_map, spts, warp_cnt, g, w, lane);
+      } else {          // a point cloud
+        const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
+        float min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
+        if constexpr (GRP) {   // group SLAM step: every session converts with its own member's format
+          const HsbGroupSessionDev& SS = P.group_sess[scan];
+          min2 = SS.sqr_min_dist;
+          max2 = SS.sqr_max_dist;
+          zmin = SS.z_min;
+          zmax = SS.z_max;
+        }
+        n = stage_from_cloud<W>(P.cloud + 3 * (size_t)beg, n, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt,
+                                g, w, lane);
+        if (P.out_origo && t == 0) {   // dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
+          P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], P.scale_to_map);
+          P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], P.scale_to_map);
+        }
       }
       if (P.out_pts) {   // fused single-scan step: the map writer reads the converted endpoints from global memory
         for (int i = t; i < n; i += GT) P.out_pts[i] = spts[i];
@@ -835,7 +846,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
         // group SLAM step: the session's endpoints and their number go to its member for the map writer (and, matched,
         // become its last-match container); the count reaches host memory before the step's sequence number (below)
         const HsbGroupSessionDev& SS = P.group_sess[scan];
-        for (int i = t; i < n; i += GT) SS.cloud_pts[i] = spts[i];
+        for (int i = t; i < n; i += GT) SS.conv_pts[i] = spts[i];
         if (t == 0) {
           *SS.kept = n;
           *SS.kept_host = n;
@@ -1048,8 +1059,8 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     if constexpr (GRP) {
       // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
       // its later map writes without matching read it (after the pose is out: only the map writers wait for this).
-      // A converted cloud is already there (cloud_pts, above).
-      if (!P.cloud) {
+      // A converted scan is already there (conv_pts, above).
+      if (!P.cloud && !P.ranges) {
         float2* keep = P.group_sess[scan].last_pts;
         for (int i = t; i < n; i += GT) keep[i] = gpts[i];
       }

@@ -109,6 +109,36 @@ class SlamProcessor {
   // the cloud format of updateCloud / updateManyCloud (the node's laser transform and filter parameters)
   void setCloudFormat(const hsb_cloud_format& fmt) { check(hsb_set_cloud_format(h_, &fmt)); }
 
+  // The node's branch without the laser tf (use_tf_scan_transformation = false, HectorMappingRos.cpp:248-254): update()
+  // from a LaserScan's raw ranges, converted on the device (hsb_slam_update_ranges).  n must equal the scan format's
+  // n_beams; poseHintWorld is the node's getLastScanMatchPose().  Returns the number of endpoints the conversion kept.
+  int updateRanges(const float* ranges, int n, const Pose& poseHintWorld, bool map_without_matching = false) {
+    const float hint[3] = {poseHintWorld.x, poseHintWorld.y, poseHintWorld.psi};
+    float out[3];
+    int updated = 0, kept = 0;
+    check(hsb_slam_update_ranges(h_, hint, ranges, n, map_without_matching ? 1 : 0, 0, out, lastScanMatchCov_, &updated,
+                                 &kept));
+    lastScanMatchPose_ = Pose{out[0], out[1], out[2]};  // :83
+    if (updated) lastMapUpdatePose_ = lastScanMatchPose_;  // :94
+    return kept;
+  }
+
+  // updateRanges() for M processors in one device pass (hsb_group_slam_update_ranges): processor s takes the ranges
+  // ranges[offsets[s] .. offsets[s+1]) (as many as its scan format's n_beams), the hint poseHintsWorld[s] and
+  // map_without_matching[s] (may be null); kept (M ints, may be null) receives each conversion's endpoint count.  Same
+  // group cache and end state as updateMany.
+  static void updateManyRanges(SlamProcessor* const* ps, int M, const float* ranges, const int* offsets,
+                               const Pose* poseHintsWorld, const int* map_without_matching = 0, int* kept = 0) {
+    stepMany(ps, M, poseHintsWorld, "updateManyRanges",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_ranges(g, hints, ranges, offsets, map_without_matching, 0, poses, cov,
+                                                   updated, kept);
+             });
+  }
+
+  // the scan format of updateRanges / updateManyRanges (the LaserScan's beam geometry and range window)
+  void setScanFormat(const hsb_scan_format& fmt) { check(hsb_set_scan_format(h_, &fmt)); }
+
   // The same step with the control flow on the host (two C-ABI calls and a round trip in between), as the
   // reference's own HectorSlamProcessor drives MapRepB200; kept for comparison and tests.
   void updateUnfused(const float* points_xy, int n, const float origo[2], const Pose& poseHintWorld,

@@ -290,6 +290,20 @@ int hsb_slam_update_nowait(hsb_handle* h, const float pose_hint_world[3], const 
 int hsb_slam_update_cloud(hsb_handle* h, const float pose_hint_world[3], const float* points_xyz, int n,
                           const double* transform, int map_without_matching, int nowait, float out_pose_world[3],
                           float cov_inout[9], int* map_updated, int* out_kept);
+/* The branch WITHOUT the laser tf (use_tf_scan_transformation = false, HectorMappingRos.cpp:248-254) in one call:
+ * rosLaserScanToDataContainer (:483-507, origo zero, :491) followed by HectorSlamProcessor::update with the last match
+ * as the start estimate.  ranges = the LaserScan's n ranges; n must equal the n_beams of the handle's scan format
+ * (hsb_set_scan_format, read at the call), otherwise HSB_ERR_INVALID_ARG.  The conversion runs in the match kernel's
+ * staging step and its endpoints stay on the device for the map writer, as in hsb_slam_update_cloud: 4 bytes per beam
+ * cross PCIe, no host round trip, three launches.  With map_without_matching the stand-alone conversion kernel
+ * converts the scan for level 0 and the coarse levels keep the last match's containers.  nowait and *out_kept as in
+ * hsb_slam_update_cloud.  A format longer than the fused conversion can stage fails with HSB_ERR_UNSUPPORTED.
+ * Pose, covariance, gate decision, kept count, every plane and the handle's end state (gate pose, last match's
+ * container, size and origo, stamps, both dirty rectangles, the pending write after nowait) are bit-identical to
+ * hsb_scan_to_points followed by hsb_slam_update(h, hint, points, kept, origo = {0, 0}, ...). */
+int hsb_slam_update_ranges(hsb_handle* h, const float pose_hint_world[3], const float* ranges, int n,
+                           int map_without_matching, int nowait, float out_pose_world[3], float cov_inout[9],
+                           int* map_updated, int* out_kept);
 /* ---- many SLAM sessions in one device pass ------------------------------------------------------*/
 /* N robots that each build their own map are N independent HectorSlamProcessors, i.e. N handles.  A group steps
  * them together: one host-to-device copy and three kernel launches per step whatever the number of members, instead
@@ -334,6 +348,18 @@ int hsb_group_slam_update(hsb_group* g, const float* hints_world, const float* p
 int hsb_group_slam_update_cloud(hsb_group* g, const float* hints_world, const float* points_xyz, const int* offsets,
                                 const double* transforms, const int* map_without_matching, int nowait,
                                 float* out_poses_world, float* cov_inout, int* map_updated, int* out_kept);
+/* The same group step from raw LaserScan ranges: hsb_slam_update_ranges for every member at once.  Session s takes
+ * ranges[offsets[s] .. offsets[s+1]), whose length must equal its member's n_beams.  Each session converts with its own
+ * member's scan format as it is at the call (beam table, beam count, range window), so robots may differ in all of
+ * these.  out_kept, hints, map_without_matching, nowait, cov_inout and map_updated as in hsb_group_slam_update_cloud;
+ * one host-to-device copy and three launches per step.  Every session's pose, covariance, gate decision and kept count
+ * are bit-identical to hsb_slam_update_ranges on its handle with the same inputs, and every member is left in the
+ * state that call leaves.  Rejected before any member changes: a member without a scan format (HSB_ERR_INVALID_ARG,
+ * the message names the session), offsets that disagree with the members' n_beams (HSB_ERR_INVALID_ARG), a scan
+ * longer than the fused conversion can stage (HSB_ERR_UNSUPPORTED, the limit and message of hsb_slam_update_ranges). */
+int hsb_group_slam_update_ranges(hsb_group* g, const float* hints_world, const float* ranges, const int* offsets,
+                                 const int* map_without_matching, int nowait, float* out_poses_world, float* cov_inout,
+                                 int* map_updated, int* out_kept);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
