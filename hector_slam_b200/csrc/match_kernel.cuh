@@ -1132,10 +1132,11 @@ __global__ void __launch_bounds__(128)
       if (out) out[b] = lh;
       if (best) {
         // arg-max over the batch (relocalisation: the most likely hypothesis): (score, index) packed so that one
-        // 64-bit atomicMax keeps the highest score and, among equals, the LOWEST index; a non-finite pose scores -1
+        // 64-bit atomicMax keeps the highest score and, among equals, the LOWEST index; a non-finite pose scores -1,
+        // and so does a NaN likelihood (an empty scan: 1 - 0/0), whose bits would otherwise pack above every score
         const float px = poses_world[3 * b], py = poses_world[3 * b + 1], pp = poses_world[3 * b + 2];
         const bool finite = fabsf(px) <= 3.4e38f && fabsf(py) <= 3.4e38f && fabsf(pp) <= 3.4e38f;
-        const float sc = finite ? lh : -1.0f;
+        const float sc = (finite && lh == lh) ? lh : -1.0f;
         unsigned u = __float_as_uint(sc);
         u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
         atomicMax(best, ((unsigned long long)u << 32) | (unsigned long long)(0xffffffffu - (unsigned)b));

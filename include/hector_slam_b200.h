@@ -445,7 +445,8 @@ int hsb_likelihood_batch_device(hsb_handle* h, int level, int B, const float* d_
                                 const int* d_offsets, int n_shared, float* d_out_likelihood, void* stream);
 /* Score AND pick (Monte-Carlo relocalisation, BASELINE config 4): the likelihood launch above with an arg-max folded
  * in — d_best4 receives {likelihood, x, y, psi} of the most likely pose of the batch (lowest index among equals; a
- * non-finite pose scores -1; an empty batch gives likelihood -1).  d_out_likelihood may be NULL.  Two launches on
+ * non-finite pose and a NaN likelihood — an empty scan, 1 - 0/0 — score -1, so neither wins over a real score; an empty
+ * batch gives likelihood -1).  d_out_likelihood may be NULL; it keeps the reference's NaN.  Two launches on
  * `stream`, nothing is synchronised: a multi-GPU caller all-gathers the 16 bytes. */
 int hsb_best_hypothesis_device(hsb_handle* h, int level, int B, const float* d_poses_world, const float* d_points_xy,
                                const int* d_offsets, int n_shared, float* d_out_likelihood, float* d_best4, void* stream);
