@@ -37,6 +37,8 @@ EXPORTED = [
     "hsb_get_match_record_floats", "hsb_match_data_record", "hsb_match_batch_record_device",
     "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update", "hsb_group_slam_update_cloud",
     "hsb_slam_update_ranges", "hsb_group_slam_update_ranges",
+    "hsb_set_laser_projection", "hsb_projected_scan_to_points", "hsb_slam_update_projected",
+    "hsb_group_slam_update_projected",
 ]
 
 
@@ -65,6 +67,11 @@ class HsbScanFormat(C.Structure):
 class HsbCloudFormat(C.Structure):
     _fields_ = [("laser_transform", C.c_double * 12), ("sqr_laser_min_dist", C.c_float), ("sqr_laser_max_dist", C.c_float),
                 ("laser_z_min_value", C.c_float), ("laser_z_max_value", C.c_float)]
+
+
+class HsbLaserProjection(C.Structure):
+    _fields_ = [("n_beams", C.c_int), ("angle_min", C.c_float), ("angle_increment", C.c_float),
+                ("range_min", C.c_float), ("range_max", C.c_float), ("range_cutoff", C.c_double)]
 
 
 class HsbError(RuntimeError):
@@ -120,6 +127,9 @@ def load_library() -> C.CDLL:
     sig("hsb_slam_update_nowait", i, vp, vp, vp, i, vp, i, vp, vp, vp)
     sig("hsb_slam_update_cloud", i, vp, vp, vp, i, vp, i, i, vp, vp, vp, vp)
     sig("hsb_slam_update_ranges", i, vp, vp, vp, i, i, i, vp, vp, vp, vp)
+    sig("hsb_set_laser_projection", i, vp, C.POINTER(HsbLaserProjection))
+    sig("hsb_projected_scan_to_points", i, vp, vp, i, vp, vp, ip, vp)
+    sig("hsb_slam_update_projected", i, vp, vp, vp, i, vp, i, i, vp, vp, vp, vp)
     sig("hsb_get_last_map_update_pose", i, vp, vp)
     sig("hsb_set_last_map_update_pose", i, vp, vp)
     sig("hsb_upload_level", i, vp, i, vp)
@@ -175,6 +185,7 @@ def load_library() -> C.CDLL:
     sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
     sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_slam_update_ranges", i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_slam_update_projected", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -493,6 +504,23 @@ class MapRepB200:
                                                     cov.ctypes.data, C.addressof(upd), C.addressof(kept)))
         return pose, cov.reshape(3, 3), bool(upd.value), int(kept.value)
 
+    def slam_update_projected(self, pose_hint_world, ranges, transform=None, map_without_matching: bool = False,
+                              nowait: bool = False, cov_inout=None):
+        """scanCallback's default branch from the LaserScan itself: raw ranges -> laser_geometry's projection (the
+        handle's set_laser_projection) -> cloud rule (set_cloud_format) -> match, gate, map write, all fused.
+        transform: 12 float64 (None = the cloud format's).  -> (pose (3,), cov (3,3), map_updated: bool, kept: int)"""
+        hint = _f32(pose_hint_world, 3)
+        r = _f32(ranges).reshape(-1)
+        T = None if transform is None else np.ascontiguousarray(transform, dtype=np.float64).reshape(12)
+        pose = np.zeros(3, np.float32)
+        cov = np.zeros(9, np.float32) if cov_inout is None else _f32(cov_inout).reshape(9).copy()
+        upd, kept = C.c_int(0), C.c_int(0)
+        self._check(self.lib.hsb_slam_update_projected(self.h, hint.ctypes.data, r.ctypes.data, r.size, _ptr(T),
+                                                       int(bool(map_without_matching)), int(bool(nowait)),
+                                                       pose.ctypes.data, cov.ctypes.data, C.addressof(upd),
+                                                       C.addressof(kept)))
+        return pose, cov.reshape(3, 3), bool(upd.value), int(kept.value)
+
     def last_map_update_pose(self) -> np.ndarray:
         out = np.zeros(3, np.float32)
         self._check(self.lib.hsb_get_last_map_update_pose(self.h, out.ctypes.data))
@@ -630,6 +658,25 @@ class MapRepB200:
         n = C.c_int()
         self._check(self.lib.hsb_cloud_to_points(self.h, p.ctypes.data if p.size else None, p.shape[0], out.ctypes.data,
                                                  C.byref(n), origo.ctypes.data))
+        return out[: n.value].copy(), origo
+
+    # -- LaserScan ranges through laser_geometry's projection, then the cloud rule ------------------
+    def set_laser_projection(self, n_beams: int, angle_min: float, angle_increment: float, range_min: float,
+                             range_max: float, range_cutoff: float = 30.0):
+        """range_cutoff: projectLaser's third argument (the node passes 30.0); < 0 means range_max."""
+        proj = HsbLaserProjection(int(n_beams), float(angle_min), float(angle_increment), float(range_min),
+                                  float(range_max), float(range_cutoff))
+        self._check(self.lib.hsb_set_laser_projection(self.h, C.byref(proj)))
+
+    def projected_scan_to_points(self, ranges, transform=None):
+        """-> (endpoints (k, 2) float32, origo (2,) float32)"""
+        r = _f32(ranges).reshape(-1)
+        T = None if transform is None else np.ascontiguousarray(transform, dtype=np.float64).reshape(12)
+        out = np.zeros((max(1, r.size), 2), np.float32)
+        origo = np.zeros(2, np.float32)
+        n = C.c_int()
+        self._check(self.lib.hsb_projected_scan_to_points(self.h, r.ctypes.data, r.size, _ptr(T), out.ctypes.data,
+                                                          C.byref(n), origo.ctypes.data))
         return out[: n.value].copy(), origo
 
     def match_batch_cloud(self, hints, points_xyz, offsets, transforms=None, want_cov: bool = True):
@@ -893,6 +940,27 @@ class SlamGroup:
                                                           offsets.ctypes.data, _ptr(mwm), int(bool(nowait)),
                                                           poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
                                                           kept.ctypes.data))
+        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+
+    def slam_update_projected(self, hints, ranges_list, transforms=None, map_without_matching=None, nowait: bool = False,
+                              cov_inout=None):
+        """The same step from the LaserScans of default-configured nodes (hsb_group_slam_update_projected): ranges_list
+        is M (n_beams_s,) arrays, or a tuple (ranges (N,), offsets (M + 1,)); transforms (M, 12) float64, None = each
+        member's cloud format.  Each member projects with its own laser projection and converts with its own cloud
+        format.  -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
+        M = self.M
+        h = _f32(hints).reshape(M, 3)
+        r, offsets = self._pack(ranges_list, 1)
+        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(M, 12)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
+        poses = np.zeros((M, 3), np.float32)
+        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
+        upd = np.zeros(M, np.int32)
+        kept = np.zeros(M, np.int32)
+        self._check(self.lib.hsb_group_slam_update_projected(self.g, h.ctypes.data, r.ctypes.data if r.size else None,
+                                                             offsets.ctypes.data, _ptr(T), _ptr(mwm), int(bool(nowait)),
+                                                             poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
+                                                             kept.ctypes.data))
         return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
 
     def _pack(self, scans, width):

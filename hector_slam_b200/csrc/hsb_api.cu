@@ -76,6 +76,9 @@ struct hsb_handle {
   hsb_cloud_format cfmt = hsb_cloud_format();
   bool cfmt_set = false;
   DevBuf d_cloud, d_cloud_off, d_cloud_tf, d_origo;
+  DevBuf d_proj_unit;   // laser_geometry's unit vectors, n_beams x double (cos, sin)
+  hsb_laser_projection proj = hsb_laser_projection();
+  bool proj_set = false;
   DevBuf d_fused_in;   // the fused single SLAM steps' upload: header, (laser transform,) cloud or ranges
   int last_n = 0;
   float last_origo[2] = {0.f, 0.f};
@@ -276,12 +279,12 @@ int fail_fused_too_long(hsb_handle* h, int max_n) {
   return fail(h, HSB_ERR_UNSUPPORTED, "scan too long for the fused conversion (%d points)", max_n);
 }
 
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false>
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
 int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int Gr,
                    const hsb::InlineScan<INL>& S = hsb::InlineScan<INL>()) {
   if (Gr <= 0 || Gr > G) Gr = G;   // groups per CTA actually launched (a G-group kernel runs with fewer: see launch_match)
   const size_t header = hsb::MatchSmem<W, G>::kHeaderBytes;
-  auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL, GRP>;
+  auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL, GRP, PROJ>;
   constexpr size_t kMaxDyn = kMaxDynSmem;
   constexpr int gt = W * 32;           // threads per scan
   int cap = 0;
@@ -713,7 +716,7 @@ int hsb_destroy(hsb_handle* h) {
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
                     &h->d_beam_cs, &h->d_ranges, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
-                    &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_fused_in};
+                    &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_fused_in, &h->d_proj_unit};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int k = 0; k < 2; ++k) {
@@ -1155,6 +1158,104 @@ int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, con
   P.out_cov = d_out_cov;
   fill_cloud_params(h, P, d_points_xyz, d_offsets, d_transforms, d_out_origo);
   return launch_match(h, P, max_points_per_scan, (cudaStream_t)stream);
+}
+
+// ---- the default path from the LaserScan: laser_geometry's projection + the cloud rule -----------
+
+int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj) {
+  if (!h || !proj) return HSB_ERR_INVALID_ARG;
+  if (proj->n_beams < 1 || proj->n_beams > (1 << 20))
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_laser_projection: n_beams is %d, must lie in [1, 2^20]", proj->n_beams);
+  if (!std::isfinite(proj->angle_min) || !std::isfinite(proj->angle_increment) || !std::isfinite(proj->range_min))
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_laser_projection: angle_min, angle_increment and range_min must be finite");
+  if (std::isnan(proj->range_cutoff)) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_laser_projection: range_cutoff is NaN");
+  if (proj->range_cutoff < 0.0 && std::isnan(proj->range_max))   // the cutoff is range_max then
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_laser_projection: range_cutoff < 0 selects range_max, which is NaN");
+  HandleScope guard(h);
+  // getUnitVectors_: cos / sin of angle_min + index * angle_increment, all double, libm
+  std::vector<double> tab((size_t)proj->n_beams * 2);
+  for (int i = 0; i < proj->n_beams; ++i) {
+    const double a = (double)proj->angle_min + (double)i * (double)proj->angle_increment;
+    tab[2 * (size_t)i] = cos(a);
+    tab[2 * (size_t)i + 1] = sin(a);
+  }
+  // a step still queued on the handle's stream may read the old table
+  HSB_CUDA(h, cudaStreamSynchronize(h->stream));
+  int s = ensure(h, h->d_proj_unit, tab.size() * sizeof(double));
+  if (s != HSB_OK) return s;
+  HSB_CUDA(h, cudaMemcpy(h->d_proj_unit.p, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice));
+  h->proj = *proj;
+  h->proj_set = true;
+  return HSB_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// projectLaser: a negative cutoff means the scan's range_max
+double projection_cutoff(const hsb_laser_projection& p) { return p.range_cutoff < 0.0 ? (double)p.range_max : p.range_cutoff; }
+
+// the projection and cloud format a projected step needs, and its beam count; `fn` names the entry point
+int check_projected(hsb_handle* h, const char* fn, int n) {
+  if (!h->proj_set) return fail(h, HSB_ERR_INVALID_ARG, "%s: hsb_set_laser_projection has not been called", fn);
+  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "%s: hsb_set_cloud_format has not been called", fn);
+  if (n != h->proj.n_beams)
+    return fail(h, HSB_ERR_INVALID_ARG, "%s: n is %d, the laser projection has %d beams", fn, n, h->proj.n_beams);
+  // every projected step converts the whole scan into the shared memory of the single step's match shape
+  if (!staging_fits<8, 1>(whole_scan_slots(n), 1)) return fail_fused_too_long(h, n);
+  return HSB_OK;
+}
+
+void fill_projected_params(const hsb_handle* h, HsbMatchParams& P, const float* d_ranges, const double* d_transforms) {
+  fill_cloud_params(h, P, nullptr, nullptr, d_transforms, nullptr);   // thresholds, default transform, scaleToMap
+  P.ranges = d_ranges;
+  P.n_beams = h->proj.n_beams;
+  P.range_min = h->proj.range_min;
+  P.range_cutoff = projection_cutoff(h->proj);
+  P.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
+}
+
+int launch_projected_conversion(hsb_handle* h, const float* d_ranges, const double* d_T, float2* d_out, int* d_n,
+                                cudaStream_t st) {
+  hsb::projected_to_points_kernel<<<1, 256, 0, st>>>(
+      d_ranges, static_cast<const double2*>(h->d_proj_unit.p), h->proj.n_beams, h->proj.range_min,
+      projection_cutoff(h->proj), d_T, h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist, h->cfmt.laser_z_min_value,
+      h->cfmt.laser_z_max_value, h->lv[0].scale, d_out, d_n);
+  HSB_CUDA(h, cudaGetLastError());
+  return HSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, const double* transform, float* out_xy,
+                                 int* out_n, float out_origo[2]) {
+  if (!h || !ranges || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
+  int s = check_projected(h, "hsb_projected_scan_to_points", n);
+  if (s != HSB_OK) return s;
+  HandleScope guard(h);
+  const double* T = transform ? transform : h->cfmt.laser_transform;
+  if ((s = ensure(h, h->d_ranges, (size_t)n * 4)) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_pts, (size_t)n * 8 + 16)) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
+  cudaStream_t st = h->stream;
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_ranges.p, ranges, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  int* d_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
+  if ((s = launch_projected_conversion(h, static_cast<const float*>(h->d_ranges.p), static_cast<const double*>(h->d_cloud_tf.p),
+                                       static_cast<float2*>(h->d_pts.p), d_n, st)) != HSB_OK)
+    return s;
+  h->launches++;
+  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaStreamSynchronize(st));
+  const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
+  if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
+  *out_n = kept;
+  if (out_origo) cloud_origo(h, T, out_origo);
+  return HSB_OK;
 }
 
 }  // extern "C"
@@ -1659,12 +1760,14 @@ int hsb_slam_update_nowait(hsb_handle* h, const float hint[3], const float* pts,
 }
 
 // What a fused single SLAM step converts on the device: a Point32 cloud in the laser frame with its laser transform
-// (hsb_slam_update_cloud), or a LaserScan's raw ranges in the handle's scan format (hsb_slam_update_ranges).
+// (hsb_slam_update_cloud), a LaserScan's raw ranges in the handle's scan format (hsb_slam_update_ranges), or raw
+// ranges projected with the handle's laser projection and then converted as a cloud (hsb_slam_update_projected).
+enum FusedKind { FUSED_CLOUD, FUSED_RANGES, FUSED_PROJECTED };
 struct FusedScan {
-  bool ranges;
-  const float* data;    // cloud: n (x, y, z) triples; ranges: n ranges
-  int n;                // cloud: points; ranges: the scan format's n_beams
-  const double* T;      // cloud: the laser transform (12 doubles)
+  FusedKind kind;
+  const float* data;    // cloud: n (x, y, z) triples; ranges / projected: n ranges
+  int n;                // cloud: points; ranges / projected: n_beams (an upper bound of the endpoints kept)
+  const double* T;      // cloud / projected: the laser transform (12 doubles)
 };
 
 // HectorMappingRos::scanCallback's conversion + HectorSlamProcessor::update (:297 / HectorSlamProcessor.h:71-113) as
@@ -1680,8 +1783,9 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
   // staging layout (floats): [0..15] header: hint, thresholds, force, [8] = 0, [9] = n (cloud offsets, as ints);
-  // cloud: [16..39] the laser transform (12 doubles), [40..] the cloud; ranges: [16..] the ranges
-  const size_t kHdr = 16, kTf = in.ranges ? 0 : 24, per_pt = in.ranges ? 1 : 3;
+  // cloud / projected: [16..39] the laser transform (12 doubles), [40..] the cloud or the ranges; ranges: [16..] the ranges
+  const bool ranges = in.kind == FUSED_RANGES, projected = in.kind == FUSED_PROJECTED;
+  const size_t kHdr = 16, kTf = ranges ? 0 : 24, per_pt = in.kind == FUSED_CLOUD ? 3 : 1;
   const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
   if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
   if (bytes > h->h_stage_bytes) {
@@ -1698,7 +1802,7 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
   hs[3] = h->min_dist; hs[4] = h->min_angle; hs[5] = map_without_matching ? 1.f : 0.f;
   reinterpret_cast<int*>(hs)[8] = 0;
   reinterpret_cast<int*>(hs)[9] = n;
-  if (!in.ranges) memcpy(hs + kHdr, in.T, 12 * sizeof(double));
+  if (!ranges) memcpy(hs + kHdr, in.T, 12 * sizeof(double));
   if (n > 0) memcpy(hs + kHdr + kTf, in.data, (size_t)n * per_pt * sizeof(float));
   cudaStream_t st = h->stream;
   HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
@@ -1712,7 +1816,7 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
   int* d_n = reinterpret_cast<int*>(d_s + 40);
   // the container's origo is known on the host: zero for a LaserScan (HectorMappingRos.cpp:491)
   float origo[2] = {0.f, 0.f};
-  if (!in.ranges) cloud_origo(h, in.T, origo);
+  if (!ranges) cloud_origo(h, in.T, origo);
   // results always travel through mapped host memory here
   const bool poll = nowait != 0;
   volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
@@ -1730,7 +1834,8 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
     P.hints = d_hdr;
     P.out_poses = d_s + 8;
     P.out_cov = h->h_pin_dev + 12;
-    if (in.ranges) fill_range_params(h, P, d_in);
+    if (ranges) fill_range_params(h, P, d_in);
+    else if (projected) fill_projected_params(h, P, d_in, d_tf);
     else fill_cloud_params(h, P, d_in, d_offs, d_tf, nullptr);
     P.out_pts = d_pts_out;
     P.out_n = d_n;
@@ -1740,12 +1845,21 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
     P.gate_out_host = h->h_pin_dev + 8;
     P.seq_host = poll ? seq_dev : nullptr;
     P.seq_value = seq_value;
-    if ((s = launch_match(h, P, n, st)) != HSB_OK) return s;
+    // (the projection is compiled into the single step's default shape only: hsb_slam_update_projected checked the tuning)
+    if (projected)
+      s = h->gather_mode == HSB_GATHER_TEX
+              ? launch_match_t<8, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, n, st, 1)
+              : launch_match_t<8, 1, hsb::MODE_LDG, 4, false, false, false, true>(h, P, n, st, 1);
+    else
+      s = launch_match(h, P, n, st);
+    if (s != HSB_OK) return s;
     h->last_n = n;   // upper bound until the kept count arrives (the writer reads the exact one on the device)
     h->last_origo[0] = origo[0];
     h->last_origo[1] = origo[1];
   } else {
-    if (in.ranges)
+    if (projected) {
+      if ((s = launch_projected_conversion(h, d_in, d_tf, d_pts_out, d_n, st)) != HSB_OK) return s;
+    } else if (ranges)
       hsb::scan_to_points_kernel<<<1, 256, 0, st>>>(d_in, static_cast<const float2*>(h->d_beam_cs.p), n, h->fmt.range_min,
                                                     range_max_c(h->fmt), h->lv[0].scale, d_pts_out, d_n);
     else
@@ -1789,7 +1903,7 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
                           int* out_kept) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
   if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  const FusedScan in = {false, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
+  const FusedScan in = {FUSED_CLOUD, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
@@ -1802,7 +1916,25 @@ int hsb_slam_update_ranges(hsb_handle* h, const float hint[3], const float* rang
   if (n != h->fmt.n_beams)
     return fail(h, HSB_ERR_INVALID_ARG, "hsb_slam_update_ranges: n is %d, the scan format has %d beams", n,
                 h->fmt.n_beams);
-  const FusedScan in = {true, ranges, n, nullptr};
+  const FusedScan in = {FUSED_RANGES, ranges, n, nullptr};
+  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
+}
+
+// ... and the default branch from the LaserScan itself (:258-297): laser_geometry's projection (:273), then
+// rosPointCloudToDataContainer (:283) + HectorSlamProcessor::update (:297)
+int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* ranges, int n, const double* transform,
+                              int map_without_matching, int nowait, float out_pose[3], float cov_inout[9],
+                              int* map_updated, int* out_kept) {
+  if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
+  int s = check_projected(h, "hsb_slam_update_projected", n);
+  if (s != HSB_OK) return s;
+  // the match shape hsb_slam_update_cloud would take under this tuning must be the one compiled with the projection
+  if (!((h->tune_warps_per_scan == 0 || h->tune_warps_per_scan == 8) && h->tune_scans_per_block <= 1 &&
+        (h->tune_unroll == 0 || h->tune_unroll == 4) && !(h->gather_mode == HSB_GATHER_TEX && h->tune_packed)))
+    return fail(h, HSB_ERR_UNSUPPORTED,
+                "hsb_slam_update_projected: no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d "
+                "unroll=%d packed=%d", h->tune_warps_per_scan, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
+  const FusedScan in = {FUSED_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
@@ -2441,9 +2573,10 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
 namespace {
 
 // What a group step's sessions bring: level-0 endpoints (hsb_group_slam_update), the node's projected point clouds
-// (hsb_group_slam_update_cloud) or raw LaserScan ranges (hsb_group_slam_update_ranges).  Clouds and ranges are
-// converted in the match kernel's staging step as hsb_slam_update_cloud / hsb_slam_update_ranges convert them.
-enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD, GROUP_RANGES };
+// (hsb_group_slam_update_cloud), raw LaserScan ranges (hsb_group_slam_update_ranges) or raw ranges to project
+// (hsb_group_slam_update_projected).  All but endpoints are converted in the match kernel's staging step as
+// hsb_slam_update_cloud / _ranges / _projected convert them.
+enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD, GROUP_RANGES, GROUP_PROJECTED };
 struct GroupInput {
   GroupInputKind kind;
   const char* fn;              // the entry point, for the error messages
@@ -2451,7 +2584,7 @@ struct GroupInput {
   const float* pts;            // endpoints: xy pairs; cloud: Point32 triples; ranges: one float per beam
   const int* offsets;          // M + 1, in points (ranges: in beams)
   const float* origo;          // endpoints: M x 2 (NULL = 0, 0)
-  const double* transforms;    // cloud: M x 12 (NULL = every member's hsb_set_cloud_format transform)
+  const double* transforms;    // cloud / projected: M x 12 (NULL = every member's hsb_set_cloud_format transform)
 };
 
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
@@ -2462,8 +2595,9 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
                float* cov_inout, int* map_updated, int* out_kept) {
   hsb_handle* h0 = g->m[0];
   const int M = (int)g->m.size(), levels = g->levels;
-  const bool cloud = in.kind == GROUP_CLOUD, ranges = in.kind == GROUP_RANGES;
-  const bool conv = cloud || ranges;   // converted on the device: the kept count decides what the session had
+  const bool cloud = in.kind == GROUP_CLOUD, ranges = in.kind == GROUP_RANGES, projected = in.kind == GROUP_PROJECTED;
+  const bool conv = cloud || ranges || projected;   // converted on the device: the kept count decides what the session had
+  const bool tf = cloud || projected;               // with a laser transform per session
   const int* offsets = in.offsets;
   if (!in.hints || !offsets || !out_poses)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
@@ -2478,8 +2612,19 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   }
   const int total = offsets[M];
   if (total > 0 && !in.pts)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : ranges ? "ranges" : "points_xy");
-  if (cloud) {
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : conv ? "ranges" : "points_xy");
+  if (projected) {
+    for (int k = 0; k < M; ++k) {
+      const hsb_handle* h = g->m[k];
+      if (!h->proj_set)
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_laser_projection has not been called on its handle",
+                    in.fn, k);
+      if (offsets[k + 1] - offsets[k] != h->proj.n_beams)
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d has %d ranges, its laser projection has %d beams", in.fn, k,
+                    offsets[k + 1] - offsets[k], h->proj.n_beams);
+    }
+  }
+  if (tf) {
     for (int k = 0; k < M; ++k)
       if (!g->m[k]->cfmt_set)
         return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_cloud_format has not been called on its handle",
@@ -2511,13 +2656,13 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   }
 
   // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments |
-  // laser transforms (cloud) | scans
+  // laser transforms (cloud, projected) | scans
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
   const size_t o_gin = al((size_t)M * 12), o_off = al(o_gin + (size_t)M * 12), o_sess = al(o_off + (size_t)(M + 1) * 4);
   const size_t o_upd = al(o_sess + (size_t)M * sizeof(HsbGroupSessionDev));
   const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_tf = al(o_lo + (size_t)M * 8);
-  const size_t o_pts = al(o_tf + (cloud ? (size_t)M * 12 * sizeof(double) : 0));
-  const size_t pt_bytes = cloud ? 12 : ranges ? 4 : 8;
+  const size_t o_pts = al(o_tf + (tf ? (size_t)M * 12 * sizeof(double) : 0));
+  const size_t pt_bytes = cloud ? 12 : conv ? 4 : 8;
   const size_t bytes = o_pts + (size_t)total * pt_bytes;
   if (bytes > g->h_stage_bytes) {
     if (g->h_stage) cudaFreeHost(g->h_stage);
@@ -2548,7 +2693,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     const int n = offsets[k + 1] - offsets[k];   // a cloud's size / a scan's beams: an upper bound of the endpoints kept
     const bool matched = !(map_without_matching && map_without_matching[k]);
     float og[2] = {0.f, 0.f};
-    if (cloud) {
+    if (tf) {
       const double* T = in.transforms ? in.transforms + 12 * (size_t)k : h->cfmt.laser_transform;
       memcpy(s_tf + 12 * (size_t)k, T, 12 * sizeof(double));
       cloud_origo(h, T, og);
@@ -2579,12 +2724,18 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
       ss.conv_pts = reinterpret_cast<float2*>(scan_points(pbuf));
       ss.kept = kept_dev + k;
       ss.kept_host = kept_mapped + k;
-      if (cloud) {
+      if (tf) {
         ss.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
         ss.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
         ss.z_min = h->cfmt.laser_z_min_value;
         ss.z_max = h->cfmt.laser_z_max_value;
-      } else {
+      }
+      if (projected) {
+        ss.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
+        ss.n_beams = h->proj.n_beams;
+        ss.range_min = h->proj.range_min;
+        ss.range_cutoff = projection_cutoff(h->proj);
+      } else if (ranges) {
         ss.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
         ss.n_beams = h->fmt.n_beams;
         ss.range_min = h->fmt.range_min;
@@ -2632,6 +2783,9 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   } else if (ranges) {   // (likewise the scan format; the offsets locate each session's ranges)
     fill_range_params(h0, P, reinterpret_cast<const float*>(d_in));
     P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  } else if (projected) {   // (likewise the projection and cloud format)
+    fill_projected_params(h0, P, reinterpret_cast<const float*>(d_in), reinterpret_cast<const double*>(ds + o_tf));
+    P.offsets = reinterpret_cast<const int*>(ds + o_off);
   } else {
     P.pts = reinterpret_cast<const float2*>(d_in);
     P.offsets = reinterpret_cast<const int*>(ds + o_off);
@@ -2645,9 +2799,14 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   P.group_lv = g->d_lv;
   P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
-  s = h0->gather_mode == HSB_GATHER_TEX
-          ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
-          : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
+  if (projected)
+    s = h0->gather_mode == HSB_GATHER_TEX
+            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true, true>(h0, P, max_n, st, 1)
+            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true, true>(h0, P, max_n, st, 1);
+  else
+    s = h0->gather_mode == HSB_GATHER_TEX
+            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
+            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
   if (s != HSB_OK) return s;
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
@@ -2743,6 +2902,14 @@ int hsb_group_slam_update_ranges(hsb_group* g, const float* hints, const float* 
                                  int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {GROUP_RANGES, "hsb_group_slam_update_ranges", hints, ranges, offsets, nullptr, nullptr};
+  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+}
+
+int hsb_group_slam_update_projected(hsb_group* g, const float* hints, const float* ranges, const int* offsets,
+                                    const double* transforms, const int* map_without_matching, int nowait,
+                                    float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {GROUP_PROJECTED, "hsb_group_slam_update_projected", hints, ranges, offsets, nullptr, transforms};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 

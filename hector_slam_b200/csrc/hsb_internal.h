@@ -40,6 +40,10 @@ struct HsbGroupSessionDev {
   const float2* beam_cs;
   int n_beams;
   float range_min, range_max_c;
+  // projected ranges (match_kernel<..., PROJ = true>): the member's hsb_set_laser_projection at step time — its double
+  // (cos, sin) table and projector cutoff (n_beams and range_min above), with the cloud format's thresholds above
+  const double2* proj_unit;
+  double range_cutoff;
 };
 
 struct HsbMatchParams {
@@ -107,6 +111,11 @@ struct HsbMatchParams {
   const HsbLevelDev* group_lv;
   const HsbGroupSessionDev* group_sess;
   unsigned* group_done;
+  // projected ranges (match_kernel<..., PROJ = true>, hsb_slam_update_projected): scan b's ranges[b * n_beams ..] are
+  // kept where (double)r < range_cutoff && r >= range_min, projected with proj_unit (n_beams x double (cos, sin)) and
+  // converted with the cloud thresholds and transform above
+  const double2* proj_unit;
+  double range_cutoff;
 };
 
 struct HsbUpdateLevelDev {

@@ -621,9 +621,8 @@ struct CloudPoint {
   float ex, ey;
   bool keep;
 };
-__device__ __forceinline__ CloudPoint cloud_point(const float* __restrict__ xyz, int i, const double* T, float min2, float max2,
-                                                  float zmin, float zmax, float scale) {
-  const float x = __ldg(xyz + 3 * (size_t)i), y = __ldg(xyz + 3 * (size_t)i + 1), z = __ldg(xyz + 3 * (size_t)i + 2);
+__device__ __forceinline__ CloudPoint cloud_point_xyz(float x, float y, float z, const double* T, float min2, float max2,
+                                                      float zmin, float zmax, float scale) {
   const float d2 = __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y));
   CloudPoint o;
   o.keep = (d2 > min2) && (d2 < max2) && !((x < 0.0f) && (d2 < 0.50f));
@@ -637,17 +636,43 @@ __device__ __forceinline__ CloudPoint cloud_point(const float* __restrict__ xyz,
   o.ey = __fmul_rn((float)by, scale);
   return o;
 }
-template <int W>
-__device__ __forceinline__ int stage_from_cloud(const float* __restrict__ xyz, int n_in, const double* T, float min2, float max2,
-                                                float zmin, float zmax, float scale, float2* dst, int* warp_cnt, int g, int w,
-                                                int lane) {
+__device__ __forceinline__ CloudPoint cloud_point(const float* __restrict__ xyz, int i, const double* T, float min2, float max2,
+                                                  float zmin, float zmax, float scale) {
+  const float x = __ldg(xyz + 3 * (size_t)i), y = __ldg(xyz + 3 * (size_t)i + 1), z = __ldg(xyz + 3 * (size_t)i + 2);
+  return cloud_point_xyz(x, y, z, T, min2, max2, zmin, zmax, scale);
+}
+
+// ---- N2, default path from the LaserScan itself: laser_geometry's projection, then the cloud rule above ----------
+// laser_geometry (ROS1 Melodic/Noetic) LaserProjection::projectLaser_ for the sensor_msgs/PointCloud output, the
+// projection the node runs before rosPointCloudToDataContainer (HectorMappingRos.cpp:273, projectLaser(scan, cloud,
+// 30.0)): beam i is kept iff (double)range < range_cutoff && range >= range_min (float compare; NaN and +-inf drop out),
+// and becomes the Point32 ((float)(range * cos_i), (float)(range * sin_i), 0) with one double product each.  The unit
+// vectors (getUnitVectors_: cos / sin of angle_min + i * angle_increment in double) arrive as a table built on the host
+// with libm.  The projected point then takes the cloud rule with z = 0 in the full tf dot product.  The two filters
+// compose into one over the beams, in beam order.
+__device__ __forceinline__ CloudPoint projected_point(const float* __restrict__ r_scan, const double2* __restrict__ unit,
+                                                      int i, float rmin, double cutoff, const double* T, float min2,
+                                                      float max2, float zmin, float zmax, float scale) {
+  const float r = __ldg(r_scan + i);
+  const double2 u = __ldg(unit + i);
+  const double rd = (double)r;
+  CloudPoint o = cloud_point_xyz((float)__dmul_rn(rd, u.x), (float)__dmul_rn(rd, u.y), 0.0f, T, min2, max2, zmin, zmax,
+                                 scale);
+  o.keep = o.keep && (rd < cutoff) && (r >= rmin);
+  return o;
+}
+// Converts points [0, n_in) with `at(i)` (a CloudPoint) and compacts the kept ones in input order into `dst`; returns
+// their number.  Warp w converts the contiguous range [w*chunk, (w+1)*chunk); with W > 1 a first pass counts each warp's
+// kept points for the cross-warp prefix.
+template <int W, typename PointAt>
+__device__ __forceinline__ int stage_compacted(int n_in, PointAt at, float2* dst, int* warp_cnt, int g, int w, int lane) {
   const int chunk = (n_in + W - 1) / W;
   const int b0 = w * chunk, b1 = min(n_in, b0 + chunk);
   int mine = 0;
   if (W > 1) {
     for (int base = b0; base < b1; base += 32) {
       const int i = base + lane;
-      const bool v = (i < b1) && cloud_point(xyz, i, T, min2, max2, zmin, zmax, scale).keep;
+      const bool v = (i < b1) && at(i).keep;
       mine += __popc(__ballot_sync(0xffffffffu, v));
     }
     if (lane == 0) warp_cnt[w] = mine;
@@ -666,7 +691,7 @@ __device__ __forceinline__ int stage_from_cloud(const float* __restrict__ xyz, i
     const int i = base + lane;
     CloudPoint p;
     p.keep = false;
-    if (i < b1) p = cloud_point(xyz, i, T, min2, max2, zmin, zmax, scale);
+    if (i < b1) p = at(i);
     const unsigned m = __ballot_sync(0xffffffffu, p.keep);
     if (p.keep) dst[off + __popc(m & ((1u << lane) - 1u))] = make_float2(p.ex, p.ey);
     off += __popc(m);
@@ -674,6 +699,22 @@ __device__ __forceinline__ int stage_from_cloud(const float* __restrict__ xyz, i
   if (W == 1) total = off;
   group_sync<W>(g);
   return total;
+}
+template <int W>
+__device__ __forceinline__ int stage_from_cloud(const float* __restrict__ xyz, int n_in, const double* T, float min2, float max2,
+                                                float zmin, float zmax, float scale, float2* dst, int* warp_cnt, int g, int w,
+                                                int lane) {
+  return stage_compacted<W>(n_in, [&](int i) { return cloud_point(xyz, i, T, min2, max2, zmin, zmax, scale); }, dst,
+                            warp_cnt, g, w, lane);
+}
+template <int W>
+__device__ __forceinline__ int stage_from_projected(const float* __restrict__ r_scan, const double2* __restrict__ unit,
+                                                    int n_beams, float rmin, double cutoff, const double* T, float min2,
+                                                    float max2, float zmin, float zmax, float scale, float2* dst,
+                                                    int* warp_cnt, int g, int w, int lane) {
+  return stage_compacted<W>(
+      n_beams, [&](int i) { return projected_point(r_scan, unit, i, rmin, cutoff, T, min2, max2, zmin, zmax, scale); },
+      dst, warp_cnt, g, w, lane);
 }
 
 // Shared-memory carve-up for G groups: [G] mbarriers | [G][2][9][32] reduction slots | points
@@ -717,7 +758,9 @@ __device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P
 }
 
 // GRP: the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv.
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false>
+// PROJ: the ranges input (P.ranges) goes through laser_geometry's projection and the cloud rule (stage_from_projected)
+// instead of rosLaserScanToDataContainer; only the instantiations the projected SLAM steps launch carry that branch.
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
 __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -804,7 +847,28 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       staged = true;
     } else if (P.ranges || P.cloud) {
       // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
-      if (P.ranges) {   // raw ranges
+      if constexpr (PROJ) {   // raw ranges, projected to a cloud in the laser frame and converted by the cloud rule
+        const float* r = P.ranges + (size_t)scan * P.n_beams;
+        const double2* unit = P.proj_unit;
+        const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
+        int nb = P.n_beams;
+        float rmin = P.range_min, min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
+        double cutoff = P.range_cutoff;
+        if constexpr (GRP) {   // group SLAM step: every session with its own member's projection and cloud format
+          const HsbGroupSessionDev& SS = P.group_sess[scan];
+          r = P.ranges + beg;
+          unit = SS.proj_unit;
+          nb = SS.n_beams;
+          rmin = SS.range_min;
+          cutoff = SS.range_cutoff;
+          min2 = SS.sqr_min_dist;
+          max2 = SS.sqr_max_dist;
+          zmin = SS.z_min;
+          zmax = SS.z_max;
+        }
+        n = stage_from_projected<W>(r, unit, nb, rmin, cutoff, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt,
+                                    g, w, lane);
+      } else if (P.ranges) {   // raw ranges
         const float* r = P.ranges + (size_t)scan * P.n_beams;
         const float2* cs = P.beam_cs;
         int nb = P.n_beams;
@@ -1086,6 +1150,19 @@ __global__ void __launch_bounds__(256)
   __shared__ int warp_cnt[32];
   const int n = stage_from_cloud<8>(xyz, n_in, T, min2, max2, zmin, zmax, scale, out, warp_cnt, 0, threadIdx.x >> 5,
                                     threadIdx.x & 31);
+  if (threadIdx.x == 0) *out_n = n;
+}
+
+__global__ void __launch_bounds__(256)
+    projected_to_points_kernel(const float* __restrict__ ranges, const double2* __restrict__ unit, int n_beams, float rmin,
+                               double cutoff, const double* __restrict__ T, float min2, float max2, float zmin, float zmax,
+                               float scale, float2* __restrict__ out, int* __restrict__ out_n) {
+  __shared__ int warp_cnt[32];
+  double Tr[12];   // the transform read once (left to ptxas, the per-point reloads spill at its 32-register choice)
+#pragma unroll
+  for (int k = 0; k < 12; ++k) Tr[k] = T[k];
+  const int n = stage_from_projected<8>(ranges, unit, n_beams, rmin, cutoff, Tr, min2, max2, zmin, zmax, scale, out,
+                                        warp_cnt, 0, threadIdx.x >> 5, threadIdx.x & 31);
   if (threadIdx.x == 0) *out_n = n;
 }
 

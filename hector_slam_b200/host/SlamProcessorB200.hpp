@@ -139,6 +139,40 @@ class SlamProcessor {
   // the scan format of updateRanges / updateManyRanges (the LaserScan's beam geometry and range window)
   void setScanFormat(const hsb_scan_format& fmt) { check(hsb_set_scan_format(h_, &fmt)); }
 
+  // The node's default branch from the LaserScan it receives (HectorMappingRos.cpp:258-297): laser_geometry's
+  // projection (:273), the cloud conversion (:283) and update() (:297) on the device (hsb_slam_update_projected).  n
+  // must equal the laser projection's n_beams; transform: the scan's tf laser transform, null = the cloud format's.
+  // Returns the number of endpoints the conversion kept.
+  int updateProjected(const float* ranges, int n, const double* transform, const Pose& poseHintWorld,
+                      bool map_without_matching = false) {
+    const float hint[3] = {poseHintWorld.x, poseHintWorld.y, poseHintWorld.psi};
+    float out[3];
+    int updated = 0, kept = 0;
+    check(hsb_slam_update_projected(h_, hint, ranges, n, transform, map_without_matching ? 1 : 0, 0, out,
+                                    lastScanMatchCov_, &updated, &kept));
+    lastScanMatchPose_ = Pose{out[0], out[1], out[2]};  // :83
+    if (updated) lastMapUpdatePose_ = lastScanMatchPose_;  // :94
+    return kept;
+  }
+
+  // updateProjected() for M processors in one device pass (hsb_group_slam_update_projected): processor s takes the
+  // ranges ranges[offsets[s] .. offsets[s+1]) (as many as its projection's n_beams) with transforms[12s..] (may be null:
+  // each processor's cloud format), the hint poseHintsWorld[s] and map_without_matching[s] (may be null); kept (M ints,
+  // may be null) receives each conversion's endpoint count.  Same group cache and end state as updateMany.
+  static void updateManyProjected(SlamProcessor* const* ps, int M, const float* ranges, const int* offsets,
+                                  const double* transforms, const Pose* poseHintsWorld, const int* map_without_matching = 0,
+                                  int* kept = 0) {
+    stepMany(ps, M, poseHintsWorld, "updateManyProjected",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_projected(g, hints, ranges, offsets, transforms, map_without_matching, 0,
+                                                      poses, cov, updated, kept);
+             });
+  }
+
+  // the laser projection of updateProjected / updateManyProjected (the LaserScan's beam geometry and projectLaser's
+  // cutoff); the cloud format (setCloudFormat) supplies the rest
+  void setLaserProjection(const hsb_laser_projection& proj) { check(hsb_set_laser_projection(h_, &proj)); }
+
   // The same step with the control flow on the host (two C-ABI calls and a round trip in between), as the
   // reference's own HectorSlamProcessor drives MapRepB200; kept for comparison and tests.
   void updateUnfused(const float* points_xy, int n, const float origo[2], const Pose& poseHintWorld,

@@ -128,6 +128,49 @@ int hsbp_update_many_ranges(void* const* ps, int M, const float* ranges, const i
   }
   return 0;
 }
+int hsbp_set_laser_projection(void* p, int n_beams, float angle_min, float angle_increment, float range_min,
+                              float range_max, double range_cutoff) {
+  hsb_laser_projection proj;
+  proj.n_beams = n_beams;
+  proj.angle_min = angle_min;
+  proj.angle_increment = angle_increment;
+  proj.range_min = range_min;
+  proj.range_max = range_max;
+  proj.range_cutoff = range_cutoff;
+  try {
+    static_cast<hsb200::SlamProcessor*>(p)->setLaserProjection(proj);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_projected(void* p, const float* ranges, int n, const double* transform, const float hint[3],
+                          int map_without_matching, int* out_kept) {
+  try {
+    const int kept = static_cast<hsb200::SlamProcessor*>(p)->updateProjected(
+        ranges, n, transform, hsb200::Pose{hint[0], hint[1], hint[2]}, map_without_matching != 0);
+    if (out_kept) *out_kept = kept;
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_many_projected(void* const* ps, int M, const float* ranges, const int* offsets, const double* transforms,
+                               const float* hints, const int* map_without_matching, int* out_kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) {
+    procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+    poses[s] = hsb200::Pose{hints[3 * s], hints[3 * s + 1], hints[3 * s + 2]};
+  }
+  try {
+    hsb200::SlamProcessor::updateManyProjected(procs.data(), M, ranges, offsets, transforms, poses.data(),
+                                               map_without_matching, out_kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

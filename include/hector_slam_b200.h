@@ -209,6 +209,41 @@ int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints_worl
                                  const int* d_offsets, int max_points_per_scan, const double* d_transforms,
                                  float* d_out_poses_world, float* d_out_cov, float* d_out_origo, void* stream);
 
+/* ---- the node's default path from the LaserScan itself ------------------------------------------*/
+/* A default node (use_tf_scan_transformation = true, HectorMappingRos.cpp:258-297) projects every scan into a
+ * sensor_msgs/PointCloud with laser_geometry, projector_.projectLaser(scan, cloud, 30.0) (:273), and converts that cloud
+ * with rosPointCloudToDataContainer (:283).  These calls take the scan's ranges and run both on the device.  The
+ * projection restates laser_geometry's LaserProjection::projectLaser_ / getUnitVectors_ (ROS1 Melodic / Noetic) for the
+ * PointCloud output:
+ *   unit vectors  c_i = cos((double)angle_min + (double)i * (double)angle_increment), s_i likewise with sin — libm's
+ *                 double functions, evaluated on the host once per hsb_set_laser_projection;
+ *   beam i kept   iff (double)range < cutoff && range >= range_min (float compare: NaN and +-inf are dropped);
+ *   Point32       ((float)((double)range * c_i), (float)((double)range * s_i), 0.0f), beam order kept.
+ * The cloud then takes the hsb_cloud_format rule of the handle as it is at the call (thresholds and, unless a call
+ * passes its own, the laser transform).  The two filters compose into one over the beams in beam order. */
+typedef struct hsb_laser_projection {
+  int    n_beams;          /* ranges.size()                                                                   */
+  float  angle_min;        /* scan.angle_min                                                                  */
+  float  angle_increment;  /* scan.angle_increment                                                            */
+  float  range_min;        /* scan.range_min   (kept: range >= range_min)                                     */
+  float  range_max;        /* scan.range_max   (the cutoff when range_cutoff < 0)                             */
+  double range_cutoff;     /* projectLaser's third argument (the node passes 30.0, :273); < 0 means range_max.
+                            * Releases differ on whether range_max also caps it: pass the value the robot's
+                            * release uses.                                                                   */
+} hsb_laser_projection;
+/* Builds the unit-vector table on the host and keeps it on the device (16 bytes per beam).  HSB_ERR_INVALID_ARG, and
+ * the handle keeps its previous projection, for n_beams outside [1, 2^20], a non-finite angle_min, angle_increment or
+ * range_min, a NaN cutoff, or a negative cutoff with a NaN range_max. */
+int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj);
+/* Projection + cloud conversion alone for one scan: ranges[n] (host, n = the projection's n_beams) -> kept endpoints
+ * in level-0 cell units, beam order (capacity n x 2), *out_n = number kept, out_origo (may be NULL) = laser position *
+ * scaleToMap.  transform: 12 doubles, rows of [R | t], NULL = the cloud format's.  Equal bit for bit to
+ * hsb_cloud_to_points on the projected cloud.  Needs hsb_set_laser_projection and hsb_set_cloud_format
+ * (HSB_ERR_INVALID_ARG, the message names what is missing); a scan longer than the fused SLAM step can stage fails with
+ * HSB_ERR_UNSUPPORTED. */
+int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, const double* transform,
+                                 float* out_points_xy, int* out_n, float out_origo[2]);
+
 /* ---- streams of batches: submit / wait ---------------------------------------------------------*/
 /* The three host-buffer batch calls above are `submit` followed by `wait`.  Used separately they let a caller keep
  * the PCIe link busy across calls: the handle owns TWO sets of device staging buffers that alternate between calls,
@@ -304,6 +339,21 @@ int hsb_slam_update_cloud(hsb_handle* h, const float pose_hint_world[3], const f
 int hsb_slam_update_ranges(hsb_handle* h, const float pose_hint_world[3], const float* ranges, int n,
                            int map_without_matching, int nowait, float out_pose_world[3], float cov_inout[9],
                            int* map_updated, int* out_kept);
+/* The DEFAULT branch of scanCallback from the LaserScan it receives (HectorMappingRos.cpp:258-297): laser_geometry's
+ * projection (:273, see hsb_laser_projection), rosPointCloudToDataContainer (:283) and HectorSlamProcessor::update (:297)
+ * in one call.  ranges = the scan's n ranges, n = the projection's n_beams (HSB_ERR_INVALID_ARG otherwise); transform
+ * as in hsb_slam_update_cloud (NULL = the cloud format's).  Both conversions run in the match kernel's staging step:
+ * 4 bytes per beam cross PCIe instead of 12 per projected point, one host-to-device copy and three launches.
+ * map_without_matching, nowait and *out_kept as in hsb_slam_update_cloud.  Needs hsb_set_laser_projection and
+ * hsb_set_cloud_format (HSB_ERR_INVALID_ARG, the message names what is missing); a scan longer than the fused
+ * conversion can stage fails with HSB_ERR_UNSUPPORTED, and so does a handle whose tuning selects a match shape other
+ * than the single step's default (8 warps, 4 gathers in flight, unpacked), the only one compiled with the projection.
+ * Pose, covariance, gate decision, kept count, every plane and the handle's end state are bit-identical to
+ * hsb_slam_update_cloud(h, hint, project(ranges), m, transform, ...), project being the restatement above and m the
+ * number of projected points. */
+int hsb_slam_update_projected(hsb_handle* h, const float pose_hint_world[3], const float* ranges, int n,
+                              const double* transform, int map_without_matching, int nowait, float out_pose_world[3],
+                              float cov_inout[9], int* map_updated, int* out_kept);
 /* ---- many SLAM sessions in one device pass ------------------------------------------------------*/
 /* N robots that each build their own map are N independent HectorSlamProcessors, i.e. N handles.  A group steps
  * them together: one host-to-device copy and three kernel launches per step whatever the number of members, instead
@@ -360,6 +410,19 @@ int hsb_group_slam_update_cloud(hsb_group* g, const float* hints_world, const fl
 int hsb_group_slam_update_ranges(hsb_group* g, const float* hints_world, const float* ranges, const int* offsets,
                                  const int* map_without_matching, int nowait, float* out_poses_world, float* cov_inout,
                                  int* map_updated, int* out_kept);
+/* The same group step from the LaserScans of default-configured nodes: hsb_slam_update_projected for every member at
+ * once.  Session s takes ranges[offsets[s] .. offsets[s+1]), whose length must equal its member's projection n_beams,
+ * and the laser transform transforms[12s..] (NULL: every member's cloud format transform).  Each session projects and
+ * converts with its own member's projection and cloud format as they are at the call.  out_kept, hints,
+ * map_without_matching, nowait, cov_inout and map_updated as in hsb_group_slam_update_cloud; one host-to-device copy
+ * and three launches per step.  Every session's results and every member's end state are bit-identical to
+ * hsb_slam_update_projected on its handle with the same inputs.  Rejected before any member changes: a member without
+ * a projection or a cloud format (HSB_ERR_INVALID_ARG, the message names the session and what is missing), offsets that
+ * disagree with the members' n_beams (HSB_ERR_INVALID_ARG), a scan longer than the fused conversion can stage
+ * (HSB_ERR_UNSUPPORTED, the limit and message of hsb_slam_update_projected). */
+int hsb_group_slam_update_projected(hsb_group* g, const float* hints_world, const float* ranges, const int* offsets,
+                                    const double* transforms, const int* map_without_matching, int nowait,
+                                    float* out_poses_world, float* cov_inout, int* map_updated, int* out_kept);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
