@@ -99,7 +99,7 @@ struct hsb_handle {
   DevBuf d_gate;           // fused SLAM step: lastMapUpdatePose[3], write-the-map flag
   float min_dist = 0.4f, min_angle = 0.13f;   // HectorSlamProcessor.h:62-63 defaults
   // tuning
-  int tune_warps_per_scan = 0, tune_scans_per_block = 0, tune_stage_smem = 1, tune_chunk = 0, tune_unroll = 0, tune_packed = 0, tune_seq = 0, tune_partial = 1, tune_prefetch = 0, tune_trace = 0, tune_pace = 0, tune_pdl = 1, tune_auto_group = 1, tune_stagger = 0;
+  int tune_warps_per_scan = 0, tune_scans_per_block = 0, tune_stage_smem = 1, tune_chunk = 0, tune_unroll = 0, tune_packed = 0, tune_seq = 0, tune_partial = 1, tune_prefetch = 0, tune_trace = 0, tune_pace = 0, tune_pdl = 1, tune_auto_group = 1, tune_stagger = 0, tune_fixpoint = 1;
   DevBuf d_trace;
   DevBuf d_best;   // arg-max accumulator of hsb_best_hypothesis_device
   DevBuf d_record; // per-evaluation record of hsb_match_data_record
@@ -333,6 +333,7 @@ int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st,
   P.sm_count = h->sm_count;
   P.prefetch = h->tune_prefetch;
   P.pace_slack = h->tune_pace;
+  P.fixpoint = h->tune_fixpoint;
   P.pts_cap = cap;
   size_t smem = header + (size_t)Gr * cap * 8;
   if (smem > 48 * 1024) {
@@ -831,6 +832,7 @@ int hsb_set_tuning(hsb_handle* h, const char* key, int value) {
   else if (!strcmp(key, "pdl")) h->tune_pdl = value;
   else if (!strcmp(key, "auto_group")) h->tune_auto_group = value;
   else if (!strcmp(key, "stagger")) h->tune_stagger = value;
+  else if (!strcmp(key, "fixpoint")) h->tune_fixpoint = value;
   else return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_tuning: unknown key '%s'", key);
   return HSB_OK;
 }

@@ -88,7 +88,11 @@ struct HsbMatchParams {
   int sm_count;             // SMs of the device (the one-scan-per-CTA shapes derive a warp's rank on its SM from blockIdx)
   int pace_slack;           // > 0: groups of a CTA keep within this many evaluations of the slowest one (see match_kernel)
   int prefetch;             // != 0: L2 bulk prefetch of the part of a scan that is read from global memory
-  // diagnostics (hsb_set_tuning "trace"): per scan 8 x u64 = {start, after coarsest level, ..., end (slot 1+levels), -, smid (slot 7)}
+  int fixpoint;             // != 0: a level's Gauss-Newton loop ends at the first evaluation that leaves the pose
+                            // bitwise unchanged (the later ones would repeat it exactly; see match_kernel)
+  // diagnostics (hsb_set_tuning "trace"): per scan 8 x u64 =
+  //   [0] start, [1 .. levels] after each level (coarsest first), [1 + levels] end,
+  //   [5] evaluations the scan actually ran (written with <= 3 levels, where slot 5 is free), [6] %warpid, [7] %smid
   unsigned long long* trace;
   // per-evaluation record (hsb_match_data_record / hsb_match_batch_record_device), nullptr = none.  Scan b owns
   // record[b * record_floats ..], record_floats = R = sum over levels of (3 + 15 * evals).  Per level, coarsest first:

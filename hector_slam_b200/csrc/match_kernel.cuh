@@ -794,6 +794,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
   // the slowest one sleeps: its issue slots and texture bandwidth go to the stragglers and all scans of the CTA end
   // within ~pace_slack evaluations of each other.  No arithmetic is involved: results are unchanged.
   const bool pace = HSB_DIAG && (G > 1) && P.pace_slack > 0;
+  const bool fixpoint = P.fixpoint != 0;   // end a level once an evaluation leaves the pose unchanged (see the loop)
   int evals_done = 0;
   if (G > 1) {
     if (threadIdx.x < 32) prog[threadIdx.x] = 0x7fffffff;   // slots of absent / finished groups never hold anyone back
@@ -970,6 +971,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     // address is formed from the kernel parameters at each store (level offsets precomputed on the host), so that the
     // evaluation loop carries no extra live register for it
     const bool recording = P.record && t == 0;
+    int evals_ran = 0;   // evaluations this scan actually ran (trace slot 5)
     if (n > 0) {
       for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
         const HsbLevelDev& L = level_desc<GRP>(P, scan, lvl);
@@ -980,6 +982,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
           rec[0] = wx; rec[1] = wy; rec[2] = wpsi;
         }
         affine_apply_exact(L.mtw, wx, wy, ex, ey);  // ScanMatcher.h:70 getMapCoordsPose
+        int ran = L.evals;                           // evaluations run at this level (fewer at a fixed point, below)
         for (int e = 0; e < L.evals; ++e) {          // ScanMatcher.h:74 + :94-97
           // OccGridMapUtil.h:70-71 and Rotation2Df (:351): sinf/cosf exactly as glibc evaluates them
           float cs, ss;
@@ -1043,14 +1046,20 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
             }
           }
           last = a;
+          bool moved = false;
           if (a.h00 != 0.0f && a.h11 != 0.0f) {  // ScanMatcher.h:201
             float d0, d1, d2;
             solve3(a, d0, d1, d2);               // :205
             if (d2 > 0.2f) d2 = 0.2f;            // :209-215
             else if (d2 < -0.2f) d2 = -0.2f;
-            ex = __fadd_rn(ex, d0);              // :217
-            ey = __fadd_rn(ey, d1);
-            epsi = __fadd_rn(epsi, d2);
+            const float nx = __fadd_rn(ex, d0);  // :217
+            const float ny = __fadd_rn(ey, d1);
+            const float npsi = __fadd_rn(epsi, d2);
+            moved = (__float_as_uint(nx) != __float_as_uint(ex)) | (__float_as_uint(ny) != __float_as_uint(ey)) |
+                    (__float_as_uint(npsi) != __float_as_uint(epsi));
+            ex = nx;
+            ey = ny;
+            epsi = npsi;
           }
           if (recording) {
             float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off + 3 + 15 * e;
@@ -1060,7 +1069,34 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
             rec[9] = a.d0;  rec[10] = a.d1; rec[11] = a.d2;
             rec[12] = ex;   rec[13] = ey;   rec[14] = epsi;
           }
+          // Fixed point: the step left the pose bit-for-bit where this evaluation ran it (or the gate made no step).
+          // Every later evaluation of the level would run at the same pose on the same map with the same endpoints in
+          // the same summation order, i.e. reproduce this one exactly — same sums, same step, same pose — so the level
+          // ends here.  The bitwise test counts -0 / +0 as moved (sinf(-0) = -0): conservative.  The pose is the same
+          // in every thread of the group, so the exit is uniform.
+          if (fixpoint && !moved) {
+            ran = e + 1;
+            break;
+          }
         }
+        if (ran < L.evals) {
+          // the skipped evaluations: `last` and the pose already are what each of them would leave
+          if (recording) {
+            for (int e = ran; e < L.evals; ++e) {
+              float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off + 3 + 15 * e;
+              rec[0] = last.h00; rec[1] = last.h01; rec[2] = last.h02;
+              rec[3] = last.h01; rec[4] = last.h11; rec[5] = last.h12;
+              rec[6] = last.h02; rec[7] = last.h12; rec[8] = last.h22;
+              rec[9] = last.d0;  rec[10] = last.d1; rec[11] = last.d2;
+              rec[12] = ex;      rec[13] = ey;      rec[14] = epsi;
+            }
+          }
+          if (pace) {   // they count as done: nobody waits for them
+            evals_done += L.evals - ran;
+            if (t == 0) prog[g] = evals_done;
+          }
+        }
+        evals_ran += ran;
         epsi = normalize_angle(epsi);                 // ScanMatcher.h:170
         affine_apply_exact(L.wtm, ex, ey, wx, wy);    // :186 getWorldCoordsPose
         wpsi = epsi;
@@ -1079,6 +1115,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     }
     if (HSB_DIAG && P.trace && t == 0) {
       P.trace[8 * (size_t)scan + 1 + P.levels] = global_timer_ns();
+      if (P.levels <= 3) P.trace[8 * (size_t)scan + 5] = (unsigned long long)evals_ran;
       P.trace[8 * (size_t)scan + 6] = warp_id();
       P.trace[8 * (size_t)scan + 7] = sm_id();
     }

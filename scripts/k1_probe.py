@@ -105,6 +105,11 @@ def timeline(label, kw):
     print(f"per-scan duration: min {dur.min():.1f} p10 {np.percentile(dur, 10):.1f} p50 {np.median(dur):.1f} "
           f"p90 {np.percentile(dur, 90):.1f} max {dur.max():.1f}")
     print("per-level duration p50 (coarse -> fine, + tail):", " ".join(f"{np.median(lv[:, k]):.1f}" for k in range(4)))
+    full = sum(rep.level_evals())
+    ran = tr[:, 5]   # evaluations each scan ran (a level ends at its first evaluation that leaves the pose unchanged)
+    hist = np.bincount(ran, minlength=full + 1)
+    print(f"evaluations run per scan (of {full}), count: " + " ".join(f"{k}:{c}" for k, c in enumerate(hist) if c) +
+          f"; {1 - ran.sum() / (full * ran.size):.1%} of all evaluations skipped")
     cnt = np.bincount(sm, minlength=torch.cuda.get_device_properties(0).multi_processor_count)
     per_sm_end = np.array([end[sm == s].max() if (sm == s).any() else 0 for s in range(cnt.size)])
     print(f"scans per SM: min {cnt[cnt > 0].min()} max {cnt.max()} (SMs used {(cnt > 0).sum()}); "
