@@ -70,12 +70,12 @@ struct hsb_handle {
   float* h_stage = nullptr;       // pinned staging for the single-scan calls (header + points, one H2D per call)
   size_t h_stage_bytes = 0;
   // raw-range input (N2)
-  DevBuf d_beam_cs, d_ranges, d_occ;
+  DevBuf d_beam_cs, d_occ;
   hsb_scan_format fmt = hsb_scan_format();
   bool fmt_set = false;
   hsb_cloud_format cfmt = hsb_cloud_format();
   bool cfmt_set = false;
-  DevBuf d_cloud, d_cloud_off, d_cloud_tf, d_origo;
+  DevBuf d_conv_in, d_cloud_tf;   // the stand-alone conversions' input (ranges or cloud) and laser transform
   DevBuf d_proj_unit;   // laser_geometry's unit vectors, n_beams x double (cos, sin)
   hsb_laser_projection proj = hsb_laser_projection();
   bool proj_set = false;
@@ -176,6 +176,34 @@ int ensure(hsb_handle* h, DevBuf& b, size_t bytes) {
   size_t want = bytes + bytes / 4 + 256;
   HSB_CUDA(h, cudaMalloc(&b.p, want));
   b.cap = want;
+  return HSB_OK;
+}
+
+// Pinned host staging `p` of `cap` bytes grown to hold `bytes` (the contents are not kept).
+template <typename T>
+int ensure_pinned(hsb_handle* h, T*& p, size_t& cap, size_t bytes) {
+  if (bytes <= cap) return HSB_OK;
+  if (p) cudaFreeHost(p);
+  p = nullptr;
+  cap = 0;
+  const size_t want = bytes < (64u << 10) ? (64u << 10) : bytes * 2;
+  HSB_CUDA(h, cudaMallocHost(reinterpret_cast<void**>(&p), want));
+  cap = want;
+  return HSB_OK;
+}
+
+// A nowait step's return: spin until the device has published `value` in the mapped word `seq` (the step's results are
+// in host memory then), checking every 4096 polls that `st` has neither failed nor finished without publishing.
+int wait_published(hsb_handle* h, volatile unsigned* seq, unsigned value, cudaStream_t st, const char* unpublished) {
+  unsigned spins = 0;
+  while (*seq != value) {
+    if ((++spins & 0xfffu) == 0) {
+      cudaError_t e = cudaStreamQuery(st);
+      if (e != cudaSuccess && e != cudaErrorNotReady) return fail(h, HSB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
+      if (e == cudaSuccess && *seq != value) return fail(h, HSB_ERR_CUDA, "%s", unpublished);
+    }
+  }
+  __sync_synchronize();
   return HSB_OK;
 }
 
@@ -288,7 +316,7 @@ int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st,
   constexpr size_t kMaxDyn = kMaxDynSmem;
   constexpr int gt = W * 32;           // threads per scan
   int cap = 0;
-  const bool fused = P.ranges || P.cloud || INL;   // conversion / inline scan: the whole scan must be staged
+  const bool fused = P.kind != HSB_IN_ENDPOINTS || INL;   // conversion / inline scan: the whole scan must be staged
   if (h->tune_stage_smem || fused) cap = whole_scan_slots(max_n);
   // resident CTAs per SM for a given dynamic shared-memory size: block, thread, register and
   // shared-memory limits (1 KB per CTA is reserved by the driver)
@@ -427,7 +455,7 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
     // Larger batches keep one scan per CTA: finished warps are replaced at once there, which a CTA-wide drain would
     // prevent.  With one warp per scan the reduction order does not depend on the CTA shape: results are the same bits.
     const long Bs = h->shape_batch > 0 ? h->shape_batch : P.B;
-    if (h->tune_auto_group && W == 1 && !P.ranges && !P.cloud && std::max<long>(Bs, P.B) <= (long)h->sm_count * 32 &&
+    if (h->tune_auto_group && W == 1 && P.kind == HSB_IN_ENDPOINTS && std::max<long>(Bs, P.B) <= (long)h->sm_count * 32 &&
         (h->tune_unroll == 0 || h->tune_unroll == 4)) {
       Gr = (int)((Bs + h->sm_count - 1) / h->sm_count);
       G = Gr <= 28 ? 28 : 32;
@@ -455,7 +483,7 @@ int launch_match_inline(hsb_handle* h, HsbMatchParams& P, const float* header, i
   P.pts = nullptr;
   P.offsets = nullptr;
   P.n_shared = n;
-  P.out_pts = reinterpret_cast<float2*>(d_pts_out);
+  P.conv.out_pts = reinterpret_cast<float2*>(d_pts_out);
   if (h->map_write_pending && st != h->stream) {
     HSB_CUDA(h, cudaEventRecord(h->ev_sync[0], h->stream));
     HSB_CUDA(h, cudaStreamWaitEvent(st, h->ev_sync[0], 0));
@@ -716,8 +744,8 @@ int hsb_destroy(hsb_handle* h) {
   cudaDeviceSynchronize();
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
-                    &h->d_beam_cs, &h->d_ranges, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
-                    &h->d_cloud, &h->d_cloud_off, &h->d_cloud_tf, &h->d_origo, &h->d_fused_in, &h->d_proj_unit};
+                    &h->d_beam_cs, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
+                    &h->d_conv_in, &h->d_cloud_tf, &h->d_fused_in, &h->d_proj_unit};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int k = 0; k < 2; ++k) {
@@ -758,14 +786,7 @@ static int upload_scan(hsb_handle* h, DevBuf& b, const float* header, int nh, co
   int s = ensure_scan_buf(h, b, n);
   if (s != HSB_OK) return s;
   const size_t bytes = kScanHeaderFloats * sizeof(float) + (size_t)n * 8;
-  if (bytes > h->h_stage_bytes) {
-    if (h->h_stage) cudaFreeHost(h->h_stage);
-    h->h_stage = nullptr;
-    h->h_stage_bytes = 0;
-    size_t cap = bytes < (64u << 10) ? (64u << 10) : bytes * 2;
-    HSB_CUDA(h, cudaMallocHost(&h->h_stage, cap));
-    h->h_stage_bytes = cap;
-  }
+  if ((s = ensure_pinned(h, h->h_stage, h->h_stage_bytes, bytes)) != HSB_OK) return s;
   memset(h->h_stage, 0, kScanHeaderFloats * sizeof(float));
   if (nh > 0) memcpy(h->h_stage, header, (size_t)nh * sizeof(float));
   if (n > 0) memcpy(h->h_stage + kScanHeaderFloats, pts, (size_t)n * 8);
@@ -1004,7 +1025,7 @@ int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const 
   return HSB_OK;
 }
 
-// ---- raw ranges (N2) ---------------------------------------------------------------------------
+// ---- converted input (N2): the node's conversions of a LaserScan or point cloud to endpoints -------
 
 int hsb_set_scan_format(hsb_handle* h, const hsb_scan_format* fmt) {
   if (!h || !fmt || fmt->n_beams < 1 || fmt->n_beams > (1 << 20)) return HSB_ERR_INVALID_ARG;
@@ -1025,66 +1046,6 @@ int hsb_set_scan_format(hsb_handle* h, const hsb_scan_format* fmt) {
   return HSB_OK;
 }
 
-// :493 maxRangeForContainer = range_max - 0.1, host fp32
-static float range_max_c(const hsb_scan_format& f) {
-  volatile float mx = f.range_max - 0.1f;
-  return mx;
-}
-
-static void fill_range_params(const hsb_handle* h, HsbMatchParams& P, const float* d_ranges) {
-  P.ranges = d_ranges;
-  P.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
-  P.n_beams = h->fmt.n_beams;
-  P.range_min = h->fmt.range_min;
-  P.range_max_c = range_max_c(h->fmt);
-  P.scale_to_map = h->lv[0].scale;
-}
-
-int hsb_scan_to_points(hsb_handle* h, const float* ranges, float* out_xy, int* out_n) {
-  if (!h || !ranges || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
-  if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
-  HandleScope guard(h);
-  const int nb = h->fmt.n_beams;
-  int s;
-  if ((s = ensure(h, h->d_ranges, (size_t)nb * 4)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_pts, (size_t)nb * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
-  cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_ranges.p, ranges, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-  HsbMatchParams P;
-  memset(&P, 0, sizeof(P));
-  fill_range_params(h, P, static_cast<const float*>(h->d_ranges.p));
-  int* d_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
-  hsb::scan_to_points_kernel<<<1, 256, 0, st>>>(P.ranges, P.beam_cs, nb, P.range_min, P.range_max_c, P.scale_to_map,
-                                                static_cast<float2*>(h->d_pts.p), d_n);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  int n = *reinterpret_cast<int*>(h->h_pin + 48);
-  if (n > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
-  *out_n = n;
-  return HSB_OK;
-}
-
-int hsb_match_batch_ranges_device(hsb_handle* h, int B, const float* d_hints, const float* d_ranges, float* d_out_poses,
-                                  float* d_out_cov, void* stream) {
-  if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
-  if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
-  if (B == 0) return HSB_OK;
-  HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  fill_range_params(h, P, d_ranges);
-  return launch_match(h, P, h->fmt.n_beams, (cudaStream_t)stream);
-}
-
-// ---- point clouds (N2, the node's default input) ------------------------------------------------
-
 int hsb_set_cloud_format(hsb_handle* h, const hsb_cloud_format* fmt) {
   if (!h || !fmt) return HSB_ERR_INVALID_ARG;
   for (int i = 0; i < 12; ++i)
@@ -1093,76 +1054,6 @@ int hsb_set_cloud_format(hsb_handle* h, const hsb_cloud_format* fmt) {
   h->cfmt_set = true;
   return HSB_OK;
 }
-
-static void fill_cloud_params(const hsb_handle* h, HsbMatchParams& P, const float* d_cloud, const int* d_offsets,
-                              const double* d_transforms, float* d_origo) {
-  P.cloud = d_cloud;
-  P.cloud_offsets = d_offsets;
-  P.cloud_tf = d_transforms;
-  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
-  P.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
-  P.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
-  P.z_min = h->cfmt.laser_z_min_value;
-  P.z_max = h->cfmt.laser_z_max_value;
-  P.scale_to_map = h->lv[0].scale;
-  P.out_origo = d_origo;
-}
-
-// The container's origo of a cloud with laser transform T (HectorMappingRos.cpp:516-517):
-// Vector2f(laserPos.x(), laserPos.y()) * scaleToMap, host fp32 without contraction
-static void cloud_origo(const hsb_handle* h, const double* T, float out[2]) {
-  volatile float ox = (float)T[3], oy = (float)T[7];
-  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
-  out[0] = sx;
-  out[1] = sy;
-}
-
-int hsb_cloud_to_points(hsb_handle* h, const float* points_xyz, int n, float* out_xy, int* out_n, float out_origo[2]) {
-  if (!h || n < 0 || (n > 0 && !points_xyz) || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  HandleScope guard(h);
-  int s;
-  if ((s = ensure(h, h->d_cloud, (size_t)(n > 0 ? n : 1) * 12)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
-  cudaStream_t st = h->stream;
-  if (n > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud.p, points_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, st));
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, h->cfmt.laser_transform, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-  int* d_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
-  hsb::cloud_to_points_kernel<<<1, 256, 0, st>>>(static_cast<const float*>(h->d_cloud.p), n, static_cast<const double*>(h->d_cloud_tf.p),
-                                                 h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist, h->cfmt.laser_z_min_value,
-                                                 h->cfmt.laser_z_max_value, h->lv[0].scale, static_cast<float2*>(h->d_pts.p), d_n);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
-  if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
-  *out_n = kept;
-  if (out_origo) cloud_origo(h, h->cfmt.laser_transform, out_origo);
-  return HSB_OK;
-}
-
-int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, const float* d_points_xyz, const int* d_offsets,
-                                 int max_points_per_scan, const double* d_transforms, float* d_out_poses, float* d_out_cov,
-                                 float* d_out_origo, void* stream) {
-  if (!h || B < 0 || !d_hints || !d_offsets || !d_out_poses || max_points_per_scan < 0) return HSB_ERR_INVALID_ARG;
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  if (B == 0) return HSB_OK;
-  if (!d_points_xyz && max_points_per_scan > 0) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  fill_cloud_params(h, P, d_points_xyz, d_offsets, d_transforms, d_out_origo);
-  return launch_match(h, P, max_points_per_scan, (cudaStream_t)stream);
-}
-
-// ---- the default path from the LaserScan: laser_geometry's projection + the cloud rule -----------
 
 int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj) {
   if (!h || !proj) return HSB_ERR_INVALID_ARG;
@@ -1195,36 +1086,107 @@ int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj) {
 
 namespace {
 
+// :493 maxRangeForContainer = range_max - 0.1, host fp32
+float range_max_c(const hsb_scan_format& f) {
+  volatile float mx = f.range_max - 0.1f;
+  return mx;
+}
+
 // projectLaser: a negative cutoff means the scan's range_max
 double projection_cutoff(const hsb_laser_projection& p) { return p.range_cutoff < 0.0 ? (double)p.range_max : p.range_cutoff; }
 
-// the projection and cloud format a projected step needs, and its beam count; `fn` names the entry point
-int check_projected(hsb_handle* h, const char* fn, int n) {
-  if (!h->proj_set) return fail(h, HSB_ERR_INVALID_ARG, "%s: hsb_set_laser_projection has not been called", fn);
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "%s: hsb_set_cloud_format has not been called", fn);
-  if (n != h->proj.n_beams)
-    return fail(h, HSB_ERR_INVALID_ARG, "%s: n is %d, the laser projection has %d beams", fn, n, h->proj.n_beams);
-  // every projected step converts the whole scan into the shared memory of the single step's match shape
-  if (!staging_fits<8, 1>(whole_scan_slots(n), 1)) return fail_fused_too_long(h, n);
+// The container's origo of a cloud with laser transform T (HectorMappingRos.cpp:516-517):
+// Vector2f(laserPos.x(), laserPos.y()) * scaleToMap, host fp32 without contraction
+void cloud_origo(const hsb_handle* h, const double* T, float out[2]) {
+  volatile float ox = (float)T[3], oy = (float)T[7];
+  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
+  out[0] = sx;
+  out[1] = sy;
+}
+
+// How h converts a scan of `kind` (not endpoints) at call time; the sink is left null.
+void fill_conv(const hsb_handle* h, HsbInputKind kind, HsbConvDev& c) {
+  memset(&c, 0, sizeof(c));
+  c.scale_to_map = h->lv[0].scale;
+  if (kind == HSB_IN_RANGES) {
+    c.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
+    c.range_min = h->fmt.range_min;
+    c.range_max_c = range_max_c(h->fmt);
+    return;
+  }
+  c.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
+  c.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
+  c.z_min = h->cfmt.laser_z_min_value;
+  c.z_max = h->cfmt.laser_z_max_value;
+  if (kind == HSB_IN_PROJECTED) {
+    c.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
+    c.range_min = h->proj.range_min;
+    c.range_cutoff = projection_cutoff(h->proj);
+  }
+}
+
+// Whether h can convert a scan of `kind` with n inputs: the formats the kind needs are set, a scan of ranges has the
+// format's beam count (n < 0: not checked) and, if `whole`, the scan fits the shared memory of the single step's match
+// shape.  The error goes to `err` and names the entry point `fn` and, if session >= 0, the group session.
+int check_input(const hsb_handle* h, hsb_handle* err, HsbInputKind kind, const char* fn, int session, int n, bool whole) {
+  char who[160];
+  if (session < 0) snprintf(who, sizeof(who), "%s", fn);
+  else snprintf(who, sizeof(who), "%s: session %d", fn, session);
+  const char* on = session < 0 ? "" : " on its handle";
+  if (kind == HSB_IN_PROJECTED && !h->proj_set)
+    return fail(err, HSB_ERR_INVALID_ARG, "%s: hsb_set_laser_projection has not been called%s", who, on);
+  if ((kind == HSB_IN_CLOUD || kind == HSB_IN_PROJECTED) && !h->cfmt_set)
+    return fail(err, HSB_ERR_INVALID_ARG, "%s: hsb_set_cloud_format has not been called%s", who, on);
+  if (kind == HSB_IN_RANGES && !h->fmt_set)
+    return fail(err, HSB_ERR_INVALID_ARG, "%s: hsb_set_scan_format has not been called%s", who, on);
+  if (n >= 0 && (kind == HSB_IN_RANGES || kind == HSB_IN_PROJECTED)) {
+    const int nb = kind == HSB_IN_RANGES ? h->fmt.n_beams : h->proj.n_beams;
+    const char* format = kind == HSB_IN_RANGES ? "scan format" : "laser projection";
+    if (n != nb && session < 0) return fail(err, HSB_ERR_INVALID_ARG, "%s: n is %d, the %s has %d beams", who, n, format, nb);
+    if (n != nb) return fail(err, HSB_ERR_INVALID_ARG, "%s has %d ranges, its %s has %d beams", who, n, format, nb);
+  }
+  if (whole && !staging_fits<8, 1>(whole_scan_slots(n), 1)) return fail_fused_too_long(err, n);
   return HSB_OK;
 }
 
-void fill_projected_params(const hsb_handle* h, HsbMatchParams& P, const float* d_ranges, const double* d_transforms) {
-  fill_cloud_params(h, P, nullptr, nullptr, d_transforms, nullptr);   // thresholds, default transform, scaleToMap
-  P.ranges = d_ranges;
-  P.n_beams = h->proj.n_beams;
-  P.range_min = h->proj.range_min;
-  P.range_cutoff = projection_cutoff(h->proj);
-  P.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
+// The stand-alone conversion of n_in inputs of `kind` at d_in (laser transform d_T) into c's sink.
+int launch_conversion(hsb_handle* h, HsbInputKind kind, const float* d_in, int n_in, const double* d_T, const HsbConvDev& c,
+                      cudaStream_t st) {
+  if (kind == HSB_IN_RANGES) hsb::conv_to_points_kernel<HSB_IN_RANGES><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
+  else if (kind == HSB_IN_CLOUD) hsb::conv_to_points_kernel<HSB_IN_CLOUD><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
+  else hsb::conv_to_points_kernel<HSB_IN_PROJECTED><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
+  h->launches++;
+  HSB_CUDA(h, cudaGetLastError());
+  return HSB_OK;
 }
 
-int launch_projected_conversion(hsb_handle* h, const float* d_ranges, const double* d_T, float2* d_out, int* d_n,
-                                cudaStream_t st) {
-  hsb::projected_to_points_kernel<<<1, 256, 0, st>>>(
-      d_ranges, static_cast<const double2*>(h->d_proj_unit.p), h->proj.n_beams, h->proj.range_min,
-      projection_cutoff(h->proj), d_T, h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist, h->cfmt.laser_z_min_value,
-      h->cfmt.laser_z_max_value, h->lv[0].scale, d_out, d_n);
-  HSB_CUDA(h, cudaGetLastError());
+// hsb_scan_to_points / hsb_cloud_to_points / hsb_projected_scan_to_points: n inputs of `kind` (host) with laser
+// transform T (host, null for ranges) -> the kept endpoints and, for a cloud, the container's origo (host)
+int to_points(hsb_handle* h, HsbInputKind kind, const float* in, int n, const double* T, float* out_xy, int* out_n,
+              float out_origo[2]) {
+  HandleScope guard(h);
+  const size_t in_bytes = (size_t)n * (kind == HSB_IN_CLOUD ? 12 : 4);
+  int s;
+  if ((s = ensure(h, h->d_conv_in, in_bytes > 0 ? in_bytes : 12)) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
+  if (T && (s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
+  cudaStream_t st = h->stream;
+  if (n > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_conv_in.p, in, in_bytes, cudaMemcpyHostToDevice, st));
+  if (T) HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
+  HsbConvDev c;
+  fill_conv(h, kind, c);
+  c.out_pts = static_cast<float2*>(h->d_pts.p);
+  c.out_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
+  if ((s = launch_conversion(h, kind, static_cast<const float*>(h->d_conv_in.p), n,
+                             T ? static_cast<const double*>(h->d_cloud_tf.p) : nullptr, c, st)) != HSB_OK)
+    return s;
+  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, c.out_n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaStreamSynchronize(st));
+  const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
+  if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
+  *out_n = kept;
+  if (T && out_origo) cloud_origo(h, T, out_origo);
   return HSB_OK;
 }
 
@@ -1232,32 +1194,72 @@ int launch_projected_conversion(hsb_handle* h, const float* d_ranges, const doub
 
 extern "C" {
 
+int hsb_scan_to_points(hsb_handle* h, const float* ranges, float* out_xy, int* out_n) {
+  if (!h || !ranges || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
+  int s = check_input(h, h, HSB_IN_RANGES, "hsb_scan_to_points", -1, -1, false);
+  if (s != HSB_OK) return s;
+  return to_points(h, HSB_IN_RANGES, ranges, h->fmt.n_beams, nullptr, out_xy, out_n, nullptr);
+}
+
+int hsb_cloud_to_points(hsb_handle* h, const float* points_xyz, int n, float* out_xy, int* out_n, float out_origo[2]) {
+  if (!h || n < 0 || (n > 0 && !points_xyz) || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
+  int s = check_input(h, h, HSB_IN_CLOUD, "hsb_cloud_to_points", -1, -1, false);
+  if (s != HSB_OK) return s;
+  return to_points(h, HSB_IN_CLOUD, points_xyz, n, h->cfmt.laser_transform, out_xy, out_n, out_origo);
+}
+
 int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, const double* transform, float* out_xy,
                                  int* out_n, float out_origo[2]) {
   if (!h || !ranges || !out_xy || !out_n) return HSB_ERR_INVALID_ARG;
-  int s = check_projected(h, "hsb_projected_scan_to_points", n);
+  int s = check_input(h, h, HSB_IN_PROJECTED, "hsb_projected_scan_to_points", -1, n, true);
   if (s != HSB_OK) return s;
+  return to_points(h, HSB_IN_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform, out_xy, out_n,
+                   out_origo);
+}
+
+int hsb_match_batch_ranges_device(hsb_handle* h, int B, const float* d_hints, const float* d_ranges, float* d_out_poses,
+                                  float* d_out_cov, void* stream) {
+  if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
+  int s = check_input(h, h, HSB_IN_RANGES, "hsb_match_batch_ranges_device", -1, -1, false);
+  if (s != HSB_OK) return s;
+  if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  const double* T = transform ? transform : h->cfmt.laser_transform;
-  if ((s = ensure(h, h->d_ranges, (size_t)n * 4)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_pts, (size_t)n * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
-  cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_ranges.p, ranges, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-  int* d_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
-  if ((s = launch_projected_conversion(h, static_cast<const float*>(h->d_ranges.p), static_cast<const double*>(h->d_cloud_tf.p),
-                                       static_cast<float2*>(h->d_pts.p), d_n, st)) != HSB_OK)
-    return s;
-  h->launches++;
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
-  if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
-  *out_n = kept;
-  if (out_origo) cloud_origo(h, T, out_origo);
-  return HSB_OK;
+  HsbMatchParams P;
+  fill_match_params(h, P);
+  P.B = B;
+  P.hints = d_hints;
+  P.out_poses = d_out_poses;
+  P.out_cov = d_out_cov;
+  P.kind = HSB_IN_RANGES;
+  P.conv_in = d_ranges;
+  P.n_shared = h->fmt.n_beams;   // scan b is d_ranges[b * n_beams ..]
+  fill_conv(h, HSB_IN_RANGES, P.conv);
+  return launch_match(h, P, h->fmt.n_beams, (cudaStream_t)stream);
+}
+
+int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, const float* d_points_xyz, const int* d_offsets,
+                                 int max_points_per_scan, const double* d_transforms, float* d_out_poses, float* d_out_cov,
+                                 float* d_out_origo, void* stream) {
+  if (!h || B < 0 || !d_hints || !d_offsets || !d_out_poses || max_points_per_scan < 0) return HSB_ERR_INVALID_ARG;
+  int s = check_input(h, h, HSB_IN_CLOUD, "hsb_match_batch_cloud_device", -1, -1, false);
+  if (s != HSB_OK) return s;
+  if (B == 0) return HSB_OK;
+  if (!d_points_xyz && max_points_per_scan > 0) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
+  HandleScope guard(h);
+  HsbMatchParams P;
+  fill_match_params(h, P);
+  P.B = B;
+  P.hints = d_hints;
+  P.out_poses = d_out_poses;
+  P.out_cov = d_out_cov;
+  P.kind = HSB_IN_CLOUD;
+  P.conv_in = d_points_xyz;
+  P.offsets = d_offsets;
+  P.cloud_tf = d_transforms;
+  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
+  P.out_origo = d_out_origo;
+  fill_conv(h, HSB_IN_CLOUD, P.conv);
+  return launch_match(h, P, max_points_per_scan, (cudaStream_t)stream);
 }
 
 }  // extern "C"
@@ -1270,9 +1272,8 @@ int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, cons
 // inputs, not by copy + the exposed tail kernel.  The blocking entry points are submit + wait.
 namespace {
 
-enum { IN_ENDPOINTS = 0, IN_RANGES = 1, IN_CLOUD = 2 };
 struct HostBatch {
-  int kind = IN_ENDPOINTS;
+  HsbInputKind kind = HSB_IN_ENDPOINTS;
   int B = 0;
   const float* hints = nullptr;
   const float* in = nullptr;        // endpoints xy | ranges | cloud xyz
@@ -1301,11 +1302,11 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
   if ((s = wait_set(h, si)) != HSB_OK) return s;   // the set is reused: its previous call must have delivered
   int max_n = 0;
   size_t in_bytes = 0, unit = 8;
-  if (hb.kind == IN_RANGES) {
+  if (hb.kind == HSB_IN_RANGES) {
     max_n = h->fmt.n_beams;
     in_bytes = (size_t)B * (size_t)h->fmt.n_beams * 4;
   } else {
-    unit = hb.kind == IN_CLOUD ? 12 : 8;
+    unit = hb.kind == HSB_IN_CLOUD ? 12 : 8;
     if (hb.offsets) {
       for (int b = 0; b < B; ++b) {
         const int n = hb.offsets[b + 1] - hb.offsets[b];
@@ -1335,7 +1336,7 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
   double* d_tf = hb.transforms ? static_cast<double*>(S.tf.p) : nullptr;
 
   std::vector<int> bounds = pipeline_bounds(B, h->tune_chunk);
-  const bool shared = hb.kind == IN_ENDPOINTS && !hb.offsets;
+  const bool shared = hb.kind == HSB_IN_ENDPOINTS && !hb.offsets;
   if (shared) bounds = std::vector<int>{0, B};   // one shared scan: nothing big to overlap
   ShapeScope shape_scope(h, B, bounds.size() - 1);
   // Stream roles: copy_stream[0] carries ALL host->device copies of all calls back to back, copy_stream[1] the kernels
@@ -1351,7 +1352,7 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
     cudaStream_t st = s1;
     if (!shared) {
       size_t p0, p1;
-      if (hb.kind == IN_RANGES) {
+      if (hb.kind == HSB_IN_RANGES) {
         p0 = (size_t)b0 * h->fmt.n_beams * 4;
         p1 = (size_t)b1 * h->fmt.n_beams * 4;
       } else {
@@ -1366,10 +1367,10 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
     HSB_CUDA(h, cudaStreamWaitEvent(s1, ready, 0));
     float* o_pose = d_poses + 3 * (size_t)b0;
     float* o_cov = d_cov ? d_cov + 9 * (size_t)b0 : nullptr;
-    if (hb.kind == IN_RANGES)
+    if (hb.kind == HSB_IN_RANGES)
       s = hsb_match_batch_ranges_device(h, b1 - b0, d_hints + 3 * (size_t)b0,
                                         reinterpret_cast<const float*>(d_in) + (size_t)b0 * h->fmt.n_beams, o_pose, o_cov, st);
-    else if (hb.kind == IN_CLOUD)
+    else if (hb.kind == HSB_IN_CLOUD)
       s = hsb_match_batch_cloud_device(h, b1 - b0, d_hints + 3 * (size_t)b0, reinterpret_cast<const float*>(d_in), d_off + b0, max_n,
                                        d_tf ? d_tf + 12 * (size_t)b0 : nullptr, o_pose, o_cov,
                                        d_origo ? d_origo + 2 * (size_t)b0 : nullptr, st);
@@ -1422,7 +1423,7 @@ int hsb_match_batch_submit(hsb_handle* h, int B, const float* hints, const float
   }
   HandleScope guard(h);
   HostBatch hb;
-  hb.kind = IN_ENDPOINTS;
+  hb.kind = HSB_IN_ENDPOINTS;
   hb.B = B;
   hb.hints = hints;
   hb.in = pts;
@@ -1442,14 +1443,14 @@ int hsb_match_batch_ranges_submit(hsb_handle* h, int B, const float* hints, cons
   int s = check_batch_args(h, B, hints, out_poses);
   if (s != HSB_OK) return s;
   if (!ranges) return HSB_ERR_INVALID_ARG;
-  if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
+  if ((s = check_input(h, h, HSB_IN_RANGES, "hsb_match_batch_ranges", -1, -1, false)) != HSB_OK) return s;
   if (B == 0) {
     if (ticket) *ticket = -1;
     return HSB_OK;
   }
   HandleScope guard(h);
   HostBatch hb;
-  hb.kind = IN_RANGES;
+  hb.kind = HSB_IN_RANGES;
   hb.B = B;
   hb.hints = hints;
   hb.in = ranges;
@@ -1466,14 +1467,14 @@ int hsb_match_batch_cloud_submit(hsb_handle* h, int B, const float* hints, const
   int s = check_batch_args(h, B, hints, out_poses);
   if (s != HSB_OK) return s;
   if (!offsets) return HSB_ERR_INVALID_ARG;
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
+  if ((s = check_input(h, h, HSB_IN_CLOUD, "hsb_match_batch_cloud", -1, -1, false)) != HSB_OK) return s;
   if (B == 0) {
     if (ticket) *ticket = -1;
     return HSB_OK;
   }
   HandleScope guard(h);
   HostBatch hb;
-  hb.kind = IN_CLOUD;
+  hb.kind = HSB_IN_CLOUD;
   hb.B = B;
   hb.hints = hints;
   hb.in = points_xyz;
@@ -1730,15 +1731,7 @@ static int slam_update_impl(hsb_handle* h, const float hint[3], const float* pts
     return s;
   if (poll) {
     // the pose is all the caller needs now; every later call on this handle is stream-ordered behind the map write
-    unsigned spins = 0;
-    while (*seq != seq_value) {
-      if ((++spins & 0xfffu) == 0) {   // every 4096 polls make sure the stream has not died underneath us
-        cudaError_t e = cudaStreamQuery(st);
-        if (e != cudaSuccess && e != cudaErrorNotReady) return fail(h, HSB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
-        if (e == cudaSuccess && *seq != seq_value) return fail(h, HSB_ERR_CUDA, "fused step finished without publishing its pose");
-      }
-    }
-    __sync_synchronize();
+    if ((s = wait_published(h, seq, seq_value, st, "fused step finished without publishing its pose")) != HSB_OK) return s;
     h->map_write_pending = true;
   } else {
     if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 8, d_s + 8, 13 * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1764,9 +1757,8 @@ int hsb_slam_update_nowait(hsb_handle* h, const float hint[3], const float* pts,
 // What a fused single SLAM step converts on the device: a Point32 cloud in the laser frame with its laser transform
 // (hsb_slam_update_cloud), a LaserScan's raw ranges in the handle's scan format (hsb_slam_update_ranges), or raw
 // ranges projected with the handle's laser projection and then converted as a cloud (hsb_slam_update_projected).
-enum FusedKind { FUSED_CLOUD, FUSED_RANGES, FUSED_PROJECTED };
 struct FusedScan {
-  FusedKind kind;
+  HsbInputKind kind;
   const float* data;    // cloud: n (x, y, z) triples; ranges / projected: n ranges
   int n;                // cloud: points; ranges / projected: n_beams (an upper bound of the endpoints kept)
   const double* T;      // cloud / projected: the laser transform (12 doubles)
@@ -1784,38 +1776,27 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
   const int n = in.n;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
-  // staging layout (floats): [0..15] header: hint, thresholds, force, [8] = 0, [9] = n (cloud offsets, as ints);
-  // cloud / projected: [16..39] the laser transform (12 doubles), [40..] the cloud or the ranges; ranges: [16..] the ranges
-  const bool ranges = in.kind == FUSED_RANGES, projected = in.kind == FUSED_PROJECTED;
-  const size_t kHdr = 16, kTf = ranges ? 0 : 24, per_pt = in.kind == FUSED_CLOUD ? 3 : 1;
+  // staging layout (floats): [0..15] header: hint, thresholds, force; cloud / projected: [16..39] the laser transform
+  // (12 doubles), [40..] the cloud or the ranges; ranges: [16..] the ranges
+  const bool ranges = in.kind == HSB_IN_RANGES;
+  const size_t kHdr = 16, kTf = ranges ? 0 : 24, per_pt = in.kind == HSB_IN_CLOUD ? 3 : 1;
   const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
   if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
-  if (bytes > h->h_stage_bytes) {
-    if (h->h_stage) cudaFreeHost(h->h_stage);
-    h->h_stage = nullptr;
-    h->h_stage_bytes = 0;
-    size_t cap = bytes < (64u << 10) ? (64u << 10) : bytes * 2;
-    HSB_CUDA(h, cudaMallocHost(&h->h_stage, cap));
-    h->h_stage_bytes = cap;
-  }
+  if ((s = ensure_pinned(h, h->h_stage, h->h_stage_bytes, bytes)) != HSB_OK) return s;
   float* hs = h->h_stage;
   memset(hs, 0, kHdr * sizeof(float));
   hs[0] = hint[0]; hs[1] = hint[1]; hs[2] = hint[2];
   hs[3] = h->min_dist; hs[4] = h->min_angle; hs[5] = map_without_matching ? 1.f : 0.f;
-  reinterpret_cast<int*>(hs)[8] = 0;
-  reinterpret_cast<int*>(hs)[9] = n;
   if (!ranges) memcpy(hs + kHdr, in.T, 12 * sizeof(double));
   if (n > 0) memcpy(hs + kHdr + kTf, in.data, (size_t)n * per_pt * sizeof(float));
   cudaStream_t st = h->stream;
   HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
   float* d_c = static_cast<float*>(h->d_fused_in.p);
   const float* d_hdr = d_c;
-  const int* d_offs = reinterpret_cast<const int*>(d_c) + 8;
-  const double* d_tf = reinterpret_cast<const double*>(d_c + kHdr);
+  const double* d_tf = ranges ? nullptr : reinterpret_cast<const double*>(d_c + kHdr);
   const float* d_in = d_c + kHdr + kTf;
   float* d_s = static_cast<float*>(h->d_scratch.p);
   float* d_gate = static_cast<float*>(h->d_gate.p);
-  int* d_n = reinterpret_cast<int*>(d_s + 40);
   // the container's origo is known on the host: zero for a LaserScan (HectorMappingRos.cpp:491)
   float origo[2] = {0.f, 0.f};
   if (!ranges) cloud_origo(h, in.T, origo);
@@ -1828,7 +1809,10 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
   int* kept_dev = reinterpret_cast<int*>(h->h_pin_dev + 24);
   DevBuf& pbuf = map_without_matching ? h->d_upd_pts : h->d_last_pts;
   if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
-  float2* d_pts_out = reinterpret_cast<float2*>(scan_points(pbuf));
+  HsbConvDev conv;
+  fill_conv(h, in.kind, conv);
+  conv.out_pts = reinterpret_cast<float2*>(scan_points(pbuf));
+  conv.out_n = reinterpret_cast<int*>(d_s + 40);
   if (!map_without_matching) {
     HsbMatchParams P;
     fill_match_params(h, P);
@@ -1836,19 +1820,19 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
     P.hints = d_hdr;
     P.out_poses = d_s + 8;
     P.out_cov = h->h_pin_dev + 12;
-    if (ranges) fill_range_params(h, P, d_in);
-    else if (projected) fill_projected_params(h, P, d_in, d_tf);
-    else fill_cloud_params(h, P, d_in, d_offs, d_tf, nullptr);
-    P.out_pts = d_pts_out;
-    P.out_n = d_n;
-    P.out_n_host = kept_dev;
+    P.kind = in.kind;
+    P.conv_in = d_in;
+    P.n_shared = n;
+    P.cloud_tf = d_tf;
+    P.conv = conv;
+    P.conv.out_n_host = kept_dev;
     P.gate_state = d_gate;
     P.gate_in = d_hdr + 3;
     P.gate_out_host = h->h_pin_dev + 8;
     P.seq_host = poll ? seq_dev : nullptr;
     P.seq_value = seq_value;
     // (the projection is compiled into the single step's default shape only: hsb_slam_update_projected checked the tuning)
-    if (projected)
+    if (in.kind == HSB_IN_PROJECTED)
       s = h->gather_mode == HSB_GATHER_TEX
               ? launch_match_t<8, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, n, st, 1)
               : launch_match_t<8, 1, hsb::MODE_LDG, 4, false, false, false, true>(h, P, n, st, 1);
@@ -1859,31 +1843,15 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
     h->last_origo[0] = origo[0];
     h->last_origo[1] = origo[1];
   } else {
-    if (projected) {
-      if ((s = launch_projected_conversion(h, d_in, d_tf, d_pts_out, d_n, st)) != HSB_OK) return s;
-    } else if (ranges)
-      hsb::scan_to_points_kernel<<<1, 256, 0, st>>>(d_in, static_cast<const float2*>(h->d_beam_cs.p), n, h->fmt.range_min,
-                                                    range_max_c(h->fmt), h->lv[0].scale, d_pts_out, d_n);
-    else
-      hsb::cloud_to_points_kernel<<<1, 256, 0, st>>>(d_in, n, d_tf, h->cfmt.sqr_laser_min_dist, h->cfmt.sqr_laser_max_dist,
-                                                     h->cfmt.laser_z_min_value, h->cfmt.laser_z_max_value, h->lv[0].scale,
-                                                     d_pts_out, d_n);
+    if ((s = launch_conversion(h, in.kind, d_in, n, d_tf, conv, st)) != HSB_OK) return s;
     hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, h->h_pin_dev + 8, nullptr, 0);
-    hsb::publish_int_kernel<<<1, 32, 0, st>>>(d_n, kept_dev, poll ? seq_dev : nullptr, seq_value);
-    h->launches += 3;
+    hsb::publish_int_kernel<<<1, 32, 0, st>>>(conv.out_n, kept_dev, poll ? seq_dev : nullptr, seq_value);
+    h->launches += 2;
     HSB_CUDA(h, cudaGetLastError());
   }
-  if ((s = enqueue_update_by_scan(h, d_pts_out, n, origo, nullptr, d_s + 8, d_gate + 3, d_n)) != HSB_OK) return s;
+  if ((s = enqueue_update_by_scan(h, conv.out_pts, n, origo, nullptr, d_s + 8, d_gate + 3, conv.out_n)) != HSB_OK) return s;
   if (poll) {
-    unsigned spins = 0;
-    while (*seq != seq_value) {
-      if ((++spins & 0xfffu) == 0) {
-        cudaError_t e = cudaStreamQuery(st);
-        if (e != cudaSuccess && e != cudaErrorNotReady) return fail(h, HSB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
-        if (e == cudaSuccess && *seq != seq_value) return fail(h, HSB_ERR_CUDA, "fused step finished without publishing its pose");
-      }
-    }
-    __sync_synchronize();
+    if ((s = wait_published(h, seq, seq_value, st, "fused step finished without publishing its pose")) != HSB_OK) return s;
     h->map_write_pending = true;
   } else {
     HSB_CUDA(h, cudaStreamSynchronize(st));
@@ -1904,8 +1872,9 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
                           int map_without_matching, int nowait, float out_pose[3], float cov_inout[9], int* map_updated,
                           int* out_kept) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
-  if (!h->cfmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_cloud_format has not been called");
-  const FusedScan in = {FUSED_CLOUD, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
+  int s = check_input(h, h, HSB_IN_CLOUD, "hsb_slam_update_cloud", -1, -1, false);
+  if (s != HSB_OK) return s;
+  const FusedScan in = {HSB_IN_CLOUD, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
@@ -1914,11 +1883,9 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
 int hsb_slam_update_ranges(hsb_handle* h, const float hint[3], const float* ranges, int n, int map_without_matching,
                            int nowait, float out_pose[3], float cov_inout[9], int* map_updated, int* out_kept) {
   if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
-  if (!h->fmt_set) return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_scan_format has not been called");
-  if (n != h->fmt.n_beams)
-    return fail(h, HSB_ERR_INVALID_ARG, "hsb_slam_update_ranges: n is %d, the scan format has %d beams", n,
-                h->fmt.n_beams);
-  const FusedScan in = {FUSED_RANGES, ranges, n, nullptr};
+  int s = check_input(h, h, HSB_IN_RANGES, "hsb_slam_update_ranges", -1, n, false);
+  if (s != HSB_OK) return s;
+  const FusedScan in = {HSB_IN_RANGES, ranges, n, nullptr};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
@@ -1928,7 +1895,7 @@ int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* r
                               int map_without_matching, int nowait, float out_pose[3], float cov_inout[9],
                               int* map_updated, int* out_kept) {
   if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
-  int s = check_projected(h, "hsb_slam_update_projected", n);
+  int s = check_input(h, h, HSB_IN_PROJECTED, "hsb_slam_update_projected", -1, n, true);
   if (s != HSB_OK) return s;
   // the match shape hsb_slam_update_cloud would take under this tuning must be the one compiled with the projection
   if (!((h->tune_warps_per_scan == 0 || h->tune_warps_per_scan == 8) && h->tune_scans_per_block <= 1 &&
@@ -1936,7 +1903,7 @@ int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* r
     return fail(h, HSB_ERR_UNSUPPORTED,
                 "hsb_slam_update_projected: no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d "
                 "unroll=%d packed=%d", h->tune_warps_per_scan, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
-  const FusedScan in = {FUSED_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform};
+  const FusedScan in = {HSB_IN_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }
 
@@ -2578,9 +2545,8 @@ namespace {
 // (hsb_group_slam_update_cloud), raw LaserScan ranges (hsb_group_slam_update_ranges) or raw ranges to project
 // (hsb_group_slam_update_projected).  All but endpoints are converted in the match kernel's staging step as
 // hsb_slam_update_cloud / _ranges / _projected convert them.
-enum GroupInputKind { GROUP_ENDPOINTS, GROUP_CLOUD, GROUP_RANGES, GROUP_PROJECTED };
 struct GroupInput {
-  GroupInputKind kind;
+  HsbInputKind kind;
   const char* fn;              // the entry point, for the error messages
   const float* hints;          // M x 3
   const float* pts;            // endpoints: xy pairs; cloud: Point32 triples; ranges: one float per beam
@@ -2597,10 +2563,11 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
                float* cov_inout, int* map_updated, int* out_kept) {
   hsb_handle* h0 = g->m[0];
   const int M = (int)g->m.size(), levels = g->levels;
-  const bool cloud = in.kind == GROUP_CLOUD, ranges = in.kind == GROUP_RANGES, projected = in.kind == GROUP_PROJECTED;
-  const bool conv = cloud || ranges || projected;   // converted on the device: the kept count decides what the session had
-  const bool tf = cloud || projected;               // with a laser transform per session
+  const bool cloud = in.kind == HSB_IN_CLOUD;
+  const bool conv = in.kind != HSB_IN_ENDPOINTS;   // converted on the device: the kept count decides what the session had
+  const bool tf = cloud || in.kind == HSB_IN_PROJECTED;   // with a laser transform per session
   const int* offsets = in.offsets;
+  int s;
   if (!in.hints || !offsets || !out_poses)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
   if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", in.fn, offsets[0]);
@@ -2615,39 +2582,13 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   const int total = offsets[M];
   if (total > 0 && !in.pts)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : conv ? "ranges" : "points_xy");
-  if (projected) {
-    for (int k = 0; k < M; ++k) {
-      const hsb_handle* h = g->m[k];
-      if (!h->proj_set)
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_laser_projection has not been called on its handle",
-                    in.fn, k);
-      if (offsets[k + 1] - offsets[k] != h->proj.n_beams)
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d has %d ranges, its laser projection has %d beams", in.fn, k,
-                    offsets[k + 1] - offsets[k], h->proj.n_beams);
-    }
-  }
-  if (tf) {
-    for (int k = 0; k < M; ++k)
-      if (!g->m[k]->cfmt_set)
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_cloud_format has not been called on its handle",
-                    in.fn, k);
-  }
-  if (ranges) {
-    for (int k = 0; k < M; ++k) {
-      const hsb_handle* h = g->m[k];
-      if (!h->fmt_set)
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: hsb_set_scan_format has not been called on its handle",
-                    in.fn, k);
-      if (offsets[k + 1] - offsets[k] != h->fmt.n_beams)
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d has %d ranges, its scan format has %d beams", in.fn, k,
-                    offsets[k + 1] - offsets[k], h->fmt.n_beams);
-    }
+  for (int k = 0; conv && k < M; ++k) {
+    if ((s = check_input(g->m[k], h0, in.kind, in.fn, k, offsets[k + 1] - offsets[k], false)) != HSB_OK) return s;
   }
   // every scan is converted whole into shared memory: the launcher's limit for the group kernel's shape
   if (conv && !staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
   DeviceGuard guard(g->device);
   cudaStream_t st = g->stream;
-  int s;
   // not before the work the members queued themselves, nor before a pending step of another group they belong to
   for (hsb_handle* h : g->m) {
     if (h->group_ev && h->group_ev != g->ev) HSB_CUDA(h0, cudaStreamWaitEvent(st, h->group_ev, 0));
@@ -2666,14 +2607,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   const size_t o_pts = al(o_tf + (tf ? (size_t)M * 12 * sizeof(double) : 0));
   const size_t pt_bytes = cloud ? 12 : conv ? 4 : 8;
   const size_t bytes = o_pts + (size_t)total * pt_bytes;
-  if (bytes > g->h_stage_bytes) {
-    if (g->h_stage) cudaFreeHost(g->h_stage);
-    g->h_stage = nullptr;
-    g->h_stage_bytes = 0;
-    const size_t cap = bytes < (64u << 10) ? (64u << 10) : bytes + bytes / 2;
-    HSB_CUDA(h0, cudaMallocHost(reinterpret_cast<void**>(&g->h_stage), cap));
-    g->h_stage_bytes = cap;
-  }
+  if ((s = ensure_pinned(h0, g->h_stage, g->h_stage_bytes, bytes)) != HSB_OK) return s;
   if ((s = ensure(h0, g->d_stage, bytes)) != HSB_OK) return s;
   char* hs = g->h_stage;
   const char* ds = static_cast<const char*>(g->d_stage.p);
@@ -2723,27 +2657,11 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     if (conv) {   // converted into the buffer the single fused step converts into
       DevBuf& pbuf = matched ? h->d_last_pts : h->d_upd_pts;
       if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
-      ss.conv_pts = reinterpret_cast<float2*>(scan_points(pbuf));
-      ss.kept = kept_dev + k;
-      ss.kept_host = kept_mapped + k;
-      if (tf) {
-        ss.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
-        ss.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
-        ss.z_min = h->cfmt.laser_z_min_value;
-        ss.z_max = h->cfmt.laser_z_max_value;
-      }
-      if (projected) {
-        ss.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
-        ss.n_beams = h->proj.n_beams;
-        ss.range_min = h->proj.range_min;
-        ss.range_cutoff = projection_cutoff(h->proj);
-      } else if (ranges) {
-        ss.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
-        ss.n_beams = h->fmt.n_beams;
-        ss.range_min = h->fmt.range_min;
-        ss.range_max_c = range_max_c(h->fmt);
-      }
-      pts0 = ss.conv_pts;
+      fill_conv(h, in.kind, ss.conv);
+      ss.conv.out_pts = reinterpret_cast<float2*>(scan_points(pbuf));
+      ss.conv.out_n = kept_dev + k;
+      ss.conv.out_n_host = kept_mapped + k;
+      pts0 = ss.conv.out_pts;
       n_dev = kept_dev + k;
     } else {
       pts0 = reinterpret_cast<const float2*>(d_in) + offsets[k];
@@ -2779,19 +2697,11 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   fill_match_params(h0, P);
   P.B = M;
   P.hints = reinterpret_cast<const float*>(ds);
-  if (cloud) {   // (the kernel takes the thresholds from the session descriptors, not from h0's format)
-    fill_cloud_params(h0, P, reinterpret_cast<const float*>(d_in), reinterpret_cast<const int*>(ds + o_off),
-                      reinterpret_cast<const double*>(ds + o_tf), nullptr);
-  } else if (ranges) {   // (likewise the scan format; the offsets locate each session's ranges)
-    fill_range_params(h0, P, reinterpret_cast<const float*>(d_in));
-    P.offsets = reinterpret_cast<const int*>(ds + o_off);
-  } else if (projected) {   // (likewise the projection and cloud format)
-    fill_projected_params(h0, P, reinterpret_cast<const float*>(d_in), reinterpret_cast<const double*>(ds + o_tf));
-    P.offsets = reinterpret_cast<const int*>(ds + o_off);
-  } else {
-    P.pts = reinterpret_cast<const float2*>(d_in);
-    P.offsets = reinterpret_cast<const int*>(ds + o_off);
-  }
+  P.kind = in.kind;   // (a converted session converts with its own descriptor)
+  if (conv) P.conv_in = reinterpret_cast<const float*>(d_in);
+  else P.pts = reinterpret_cast<const float2*>(d_in);
+  P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  if (tf) P.cloud_tf = reinterpret_cast<const double*>(ds + o_tf);
   P.out_poses = g->d_res;
   P.out_cov = g->h_res_dev + 4 * (size_t)M;
   P.gate_in = reinterpret_cast<const float*>(ds + o_gin);
@@ -2801,7 +2711,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   P.group_lv = g->d_lv;
   P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
-  if (projected)
+  if (in.kind == HSB_IN_PROJECTED)
     s = h0->gather_mode == HSB_GATHER_TEX
             ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true, true>(h0, P, max_n, st, 1)
             : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true, true>(h0, P, max_n, st, 1);
@@ -2851,15 +2761,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
 
   if (nowait) {   // return when every pose has arrived; the map writes continue on the group's stream
     volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(g->h_res + 13 * (size_t)M);
-    unsigned spins = 0;
-    while (*seq != P.seq_value) {
-      if ((++spins & 0xfffu) == 0) {
-        cudaError_t e = cudaStreamQuery(st);
-        if (e != cudaSuccess && e != cudaErrorNotReady) return fail(h0, HSB_ERR_CUDA, "stream failed: %s", cudaGetErrorString(e));
-        if (e == cudaSuccess && *seq != P.seq_value) return fail(h0, HSB_ERR_CUDA, "group step finished without publishing its poses");
-      }
-    }
-    __sync_synchronize();
+    if ((s = wait_published(h0, seq, P.seq_value, st, "group step finished without publishing its poses")) != HSB_OK) return s;
   } else {
     HSB_CUDA(h0, cudaStreamSynchronize(st));   // :93 onMapUpdated for every member
   }
@@ -2887,7 +2789,7 @@ extern "C" {
 int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_xy, const int* offsets, const float* origo,
                           const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  const GroupInput in = {GROUP_ENDPOINTS, "hsb_group_slam_update", hints, points_xy, offsets, origo, nullptr};
+  const GroupInput in = {HSB_IN_ENDPOINTS, "hsb_group_slam_update", hints, points_xy, offsets, origo, nullptr};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, nullptr);
 }
 
@@ -2895,7 +2797,7 @@ int hsb_group_slam_update_cloud(hsb_group* g, const float* hints, const float* p
                                 const double* transforms, const int* map_without_matching, int nowait, float* out_poses,
                                 float* cov_inout, int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  const GroupInput in = {GROUP_CLOUD, "hsb_group_slam_update_cloud", hints, points_xyz, offsets, nullptr, transforms};
+  const GroupInput in = {HSB_IN_CLOUD, "hsb_group_slam_update_cloud", hints, points_xyz, offsets, nullptr, transforms};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 
@@ -2903,7 +2805,7 @@ int hsb_group_slam_update_ranges(hsb_group* g, const float* hints, const float* 
                                  const int* map_without_matching, int nowait, float* out_poses, float* cov_inout,
                                  int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  const GroupInput in = {GROUP_RANGES, "hsb_group_slam_update_ranges", hints, ranges, offsets, nullptr, nullptr};
+  const GroupInput in = {HSB_IN_RANGES, "hsb_group_slam_update_ranges", hints, ranges, offsets, nullptr, nullptr};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 
@@ -2911,7 +2813,7 @@ int hsb_group_slam_update_projected(hsb_group* g, const float* hints, const floa
                                     const double* transforms, const int* map_without_matching, int nowait,
                                     float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  const GroupInput in = {GROUP_PROJECTED, "hsb_group_slam_update_projected", hints, ranges, offsets, nullptr, transforms};
+  const GroupInput in = {HSB_IN_PROJECTED, "hsb_group_slam_update_projected", hints, ranges, offsets, nullptr, transforms};
   return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 

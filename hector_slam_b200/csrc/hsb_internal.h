@@ -22,28 +22,40 @@ struct HsbLevelDev {
   int rec_off;               // where this level's part of a scan's per-evaluation record starts (HsbMatchParams::record)
 };
 
-// One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges): the member handle's state the match
-// kernel touches.
+// What a scan arrives as: level-0 endpoints, or an input the match kernel's staging step converts to them —
+// LaserScan ranges (rosLaserScanToDataContainer), a Point32 cloud in the laser frame (rosPointCloudToDataContainer) or
+// LaserScan ranges projected by laser_geometry and then converted as a cloud.
+enum HsbInputKind { HSB_IN_ENDPOINTS, HSB_IN_RANGES, HSB_IN_CLOUD, HSB_IN_PROJECTED };
+
+// How a handle converts a scan (its hsb_set_scan_format / _cloud_format / _laser_projection at call time), and where
+// the converted endpoints go.  Only the fields of the scan's kind are set.  (A scan of ranges has exactly the format's
+// beam count, checked on the host: the kernels take it from the scan's length.)
+struct HsbConvDev {
+  // ranges: the (cos, sin) table of the accumulated beam angle, kept where range_min < r < range_max_c;
+  // projected: kept where (double)r < range_cutoff && r >= range_min, projected with proj_unit (double (cos, sin))
+  const float2* beam_cs;
+  const double2* proj_unit;
+  float range_min, range_max_c;
+  double range_cutoff;
+  // cloud and projected: the thresholds of the cloud rule
+  float sqr_min_dist, sqr_max_dist, z_min, z_max;
+  float scale_to_map;
+  // the sink (SLAM steps and the stand-alone conversion; null for batch matches): the compacted endpoints go to
+  // out_pts, their number to device memory (out_n, the map writer's n_dev) and, if set, to mapped host memory
+  // (out_n_host, written before the step's sequence number is published)
+  float2* out_pts;
+  int* out_n;
+  int* out_n_host;
+};
+
+// One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges / _projected): the member handle's state
+// the match kernel touches.
 struct HsbGroupSessionDev {
   float* gate_state;   // the member's lastMapUpdatePose[3] and write flag (hsb_handle::d_gate)
   float2* last_pts;    // the member's "containers of the last match": a matched scan's endpoints are copied here
-  // converted input (HsbMatchParams::cloud or ::ranges set): the converted endpoints go to conv_pts (the member's
-  // last-match container when the session matches, its update-scan buffer when not), their number to kept (device
-  // memory, the map writer's n_dev) and to kept_host (the group's mapped host block, before the step's sequence number
-  // is published)
-  float2* conv_pts;
-  int* kept;
-  int* kept_host;
-  // point clouds: the member's hsb_set_cloud_format thresholds at step time
-  float sqr_min_dist, sqr_max_dist, z_min, z_max;
-  // raw ranges: the member's hsb_set_scan_format at step time — its (cos, sin) table, beam count and range window
-  const float2* beam_cs;
-  int n_beams;
-  float range_min, range_max_c;
-  // projected ranges (match_kernel<..., PROJ = true>): the member's hsb_set_laser_projection at step time — its double
-  // (cos, sin) table and projector cutoff (n_beams and range_min above), with the cloud format's thresholds above
-  const double2* proj_unit;
-  double range_cutoff;
+  // converted input: the member's format; the sink is its last-match container when the session matches, its
+  // update-scan buffer when not
+  HsbConvDev conv;
 };
 
 struct HsbMatchParams {
@@ -51,33 +63,24 @@ struct HsbMatchParams {
   int levels;
   int B;
   const float* hints;   // B x 3
-  const float2* pts;    // all scans, interleaved xy
-  const int* offsets;   // B + 1, or nullptr in shared-scan mode
+  // Scan b's input is [offsets[b], offsets[b+1]) — endpoints, ranges or cloud points — or, without offsets, n_shared
+  // inputs: the same endpoints for every scan (shared-scan mode), or scan b's own converted input at b * n_shared.
+  HsbInputKind kind;
+  const float2* pts;    // endpoints, interleaved xy
+  const float* conv_in; // converted input: one float per range, or Point32 (x, y, z) triples
+  const int* offsets;   // B + 1, or nullptr
   int n_shared;
   float* out_poses;     // B x 3
   float* out_cov;       // B x 9 or nullptr
   int pts_cap;          // points of smem staging per scan group (0 = read points from global)
-  // raw-range input (N2: rosLaserScanToDataContainer fused into the staging step); ranges == nullptr
-  // selects the endpoint input above
-  const float* ranges;      // B x n_beams
-  const float2* beam_cs;    // n_beams x (cos, sin) of the accumulated beam angle
-  int n_beams;
-  float range_min, range_max_c;  // keep range_min < r < range_max - 0.1
-  float scale_to_map;
-  // point-cloud input (N2, the node's default path: rosPointCloudToDataContainer fused into the staging step);
-  // cloud == nullptr selects one of the inputs above.  Scan b is the Point32 triples cloud[3*cloud_offsets[b] ..
-  // 3*cloud_offsets[b+1]); its laser transform is cloud_tf + 12*b (rows of [R | t], double) or, if that is null, cloud_tf0.
-  const float* cloud;
-  const int* cloud_offsets;
+  // how converted input becomes endpoints (N2: the node's conversions fused into the staging step), and where the
+  // endpoints go (fused single SLAM step; with an inline scan, where its endpoints go)
+  HsbConvDev conv;
+  // cloud and projected: scan b's laser transform is cloud_tf + 12*b (rows of [R | t], double) or, if that is null,
+  // cloud_tf0
   const double* cloud_tf;
   double cloud_tf0[12];
-  float sqr_min_dist, sqr_max_dist, z_min, z_max;
-  float* out_origo;         // B x 2 (may be null): dataContainer origo = laser position * scaleToMap
-  // fused single-scan SLAM step from a point cloud or raw ranges (B == 1): the converted endpoints are also written out
-  // for the map writer, their number goes to device memory (out_n) and to mapped host memory (out_n_host)
-  float2* out_pts;
-  int* out_n;
-  int* out_n_host;
+  float* out_origo;         // cloud: B x 2 (may be null): dataContainer origo = laser position * scaleToMap
   // fused SLAM step (B == 1): the gate of HectorSlamProcessor::update evaluated in the kernel's epilogue
   float* gate_state;        // [0..2] lastMapUpdatePose, [3] flag out; nullptr = no gate
   const float* gate_in;     // minDist, minAngle, force
@@ -107,19 +110,12 @@ struct HsbMatchParams {
   // group_lv[b * levels ..] (built once per group) instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done
-  // counts the sessions that have finished: the last one publishes seq_value to seq_host.  With cloud input a session
-  // reads its thresholds from group_sess[b] (sqr_min_dist .. z_max above are unused); with ranges input its ranges are
-  // ranges[offsets[b] .. offsets[b+1]) and its format comes from group_sess[b] (beam_cs .. range_max_c above are
-  // unused).  Either way a set map_without_matching flag still converts the scan for the map writer: only the match is
-  // skipped.
+  // counts the sessions that have finished: the last one publishes seq_value to seq_host.  A converted session converts
+  // with group_sess[b].conv (conv above is unused); a set map_without_matching flag still converts the scan for the map
+  // writer: only the match is skipped.
   const HsbLevelDev* group_lv;
   const HsbGroupSessionDev* group_sess;
   unsigned* group_done;
-  // projected ranges (match_kernel<..., PROJ = true>, hsb_slam_update_projected): scan b's ranges[b * n_beams ..] are
-  // kept where (double)r < range_cutoff && r >= range_min, projected with proj_unit (n_beams x double (cos, sin)) and
-  // converted with the cloud thresholds and transform above
-  const double2* proj_unit;
-  double range_cutoff;
 };
 
 struct HsbUpdateLevelDev {

@@ -757,9 +757,16 @@ __device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P
   else return P.lv[lvl];
 }
 
+// Conversion descriptor of scan `scan`: the kernel parameters' (one handle), or the session's (group SLAM step).
+template <bool GRP>
+__device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, int scan) {
+  if constexpr (GRP) return P.group_sess[scan].conv;
+  else return P.conv;
+}
+
 // GRP: the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv.
-// PROJ: the ranges input (P.ranges) goes through laser_geometry's projection and the cloud rule (stage_from_projected)
-// instead of rosLaserScanToDataContainer; only the instantiations the projected SLAM steps launch carry that branch.
+// PROJ: converted input is HSB_IN_PROJECTED (laser_geometry's projection and the cloud rule, stage_from_projected); only
+// the instantiations the projected SLAM steps launch carry that branch.
 template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
 __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
@@ -816,19 +823,18 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
   uint32_t phase = 0;
   int red_flip = 0;
   for (int scan = blockIdx.x * Gr + g; scan < P.B; scan += gridDim.x * Gr) {
-    int beg, n;
-    if (P.cloud) {
-      beg = P.cloud_offsets[scan];
-      n = P.cloud_offsets[scan + 1] - beg;   // input points; replaced by the number kept below
-    } else if (P.offsets) {
+    // the scan's input [beg, beg + n): endpoints, or the ranges / cloud points a conversion replaces by the kept endpoints
+    size_t beg;
+    int n;
+    if (P.offsets) {
       beg = P.offsets[scan];
-      n = P.offsets[scan + 1] - beg;
+      n = P.offsets[scan + 1] - (int)beg;
     } else {
-      beg = 0;
       n = P.n_shared;
+      beg = P.kind == HSB_IN_ENDPOINTS ? 0 : (size_t)scan * n;
     }
     if constexpr (GRP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
-      if (!P.cloud && !P.ranges && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a conversion runs first, below)
+      if (P.kind == HSB_IN_ENDPOINTS && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a conversion runs first, below)
     }
     const float2* __restrict__ gpts = P.pts + beg;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
@@ -841,81 +847,39 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       for (int i = t; i < n; i += GT) {
         const float2 v = S.pts[i];
         spts[i] = v;
-        if (P.out_pts) P.out_pts[i] = v;
+        if (P.conv.out_pts) P.conv.out_pts[i] = v;
       }
       group_sync<W>(g);
       ns = n;
       staged = true;
-    } else if (P.ranges || P.cloud) {
+    } else if (P.kind != HSB_IN_ENDPOINTS) {
       // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
+      const HsbConvDev& C = conv_desc<GRP>(P, scan);
+      const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
       if constexpr (PROJ) {   // raw ranges, projected to a cloud in the laser frame and converted by the cloud rule
-        const float* r = P.ranges + (size_t)scan * P.n_beams;
-        const double2* unit = P.proj_unit;
-        const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
-        int nb = P.n_beams;
-        float rmin = P.range_min, min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
-        double cutoff = P.range_cutoff;
-        if constexpr (GRP) {   // group SLAM step: every session with its own member's projection and cloud format
-          const HsbGroupSessionDev& SS = P.group_sess[scan];
-          r = P.ranges + beg;
-          unit = SS.proj_unit;
-          nb = SS.n_beams;
-          rmin = SS.range_min;
-          cutoff = SS.range_cutoff;
-          min2 = SS.sqr_min_dist;
-          max2 = SS.sqr_max_dist;
-          zmin = SS.z_min;
-          zmax = SS.z_max;
-        }
-        n = stage_from_projected<W>(r, unit, nb, rmin, cutoff, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt,
-                                    g, w, lane);
-      } else if (P.ranges) {   // raw ranges
-        const float* r = P.ranges + (size_t)scan * P.n_beams;
-        const float2* cs = P.beam_cs;
-        int nb = P.n_beams;
-        float rmin = P.range_min, rmaxc = P.range_max_c;
-        if constexpr (GRP) {   // group SLAM step: every session converts its own slice with its own member's format
-          const HsbGroupSessionDev& SS = P.group_sess[scan];
-          r = P.ranges + beg;
-          cs = SS.beam_cs;
-          nb = SS.n_beams;
-          rmin = SS.range_min;
-          rmaxc = SS.range_max_c;
-        }
-        n = stage_from_ranges<W>(r, cs, nb, rmin, rmaxc, P.scale_to_map, spts, warp_cnt, g, w, lane);
+        n = stage_from_projected<W>(P.conv_in + beg, C.proj_unit, n, C.range_min, C.range_cutoff, T, C.sqr_min_dist,
+                                    C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map, spts, warp_cnt, g, w, lane);
+      } else if (P.kind == HSB_IN_RANGES) {
+        n = stage_from_ranges<W>(P.conv_in + beg, C.beam_cs, n, C.range_min, C.range_max_c, C.scale_to_map, spts,
+                                 warp_cnt, g, w, lane);
       } else {          // a point cloud
-        const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
-        float min2 = P.sqr_min_dist, max2 = P.sqr_max_dist, zmin = P.z_min, zmax = P.z_max;
-        if constexpr (GRP) {   // group SLAM step: every session converts with its own member's format
-          const HsbGroupSessionDev& SS = P.group_sess[scan];
-          min2 = SS.sqr_min_dist;
-          max2 = SS.sqr_max_dist;
-          zmin = SS.z_min;
-          zmax = SS.z_max;
-        }
-        n = stage_from_cloud<W>(P.cloud + 3 * (size_t)beg, n, T, min2, max2, zmin, zmax, P.scale_to_map, spts, warp_cnt,
-                                g, w, lane);
+        n = stage_from_cloud<W>(P.conv_in + 3 * beg, n, T, C.sqr_min_dist, C.sqr_max_dist, C.z_min, C.z_max,
+                                C.scale_to_map, spts, warp_cnt, g, w, lane);
         if (P.out_origo && t == 0) {   // dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
-          P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], P.scale_to_map);
-          P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], P.scale_to_map);
+          P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], C.scale_to_map);
+          P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], C.scale_to_map);
         }
       }
-      if (P.out_pts) {   // fused single-scan step: the map writer reads the converted endpoints from global memory
-        for (int i = t; i < n; i += GT) P.out_pts[i] = spts[i];
+      if (C.out_pts) {
+        // SLAM step: the endpoints and their number go to the map writer (and, matched, become the last-match
+        // container); the count reaches host memory before the step's sequence number (below)
+        for (int i = t; i < n; i += GT) C.out_pts[i] = spts[i];
         if (t == 0) {
-          *P.out_n = n;
-          if (P.out_n_host) *P.out_n_host = n;
+          *C.out_n = n;
+          if (C.out_n_host) *C.out_n_host = n;
         }
       }
       if constexpr (GRP) {
-        // group SLAM step: the session's endpoints and their number go to its member for the map writer (and, matched,
-        // become its last-match container); the count reaches host memory before the step's sequence number (below)
-        const HsbGroupSessionDev& SS = P.group_sess[scan];
-        for (int i = t; i < n; i += GT) SS.conv_pts[i] = spts[i];
-        if (t == 0) {
-          *SS.kept = n;
-          *SS.kept_host = n;
-        }
         if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // map_without_matching: converted for the writer, not matched
       }
       ns = n;
@@ -1160,8 +1124,8 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     if constexpr (GRP) {
       // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
       // its later map writes without matching read it (after the pose is out: only the map writers wait for this).
-      // A converted scan is already there (conv_pts, above).
-      if (!P.cloud && !P.ranges) {
+      // A converted scan is already there (the conversion's sink, above).
+      if (P.kind == HSB_IN_ENDPOINTS) {
         float2* keep = P.group_sess[scan].last_pts;
         for (int i = t; i < n; i += GT) keep[i] = gpts[i];
       }
@@ -1171,36 +1135,28 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
   if (pace && t == 0) prog[g] = 0x7fffffff;   // this group is done: nobody waits for it any more
 }
 
-// The conversion alone (one scan, one CTA of 8 warps), for the N2 parity tests.
+// The conversion alone (one scan of n_in ranges or cloud points, laser transform T; one CTA of 8 warps) into C's sink:
+// the stand-alone conversion calls and the SLAM steps without matching.
+template <int KIND>
 __global__ void __launch_bounds__(256)
-    scan_to_points_kernel(const float* __restrict__ ranges, const float2* __restrict__ beam_cs, int n_beams, float rmin,
-                          float rmaxc, float scale, float2* __restrict__ out, int* __restrict__ out_n) {
+    conv_to_points_kernel(const float* __restrict__ in, int n_in, const double* __restrict__ T, const HsbConvDev C) {
   __shared__ int warp_cnt[32];
-  const int n = stage_from_ranges<8>(ranges, beam_cs, n_beams, rmin, rmaxc, scale, out, warp_cnt, 0, threadIdx.x >> 5,
-                                     threadIdx.x & 31);
-  if (threadIdx.x == 0) *out_n = n;
-}
-
-__global__ void __launch_bounds__(256)
-    cloud_to_points_kernel(const float* __restrict__ xyz, int n_in, const double* __restrict__ T, float min2, float max2, float zmin,
-                           float zmax, float scale, float2* __restrict__ out, int* __restrict__ out_n) {
-  __shared__ int warp_cnt[32];
-  const int n = stage_from_cloud<8>(xyz, n_in, T, min2, max2, zmin, zmax, scale, out, warp_cnt, 0, threadIdx.x >> 5,
-                                    threadIdx.x & 31);
-  if (threadIdx.x == 0) *out_n = n;
-}
-
-__global__ void __launch_bounds__(256)
-    projected_to_points_kernel(const float* __restrict__ ranges, const double2* __restrict__ unit, int n_beams, float rmin,
-                               double cutoff, const double* __restrict__ T, float min2, float max2, float zmin, float zmax,
-                               float scale, float2* __restrict__ out, int* __restrict__ out_n) {
-  __shared__ int warp_cnt[32];
-  double Tr[12];   // the transform read once (left to ptxas, the per-point reloads spill at its 32-register choice)
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int n;
+  if constexpr (KIND == HSB_IN_RANGES) {
+    n = stage_from_ranges<8>(in, C.beam_cs, n_in, C.range_min, C.range_max_c, C.scale_to_map, C.out_pts, warp_cnt, 0, w,
+                             lane);
+  } else if constexpr (KIND == HSB_IN_CLOUD) {
+    n = stage_from_cloud<8>(in, n_in, T, C.sqr_min_dist, C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map, C.out_pts,
+                            warp_cnt, 0, w, lane);
+  } else {
+    double Tr[12];   // the transform read once (left to ptxas, the per-point reloads spill at its 32-register choice)
 #pragma unroll
-  for (int k = 0; k < 12; ++k) Tr[k] = T[k];
-  const int n = stage_from_projected<8>(ranges, unit, n_beams, rmin, cutoff, Tr, min2, max2, zmin, zmax, scale, out,
-                                        warp_cnt, 0, threadIdx.x >> 5, threadIdx.x & 31);
-  if (threadIdx.x == 0) *out_n = n;
+    for (int k = 0; k < 12; ++k) Tr[k] = T[k];
+    n = stage_from_projected<8>(in, C.proj_unit, n_in, C.range_min, C.range_cutoff, Tr, C.sqr_min_dist, C.sqr_max_dist,
+                                C.z_min, C.z_max, C.scale_to_map, C.out_pts, warp_cnt, 0, w, lane);
+  }
+  if (threadIdx.x == 0) *C.out_n = n;
 }
 
 // N3: OccGridMapUtil::getLikelihoodForState (OccGridMapUtil.h:189-221) for one state (map coordinates of the level),
