@@ -38,7 +38,8 @@ EXPORTED = [
     "hsb_group_create", "hsb_group_destroy", "hsb_group_slam_update", "hsb_group_slam_update_cloud",
     "hsb_slam_update_ranges", "hsb_group_slam_update_ranges",
     "hsb_set_laser_projection", "hsb_projected_scan_to_points", "hsb_slam_update_projected",
-    "hsb_group_slam_update_projected",
+    "hsb_group_slam_update_projected", "hsb_match_batch_projected", "hsb_match_batch_projected_submit",
+    "hsb_match_batch_projected_device",
 ]
 
 
@@ -130,6 +131,9 @@ def load_library() -> C.CDLL:
     sig("hsb_set_laser_projection", i, vp, C.POINTER(HsbLaserProjection))
     sig("hsb_projected_scan_to_points", i, vp, vp, i, vp, vp, ip, vp)
     sig("hsb_slam_update_projected", i, vp, vp, vp, i, vp, i, i, vp, vp, vp, vp)
+    sig("hsb_match_batch_projected", i, vp, i, vp, vp, vp, vp, vp, vp)
+    sig("hsb_match_batch_projected_submit", i, vp, i, vp, vp, vp, vp, vp, vp, ip)
+    sig("hsb_match_batch_projected_device", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_get_last_map_update_pose", i, vp, vp)
     sig("hsb_set_last_map_update_pose", i, vp, vp)
     sig("hsb_upload_level", i, vp, i, vp)
@@ -678,6 +682,36 @@ class MapRepB200:
         self._check(self.lib.hsb_projected_scan_to_points(self.h, r.ctypes.data, r.size, _ptr(T), out.ctypes.data,
                                                           C.byref(n), origo.ctypes.data))
         return out[: n.value].copy(), origo
+
+    def match_batch_projected(self, hints, ranges, transforms=None, want_cov: bool = True):
+        """A default node's LaserScans matched in one batch: ranges (B, n_beams) float32, n_beams = the projection's;
+        transforms (B, 12) float64 or None (the cloud format's).  -> (poses (B, 3), cov (B, 3, 3) | None, origo (B, 2))"""
+        B = int(hints.shape[0])
+        if isinstance(hints, np.ndarray):
+            hints = _f32(hints).reshape(-1, 3)
+        if isinstance(ranges, np.ndarray):
+            ranges = _f32(ranges).reshape(B, -1) if B else _f32(ranges)
+        if transforms is not None:
+            transforms = np.ascontiguousarray(transforms, dtype=np.float64).reshape(B, 12)
+        poses = np.zeros((B, 3), np.float32)
+        cov = np.zeros((B, 9), np.float32) if want_cov else None
+        origo = np.zeros((B, 2), np.float32)
+        self._check(self.lib.hsb_match_batch_projected(self.h, B, _ptr(hints), _ptr(ranges), _ptr(transforms),
+                                                       poses.ctypes.data, _ptr(cov), origo.ctypes.data))
+        return poses, (cov.reshape(B, 3, 3) if want_cov else None), origo
+
+    def match_batch_projected_submit(self, hints, ranges, out_poses, out_cov=None, out_origo=None,
+                                     transforms=None) -> int:
+        t = C.c_int(-1)
+        self._check(self.lib.hsb_match_batch_projected_submit(self.h, int(hints.shape[0]), _ptr(hints), _ptr(ranges),
+                                                              _ptr(transforms), _ptr(out_poses), _ptr(out_cov),
+                                                              _ptr(out_origo), C.byref(t)))
+        return t.value
+
+    def match_batch_projected_device(self, B: int, d_hints: int, d_ranges: int, d_transforms: int | None,
+                                     d_out_poses: int, d_out_cov: int | None, d_out_origo: int | None, stream: int = 0):
+        self._check(self.lib.hsb_match_batch_projected_device(self.h, int(B), d_hints, d_ranges, d_transforms,
+                                                              d_out_poses, d_out_cov, d_out_origo, stream))
 
     def match_batch_cloud(self, hints, points_xyz, offsets, transforms=None, want_cov: bool = True):
         """-> (poses (B, 3), cov (B, 3, 3) | None, origo (B, 2))"""

@@ -426,6 +426,28 @@ int launch_match_mode(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t 
   return fail(h, HSB_ERR_INVALID_ARG, "unsupported tuning warps_per_scan=%d scans_per_block=%d unroll=%d", W, G, U);
 }
 
+// Projected input (HSB_IN_PROJECTED): the match kernels compiled with the projection (match_kernel PROJ).  They are the
+// shapes launch_match selects for a converted batch under the default tuning — W in {1, 2, 4, 8}, one scan per CTA (a
+// converted batch never takes the auto-group path), 4 gathers in flight, unpacked — so a projected batch matches in the
+// shape a cloud batch of the same size takes.  The entry points reject any other tuning before they queue anything
+// (check_projected_tuning); this is the launcher's own guard.
+int launch_match_projected(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int W, int G, int U) {
+  const bool tex = h->gather_mode == HSB_GATHER_TEX;
+  if (G == 1 && U == 4 && !(tex && h->tune_packed)) {
+#define HSB_PROJ_CASE(w)                                                                                     \
+  if (W == w)                                                                                                \
+    return tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, max_n, st, 1)      \
+               : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, false, true>(h, P, max_n, st, 1);
+    HSB_PROJ_CASE(1);
+    HSB_PROJ_CASE(2);
+    HSB_PROJ_CASE(4);
+    HSB_PROJ_CASE(8);
+#undef HSB_PROJ_CASE
+  }
+  return fail(h, HSB_ERR_UNSUPPORTED, "no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d unroll=%d",
+              W, G, U);
+}
+
 int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   if (h->map_write_pending && st != h->stream) {
     // hsb_slam_update_nowait left a map write running on the handle's stream: a match on another stream waits for it
@@ -462,6 +484,7 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
     }
   }
   int U = h->tune_unroll > 0 ? h->tune_unroll : 4;
+  if (P.kind == HSB_IN_PROJECTED) return launch_match_projected(h, P, max_n, st, W, G, U);
   if (h->gather_mode == HSB_GATHER_TEX) return launch_match_mode<hsb::MODE_TEX>(h, P, max_n, st, W, G, U, Gr);
   return launch_match_mode<hsb::MODE_LDG>(h, P, max_n, st, W, G, U, Gr);
 }
@@ -1149,6 +1172,35 @@ int check_input(const hsb_handle* h, hsb_handle* err, HsbInputKind kind, const c
   return HSB_OK;
 }
 
+// Whether h's tuning selects a match shape compiled with the projection (launch_match_projected): one scan per CTA,
+// 4 gathers in flight, unpacked, and 8 warps per scan (`single`: the single step's shape) or any of 1, 2, 4, 8 (a batch).
+// HSB_ERR_UNSUPPORTED naming the entry point `fn` otherwise.
+int check_projected_tuning(hsb_handle* h, const char* fn, bool single) {
+  const int W = h->tune_warps_per_scan;
+  const bool width = W == 0 || W == 8 || (!single && (W == 1 || W == 2 || W == 4));
+  if (width && h->tune_scans_per_block <= 1 && (h->tune_unroll == 0 || h->tune_unroll == 4) &&
+      !(h->gather_mode == HSB_GATHER_TEX && h->tune_packed))
+    return HSB_OK;
+  return fail(h, HSB_ERR_UNSUPPORTED,
+              "%s: no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d unroll=%d packed=%d", fn,
+              W, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
+}
+
+// Everything a projected batch call checks before it queues anything: the formats, the scan length and the tuning.
+int check_projected_batch(hsb_handle* h, const char* fn) {
+  int s = check_input(h, h, HSB_IN_PROJECTED, fn, -1, h->proj.n_beams, true);
+  if (s != HSB_OK) return s;
+  return check_projected_tuning(h, fn, false);
+}
+
+// The beam count of a fixed-length kind (ranges: the scan format's, projected: the laser projection's), 0 for the kinds
+// whose scans have their own lengths (endpoints, cloud).
+int fixed_beams(const hsb_handle* h, HsbInputKind kind) {
+  if (kind == HSB_IN_RANGES) return h->fmt.n_beams;
+  if (kind == HSB_IN_PROJECTED) return h->proj.n_beams;
+  return 0;
+}
+
 // The stand-alone conversion of n_in inputs of `kind` at d_in (laser transform d_T) into c's sink.
 int launch_conversion(hsb_handle* h, HsbInputKind kind, const float* d_in, int n_in, const double* d_T, const HsbConvDev& c,
                       cudaStream_t st) {
@@ -1262,9 +1314,33 @@ int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, con
   return launch_match(h, P, max_points_per_scan, (cudaStream_t)stream);
 }
 
+int hsb_match_batch_projected_device(hsb_handle* h, int B, const float* d_hints, const float* d_ranges,
+                                     const double* d_transforms, float* d_out_poses, float* d_out_cov, float* d_out_origo,
+                                     void* stream) {
+  if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
+  int s = check_projected_batch(h, "hsb_match_batch_projected_device");
+  if (s != HSB_OK) return s;
+  if (B == 0) return HSB_OK;
+  HandleScope guard(h);
+  HsbMatchParams P;
+  fill_match_params(h, P);
+  P.B = B;
+  P.hints = d_hints;
+  P.out_poses = d_out_poses;
+  P.out_cov = d_out_cov;
+  P.kind = HSB_IN_PROJECTED;
+  P.conv_in = d_ranges;
+  P.n_shared = h->proj.n_beams;   // scan b is d_ranges[b * n_beams ..]
+  P.cloud_tf = d_transforms;
+  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
+  P.out_origo = d_out_origo;
+  fill_conv(h, HSB_IN_PROJECTED, P.conv);
+  return launch_match(h, P, h->proj.n_beams, (cudaStream_t)stream);
+}
+
 }  // extern "C"
 
-// ---- host-buffer batch calls: one pipelined implementation for the three input formats -----------
+// ---- host-buffer batch calls: one pipelined implementation for the four input formats ------------
 // A call is cut into chunks (pipeline_bounds); chunk c's host->device copy runs on copy stream c%2 while chunk
 // c-1 is being matched, results stream back behind each kernel.  Two staging SETS of device buffers alternate
 // between calls, so that — with the submit / wait form — call k+1's first copies already travel while call k's
@@ -1276,10 +1352,10 @@ struct HostBatch {
   HsbInputKind kind = HSB_IN_ENDPOINTS;
   int B = 0;
   const float* hints = nullptr;
-  const float* in = nullptr;        // endpoints xy | ranges | cloud xyz
+  const float* in = nullptr;        // endpoints xy | ranges (ranges, projected) | cloud xyz
   const int* offsets = nullptr;     // endpoints (NULL = shared scan) | cloud
   int n_shared = 0;
-  const double* transforms = nullptr;
+  const double* transforms = nullptr;   // cloud, projected
   float* out_poses = nullptr;
   float* out_cov = nullptr;
   float* out_origo = nullptr;
@@ -1302,9 +1378,11 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
   if ((s = wait_set(h, si)) != HSB_OK) return s;   // the set is reused: its previous call must have delivered
   int max_n = 0;
   size_t in_bytes = 0, unit = 8;
-  if (hb.kind == HSB_IN_RANGES) {
-    max_n = h->fmt.n_beams;
-    in_bytes = (size_t)B * (size_t)h->fmt.n_beams * 4;
+  const int nb = fixed_beams(h, hb.kind);   // ranges / projected: scan b is in[b * nb .. (b + 1) * nb)
+  if (nb > 0) {
+    max_n = nb;
+    unit = 4;
+    in_bytes = (size_t)B * (size_t)nb * unit;
   } else {
     unit = hb.kind == HSB_IN_CLOUD ? 12 : 8;
     if (hb.offsets) {
@@ -1352,9 +1430,9 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
     cudaStream_t st = s1;
     if (!shared) {
       size_t p0, p1;
-      if (hb.kind == HSB_IN_RANGES) {
-        p0 = (size_t)b0 * h->fmt.n_beams * 4;
-        p1 = (size_t)b1 * h->fmt.n_beams * 4;
+      if (nb > 0) {
+        p0 = (size_t)b0 * nb * unit;
+        p1 = (size_t)b1 * nb * unit;
       } else {
         p0 = (size_t)hb.offsets[b0] * unit;
         p1 = (size_t)hb.offsets[b1] * unit;
@@ -1369,7 +1447,12 @@ int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
     float* o_cov = d_cov ? d_cov + 9 * (size_t)b0 : nullptr;
     if (hb.kind == HSB_IN_RANGES)
       s = hsb_match_batch_ranges_device(h, b1 - b0, d_hints + 3 * (size_t)b0,
-                                        reinterpret_cast<const float*>(d_in) + (size_t)b0 * h->fmt.n_beams, o_pose, o_cov, st);
+                                        reinterpret_cast<const float*>(d_in) + (size_t)b0 * nb, o_pose, o_cov, st);
+    else if (hb.kind == HSB_IN_PROJECTED)
+      s = hsb_match_batch_projected_device(h, b1 - b0, d_hints + 3 * (size_t)b0,
+                                           reinterpret_cast<const float*>(d_in) + (size_t)b0 * nb,
+                                           d_tf ? d_tf + 12 * (size_t)b0 : nullptr, o_pose, o_cov,
+                                           d_origo ? d_origo + 2 * (size_t)b0 : nullptr, st);
     else if (hb.kind == HSB_IN_CLOUD)
       s = hsb_match_batch_cloud_device(h, b1 - b0, d_hints + 3 * (size_t)b0, reinterpret_cast<const float*>(d_in), d_off + b0, max_n,
                                        d_tf ? d_tf + 12 * (size_t)b0 : nullptr, o_pose, o_cov,
@@ -1488,6 +1571,34 @@ int hsb_match_batch_cloud_submit(hsb_handle* h, int B, const float* hints, const
 int hsb_match_batch_cloud(hsb_handle* h, int B, const float* hints, const float* points_xyz, const int* offsets,
                           const double* transforms, float* out_poses, float* out_cov, float* out_origo) {
   return hsb_match_batch_cloud_submit(h, B, hints, points_xyz, offsets, transforms, out_poses, out_cov, out_origo, nullptr);
+}
+
+int hsb_match_batch_projected_submit(hsb_handle* h, int B, const float* hints, const float* ranges,
+                                     const double* transforms, float* out_poses, float* out_cov, float* out_origo,
+                                     int* ticket) {
+  int s = check_batch_args(h, B, hints, out_poses);
+  if (s != HSB_OK) return s;
+  if (!ranges) return HSB_ERR_INVALID_ARG;
+  if ((s = check_projected_batch(h, "hsb_match_batch_projected")) != HSB_OK) return s;
+  if (B == 0) {
+    if (ticket) *ticket = -1;
+    return HSB_OK;
+  }
+  HandleScope guard(h);
+  HostBatch hb;
+  hb.kind = HSB_IN_PROJECTED;
+  hb.B = B;
+  hb.hints = hints;
+  hb.in = ranges;
+  hb.transforms = transforms;
+  hb.out_poses = out_poses;
+  hb.out_cov = out_cov;
+  hb.out_origo = out_origo;
+  return run_host_batch(h, hb, ticket);
+}
+int hsb_match_batch_projected(hsb_handle* h, int B, const float* hints, const float* ranges, const double* transforms,
+                              float* out_poses, float* out_cov, float* out_origo) {
+  return hsb_match_batch_projected_submit(h, B, hints, ranges, transforms, out_poses, out_cov, out_origo, nullptr);
 }
 
 int hsb_match_batch_wait(hsb_handle* h, int ticket) {
@@ -1831,14 +1942,8 @@ static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& 
     P.gate_out_host = h->h_pin_dev + 8;
     P.seq_host = poll ? seq_dev : nullptr;
     P.seq_value = seq_value;
-    // (the projection is compiled into the single step's default shape only: hsb_slam_update_projected checked the tuning)
-    if (in.kind == HSB_IN_PROJECTED)
-      s = h->gather_mode == HSB_GATHER_TEX
-              ? launch_match_t<8, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, n, st, 1)
-              : launch_match_t<8, 1, hsb::MODE_LDG, 4, false, false, false, true>(h, P, n, st, 1);
-    else
-      s = launch_match(h, P, n, st);
-    if (s != HSB_OK) return s;
+    // (a projected step takes the single step's default shape: hsb_slam_update_projected checked the tuning)
+    if ((s = launch_match(h, P, n, st)) != HSB_OK) return s;
     h->last_n = n;   // upper bound until the kept count arrives (the writer reads the exact one on the device)
     h->last_origo[0] = origo[0];
     h->last_origo[1] = origo[1];
@@ -1897,12 +2002,7 @@ int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* r
   if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
   int s = check_input(h, h, HSB_IN_PROJECTED, "hsb_slam_update_projected", -1, n, true);
   if (s != HSB_OK) return s;
-  // the match shape hsb_slam_update_cloud would take under this tuning must be the one compiled with the projection
-  if (!((h->tune_warps_per_scan == 0 || h->tune_warps_per_scan == 8) && h->tune_scans_per_block <= 1 &&
-        (h->tune_unroll == 0 || h->tune_unroll == 4) && !(h->gather_mode == HSB_GATHER_TEX && h->tune_packed)))
-    return fail(h, HSB_ERR_UNSUPPORTED,
-                "hsb_slam_update_projected: no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d "
-                "unroll=%d packed=%d", h->tune_warps_per_scan, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
+  if ((s = check_projected_tuning(h, "hsb_slam_update_projected", true)) != HSB_OK) return s;
   const FusedScan in = {HSB_IN_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform};
   return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
 }

@@ -80,7 +80,7 @@ struct HsbMatchParams {
   // cloud_tf0
   const double* cloud_tf;
   double cloud_tf0[12];
-  float* out_origo;         // cloud: B x 2 (may be null): dataContainer origo = laser position * scaleToMap
+  float* out_origo;         // cloud and projected: B x 2 (may be null): dataContainer origo = laser position * scaleToMap
   // fused SLAM step (B == 1): the gate of HectorSlamProcessor::update evaluated in the kernel's epilogue
   float* gate_state;        // [0..2] lastMapUpdatePose, [3] flag out; nullptr = no gate
   const float* gate_in;     // minDist, minAngle, force

@@ -766,7 +766,8 @@ __device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, 
 
 // GRP: the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv.
 // PROJ: converted input is HSB_IN_PROJECTED (laser_geometry's projection and the cloud rule, stage_from_projected); only
-// the instantiations the projected SLAM steps launch carry that branch.
+// the instantiations the projected SLAM steps and batch matches launch carry that branch (hsb_api.cu
+// launch_match_projected).
 template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
 __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
@@ -856,19 +857,25 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
       const HsbConvDev& C = conv_desc<GRP>(P, scan);
       const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
+      // cloud and projected: dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
+      // (called inside both branches: after their join it would cost the unrelated instantiations a register)
+      const auto store_origo = [&] {
+        if (P.out_origo && t == 0) {
+          P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], C.scale_to_map);
+          P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], C.scale_to_map);
+        }
+      };
       if constexpr (PROJ) {   // raw ranges, projected to a cloud in the laser frame and converted by the cloud rule
         n = stage_from_projected<W>(P.conv_in + beg, C.proj_unit, n, C.range_min, C.range_cutoff, T, C.sqr_min_dist,
                                     C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map, spts, warp_cnt, g, w, lane);
+        store_origo();
       } else if (P.kind == HSB_IN_RANGES) {
         n = stage_from_ranges<W>(P.conv_in + beg, C.beam_cs, n, C.range_min, C.range_max_c, C.scale_to_map, spts,
                                  warp_cnt, g, w, lane);
       } else {          // a point cloud
         n = stage_from_cloud<W>(P.conv_in + 3 * beg, n, T, C.sqr_min_dist, C.sqr_max_dist, C.z_min, C.z_max,
                                 C.scale_to_map, spts, warp_cnt, g, w, lane);
-        if (P.out_origo && t == 0) {   // dataContainer.setOrigo(Vector2f(laserPos.x(), laserPos.y()) * scaleToMap)  (:516-517)
-          P.out_origo[2 * (size_t)scan] = __fmul_rn((float)T[3], C.scale_to_map);
-          P.out_origo[2 * (size_t)scan + 1] = __fmul_rn((float)T[7], C.scale_to_map);
-        }
+        store_origo();
       }
       if (C.out_pts) {
         // SLAM step: the endpoints and their number go to the map writer (and, matched, become the last-match

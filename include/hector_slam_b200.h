@@ -243,9 +243,27 @@ int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj);
  * HSB_ERR_UNSUPPORTED. */
 int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, const double* transform,
                                  float* out_points_xy, int* out_n, float out_origo[2]);
+/* hsb_match_batch with both conversions fused into the match kernel's staging step, for replaying or relocalising a
+ * default node's LaserScans: scan b is ranges[b*n_beams .. (b+1)*n_beams), n_beams = the laser projection's.
+ * `transforms` (B x 12 doubles, rows of [R | t], may be NULL) and out_origo (B x 2, may be NULL: each container's
+ * origo, laser position * scaleToMap) as in hsb_match_batch_cloud.  4 bytes per beam cross PCIe instead of 12 per
+ * projected point.  An all-dropped scan returns its hint and an all-zero covariance; the "last match" containers are not
+ * touched.  Each scan's pose, covariance and origo are bit-identical to hsb_match_batch_cloud on the cloud the
+ * restatement above projects from that scan, with the same transforms, in the same launch shape, and to
+ * hsb_match_batch on the endpoints hsb_projected_scan_to_points returns.  Rejected before anything is queued:
+ * HSB_ERR_INVALID_ARG for NULL pointers, B < 0 or a handle without hsb_set_laser_projection or hsb_set_cloud_format
+ * (the message names what is missing); HSB_ERR_UNSUPPORTED for a projection longer than the fused conversion can stage,
+ * and for a tuning that selects a match shape without the projection — the projection is compiled into the shapes a
+ * batch takes by default (1, 2, 4 or 8 warps per scan, one scan per CTA, 4 gathers in flight, unpacked).  B = 0 returns
+ * HSB_OK.  Host buffers (submit / wait form below) / device buffers + stream. */
+int hsb_match_batch_projected(hsb_handle* h, int B, const float* hints_world, const float* ranges,
+                              const double* transforms, float* out_poses_world, float* out_cov, float* out_origo);
+int hsb_match_batch_projected_device(hsb_handle* h, int B, const float* d_hints_world, const float* d_ranges,
+                                     const double* d_transforms, float* d_out_poses_world, float* d_out_cov,
+                                     float* d_out_origo, void* stream);
 
 /* ---- streams of batches: submit / wait ---------------------------------------------------------*/
-/* The three host-buffer batch calls above are `submit` followed by `wait`.  Used separately they let a caller keep
+/* The four host-buffer batch calls above are `submit` followed by `wait`.  Used separately they let a caller keep
  * the PCIe link busy across calls: the handle owns TWO sets of device staging buffers that alternate between calls,
  * so the copies of call k+1 travel while the last chunk of call k is still being matched.
  *   submit  queues the copies and kernels of one batch and returns a ticket (it blocks only while the staging set it
@@ -262,6 +280,9 @@ int hsb_match_batch_ranges_submit(hsb_handle* h, int B, const float* hints_world
 int hsb_match_batch_cloud_submit(hsb_handle* h, int B, const float* hints_world, const float* points_xyz, const int* offsets,
                                  const double* transforms, float* out_poses_world, float* out_cov, float* out_origo,
                                  int* ticket);
+int hsb_match_batch_projected_submit(hsb_handle* h, int B, const float* hints_world, const float* ranges,
+                                     const double* transforms, float* out_poses_world, float* out_cov,
+                                     float* out_origo, int* ticket);
 int hsb_match_batch_wait(hsb_handle* h, int ticket);
 /* Page-locked host memory for those buffers (cudaHostAlloc, allocated by the calling thread: bind the thread to the
  * GPU's NUMA node first if the host has several).  NULL on failure. */
