@@ -426,14 +426,20 @@ int launch_match_mode(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t 
   return fail(h, HSB_ERR_INVALID_ARG, "unsupported tuning warps_per_scan=%d scans_per_block=%d unroll=%d", W, G, U);
 }
 
-// Projected input (HSB_IN_PROJECTED): the match kernels compiled with the projection (match_kernel PROJ).  They are the
-// shapes launch_match selects for a converted batch under the default tuning — W in {1, 2, 4, 8}, one scan per CTA (a
-// converted batch never takes the auto-group path), 4 gathers in flight, unpacked — so a projected batch matches in the
-// shape a cloud batch of the same size takes.  The entry points reject any other tuning before they queue anything
-// (check_projected_tuning); this is the launcher's own guard.
+// Projected input (HSB_IN_PROJECTED): whether the match kernel is compiled with the projection (match_kernel PROJ) for
+// the launch shape W warps per scan, G scans per CTA, U gathers in flight.  The shapes are the ones launch_match selects
+// for a converted batch under the default tuning — W in {1, 2, 4, 8}, one scan per CTA (a converted batch never takes
+// the auto-group path), 4 gathers in flight, unpacked — so a projected batch matches in the shape a cloud batch of the
+// same size takes.
+bool has_projected_kernel(const hsb_handle* h, int W, int G, int U) {
+  return (W == 1 || W == 2 || W == 4 || W == 8) && G == 1 && U == 4 && !(h->gather_mode == HSB_GATHER_TEX && h->tune_packed);
+}
+
+// The entry points reject a tuning without a projected kernel before they queue anything (check_projected_tuning);
+// this is the launcher's own guard.
 int launch_match_projected(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int W, int G, int U) {
-  const bool tex = h->gather_mode == HSB_GATHER_TEX;
-  if (G == 1 && U == 4 && !(tex && h->tune_packed)) {
+  if (has_projected_kernel(h, W, G, U)) {
+    const bool tex = h->gather_mode == HSB_GATHER_TEX;
 #define HSB_PROJ_CASE(w)                                                                                     \
   if (W == w)                                                                                                \
     return tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, max_n, st, 1)      \
@@ -489,30 +495,29 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   return launch_match_mode<hsb::MODE_LDG>(h, P, max_n, st, W, G, U, Gr);
 }
 
-// Single-scan launch with the scan INSIDE the kernel parameters (hsb_match_data, hsb_slam_update; match_kernel.cuh
-// InlineScan): the shape a single scan always takes (8 warps, 4 gathers in flight), so results equal the copy path's.
+// Whether a single scan of n endpoints (hsb_match_data, hsb_slam_update) travels INSIDE the kernel parameters
+// (match_kernel.cuh InlineScan): tuning "inline_scan", and a tuning that leaves the single scan its usual shape.
 bool inline_scan_applies(const hsb_handle* h, int n) {
   return h->tune_inline_scan && n <= HSB_INLINE_MAX_POINTS && (h->tune_warps_per_scan == 0 || h->tune_warps_per_scan == 8) &&
          h->tune_scans_per_block <= 1 && (h->tune_unroll == 0 || h->tune_unroll == 4) && !h->tune_packed && h->tune_seq <= 1;
 }
-int launch_match_inline(hsb_handle* h, HsbMatchParams& P, const float* header, int nh, const float* pts, int n, float* d_pts_out,
-                        cudaStream_t st) {
+
+// The single-scan match of hsb_match_data and the SLAM steps on the handle's stream: P describes one scan of P.n_shared
+// inputs staged on the device.  With `inl` (inline_scan_applies) the host's header (nh floats) and endpoints are sent in
+// the kernel parameters instead, in the shape a single scan always takes (8 warps, 4 gathers in flight), so results
+// equal the staged path's; the kernel writes the endpoints to P.pts, where the map writer reads them.
+int launch_match_single(hsb_handle* h, HsbMatchParams& P, bool inl, const float* header, int nh, const float* pts) {
+  const int n = P.n_shared;
+  if (!inl) return launch_match(h, P, n, h->stream);
   hsb::InlineScan<true>& S = h->inline_scan;
   memset(S.header, 0, sizeof(S.header));
   if (nh > 0) memcpy(S.header, header, (size_t)nh * sizeof(float));
   if (n > 0) memcpy(S.pts, pts, (size_t)n * 8);
-  P.B = 1;
+  P.conv.out_pts = const_cast<float2*>(P.pts);
   P.hints = nullptr;
   P.pts = nullptr;
-  P.offsets = nullptr;
-  P.n_shared = n;
-  P.conv.out_pts = reinterpret_cast<float2*>(d_pts_out);
-  if (h->map_write_pending && st != h->stream) {
-    HSB_CUDA(h, cudaEventRecord(h->ev_sync[0], h->stream));
-    HSB_CUDA(h, cudaStreamWaitEvent(st, h->ev_sync[0], 0));
-  }
-  if (h->gather_mode == HSB_GATHER_TEX) return launch_match_t<8, 1, hsb::MODE_TEX, 4, false, true>(h, P, n, st, 1, S);
-  return launch_match_t<8, 1, hsb::MODE_LDG, 4, false, true>(h, P, n, st, 1, S);
+  if (h->gather_mode == HSB_GATHER_TEX) return launch_match_t<8, 1, hsb::MODE_TEX, 4, false, true>(h, P, n, h->stream, 1, S);
+  return launch_match_t<8, 1, hsb::MODE_LDG, 4, false, true>(h, P, n, h->stream, 1, S);
 }
 
 // Copy/compute pipeline of the host-buffer batch calls.  A call of >= 2048 scans travels in TWO halves: the second
@@ -905,59 +910,130 @@ int hsb_world_coords_pose(const hsb_handle* h, int level, const float map[3], fl
   return HSB_OK;
 }
 
+}  // extern "C"
+
 // ---- matching ----------------------------------------------------------------------------------
 
+namespace {
+
+// :493 maxRangeForContainer = range_max - 0.1, host fp32
+float range_max_c(const hsb_scan_format& f) {
+  volatile float mx = f.range_max - 0.1f;
+  return mx;
+}
+
+// projectLaser: a negative cutoff means the scan's range_max
+double projection_cutoff(const hsb_laser_projection& p) { return p.range_cutoff < 0.0 ? (double)p.range_max : p.range_cutoff; }
+
+// The container's origo of a cloud with laser transform T (HectorMappingRos.cpp:516-517):
+// Vector2f(laserPos.x(), laserPos.y()) * scaleToMap, host fp32 without contraction
+void cloud_origo(const hsb_handle* h, const double* T, float out[2]) {
+  volatile float ox = (float)T[3], oy = (float)T[7];
+  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
+  out[0] = sx;
+  out[1] = sy;
+}
+
+// How h converts a scan of `kind` (not endpoints) at call time; the sink is left null.
+void fill_conv(const hsb_handle* h, HsbInputKind kind, HsbConvDev& c) {
+  memset(&c, 0, sizeof(c));
+  c.scale_to_map = h->lv[0].scale;
+  if (kind == HSB_IN_RANGES) {
+    c.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
+    c.range_min = h->fmt.range_min;
+    c.range_max_c = range_max_c(h->fmt);
+    return;
+  }
+  c.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
+  c.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
+  c.z_min = h->cfmt.laser_z_min_value;
+  c.z_max = h->cfmt.laser_z_max_value;
+  if (kind == HSB_IN_PROJECTED) {
+    c.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
+    c.range_min = h->proj.range_min;
+    c.range_cutoff = projection_cutoff(h->proj);
+  }
+}
+
+// A scan, or a batch of scans, of one input kind.
+struct ScanIn {
+  HsbInputKind kind;
+  const float* in;        // endpoints: xy pairs; cloud: xyz triples; ranges / projected: one range per beam
+  const int* offsets;     // B + 1 bounds of the scans in `in`, in points (NULL: every scan has n_shared inputs)
+  int n_shared;
+  int max_n;              // the longest scan
+  const double* tf;       // cloud / projected: B x 12 laser transforms (NULL: the cloud format's)
+};
+
+// The match kernel's description of `sc` (device memory): the input, its layout and h's conversion of it.
+void fill_scan(const hsb_handle* h, const ScanIn& sc, HsbMatchParams& P) {
+  P.kind = sc.kind;
+  P.offsets = sc.offsets;
+  P.n_shared = sc.offsets ? 0 : sc.n_shared;
+  if (sc.kind == HSB_IN_ENDPOINTS) {
+    P.pts = reinterpret_cast<const float2*>(sc.in);
+    return;
+  }
+  P.conv_in = sc.in;
+  P.cloud_tf = sc.tf;
+  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
+  fill_conv(h, sc.kind, P.conv);
+}
+
 // R of HsbMatchParams::record: floats of one scan's per-evaluation record
-static int record_floats(const hsb_handle* h) {
+int record_floats(const hsb_handle* h) {
   int r = 0;
   for (int l = 0; l < h->levels; ++l) r += 3 + 15 * h->lv[l].evals;
   return r;
 }
 
-int hsb_get_match_record_floats(const hsb_handle* h) { return h ? record_floats(h) : HSB_ERR_INVALID_ARG; }
+// The batch match of every input kind on device buffers (the hsb_match_batch*_device calls, and each chunk of the
+// host-buffer calls): B scans `sc` with their hints; poses B x 3, covariances B x 9 (or NULL), origo B x 2 (cloud and
+// projected, or NULL), per-evaluation records B x R (or NULL).  The caller has checked the arguments.
+int match_batch(hsb_handle* h, int B, const float* hints, const ScanIn& sc, float* out_poses, float* out_cov,
+                float* out_origo, float* record, cudaStream_t st) {
+  HsbMatchParams P;
+  fill_match_params(h, P);
+  P.B = B;
+  P.hints = hints;
+  fill_scan(h, sc, P);
+  P.out_poses = out_poses;
+  P.out_cov = out_cov;
+  P.out_origo = out_origo;
+  P.record = record;
+  P.record_floats = record_floats(h);
+  return launch_match(h, P, std::max(sc.max_n, 0), st);
+}
 
-static int match_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets, int n_shared,
-                        int max_points_per_scan, float* d_out_poses, float* d_out_cov, float* gate_state, const float* gate_in,
-                        float* gate_out_host, cudaStream_t stream, unsigned* seq_host = nullptr, unsigned seq_value = 0,
-                        float* d_record = nullptr) {
+int match_endpoints_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets, int n_shared,
+                           int max_points_per_scan, float* d_out_poses, float* d_out_cov, float* d_record, void* stream) {
   if (!h || B < 0 || !d_hints || !d_out_poses) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   if (!d_offsets && n_shared < 0) return fail(h, HSB_ERR_INVALID_ARG, "shared-scan mode needs n_shared >= 0");
   if (!d_pts && (d_offsets || n_shared > 0)) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
   HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.pts = reinterpret_cast<const float2*>(d_pts);
-  P.offsets = d_offsets;
-  P.n_shared = d_offsets ? 0 : n_shared;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  P.gate_state = gate_state;   // fused SLAM step only (B == 1)
-  P.gate_in = gate_in;
-  P.gate_out_host = gate_out_host;
-  P.seq_host = seq_host;
-  P.seq_value = seq_value;
-  P.record = d_record;
-  P.record_floats = record_floats(h);
-  int max_n = d_offsets ? max_points_per_scan : n_shared;
-  if (max_n < 0) max_n = 0;
-  return launch_match(h, P, max_n, stream);
+  const ScanIn sc = {HSB_IN_ENDPOINTS, d_pts, d_offsets, n_shared, d_offsets ? max_points_per_scan : n_shared, nullptr};
+  return match_batch(h, B, d_hints, sc, d_out_poses, d_out_cov, nullptr, d_record, (cudaStream_t)stream);
 }
+
+}  // namespace
+
+extern "C" {
+
+int hsb_get_match_record_floats(const hsb_handle* h) { return h ? record_floats(h) : HSB_ERR_INVALID_ARG; }
 
 int hsb_match_batch_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets,
                            int n_shared, int max_points_per_scan, float* d_out_poses, float* d_out_cov, void* stream) {
-  return match_device(h, B, d_hints, d_pts, d_offsets, n_shared, max_points_per_scan, d_out_poses, d_out_cov, nullptr, nullptr,
-                      nullptr, (cudaStream_t)stream);
+  return match_endpoints_device(h, B, d_hints, d_pts, d_offsets, n_shared, max_points_per_scan, d_out_poses, d_out_cov,
+                                nullptr, stream);
 }
 
 int hsb_match_batch_record_device(hsb_handle* h, int B, const float* d_hints, const float* d_pts, const int* d_offsets,
                                   int n_shared, int max_points_per_scan, float* d_out_poses, float* d_out_cov, float* d_record,
                                   void* stream) {
   if (!d_record) return HSB_ERR_INVALID_ARG;
-  return match_device(h, B, d_hints, d_pts, d_offsets, n_shared, max_points_per_scan, d_out_poses, d_out_cov, nullptr, nullptr,
-                      nullptr, (cudaStream_t)stream, nullptr, 0, d_record);
+  return match_endpoints_device(h, B, d_hints, d_pts, d_offsets, n_shared, max_points_per_scan, d_out_poses, d_out_cov,
+                                d_record, stream);
 }
 
 static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2], float out_pose[3],
@@ -976,31 +1052,26 @@ static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts,
   // the kernel writes pose + Hessian straight into mapped host memory: no device-to-host copy operation on the
   // critical path (reading the scan from host memory the same way was slower than copying it)
   const bool host_out = h->tune_host_out != 0;
-  float* o_pose = host_out ? h->h_pin_dev + 4 : d_s + 4;
-  float* o_cov = host_out ? h->h_pin_dev + 8 : d_s + 8;
   const int R = record_floats(h);
   float* d_rec = nullptr;
   if (record_out) {
     if ((s = ensure(h, h->d_record, (size_t)R * sizeof(float))) != HSB_OK) return s;
     d_rec = static_cast<float*>(h->d_record.p);
   }
-  if (inline_scan_applies(h, n)) {
-    // ... and the scan goes in with the launch itself: no host-to-device copy operation either; the kernel leaves
-    // the endpoints in d_last_pts for hsb_update_by_scan's coarse levels
-    if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
-    HsbMatchParams P;
-    fill_match_params(h, P);
-    P.out_poses = o_pose;
-    P.out_cov = o_cov;
-    P.record = d_rec;
-    P.record_floats = R;
-    s = launch_match_inline(h, P, hint, 3, pts, n, scan_points(h->d_last_pts), st);
-  } else {
-    if ((s = upload_scan(h, h->d_last_pts, hint, 3, pts, n, st)) != HSB_OK) return s;   // header [0..2] = hint
-    s = match_device(h, 1, scan_header(h->d_last_pts), scan_points(h->d_last_pts), nullptr, n, n, o_pose, o_cov, nullptr,
-                     nullptr, nullptr, st, nullptr, 0, d_rec);
-  }
-  if (s != HSB_OK) return s;
+  // the scan goes into the container of the last match (header [0..2] = hint) — or in with the launch itself
+  // (inline_scan): no host-to-device copy operation either
+  const bool inl = inline_scan_applies(h, n);
+  if ((s = inl ? ensure_scan_buf(h, h->d_last_pts, n) : upload_scan(h, h->d_last_pts, hint, 3, pts, n, st)) != HSB_OK) return s;
+  HsbMatchParams P;
+  fill_match_params(h, P);
+  P.B = 1;
+  P.hints = scan_header(h->d_last_pts);
+  fill_scan(h, {HSB_IN_ENDPOINTS, scan_points(h->d_last_pts), nullptr, n, n, nullptr}, P);
+  P.out_poses = host_out ? h->h_pin_dev + 4 : d_s + 4;
+  P.out_cov = host_out ? h->h_pin_dev + 8 : d_s + 8;
+  P.record = d_rec;
+  P.record_floats = R;
+  if ((s = launch_match_single(h, P, inl, hint, 3, pts)) != HSB_OK) return s;
   if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 4, d_s + 4, 13 * sizeof(float), cudaMemcpyDeviceToHost, st));
   if (record_out) HSB_CUDA(h, cudaMemcpyAsync(record_out, d_rec, (size_t)R * sizeof(float), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
@@ -1109,45 +1180,6 @@ int hsb_set_laser_projection(hsb_handle* h, const hsb_laser_projection* proj) {
 
 namespace {
 
-// :493 maxRangeForContainer = range_max - 0.1, host fp32
-float range_max_c(const hsb_scan_format& f) {
-  volatile float mx = f.range_max - 0.1f;
-  return mx;
-}
-
-// projectLaser: a negative cutoff means the scan's range_max
-double projection_cutoff(const hsb_laser_projection& p) { return p.range_cutoff < 0.0 ? (double)p.range_max : p.range_cutoff; }
-
-// The container's origo of a cloud with laser transform T (HectorMappingRos.cpp:516-517):
-// Vector2f(laserPos.x(), laserPos.y()) * scaleToMap, host fp32 without contraction
-void cloud_origo(const hsb_handle* h, const double* T, float out[2]) {
-  volatile float ox = (float)T[3], oy = (float)T[7];
-  volatile float sx = ox * h->lv[0].scale, sy = oy * h->lv[0].scale;
-  out[0] = sx;
-  out[1] = sy;
-}
-
-// How h converts a scan of `kind` (not endpoints) at call time; the sink is left null.
-void fill_conv(const hsb_handle* h, HsbInputKind kind, HsbConvDev& c) {
-  memset(&c, 0, sizeof(c));
-  c.scale_to_map = h->lv[0].scale;
-  if (kind == HSB_IN_RANGES) {
-    c.beam_cs = static_cast<const float2*>(h->d_beam_cs.p);
-    c.range_min = h->fmt.range_min;
-    c.range_max_c = range_max_c(h->fmt);
-    return;
-  }
-  c.sqr_min_dist = h->cfmt.sqr_laser_min_dist;
-  c.sqr_max_dist = h->cfmt.sqr_laser_max_dist;
-  c.z_min = h->cfmt.laser_z_min_value;
-  c.z_max = h->cfmt.laser_z_max_value;
-  if (kind == HSB_IN_PROJECTED) {
-    c.proj_unit = static_cast<const double2*>(h->d_proj_unit.p);
-    c.range_min = h->proj.range_min;
-    c.range_cutoff = projection_cutoff(h->proj);
-  }
-}
-
 // Whether h can convert a scan of `kind` with n inputs: the formats the kind needs are set, a scan of ranges has the
 // format's beam count (n < 0: not checked) and, if `whole`, the scan fits the shared memory of the single step's match
 // shape.  The error goes to `err` and names the entry point `fn` and, if session >= 0, the group session.
@@ -1172,24 +1204,26 @@ int check_input(const hsb_handle* h, hsb_handle* err, HsbInputKind kind, const c
   return HSB_OK;
 }
 
-// Whether h's tuning selects a match shape compiled with the projection (launch_match_projected): one scan per CTA,
-// 4 gathers in flight, unpacked, and 8 warps per scan (`single`: the single step's shape) or any of 1, 2, 4, 8 (a batch).
-// HSB_ERR_UNSUPPORTED naming the entry point `fn` otherwise.
+// Whether h's tuning selects a match shape compiled with the projection (has_projected_kernel), with 8 warps per scan
+// for the single step (`single`).  HSB_ERR_UNSUPPORTED naming the entry point `fn` otherwise.
 int check_projected_tuning(hsb_handle* h, const char* fn, bool single) {
-  const int W = h->tune_warps_per_scan;
-  const bool width = W == 0 || W == 8 || (!single && (W == 1 || W == 2 || W == 4));
-  if (width && h->tune_scans_per_block <= 1 && (h->tune_unroll == 0 || h->tune_unroll == 4) &&
-      !(h->gather_mode == HSB_GATHER_TEX && h->tune_packed))
-    return HSB_OK;
+  // the shape launch_match picks: warps_per_scan = 0 picks 8 for a single scan and one of 1, 2, 4, 8 for a batch
+  const int W = h->tune_warps_per_scan == 0 ? 8 : h->tune_warps_per_scan;
+  const int G = h->tune_scans_per_block <= 1 ? 1 : h->tune_scans_per_block;
+  const int U = h->tune_unroll == 0 ? 4 : h->tune_unroll;
+  if (has_projected_kernel(h, W, G, U) && (!single || W == 8)) return HSB_OK;
   return fail(h, HSB_ERR_UNSUPPORTED,
               "%s: no projected-scan kernel for tuning warps_per_scan=%d scans_per_block=%d unroll=%d packed=%d", fn,
-              W, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
+              h->tune_warps_per_scan, h->tune_scans_per_block, h->tune_unroll, h->tune_packed);
 }
 
-// Everything a projected batch call checks before it queues anything: the formats, the scan length and the tuning.
-int check_projected_batch(hsb_handle* h, const char* fn) {
-  int s = check_input(h, h, HSB_IN_PROJECTED, fn, -1, h->proj.n_beams, true);
-  if (s != HSB_OK) return s;
+// Everything a batch call of `kind` checks on the handle before it queues anything: the formats the kind needs and,
+// for projected input, the scan length and the tuning.
+int check_batch_input(hsb_handle* h, HsbInputKind kind, const char* fn) {
+  if (kind == HSB_IN_ENDPOINTS) return HSB_OK;
+  const bool proj = kind == HSB_IN_PROJECTED;
+  int s = check_input(h, h, kind, fn, -1, proj ? h->proj.n_beams : -1, proj);
+  if (s != HSB_OK || !proj) return s;
   return check_projected_tuning(h, fn, false);
 }
 
@@ -1272,70 +1306,39 @@ int hsb_projected_scan_to_points(hsb_handle* h, const float* ranges, int n, cons
 int hsb_match_batch_ranges_device(hsb_handle* h, int B, const float* d_hints, const float* d_ranges, float* d_out_poses,
                                   float* d_out_cov, void* stream) {
   if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
-  int s = check_input(h, h, HSB_IN_RANGES, "hsb_match_batch_ranges_device", -1, -1, false);
+  int s = check_batch_input(h, HSB_IN_RANGES, "hsb_match_batch_ranges_device");
   if (s != HSB_OK) return s;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  P.kind = HSB_IN_RANGES;
-  P.conv_in = d_ranges;
-  P.n_shared = h->fmt.n_beams;   // scan b is d_ranges[b * n_beams ..]
-  fill_conv(h, HSB_IN_RANGES, P.conv);
-  return launch_match(h, P, h->fmt.n_beams, (cudaStream_t)stream);
+  const int nb = h->fmt.n_beams;   // scan b is d_ranges[b * n_beams ..]
+  return match_batch(h, B, d_hints, {HSB_IN_RANGES, d_ranges, nullptr, nb, nb, nullptr}, d_out_poses, d_out_cov, nullptr,
+                     nullptr, (cudaStream_t)stream);
 }
 
 int hsb_match_batch_cloud_device(hsb_handle* h, int B, const float* d_hints, const float* d_points_xyz, const int* d_offsets,
                                  int max_points_per_scan, const double* d_transforms, float* d_out_poses, float* d_out_cov,
                                  float* d_out_origo, void* stream) {
   if (!h || B < 0 || !d_hints || !d_offsets || !d_out_poses || max_points_per_scan < 0) return HSB_ERR_INVALID_ARG;
-  int s = check_input(h, h, HSB_IN_CLOUD, "hsb_match_batch_cloud_device", -1, -1, false);
+  int s = check_batch_input(h, HSB_IN_CLOUD, "hsb_match_batch_cloud_device");
   if (s != HSB_OK) return s;
   if (B == 0) return HSB_OK;
   if (!d_points_xyz && max_points_per_scan > 0) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
   HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  P.kind = HSB_IN_CLOUD;
-  P.conv_in = d_points_xyz;
-  P.offsets = d_offsets;
-  P.cloud_tf = d_transforms;
-  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
-  P.out_origo = d_out_origo;
-  fill_conv(h, HSB_IN_CLOUD, P.conv);
-  return launch_match(h, P, max_points_per_scan, (cudaStream_t)stream);
+  return match_batch(h, B, d_hints, {HSB_IN_CLOUD, d_points_xyz, d_offsets, 0, max_points_per_scan, d_transforms},
+                     d_out_poses, d_out_cov, d_out_origo, nullptr, (cudaStream_t)stream);
 }
 
 int hsb_match_batch_projected_device(hsb_handle* h, int B, const float* d_hints, const float* d_ranges,
                                      const double* d_transforms, float* d_out_poses, float* d_out_cov, float* d_out_origo,
                                      void* stream) {
   if (!h || B < 0 || !d_hints || !d_ranges || !d_out_poses) return HSB_ERR_INVALID_ARG;
-  int s = check_projected_batch(h, "hsb_match_batch_projected_device");
+  int s = check_batch_input(h, HSB_IN_PROJECTED, "hsb_match_batch_projected_device");
   if (s != HSB_OK) return s;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  HsbMatchParams P;
-  fill_match_params(h, P);
-  P.B = B;
-  P.hints = d_hints;
-  P.out_poses = d_out_poses;
-  P.out_cov = d_out_cov;
-  P.kind = HSB_IN_PROJECTED;
-  P.conv_in = d_ranges;
-  P.n_shared = h->proj.n_beams;   // scan b is d_ranges[b * n_beams ..]
-  P.cloud_tf = d_transforms;
-  memcpy(P.cloud_tf0, h->cfmt.laser_transform, sizeof(P.cloud_tf0));
-  P.out_origo = d_out_origo;
-  fill_conv(h, HSB_IN_PROJECTED, P.conv);
-  return launch_match(h, P, h->proj.n_beams, (cudaStream_t)stream);
+  const int nb = h->proj.n_beams;   // scan b is d_ranges[b * n_beams ..]
+  return match_batch(h, B, d_hints, {HSB_IN_PROJECTED, d_ranges, nullptr, nb, nb, d_transforms}, d_out_poses, d_out_cov,
+                     d_out_origo, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"
@@ -1348,19 +1351,6 @@ int hsb_match_batch_projected_device(hsb_handle* h, int B, const float* d_hints,
 // inputs, not by copy + the exposed tail kernel.  The blocking entry points are submit + wait.
 namespace {
 
-struct HostBatch {
-  HsbInputKind kind = HSB_IN_ENDPOINTS;
-  int B = 0;
-  const float* hints = nullptr;
-  const float* in = nullptr;        // endpoints xy | ranges (ranges, projected) | cloud xyz
-  const int* offsets = nullptr;     // endpoints (NULL = shared scan) | cloud
-  int n_shared = 0;
-  const double* transforms = nullptr;   // cloud, projected
-  float* out_poses = nullptr;
-  float* out_cov = nullptr;
-  float* out_origo = nullptr;
-};
-
 int wait_set(hsb_handle* h, int s) {
   BatchSet& S = h->bset[s];
   if (!S.busy) return HSB_OK;
@@ -1370,125 +1360,105 @@ int wait_set(hsb_handle* h, int s) {
   return HSB_OK;
 }
 
-int submit_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
-  const int B = hb.B;
+// The host-buffer batch call `fn` of every input kind: B scans `sc` (host memory; the longest is found here) with their
+// hints, results into host memory.  Everything that can reject the call is checked before anything is queued, and
+// B == 0 returns after the checks.  With a ticket the call returns once everything is queued (hsb_match_batch_wait),
+// without one it waits.
+int submit_batch(hsb_handle* h, const char* fn, int B, const float* hints, const ScanIn& sc, float* out_poses,
+                 float* out_cov, float* out_origo, int* ticket) {
+  if (!h || B < 0 || !hints || !out_poses) return HSB_ERR_INVALID_ARG;
+  // what a converted kind cannot do without: a cloud's offsets, the ranges
+  if (sc.kind != HSB_IN_ENDPOINTS && (sc.kind == HSB_IN_CLOUD ? !sc.offsets : !sc.in)) return HSB_ERR_INVALID_ARG;
+  int s = check_batch_input(h, sc.kind, fn);
+  if (s != HSB_OK) return s;
+  if (B == 0) {
+    if (ticket) *ticket = -1;
+    return HSB_OK;
+  }
+  if (!sc.offsets && sc.n_shared < 0) return fail(h, HSB_ERR_INVALID_ARG, "%s: shared-scan mode needs n_shared >= 0", fn);
+  HandleScope guard(h);
   const int si = h->next_set;
   BatchSet& S = h->bset[si];
-  int s;
   if ((s = wait_set(h, si)) != HSB_OK) return s;   // the set is reused: its previous call must have delivered
   int max_n = 0;
   size_t in_bytes = 0, unit = 8;
-  const int nb = fixed_beams(h, hb.kind);   // ranges / projected: scan b is in[b * nb .. (b + 1) * nb)
+  const int nb = fixed_beams(h, sc.kind);   // ranges / projected: scan b is in[b * nb .. (b + 1) * nb)
   if (nb > 0) {
     max_n = nb;
     unit = 4;
     in_bytes = (size_t)B * (size_t)nb * unit;
   } else {
-    unit = hb.kind == HSB_IN_CLOUD ? 12 : 8;
-    if (hb.offsets) {
+    unit = sc.kind == HSB_IN_CLOUD ? 12 : 8;
+    if (sc.offsets) {
       for (int b = 0; b < B; ++b) {
-        const int n = hb.offsets[b + 1] - hb.offsets[b];
+        const int n = sc.offsets[b + 1] - sc.offsets[b];
         if (n < 0) return fail(h, HSB_ERR_INVALID_ARG, "offsets must be non-decreasing");
         max_n = std::max(max_n, n);
       }
-      in_bytes = (size_t)hb.offsets[B] * unit;
+      in_bytes = (size_t)sc.offsets[B] * unit;
     } else {
-      max_n = hb.n_shared > 0 ? hb.n_shared : 0;
+      max_n = sc.n_shared > 0 ? sc.n_shared : 0;
       in_bytes = (size_t)max_n * unit;
     }
-    if (in_bytes > 0 && !hb.in) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
+    if (in_bytes > 0 && !sc.in) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
   }
   if ((s = ensure(h, S.hints, (size_t)B * 12)) != HSB_OK) return s;
   if ((s = ensure(h, S.in, in_bytes + 16)) != HSB_OK) return s;
   if ((s = ensure(h, S.offsets, (size_t)(B + 1) * 4)) != HSB_OK) return s;
   if ((s = ensure(h, S.poses, (size_t)B * 12)) != HSB_OK) return s;
-  if (hb.out_cov && (s = ensure(h, S.cov, (size_t)B * 36)) != HSB_OK) return s;
-  if (hb.out_origo && (s = ensure(h, S.origo, (size_t)B * 8)) != HSB_OK) return s;
-  if (hb.transforms && (s = ensure(h, S.tf, (size_t)B * 12 * sizeof(double))) != HSB_OK) return s;
+  if (out_cov && (s = ensure(h, S.cov, (size_t)B * 36)) != HSB_OK) return s;
+  if (out_origo && (s = ensure(h, S.origo, (size_t)B * 8)) != HSB_OK) return s;
+  if (sc.tf && (s = ensure(h, S.tf, (size_t)B * 12 * sizeof(double))) != HSB_OK) return s;
   float* d_hints = static_cast<float*>(S.hints.p);
   char* d_in = static_cast<char*>(S.in.p);
   int* d_off = static_cast<int*>(S.offsets.p);
   float* d_poses = static_cast<float*>(S.poses.p);
-  float* d_cov = hb.out_cov ? static_cast<float*>(S.cov.p) : nullptr;
-  float* d_origo = hb.out_origo ? static_cast<float*>(S.origo.p) : nullptr;
-  double* d_tf = hb.transforms ? static_cast<double*>(S.tf.p) : nullptr;
+  float* d_cov = out_cov ? static_cast<float*>(S.cov.p) : nullptr;
+  float* d_origo = out_origo ? static_cast<float*>(S.origo.p) : nullptr;
+  double* d_tf = sc.tf ? static_cast<double*>(S.tf.p) : nullptr;
 
   std::vector<int> bounds = pipeline_bounds(B, h->tune_chunk);
-  const bool shared = hb.kind == HSB_IN_ENDPOINTS && !hb.offsets;
+  const bool shared = sc.kind == HSB_IN_ENDPOINTS && !sc.offsets;
   if (shared) bounds = std::vector<int>{0, B};   // one shared scan: nothing big to overlap
   ShapeScope shape_scope(h, B, bounds.size() - 1);
   // Stream roles: copy_stream[0] carries ALL host->device copies of all calls back to back, copy_stream[1] the kernels
   // and the result copies; a chunk's kernel waits for its copy through an event, so the copy engine never queues behind
   // a kernel.
   cudaStream_t s0 = h->copy_stream[0], s1 = h->copy_stream[1];
-  if (hb.offsets) HSB_CUDA(h, cudaMemcpyAsync(d_off, hb.offsets, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, s0));
-  if (shared && in_bytes > 0) HSB_CUDA(h, cudaMemcpyAsync(d_in, hb.in, in_bytes, cudaMemcpyHostToDevice, s0));
-  HSB_CUDA(h, cudaMemcpyAsync(d_hints, hb.hints, (size_t)B * 12, cudaMemcpyHostToDevice, s0));
-  if (d_tf) HSB_CUDA(h, cudaMemcpyAsync(d_tf, hb.transforms, (size_t)B * 12 * sizeof(double), cudaMemcpyHostToDevice, s0));
+  if (sc.offsets) HSB_CUDA(h, cudaMemcpyAsync(d_off, sc.offsets, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, s0));
+  if (shared && in_bytes > 0) HSB_CUDA(h, cudaMemcpyAsync(d_in, sc.in, in_bytes, cudaMemcpyHostToDevice, s0));
+  HSB_CUDA(h, cudaMemcpyAsync(d_hints, hints, (size_t)B * 12, cudaMemcpyHostToDevice, s0));
+  if (d_tf) HSB_CUDA(h, cudaMemcpyAsync(d_tf, sc.tf, (size_t)B * 12 * sizeof(double), cudaMemcpyHostToDevice, s0));
   for (size_t ci = 0; ci + 1 < bounds.size(); ++ci) {
     const int b0 = bounds[ci], b1 = bounds[ci + 1];
-    cudaStream_t st = s1;
     if (!shared) {
-      size_t p0, p1;
-      if (nb > 0) {
-        p0 = (size_t)b0 * nb * unit;
-        p1 = (size_t)b1 * nb * unit;
-      } else {
-        p0 = (size_t)hb.offsets[b0] * unit;
-        p1 = (size_t)hb.offsets[b1] * unit;
-      }
+      const size_t p0 = (nb > 0 ? (size_t)b0 * nb : (size_t)sc.offsets[b0]) * unit;
+      const size_t p1 = (nb > 0 ? (size_t)b1 * nb : (size_t)sc.offsets[b1]) * unit;
       if (p1 > p0)
-        HSB_CUDA(h, cudaMemcpyAsync(d_in + p0, reinterpret_cast<const char*>(hb.in) + p0, p1 - p0, cudaMemcpyHostToDevice, s0));
+        HSB_CUDA(h, cudaMemcpyAsync(d_in + p0, reinterpret_cast<const char*>(sc.in) + p0, p1 - p0, cudaMemcpyHostToDevice, s0));
     }
     cudaEvent_t ready = S.chunk_ready[ci < 8 ? ci : 7];
     HSB_CUDA(h, cudaEventRecord(ready, s0));           // hints / offsets / this chunk's input are on the device
     HSB_CUDA(h, cudaStreamWaitEvent(s1, ready, 0));
+    // the chunk's scans on the device (offsets index the whole input, fixed-length scans start at the chunk's first)
+    const ScanIn chunk = {sc.kind, reinterpret_cast<const float*>(d_in) + (size_t)b0 * nb, sc.offsets ? d_off + b0 : nullptr,
+                          nb > 0 ? nb : sc.n_shared, max_n, d_tf ? d_tf + 12 * (size_t)b0 : nullptr};
     float* o_pose = d_poses + 3 * (size_t)b0;
     float* o_cov = d_cov ? d_cov + 9 * (size_t)b0 : nullptr;
-    if (hb.kind == HSB_IN_RANGES)
-      s = hsb_match_batch_ranges_device(h, b1 - b0, d_hints + 3 * (size_t)b0,
-                                        reinterpret_cast<const float*>(d_in) + (size_t)b0 * nb, o_pose, o_cov, st);
-    else if (hb.kind == HSB_IN_PROJECTED)
-      s = hsb_match_batch_projected_device(h, b1 - b0, d_hints + 3 * (size_t)b0,
-                                           reinterpret_cast<const float*>(d_in) + (size_t)b0 * nb,
-                                           d_tf ? d_tf + 12 * (size_t)b0 : nullptr, o_pose, o_cov,
-                                           d_origo ? d_origo + 2 * (size_t)b0 : nullptr, st);
-    else if (hb.kind == HSB_IN_CLOUD)
-      s = hsb_match_batch_cloud_device(h, b1 - b0, d_hints + 3 * (size_t)b0, reinterpret_cast<const float*>(d_in), d_off + b0, max_n,
-                                       d_tf ? d_tf + 12 * (size_t)b0 : nullptr, o_pose, o_cov,
-                                       d_origo ? d_origo + 2 * (size_t)b0 : nullptr, st);
-    else
-      s = hsb_match_batch_device(h, b1 - b0, d_hints + 3 * (size_t)b0, reinterpret_cast<const float*>(d_in),
-                                 hb.offsets ? d_off + b0 : nullptr, hb.n_shared, max_n, o_pose, o_cov, st);
-    if (s != HSB_OK) return s;
-    HSB_CUDA(h, cudaMemcpyAsync(hb.out_poses + 3 * (size_t)b0, o_pose, (size_t)(b1 - b0) * 12, cudaMemcpyDeviceToHost, st));
-    if (hb.out_cov)
-      HSB_CUDA(h, cudaMemcpyAsync(hb.out_cov + 9 * (size_t)b0, o_cov, (size_t)(b1 - b0) * 36, cudaMemcpyDeviceToHost, st));
-    if (hb.out_origo)
-      HSB_CUDA(h, cudaMemcpyAsync(hb.out_origo + 2 * (size_t)b0, d_origo + 2 * (size_t)b0, (size_t)(b1 - b0) * 8,
-                                  cudaMemcpyDeviceToHost, st));
+    float* o_origo = d_origo ? d_origo + 2 * (size_t)b0 : nullptr;
+    if ((s = match_batch(h, b1 - b0, d_hints + 3 * (size_t)b0, chunk, o_pose, o_cov, o_origo, nullptr, s1)) != HSB_OK) return s;
+    HSB_CUDA(h, cudaMemcpyAsync(out_poses + 3 * (size_t)b0, o_pose, (size_t)(b1 - b0) * 12, cudaMemcpyDeviceToHost, s1));
+    if (out_cov)
+      HSB_CUDA(h, cudaMemcpyAsync(out_cov + 9 * (size_t)b0, o_cov, (size_t)(b1 - b0) * 36, cudaMemcpyDeviceToHost, s1));
+    if (out_origo)
+      HSB_CUDA(h, cudaMemcpyAsync(out_origo + 2 * (size_t)b0, o_origo, (size_t)(b1 - b0) * 8, cudaMemcpyDeviceToHost, s1));
   }
   HSB_CUDA(h, cudaEventRecord(S.done[0], h->copy_stream[0]));
   HSB_CUDA(h, cudaEventRecord(S.done[1], h->copy_stream[1]));
   S.busy = true;
   h->next_set = si ^ 1;
-  if (ticket) *ticket = si;
-  return HSB_OK;
-}
-
-int run_host_batch(hsb_handle* h, const HostBatch& hb, int* ticket) {
-  int t = 0;
-  int s = submit_host_batch(h, hb, &t);
-  if (s != HSB_OK) return s;
-  if (ticket) {
-    *ticket = t;
-    return HSB_OK;
-  }
-  return wait_set(h, t);
-}
-
-int check_batch_args(hsb_handle* h, int B, const float* hints, float* out_poses) {
-  if (!h || B < 0 || !hints || !out_poses) return HSB_ERR_INVALID_ARG;
+  if (!ticket) return wait_set(h, si);
+  *ticket = si;
   return HSB_OK;
 }
 
@@ -1498,23 +1468,8 @@ extern "C" {
 
 int hsb_match_batch_submit(hsb_handle* h, int B, const float* hints, const float* pts, const int* offsets, int n_shared,
                            float* out_poses, float* out_cov, int* ticket) {
-  int s = check_batch_args(h, B, hints, out_poses);
-  if (s != HSB_OK) return s;
-  if (B == 0) {
-    if (ticket) *ticket = -1;
-    return HSB_OK;
-  }
-  HandleScope guard(h);
-  HostBatch hb;
-  hb.kind = HSB_IN_ENDPOINTS;
-  hb.B = B;
-  hb.hints = hints;
-  hb.in = pts;
-  hb.offsets = offsets;
-  hb.n_shared = n_shared;
-  hb.out_poses = out_poses;
-  hb.out_cov = out_cov;
-  return run_host_batch(h, hb, ticket);
+  return submit_batch(h, "hsb_match_batch", B, hints, {HSB_IN_ENDPOINTS, pts, offsets, n_shared, 0, nullptr}, out_poses,
+                      out_cov, nullptr, ticket);
 }
 int hsb_match_batch(hsb_handle* h, int B, const float* hints, const float* pts, const int* offsets, int n_shared,
                     float* out_poses, float* out_cov) {
@@ -1523,23 +1478,8 @@ int hsb_match_batch(hsb_handle* h, int B, const float* hints, const float* pts, 
 
 int hsb_match_batch_ranges_submit(hsb_handle* h, int B, const float* hints, const float* ranges, float* out_poses,
                                   float* out_cov, int* ticket) {
-  int s = check_batch_args(h, B, hints, out_poses);
-  if (s != HSB_OK) return s;
-  if (!ranges) return HSB_ERR_INVALID_ARG;
-  if ((s = check_input(h, h, HSB_IN_RANGES, "hsb_match_batch_ranges", -1, -1, false)) != HSB_OK) return s;
-  if (B == 0) {
-    if (ticket) *ticket = -1;
-    return HSB_OK;
-  }
-  HandleScope guard(h);
-  HostBatch hb;
-  hb.kind = HSB_IN_RANGES;
-  hb.B = B;
-  hb.hints = hints;
-  hb.in = ranges;
-  hb.out_poses = out_poses;
-  hb.out_cov = out_cov;
-  return run_host_batch(h, hb, ticket);
+  return submit_batch(h, "hsb_match_batch_ranges", B, hints, {HSB_IN_RANGES, ranges, nullptr, 0, 0, nullptr}, out_poses,
+                      out_cov, nullptr, ticket);
 }
 int hsb_match_batch_ranges(hsb_handle* h, int B, const float* hints, const float* ranges, float* out_poses, float* out_cov) {
   return hsb_match_batch_ranges_submit(h, B, hints, ranges, out_poses, out_cov, nullptr);
@@ -1547,26 +1487,8 @@ int hsb_match_batch_ranges(hsb_handle* h, int B, const float* hints, const float
 
 int hsb_match_batch_cloud_submit(hsb_handle* h, int B, const float* hints, const float* points_xyz, const int* offsets,
                                  const double* transforms, float* out_poses, float* out_cov, float* out_origo, int* ticket) {
-  int s = check_batch_args(h, B, hints, out_poses);
-  if (s != HSB_OK) return s;
-  if (!offsets) return HSB_ERR_INVALID_ARG;
-  if ((s = check_input(h, h, HSB_IN_CLOUD, "hsb_match_batch_cloud", -1, -1, false)) != HSB_OK) return s;
-  if (B == 0) {
-    if (ticket) *ticket = -1;
-    return HSB_OK;
-  }
-  HandleScope guard(h);
-  HostBatch hb;
-  hb.kind = HSB_IN_CLOUD;
-  hb.B = B;
-  hb.hints = hints;
-  hb.in = points_xyz;
-  hb.offsets = offsets;
-  hb.transforms = transforms;
-  hb.out_poses = out_poses;
-  hb.out_cov = out_cov;
-  hb.out_origo = out_origo;
-  return run_host_batch(h, hb, ticket);
+  return submit_batch(h, "hsb_match_batch_cloud", B, hints, {HSB_IN_CLOUD, points_xyz, offsets, 0, 0, transforms},
+                      out_poses, out_cov, out_origo, ticket);
 }
 int hsb_match_batch_cloud(hsb_handle* h, int B, const float* hints, const float* points_xyz, const int* offsets,
                           const double* transforms, float* out_poses, float* out_cov, float* out_origo) {
@@ -1576,25 +1498,8 @@ int hsb_match_batch_cloud(hsb_handle* h, int B, const float* hints, const float*
 int hsb_match_batch_projected_submit(hsb_handle* h, int B, const float* hints, const float* ranges,
                                      const double* transforms, float* out_poses, float* out_cov, float* out_origo,
                                      int* ticket) {
-  int s = check_batch_args(h, B, hints, out_poses);
-  if (s != HSB_OK) return s;
-  if (!ranges) return HSB_ERR_INVALID_ARG;
-  if ((s = check_projected_batch(h, "hsb_match_batch_projected")) != HSB_OK) return s;
-  if (B == 0) {
-    if (ticket) *ticket = -1;
-    return HSB_OK;
-  }
-  HandleScope guard(h);
-  HostBatch hb;
-  hb.kind = HSB_IN_PROJECTED;
-  hb.B = B;
-  hb.hints = hints;
-  hb.in = ranges;
-  hb.transforms = transforms;
-  hb.out_poses = out_poses;
-  hb.out_cov = out_cov;
-  hb.out_origo = out_origo;
-  return run_host_batch(h, hb, ticket);
+  return submit_batch(h, "hsb_match_batch_projected", B, hints, {HSB_IN_PROJECTED, ranges, nullptr, 0, 0, transforms},
+                      out_poses, out_cov, out_origo, ticket);
 }
 int hsb_match_batch_projected(hsb_handle* h, int B, const float* hints, const float* ranges, const double* transforms,
                               float* out_poses, float* out_cov, float* out_origo) {
@@ -1720,10 +1625,43 @@ static void fill_update_level(hsb_handle* h, int l, HsbUpdateLevelDev& d) {
   d.slot = L.parity;
 }
 
-// MapRepMultiMap::updateByScan (MapRepMultiMap.h:134-147) as launches on h->stream; level 0 reads `d_pts0`,
-// the coarse levels the container the last matchData left behind (:143).  pose_dev / gate_flag: see HsbUpdateParams.
-static int enqueue_update_by_scan(hsb_handle* h, const float2* d_pts0, int n, const float origo[2], const float pose[3],
-                                  const float* pose_dev, const float* gate_flag, const int* n_dev = nullptr) {
+// MapRepMultiMap::updateByScan (MapRepMultiMap.h:134-147) for one scan of h: its map-writer level descriptors
+// d[0 .. levels).  Level 0 reads this scan (`pts`, n; converted input: the kept count the device holds at n_dev, n is an
+// upper bound); the coarse levels read it too if it has just become the last match's container (`matched`), and
+// otherwise the container the last matchData left behind (:143).  Advances the stamp bases (a wrap clears the stamps on
+// `st`) and writer slots of the active levels, and raises *max_n to the longest active scan.
+static int fill_update_levels(hsb_handle* h, HsbUpdateLevelDev* d, const float2* pts, int n, const int* n_dev,
+                              const float origo[2], bool matched, cudaStream_t st, int* max_n) {
+  for (int l = 0; l < h->levels; ++l) {
+    fill_update_level(h, l, d[l]);
+    d[l].pt_scale = (float)(1.0 / pow(2.0, (double)l));
+    if (l == 0 || matched) {
+      d[l].pts = pts;
+      d[l].n = n;
+      d[l].n_dev = n_dev;
+      d[l].origo_x = origo ? origo[0] : 0.f;
+      d[l].origo_y = origo ? origo[1] : 0.f;
+    } else {
+      d[l].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+      d[l].n = h->last_n;
+      d[l].origo_x = h->last_origo[0];
+      d[l].origo_y = h->last_origo[1];
+    }
+    // an empty container still advances the stamps in the reference (OccGridMapBase.h:164-167); no-op here
+    d[l].active = d[l].n > 0;
+    if (d[l].active) {
+      const int s = next_stamp_base(h, l, &d[l].stamp_base, st);
+      if (s != HSB_OK) return s;
+      *max_n = std::max(*max_n, d[l].n);
+    }
+  }
+  return HSB_OK;
+}
+
+// The map write of hsb_update_by_scan and the single SLAM steps (fill_update_levels) as launches on h->stream.
+// pose_dev / gate_flag: see HsbUpdateParams.
+static int enqueue_update_by_scan(hsb_handle* h, const float2* pts, int n, const int* n_dev, const float origo[2],
+                                  bool matched, const float pose[3], const float* pose_dev, const float* gate_flag) {
   HsbUpdateParams P;
   memset(&P, 0, sizeof(P));
   P.levels = h->levels;
@@ -1732,31 +1670,9 @@ static int enqueue_update_by_scan(hsb_handle* h, const float2* d_pts0, int n, co
   P.gate_flag = gate_flag;
   P.log_odds_free = h->log_odds_free;
   P.log_odds_occ = h->log_odds_occ;
-  int max_n = 0, s;
-  for (int l = 0; l < h->levels; ++l) {
-    HsbUpdateLevelDev& d = P.lv[l];
-    fill_update_level(h, l, d);
-    d.pt_scale = (float)(1.0 / pow(2.0, (double)l));
-    if (l == 0) {  // MapRepMultiMap.h:140-141
-      d.pts = d_pts0;
-      d.n = n;
-      d.n_dev = n_dev;   // fused point-cloud step: `n` is the cloud's size, the kept endpoints are counted on the device
-      d.origo_x = origo ? origo[0] : 0.f;
-      d.origo_y = origo ? origo[1] : 0.f;
-    } else {  // :143 — the container left behind by the last matchData
-      d.pts = reinterpret_cast<const float2*>(scan_points(h->d_last_pts));
-      d.n = h->last_n;
-      d.n_dev = (n_dev && d.pts == d_pts0) ? n_dev : nullptr;   // ... which is this very scan when the step matched it
-      d.origo_x = h->last_origo[0];
-      d.origo_y = h->last_origo[1];
-    }
-    // an empty container still advances the stamps in the reference (OccGridMapBase.h:164-167); no-op here
-    d.active = d.n > 0;
-    if (d.active) {
-      if ((s = next_stamp_base(h, l, &d.stamp_base, h->stream)) != HSB_OK) return s;
-      if (d.n > max_n) max_n = d.n;
-    }
-  }
+  int max_n = 0;
+  const int s = fill_update_levels(h, P.lv, pts, n, n_dev, origo, matched, h->stream, &max_n);
+  if (s != HSB_OK) return s;
   return run_update(h, P, max_n);
 }
 
@@ -1766,7 +1682,8 @@ int hsb_update_by_scan(hsb_handle* h, const float* pts, int n, const float origo
   int s;
   cudaStream_t st = h->stream;
   if ((s = upload_scan(h, h->d_upd_pts, nullptr, 0, pts, n, st)) != HSB_OK) return s;
-  if ((s = enqueue_update_by_scan(h, reinterpret_cast<const float2*>(scan_points(h->d_upd_pts)), n, origo, pose, nullptr, nullptr)) != HSB_OK)
+  if ((s = enqueue_update_by_scan(h, reinterpret_cast<const float2*>(scan_points(h->d_upd_pts)), n, nullptr, origo, false,
+                                  pose, nullptr, nullptr)) != HSB_OK)
     return s;
   HSB_CUDA(h, cudaStreamSynchronize(st));
   return HSB_OK;
@@ -1783,63 +1700,118 @@ int hsb_set_map_update_min_angle_diff(hsb_handle* h, float min_angle) {
   return HSB_OK;
 }
 
-static int slam_update_impl(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
-                            int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated, bool wait_map) {
-  if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
+// HectorSlamProcessor::update (HectorSlamProcessor.h:71-113) for one scan `in` (host memory, n_shared inputs) of any
+// kind, after the node's conversion for converted input (HectorMappingRos::scanCallback :297): match with the gate in
+// its epilogue, then the map write, behind ONE host-to-device copy.  Converted input is converted by the match kernel's
+// staging step, which also writes the endpoints out for the map writer and leaves their number on the device (the
+// writer reads it there), so no host round trip appears between conversion, match, gate and map write.  origo: the
+// endpoints' container origo (NULL = 0, 0); a converted scan's follows from its laser transform.  nowait: return when
+// the pose has arrived, the map write continues on the handle's stream.
+static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const float origo_in[2], int map_without_matching,
+                     bool nowait, float out_pose[3], float cov_inout[9], int* map_updated, int* out_kept) {
   HandleScope guard(h);
   int s;
+  const int n = in.n_shared;   // converted: a cloud's points or a scan's beams, an upper bound of the endpoints kept
+  const bool conv = in.kind != HSB_IN_ENDPOINTS;
   if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
-  // scan header: [0..2] hint, [3..5] minDist / minAngle / force; scratch: [8..10] pose, [11] flag, [12..20] cov
+  // scratch: [8..10] pose, [11] flag, [12..20] cov, [40] the kept-endpoint count of converted input
   float* d_s = static_cast<float*>(h->d_scratch.p);
   float* d_gate = static_cast<float*>(h->d_gate.p);
+  int* n_dev = conv ? reinterpret_cast<int*>(d_s + 40) : nullptr;
   cudaStream_t st = h->stream;
+  // results (pose, flag, Hessian, kept count) are written into mapped host memory by the kernels themselves: the step
+  // is one host-to-device copy and three launches (match with the gate in its epilogue, mark, apply — the latter two
+  // with programmatic dependent launch).  Endpoint steps only: tuning host_out = 0 copies them back instead.
+  const bool host_out = conv || h->tune_host_out != 0;
+  const bool poll = host_out && nowait;   // return when the pose has arrived; the map write continues on the stream
+  volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
+  unsigned* seq_dev = reinterpret_cast<unsigned*>(h->h_pin_dev + 22);
+  const unsigned seq_value = ++h->step_seq;
+  int* kept_host = reinterpret_cast<int*>(h->h_pin + 24);
+  int* kept_dev = reinterpret_cast<int*>(h->h_pin_dev + 24);
   // without matching the reference leaves the coarse containers alone (HectorSlamProcessor.h:77-81,
   // MapRepMultiMap.h:143): only level 0 sees this scan
   DevBuf& pbuf = map_without_matching ? h->d_upd_pts : h->d_last_pts;
   const float header[6] = {hint[0], hint[1], hint[2], h->min_dist, h->min_angle, map_without_matching ? 1.f : 0.f};
-  // results (pose, flag, Hessian) are written into mapped host memory by the kernels themselves: the step is one
-  // host-to-device copy and three launches (match with the gate in its epilogue, mark, apply — the latter two with
-  // programmatic dependent launch)
-  const bool host_out = h->tune_host_out != 0;
-  const bool poll = host_out && !wait_map;   // return when the pose has arrived; the map write continues on the stream
-  volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
-  unsigned* seq_dev = reinterpret_cast<unsigned*>(h->h_pin_dev + 22);
-  const unsigned seq_value = ++h->step_seq;
-  const bool inl = !map_without_matching && inline_scan_applies(h, n);   // header + scan travel in the match launch
-  if (inl) s = ensure_scan_buf(h, pbuf, n);
-  else s = upload_scan(h, pbuf, header, 6, pts, n, st);
-  if (s != HSB_OK) return s;
-  const float* d_hdr = scan_header(pbuf);
-  const float* d_pose_in = d_hdr;  // the hint, unless matched below
+  const bool inl = !conv && !map_without_matching && inline_scan_applies(h, n);   // header + scan travel in the match launch
+  float origo[2] = {0.f, 0.f};
+  const float* d_hdr;   // the header on the device: [0..2] hint, [3..5] minDist / minAngle / force
+  ScanIn dev;           // the scan on the device
+  if (!conv) {
+    // staging, endpoints: header + points straight into the container the map writer reads
+    if ((s = inl ? ensure_scan_buf(h, pbuf, n) : upload_scan(h, pbuf, header, 6, in.in, n, st)) != HSB_OK) return s;
+    d_hdr = scan_header(pbuf);
+    dev = {HSB_IN_ENDPOINTS, scan_points(pbuf), nullptr, n, n, nullptr};
+    if (origo_in) memcpy(origo, origo_in, sizeof(origo));
+  } else {
+    // staging, converted input (floats): [0..15] header; cloud / projected: [16..39] the laser transform (12 doubles),
+    // [40..] the cloud or the ranges; ranges: [16..] the ranges.  The conversion writes the endpoints into the container.
+    const size_t kHdr = 16, kTf = in.tf ? 24 : 0, per_pt = in.kind == HSB_IN_CLOUD ? 3 : 1;
+    const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
+    if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
+    if ((s = ensure_pinned(h, h->h_stage, h->h_stage_bytes, bytes)) != HSB_OK) return s;
+    float* hs = h->h_stage;
+    memset(hs, 0, kHdr * sizeof(float));
+    memcpy(hs, header, sizeof(header));
+    if (in.tf) memcpy(hs + kHdr, in.tf, 12 * sizeof(double));
+    if (n > 0) memcpy(hs + kHdr + kTf, in.in, (size_t)n * per_pt * sizeof(float));
+    HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
+    if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
+    const float* d_c = static_cast<const float*>(h->d_fused_in.p);
+    d_hdr = d_c;
+    dev = {in.kind, d_c + kHdr + kTf, nullptr, n, n, in.tf ? reinterpret_cast<const double*>(d_c + kHdr) : nullptr};
+    if (in.tf) cloud_origo(h, in.tf, origo);   // a LaserScan's origo is zero (HectorMappingRos.cpp:491)
+  }
+  float2* d_pts = reinterpret_cast<float2*>(scan_points(pbuf));
   if (!map_without_matching) {
-    h->last_n = n;
-    h->last_origo[0] = origo ? origo[0] : 0.f;
-    h->last_origo[1] = origo ? origo[1] : 0.f;
     // :78 match, and :83-89 the gate in the same kernel's epilogue (an empty scan still passes through it: pose = hint)
-    if (inl) {
-      HsbMatchParams P;
-      fill_match_params(h, P);
-      P.out_poses = d_s + 8;
-      P.out_cov = host_out ? h->h_pin_dev + 12 : d_s + 12;
-      P.gate_state = d_gate;
-      P.gate_out_host = host_out ? h->h_pin_dev + 8 : nullptr;
-      P.seq_host = poll ? seq_dev : nullptr;
-      P.seq_value = seq_value;
-      s = launch_match_inline(h, P, header, 6, pts, n, scan_points(pbuf), st);
-    } else {
-      s = match_device(h, 1, d_hdr, scan_points(pbuf), nullptr, n, n, d_s + 8, host_out ? h->h_pin_dev + 12 : d_s + 12, d_gate,
-                       d_hdr + 3, host_out ? h->h_pin_dev + 8 : nullptr, st, poll ? seq_dev : nullptr, seq_value);
+    HsbMatchParams P;
+    fill_match_params(h, P);
+    P.B = 1;
+    P.hints = d_hdr;
+    fill_scan(h, dev, P);
+    if (conv) {
+      P.conv.out_pts = d_pts;
+      P.conv.out_n = n_dev;
+      P.conv.out_n_host = kept_dev;
+    }
+    P.out_poses = d_s + 8;
+    P.out_cov = host_out ? h->h_pin_dev + 12 : d_s + 12;
+    P.gate_state = d_gate;
+    P.gate_in = d_hdr + 3;
+    P.gate_out_host = host_out ? h->h_pin_dev + 8 : nullptr;
+    P.seq_host = poll ? seq_dev : nullptr;
+    P.seq_value = seq_value;
+    // (a projected step takes the single step's default shape: hsb_slam_update_projected checked the tuning)
+    s = launch_match_single(h, P, inl, header, 6, in.in);
+    // the scan is the last match's container now (endpoints: since the staging copy, whether or not the match launched)
+    if (s == HSB_OK || !conv) {
+      h->last_n = n;   // (converted: an upper bound until the kept count arrives; the writer reads the exact one on the device)
+      h->last_origo[0] = origo[0];
+      h->last_origo[1] = origo[1];
     }
     if (s != HSB_OK) return s;
-  } else {
-    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_pose_in, d_s + 8, host_out ? h->h_pin_dev + 8 : nullptr,
-                                            poll ? seq_dev : nullptr, seq_value);  // :80, :89
+  } else if (!conv) {
+    // without matching, endpoints: the gate alone (:80, :89)
+    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, host_out ? h->h_pin_dev + 8 : nullptr,
+                                            poll ? seq_dev : nullptr, seq_value);
     h->launches += 1;
     HSB_CUDA(h, cudaGetLastError());
+  } else {
+    // without matching, converted input: the stand-alone conversion kernel, the gate, then the kept count's publication
+    HsbConvDev c;
+    fill_conv(h, in.kind, c);
+    c.out_pts = d_pts;
+    c.out_n = n_dev;
+    if ((s = launch_conversion(h, in.kind, dev.in, n, dev.tf, c, st)) != HSB_OK) return s;
+    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, h->h_pin_dev + 8, nullptr, 0);
+    hsb::publish_int_kernel<<<1, 32, 0, st>>>(n_dev, kept_dev, poll ? seq_dev : nullptr, seq_value);
+    h->launches += 2;
+    HSB_CUDA(h, cudaGetLastError());
   }
-  if ((s = enqueue_update_by_scan(h, reinterpret_cast<const float2*>(scan_points(pbuf)), n, origo, nullptr, d_s + 8, d_gate + 3)) != HSB_OK)  // :91
-    return s;
+  if ((s = enqueue_update_by_scan(h, d_pts, n, n_dev, origo, !map_without_matching, nullptr, d_s + 8, d_gate + 3)) != HSB_OK)
+    return s;   // :91
   if (poll) {
     // the pose is all the caller needs now; every later call on this handle is stream-ordered behind the map write
     if ((s = wait_published(h, seq, seq_value, st, "fused step finished without publishing its pose")) != HSB_OK) return s;
@@ -1849,126 +1821,28 @@ static int slam_update_impl(hsb_handle* h, const float hint[3], const float* pts
     HSB_CUDA(h, cudaStreamSynchronize(st));  // :93 onMapUpdated — the probability plane is current
     h->map_write_pending = false;
   }
-  memcpy(out_pose, h->h_pin + 8, 3 * sizeof(float));
-  if (map_updated) *map_updated = h->h_pin[11] != 0.f;
-  if (cov_inout && n > 0 && !map_without_matching) memcpy(cov_inout, h->h_pin + 12, 9 * sizeof(float));
-  return HSB_OK;
-}
-
-int hsb_slam_update(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
-                    int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated) {
-  return slam_update_impl(h, hint, pts, n, origo, map_without_matching, out_pose, cov_inout, map_updated, true);
-}
-
-int hsb_slam_update_nowait(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
-                           int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated) {
-  return slam_update_impl(h, hint, pts, n, origo, map_without_matching, out_pose, cov_inout, map_updated, false);
-}
-
-// What a fused single SLAM step converts on the device: a Point32 cloud in the laser frame with its laser transform
-// (hsb_slam_update_cloud), a LaserScan's raw ranges in the handle's scan format (hsb_slam_update_ranges), or raw
-// ranges projected with the handle's laser projection and then converted as a cloud (hsb_slam_update_projected).
-struct FusedScan {
-  HsbInputKind kind;
-  const float* data;    // cloud: n (x, y, z) triples; ranges / projected: n ranges
-  int n;                // cloud: points; ranges / projected: n_beams (an upper bound of the endpoints kept)
-  const double* T;      // cloud / projected: the laser transform (12 doubles)
-};
-
-// HectorMappingRos::scanCallback's conversion + HectorSlamProcessor::update (:297 / HectorSlamProcessor.h:71-113) as
-// one step.  The scan is converted by the match kernel's staging step; the converted endpoints, which the map writer
-// needs too, are written out by the same kernel and their number stays on the device (the writer reads it there), so no
-// host round trip appears between conversion, match, gate and map write.  Without matching the stand-alone conversion
-// kernel converts the scan and the gate runs alone.
-static int fused_slam_step(hsb_handle* h, const float hint[3], const FusedScan& in, int map_without_matching, int nowait,
-                           float out_pose[3], float cov_inout[9], int* map_updated, int* out_kept) {
-  HandleScope guard(h);
-  int s;
-  const int n = in.n;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
-  if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
-  // staging layout (floats): [0..15] header: hint, thresholds, force; cloud / projected: [16..39] the laser transform
-  // (12 doubles), [40..] the cloud or the ranges; ranges: [16..] the ranges
-  const bool ranges = in.kind == HSB_IN_RANGES;
-  const size_t kHdr = 16, kTf = ranges ? 0 : 24, per_pt = in.kind == HSB_IN_CLOUD ? 3 : 1;
-  const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
-  if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
-  if ((s = ensure_pinned(h, h->h_stage, h->h_stage_bytes, bytes)) != HSB_OK) return s;
-  float* hs = h->h_stage;
-  memset(hs, 0, kHdr * sizeof(float));
-  hs[0] = hint[0]; hs[1] = hint[1]; hs[2] = hint[2];
-  hs[3] = h->min_dist; hs[4] = h->min_angle; hs[5] = map_without_matching ? 1.f : 0.f;
-  if (!ranges) memcpy(hs + kHdr, in.T, 12 * sizeof(double));
-  if (n > 0) memcpy(hs + kHdr + kTf, in.data, (size_t)n * per_pt * sizeof(float));
-  cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
-  float* d_c = static_cast<float*>(h->d_fused_in.p);
-  const float* d_hdr = d_c;
-  const double* d_tf = ranges ? nullptr : reinterpret_cast<const double*>(d_c + kHdr);
-  const float* d_in = d_c + kHdr + kTf;
-  float* d_s = static_cast<float*>(h->d_scratch.p);
-  float* d_gate = static_cast<float*>(h->d_gate.p);
-  // the container's origo is known on the host: zero for a LaserScan (HectorMappingRos.cpp:491)
-  float origo[2] = {0.f, 0.f};
-  if (!ranges) cloud_origo(h, in.T, origo);
-  // results always travel through mapped host memory here
-  const bool poll = nowait != 0;
-  volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
-  unsigned* seq_dev = reinterpret_cast<unsigned*>(h->h_pin_dev + 22);
-  const unsigned seq_value = ++h->step_seq;
-  int* kept_host = reinterpret_cast<int*>(h->h_pin + 24);
-  int* kept_dev = reinterpret_cast<int*>(h->h_pin_dev + 24);
-  DevBuf& pbuf = map_without_matching ? h->d_upd_pts : h->d_last_pts;
-  if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
-  HsbConvDev conv;
-  fill_conv(h, in.kind, conv);
-  conv.out_pts = reinterpret_cast<float2*>(scan_points(pbuf));
-  conv.out_n = reinterpret_cast<int*>(d_s + 40);
-  if (!map_without_matching) {
-    HsbMatchParams P;
-    fill_match_params(h, P);
-    P.B = 1;
-    P.hints = d_hdr;
-    P.out_poses = d_s + 8;
-    P.out_cov = h->h_pin_dev + 12;
-    P.kind = in.kind;
-    P.conv_in = d_in;
-    P.n_shared = n;
-    P.cloud_tf = d_tf;
-    P.conv = conv;
-    P.conv.out_n_host = kept_dev;
-    P.gate_state = d_gate;
-    P.gate_in = d_hdr + 3;
-    P.gate_out_host = h->h_pin_dev + 8;
-    P.seq_host = poll ? seq_dev : nullptr;
-    P.seq_value = seq_value;
-    // (a projected step takes the single step's default shape: hsb_slam_update_projected checked the tuning)
-    if ((s = launch_match(h, P, n, st)) != HSB_OK) return s;
-    h->last_n = n;   // upper bound until the kept count arrives (the writer reads the exact one on the device)
-    h->last_origo[0] = origo[0];
-    h->last_origo[1] = origo[1];
-  } else {
-    if ((s = launch_conversion(h, in.kind, d_in, n, d_tf, conv, st)) != HSB_OK) return s;
-    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, h->h_pin_dev + 8, nullptr, 0);
-    hsb::publish_int_kernel<<<1, 32, 0, st>>>(conv.out_n, kept_dev, poll ? seq_dev : nullptr, seq_value);
-    h->launches += 2;
-    HSB_CUDA(h, cudaGetLastError());
-  }
-  if ((s = enqueue_update_by_scan(h, conv.out_pts, n, origo, nullptr, d_s + 8, d_gate + 3, conv.out_n)) != HSB_OK) return s;
-  if (poll) {
-    if ((s = wait_published(h, seq, seq_value, st, "fused step finished without publishing its pose")) != HSB_OK) return s;
-    h->map_write_pending = true;
-  } else {
-    HSB_CUDA(h, cudaStreamSynchronize(st));
-    h->map_write_pending = false;
-  }
-  const int kept = *kept_host;
-  if (!map_without_matching) h->last_n = kept;
+  // the endpoints the step had: known on the host for endpoints, counted on the device for converted input
+  const int kept = conv ? *kept_host : n;
+  if (conv && !map_without_matching) h->last_n = kept;
   memcpy(out_pose, h->h_pin + 8, 3 * sizeof(float));
   if (map_updated) *map_updated = h->h_pin[11] != 0.f;
   if (cov_inout && kept > 0 && !map_without_matching) memcpy(cov_inout, h->h_pin + 12, 9 * sizeof(float));
   if (out_kept) *out_kept = kept;
   return HSB_OK;
+}
+
+int hsb_slam_update(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
+                    int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated) {
+  if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
+  return slam_step(h, hint, {HSB_IN_ENDPOINTS, pts, nullptr, n, n, nullptr}, origo, map_without_matching, false, out_pose,
+                   cov_inout, map_updated, nullptr);
+}
+
+int hsb_slam_update_nowait(hsb_handle* h, const float hint[3], const float* pts, int n, const float origo[2],
+                           int map_without_matching, float out_pose[3], float cov_inout[9], int* map_updated) {
+  if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
+  return slam_step(h, hint, {HSB_IN_ENDPOINTS, pts, nullptr, n, n, nullptr}, origo, map_without_matching, true, out_pose,
+                   cov_inout, map_updated, nullptr);
 }
 
 // HectorMappingRos::scanCallback's default branch in one call: rosPointCloudToDataContainer (HectorMappingRos.cpp:283,
@@ -1979,8 +1853,8 @@ int hsb_slam_update_cloud(hsb_handle* h, const float hint[3], const float* point
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !points_xyz)) return HSB_ERR_INVALID_ARG;
   int s = check_input(h, h, HSB_IN_CLOUD, "hsb_slam_update_cloud", -1, -1, false);
   if (s != HSB_OK) return s;
-  const FusedScan in = {HSB_IN_CLOUD, points_xyz, n, transform ? transform : h->cfmt.laser_transform};
-  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
+  const ScanIn in = {HSB_IN_CLOUD, points_xyz, nullptr, n, n, transform ? transform : h->cfmt.laser_transform};
+  return slam_step(h, hint, in, nullptr, map_without_matching, nowait != 0, out_pose, cov_inout, map_updated, out_kept);
 }
 
 // ... and its branch without the laser tf (use_tf_scan_transformation = false, :248-254): rosLaserScanToDataContainer
@@ -1990,8 +1864,8 @@ int hsb_slam_update_ranges(hsb_handle* h, const float hint[3], const float* rang
   if (!h || !hint || !out_pose || !ranges) return HSB_ERR_INVALID_ARG;
   int s = check_input(h, h, HSB_IN_RANGES, "hsb_slam_update_ranges", -1, n, false);
   if (s != HSB_OK) return s;
-  const FusedScan in = {HSB_IN_RANGES, ranges, n, nullptr};
-  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
+  return slam_step(h, hint, {HSB_IN_RANGES, ranges, nullptr, n, n, nullptr}, nullptr, map_without_matching, nowait != 0,
+                   out_pose, cov_inout, map_updated, out_kept);
 }
 
 // ... and the default branch from the LaserScan itself (:258-297): laser_geometry's projection (:273), then
@@ -2003,8 +1877,8 @@ int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* r
   int s = check_input(h, h, HSB_IN_PROJECTED, "hsb_slam_update_projected", -1, n, true);
   if (s != HSB_OK) return s;
   if ((s = check_projected_tuning(h, "hsb_slam_update_projected", true)) != HSB_OK) return s;
-  const FusedScan in = {HSB_IN_PROJECTED, ranges, n, transform ? transform : h->cfmt.laser_transform};
-  return fused_slam_step(h, hint, in, map_without_matching, nowait, out_pose, cov_inout, map_updated, out_kept);
+  const ScanIn in = {HSB_IN_PROJECTED, ranges, nullptr, n, n, transform ? transform : h->cfmt.laser_transform};
+  return slam_step(h, hint, in, nullptr, map_without_matching, nowait != 0, out_pose, cov_inout, map_updated, out_kept);
 }
 
 int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
@@ -2766,29 +2640,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     } else {
       pts0 = reinterpret_cast<const float2*>(d_in) + offsets[k];
     }
-    // MapRepMultiMap::updateByScan: level 0 from this scan, the coarse levels from the last match's container (:143)
-    for (int l = 0; l < levels; ++l) {
-      HsbUpdateLevelDev& d = s_upd[(size_t)k * levels + l];
-      fill_update_level(h, l, d);
-      d.pt_scale = (float)(1.0 / pow(2.0, (double)l));
-      if (l == 0 || matched) {
-        d.pts = pts0;
-        d.n = n;
-        d.n_dev = n_dev;
-        d.origo_x = og[0];
-        d.origo_y = og[1];
-      } else {
-        d.pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
-        d.n = h->last_n;
-        d.origo_x = h->last_origo[0];
-        d.origo_y = h->last_origo[1];
-      }
-      d.active = d.n > 0;
-      if (d.active) {
-        if ((s = next_stamp_base(h, l, &d.stamp_base, st)) != HSB_OK) return s;
-        max_upd = std::max(max_upd, d.n);
-      }
-    }
+    if ((s = fill_update_levels(h, s_upd + (size_t)k * levels, pts0, n, n_dev, og, matched, st, &max_upd)) != HSB_OK) return s;
   }
   HSB_CUDA(h0, cudaMemcpyAsync(g->d_stage.p, hs, bytes, cudaMemcpyHostToDevice, st));
 
@@ -2797,11 +2649,9 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   fill_match_params(h0, P);
   P.B = M;
   P.hints = reinterpret_cast<const float*>(ds);
-  P.kind = in.kind;   // (a converted session converts with its own descriptor)
-  if (conv) P.conv_in = reinterpret_cast<const float*>(d_in);
-  else P.pts = reinterpret_cast<const float2*>(d_in);
-  P.offsets = reinterpret_cast<const int*>(ds + o_off);
-  if (tf) P.cloud_tf = reinterpret_cast<const double*>(ds + o_tf);
+  // (a converted session converts with its own descriptor, HsbGroupSessionDev::conv)
+  fill_scan(h0, {in.kind, reinterpret_cast<const float*>(d_in), reinterpret_cast<const int*>(ds + o_off), 0, max_n,
+                 tf ? reinterpret_cast<const double*>(ds + o_tf) : nullptr}, P);
   P.out_poses = g->d_res;
   P.out_cov = g->h_res_dev + 4 * (size_t)M;
   P.gate_in = reinterpret_cast<const float*>(ds + o_gin);
