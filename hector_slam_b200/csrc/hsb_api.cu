@@ -2370,7 +2370,16 @@ void* hsb_level_logodds_device_ptr(hsb_handle* h, int level) {
 int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
   if (!h || level < 0 || level >= h->levels) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  return refresh_level(h, level, (cudaStream_t)stream);
+  int s = refresh_level(h, level, (cudaStream_t)stream);
+  if (s != HSB_OK) return s;
+  // the plane was written from outside (a full-plane broadcast): the host mirror has to re-read the whole level, so the
+  // mirror rectangle becomes the level, in order on `stream`.  The replication rectangle is left alone: marking it
+  // would make a replica re-ship a whole plane it has only received.
+  Level& L = h->lv[level];
+  if (!L.dirty) return HSB_OK;
+  const int full[4] = {0, 0, L.sx - 1, L.sy - 1};
+  HSB_CUDA(h, cudaMemcpyAsync(L.dirty + 4, full, sizeof(full), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return HSB_OK;
 }
 
 }  // extern "C"

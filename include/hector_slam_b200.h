@@ -463,7 +463,10 @@ int hsb_download_level(hsb_handle* h, int level, float* logodds_host_out);
 /* probability plane P = e^l / (e^l + 1) (GridMapLogOdds.h:163-166) as the match kernel sees it */
 int hsb_download_prob(hsb_handle* h, int level, float* prob_host_out);
 /* device address of the level's log-odds plane (for NCCL broadcast of map replicas) and a full
- * recompute of the probability planes after such an external write */
+ * recompute of the probability plane and texture twin after such an external write, on `stream`.
+ * hsb_refresh_level also sets the level's mirror rectangle (hsb_get_mirror_dirty_rect) to the whole
+ * level, in order on `stream`, so that a host mirror re-reads the plane; the replication rectangle
+ * (hsb_get_dirty_rect) is left as it is, so a replica does not ship back a plane it only received. */
 void* hsb_level_logodds_device_ptr(hsb_handle* h, int level);
 int hsb_refresh_level(hsb_handle* h, int level, void* stream);
 
