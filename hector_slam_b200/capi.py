@@ -40,6 +40,8 @@ EXPORTED = [
     "hsb_set_laser_projection", "hsb_projected_scan_to_points", "hsb_slam_update_projected",
     "hsb_group_slam_update_projected", "hsb_match_batch_projected", "hsb_match_batch_projected_submit",
     "hsb_match_batch_projected_device",
+    "hsb_group_slam_update_subset", "hsb_group_slam_update_cloud_subset", "hsb_group_slam_update_ranges_subset",
+    "hsb_group_slam_update_projected_subset",
 ]
 
 
@@ -190,6 +192,10 @@ def load_library() -> C.CDLL:
     sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_slam_update_ranges", i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_slam_update_projected", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_slam_update_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
+    sig("hsb_group_slam_update_cloud_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_slam_update_ranges_subset", i, vp, i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_slam_update_projected_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -920,90 +926,113 @@ class SlamGroup:
         if st != 0:
             raise HsbError(st, (self.lib.hsb_last_error(self.reps[0].h) or b"").decode())
 
-    def slam_update(self, hints, scans, origo=None, map_without_matching=None, nowait: bool = False, cov_inout=None):
+    def slam_update(self, hints, scans, origo=None, map_without_matching=None, nowait: bool = False, cov_inout=None,
+                    members=None):
         """scans: M (n_s, 2) endpoint arrays, or a tuple (points (N, 2), offsets (M + 1,)).  hints (M, 3), origo (M, 2),
         map_without_matching (M,) bools.  -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool); a cov entry keeps its
-        cov_inout value (zeros if None) where the session matched nothing."""
-        M = self.M
-        h = _f32(hints).reshape(M, 3)
-        pts, offsets = self._pack(scans, 2)
-        og = None if origo is None else _f32(origo).reshape(M, 2)
-        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
-        poses = np.zeros((M, 3), np.float32)
-        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
-        upd = np.zeros(M, np.int32)
-        self._check(self.lib.hsb_group_slam_update(self.g, h.ctypes.data, pts.ctypes.data if pts.size else None,
-                                                   offsets.ctypes.data, _ptr(og), _ptr(mwm), int(bool(nowait)),
-                                                   poses.ctypes.data, cov.ctypes.data, upd.ctypes.data))
-        return poses, cov.reshape(M, 3, 3), upd.astype(bool)
+        cov_inout value (zeros if None) where the session matched nothing.
+        members: step only these members (indices into the group's handles, in session order,
+        hsb_group_slam_update_subset); every per-session argument and result then has len(members) entries."""
+        K, mem = self._sessions(members)
+        h = _f32(hints).reshape(K, 3)
+        pts, offsets = self._pack(scans, 2, K)
+        og = None if origo is None else _f32(origo).reshape(K, 2)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(K)
+        poses = np.zeros((K, 3), np.float32)
+        cov = np.zeros((K, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(K, 9).copy()
+        upd = np.zeros(K, np.int32)
+        args = (h.ctypes.data, pts.ctypes.data if pts.size else None, offsets.ctypes.data, _ptr(og), _ptr(mwm),
+                int(bool(nowait)), poses.ctypes.data, cov.ctypes.data, upd.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_slam_update(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_slam_update_subset(self.g, K, _ptr(mem), *args))
+        return poses, cov.reshape(K, 3, 3), upd.astype(bool)
 
     def slam_update_cloud(self, hints, clouds, transforms=None, map_without_matching=None, nowait: bool = False,
-                          cov_inout=None):
+                          cov_inout=None, members=None):
         """The same step from the node's default input (hsb_group_slam_update_cloud): clouds are M (n_s, 3) Point32
         arrays in the laser frame, or a tuple (points (N, 3), offsets (M + 1,)); transforms (M, 12) float64 laser
         transforms, None = each member's cloud format.  Each member converts with its own cloud format's thresholds.
+        members as in slam_update (hsb_group_slam_update_cloud_subset).
         -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
-        M = self.M
-        h = _f32(hints).reshape(M, 3)
-        pts, offsets = self._pack(clouds, 3)
-        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(M, 12)
-        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
-        poses = np.zeros((M, 3), np.float32)
-        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
-        upd = np.zeros(M, np.int32)
-        kept = np.zeros(M, np.int32)
-        self._check(self.lib.hsb_group_slam_update_cloud(self.g, h.ctypes.data, pts.ctypes.data if pts.size else None,
-                                                         offsets.ctypes.data, _ptr(T), _ptr(mwm), int(bool(nowait)),
-                                                         poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
-                                                         kept.ctypes.data))
-        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+        K, mem = self._sessions(members)
+        h = _f32(hints).reshape(K, 3)
+        pts, offsets = self._pack(clouds, 3, K)
+        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(K, 12)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(K)
+        poses = np.zeros((K, 3), np.float32)
+        cov = np.zeros((K, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(K, 9).copy()
+        upd = np.zeros(K, np.int32)
+        kept = np.zeros(K, np.int32)
+        args = (h.ctypes.data, pts.ctypes.data if pts.size else None, offsets.ctypes.data, _ptr(T), _ptr(mwm),
+                int(bool(nowait)), poses.ctypes.data, cov.ctypes.data, upd.ctypes.data, kept.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_slam_update_cloud(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_slam_update_cloud_subset(self.g, K, _ptr(mem), *args))
+        return poses, cov.reshape(K, 3, 3), upd.astype(bool), kept.astype(int)
 
-    def slam_update_ranges(self, hints, ranges_list, map_without_matching=None, nowait: bool = False, cov_inout=None):
+    def slam_update_ranges(self, hints, ranges_list, map_without_matching=None, nowait: bool = False, cov_inout=None,
+                           members=None):
         """The same step from raw LaserScan ranges (hsb_group_slam_update_ranges): ranges_list is M (n_beams_s,) arrays,
-        or a tuple (ranges (N,), offsets (M + 1,)).  Each member converts with its own scan format.
+        or a tuple (ranges (N,), offsets (M + 1,)).  Each member converts with its own scan format.  members as in
+        slam_update (hsb_group_slam_update_ranges_subset).
         -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
-        M = self.M
-        h = _f32(hints).reshape(M, 3)
-        r, offsets = self._pack(ranges_list, 1)
-        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
-        poses = np.zeros((M, 3), np.float32)
-        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
-        upd = np.zeros(M, np.int32)
-        kept = np.zeros(M, np.int32)
-        self._check(self.lib.hsb_group_slam_update_ranges(self.g, h.ctypes.data, r.ctypes.data if r.size else None,
-                                                          offsets.ctypes.data, _ptr(mwm), int(bool(nowait)),
-                                                          poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
-                                                          kept.ctypes.data))
-        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+        K, mem = self._sessions(members)
+        h = _f32(hints).reshape(K, 3)
+        r, offsets = self._pack(ranges_list, 1, K)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(K)
+        poses = np.zeros((K, 3), np.float32)
+        cov = np.zeros((K, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(K, 9).copy()
+        upd = np.zeros(K, np.int32)
+        kept = np.zeros(K, np.int32)
+        args = (h.ctypes.data, r.ctypes.data if r.size else None, offsets.ctypes.data, _ptr(mwm), int(bool(nowait)),
+                poses.ctypes.data, cov.ctypes.data, upd.ctypes.data, kept.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_slam_update_ranges(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_slam_update_ranges_subset(self.g, K, _ptr(mem), *args))
+        return poses, cov.reshape(K, 3, 3), upd.astype(bool), kept.astype(int)
 
     def slam_update_projected(self, hints, ranges_list, transforms=None, map_without_matching=None, nowait: bool = False,
-                              cov_inout=None):
+                              cov_inout=None, members=None):
         """The same step from the LaserScans of default-configured nodes (hsb_group_slam_update_projected): ranges_list
         is M (n_beams_s,) arrays, or a tuple (ranges (N,), offsets (M + 1,)); transforms (M, 12) float64, None = each
         member's cloud format.  Each member projects with its own laser projection and converts with its own cloud
-        format.  -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
-        M = self.M
-        h = _f32(hints).reshape(M, 3)
-        r, offsets = self._pack(ranges_list, 1)
-        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(M, 12)
-        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(M)
-        poses = np.zeros((M, 3), np.float32)
-        cov = np.zeros((M, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(M, 9).copy()
-        upd = np.zeros(M, np.int32)
-        kept = np.zeros(M, np.int32)
-        self._check(self.lib.hsb_group_slam_update_projected(self.g, h.ctypes.data, r.ctypes.data if r.size else None,
-                                                             offsets.ctypes.data, _ptr(T), _ptr(mwm), int(bool(nowait)),
-                                                             poses.ctypes.data, cov.ctypes.data, upd.ctypes.data,
-                                                             kept.ctypes.data))
-        return poses, cov.reshape(M, 3, 3), upd.astype(bool), kept.astype(int)
+        format.  members as in slam_update (hsb_group_slam_update_projected_subset).
+        -> (poses (M, 3), covs (M, 3, 3), updated (M,) bool, kept (M,) int: endpoints each conversion kept)"""
+        K, mem = self._sessions(members)
+        h = _f32(hints).reshape(K, 3)
+        r, offsets = self._pack(ranges_list, 1, K)
+        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(K, 12)
+        mwm = None if map_without_matching is None else np.ascontiguousarray(map_without_matching, np.int32).reshape(K)
+        poses = np.zeros((K, 3), np.float32)
+        cov = np.zeros((K, 9), np.float32) if cov_inout is None else _f32(cov_inout).reshape(K, 9).copy()
+        upd = np.zeros(K, np.int32)
+        kept = np.zeros(K, np.int32)
+        args = (h.ctypes.data, r.ctypes.data if r.size else None, offsets.ctypes.data, _ptr(T), _ptr(mwm),
+                int(bool(nowait)), poses.ctypes.data, cov.ctypes.data, upd.ctypes.data, kept.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_slam_update_projected(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_slam_update_projected_subset(self.g, K, _ptr(mem), *args))
+        return poses, cov.reshape(K, 3, 3), upd.astype(bool), kept.astype(int)
 
-    def _pack(self, scans, width):
-        """M per-session arrays (n_s, width), or a tuple (points (N, width), offsets (M + 1,)) -> (points, offsets)."""
+    def _sessions(self, members):
+        """-> (sessions of the step, the member list as int32, or None for a step of every member)"""
+        if members is None:
+            return self.M, None
+        mem = np.ascontiguousarray(members, dtype=np.int32).reshape(-1)
+        return mem.shape[0], mem
+
+    def _pack(self, scans, width, n):
+        """n per-session arrays (n_s, width), or a tuple (points (N, width), offsets (n + 1,)) -> (points, offsets)."""
         if isinstance(scans, tuple):
             return _f32(scans[0]).reshape(-1, width), np.ascontiguousarray(scans[1], dtype=np.int32)
         scans = [_f32(s).reshape(-1, width) for s in scans]
-        assert len(scans) == self.M, (len(scans), self.M)
-        offsets = np.zeros(self.M + 1, np.int32)
+        assert len(scans) == n, (len(scans), n)
+        offsets = np.zeros(n + 1, np.int32)
         offsets[1:] = np.cumsum([s.shape[0] for s in scans])
         return (np.concatenate(scans) if offsets[-1] else np.zeros((0, width), np.float32)), offsets
 

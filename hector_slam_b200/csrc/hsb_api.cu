@@ -677,6 +677,9 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
   HSB_CUDA_C(cudaMemset(h->d_dirty_all, 0, (HSB_MAX_LEVELS * 8 + 4) * sizeof(int)));
   HSB_CUDA_C(cudaHostAlloc(&h->h_pin, 64 * sizeof(float), cudaHostAllocMapped));
   HSB_CUDA_C(cudaHostGetDevicePointer(&h->h_pin_dev, h->h_pin, 0));
+  // pinned memory comes back from earlier allocations with their contents: a nowait step polls h_pin[22] for its
+  // sequence number (1, 2, ...), which must not be there before the step publishes it
+  memset(h->h_pin, 0, 64 * sizeof(float));
 
   h->gather_mode = cfg->gather_mode == HSB_GATHER_LDG ? HSB_GATHER_LDG : HSB_GATHER_TEX;  // AUTO -> TEX (measured faster)
   // The texture twin is a CUDA array with texture gather, whose extent the device limits (maxTexture2DGather, 32768 x
@@ -2392,16 +2395,20 @@ int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
 // (stamp bases, writer slots, the last match's container size and origo) is advanced here exactly as it advances there.
 
 struct hsb_group {
-  std::vector<hsb_handle*> m;      // the members, in session order
+  std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create was given them
+  std::vector<int> all;            // 0 .. M-1: the member list of a step of every member
+  std::vector<unsigned char> listed;   // scratch of a step's member-list check, M flags
   int device = 0;
   int levels = 0;
   cudaStream_t stream = nullptr;   // every step of the group runs here
   cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
-  HsbLevelDev* d_lv = nullptr;     // M x levels match-kernel level descriptors (a handle's planes never move)
-  // M x 4 (pose, write flag) for the map writer, the finished-session counter (4 words), then M kept-endpoint counts of a
-  // cloud or ranges step (ints, the map writer's n_dev)
+  // M x levels match-kernel level descriptors, member-major (a handle's planes never move); a session reads its
+  // member's row (HsbGroupSessionDev::member)
+  HsbLevelDev* d_lv = nullptr;
+  // per session (at most M) 4 floats (pose, write flag) for the map writer, the finished-session counter (4 words), then
+  // the sessions' kept-endpoint counts of a converted step (ints, the map writer's n_dev)
   float* d_res = nullptr;
-  // mapped pinned: M x 4 (pose, flag), M x 9 Hessian, the sequence number (4 words), M kept-endpoint counts (ints)
+  // mapped pinned, per session: 4 (pose, flag), then 9 Hessian; the sequence number (4 words), kept-endpoint counts (ints)
   float* h_res = nullptr;
   float* h_res_dev = nullptr;      // device alias of h_res
   char* h_stage = nullptr;         // pinned staging of the step's host-to-device copy
@@ -2476,6 +2483,9 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
   hsb_group* g = new (std::nothrow) hsb_group();
   if (!g) return group_fail(h0, HSB_ERR_OUT_OF_MEMORY, "hsb_group_create: out of host memory");
   g->m.assign(handles, handles + M);
+  g->all.resize(M);
+  for (int s = 0; s < M; ++s) g->all[s] = s;
+  g->listed.assign(M, 0);
   g->device = h0->device;
   g->levels = h0->levels;
 #define HSB_GROUP_CUDA(expr)                                                                                 \
@@ -2527,25 +2537,38 @@ namespace {
 // What a group step's sessions bring: level-0 endpoints (hsb_group_slam_update), the node's projected point clouds
 // (hsb_group_slam_update_cloud), raw LaserScan ranges (hsb_group_slam_update_ranges) or raw ranges to project
 // (hsb_group_slam_update_projected).  All but endpoints are converted in the match kernel's staging step as
-// hsb_slam_update_cloud / _ranges / _projected convert them.
+// hsb_slam_update_cloud / _ranges / _projected convert them.  Every array has one entry per session (K).
 struct GroupInput {
   HsbInputKind kind;
   const char* fn;              // the entry point, for the error messages
-  const float* hints;          // M x 3
+  const float* hints;          // K x 3
   const float* pts;            // endpoints: xy pairs; cloud: Point32 triples; ranges: one float per beam
-  const int* offsets;          // M + 1, in points (ranges: in beams)
-  const float* origo;          // endpoints: M x 2 (NULL = 0, 0)
-  const double* transforms;    // cloud / projected: M x 12 (NULL = every member's hsb_set_cloud_format transform)
+  const int* offsets;          // K + 1, in points (ranges: in beams)
+  const float* origo;          // endpoints: K x 2 (NULL = 0, 0)
+  const double* transforms;    // cloud / projected: K x 12 (NULL = every session's member's hsb_set_cloud_format transform)
 };
 
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
 constexpr int kGroupW = 8;
 
-// One group step of any input kind.  Everything that can reject the step is checked before any member's state moves.
-int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matching, int nowait, float* out_poses,
-               float* cov_inout, int* map_updated, int* out_kept) {
-  hsb_handle* h0 = g->m[0];
+// One group step of any input kind over K of the group's members: session k steps member members[k] (a step of every
+// member passes K = M and g->all).  Members not listed are neither read nor changed.  Everything that can reject the
+// step is checked before any member's state moves.
+int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, const int* map_without_matching,
+               int nowait, float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is stepped
   const int M = (int)g->m.size(), levels = g->levels;
+  if (K < 0 || K > M) return fail(h0, HSB_ERR_INVALID_ARG, "%s: K is %d, must be in [0, %d]", in.fn, K, M);
+  if (K == 0) return HSB_OK;
+  if (!members) return fail(h0, HSB_ERR_INVALID_ARG, "%s: members is NULL with K = %d", in.fn, K);
+  std::fill(g->listed.begin(), g->listed.end(), 0);
+  for (int k = 0; k < K; ++k) {
+    const int j = members[k];
+    if (j < 0 || j >= M)
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is outside [0, %d)", in.fn, k, j, M);
+    if (g->listed[j]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is listed twice", in.fn, k, j);
+    g->listed[j] = 1;
+  }
   const bool cloud = in.kind == HSB_IN_CLOUD;
   const bool conv = in.kind != HSB_IN_ENDPOINTS;   // converted on the device: the kept count decides what the session had
   const bool tf = cloud || in.kind == HSB_IN_PROJECTED;   // with a laser transform per session
@@ -2555,25 +2578,27 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
   if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", in.fn, offsets[0]);
   int max_n = 0;
-  for (int k = 0; k < M; ++k) {
+  for (int k = 0; k < K; ++k) {
     const int n = offsets[k + 1] - offsets[k];
     if (n < 0)
       return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets decrease at session %d (%d -> %d)", in.fn, k, offsets[k],
                   offsets[k + 1]);
     max_n = std::max(max_n, n);
   }
-  const int total = offsets[M];
+  const int total = offsets[K];
   if (total > 0 && !in.pts)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : conv ? "ranges" : "points_xy");
-  for (int k = 0; conv && k < M; ++k) {
-    if ((s = check_input(g->m[k], h0, in.kind, in.fn, k, offsets[k + 1] - offsets[k], false)) != HSB_OK) return s;
+  for (int k = 0; conv && k < K; ++k) {
+    if ((s = check_input(g->m[members[k]], h0, in.kind, in.fn, k, offsets[k + 1] - offsets[k], false)) != HSB_OK)
+      return s;
   }
   // every scan is converted whole into shared memory: the launcher's limit for the group kernel's shape
   if (conv && !staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
   DeviceGuard guard(g->device);
   cudaStream_t st = g->stream;
   // not before the work the members queued themselves, nor before a pending step of another group they belong to
-  for (hsb_handle* h : g->m) {
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
     if (h->group_ev && h->group_ev != g->ev) HSB_CUDA(h0, cudaStreamWaitEvent(st, h->group_ev, 0));
     if (h->queued) {
       if ((s = order_before(h, st, true)) != HSB_OK) return s;
@@ -2584,10 +2609,10 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments |
   // laser transforms (cloud, projected) | scans
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_gin = al((size_t)M * 12), o_off = al(o_gin + (size_t)M * 12), o_sess = al(o_off + (size_t)(M + 1) * 4);
-  const size_t o_upd = al(o_sess + (size_t)M * sizeof(HsbGroupSessionDev));
-  const size_t o_lo = al(o_upd + (size_t)M * levels * sizeof(HsbUpdateLevelDev)), o_tf = al(o_lo + (size_t)M * 8);
-  const size_t o_pts = al(o_tf + (tf ? (size_t)M * 12 * sizeof(double) : 0));
+  const size_t o_gin = al((size_t)K * 12), o_off = al(o_gin + (size_t)K * 12), o_sess = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_upd = al(o_sess + (size_t)K * sizeof(HsbGroupSessionDev));
+  const size_t o_lo = al(o_upd + (size_t)K * levels * sizeof(HsbUpdateLevelDev)), o_tf = al(o_lo + (size_t)K * 8);
+  const size_t o_pts = al(o_tf + (tf ? (size_t)K * 12 * sizeof(double) : 0));
   const size_t pt_bytes = cloud ? 12 : conv ? 4 : 8;
   const size_t bytes = o_pts + (size_t)total * pt_bytes;
   if ((s = ensure_pinned(h0, g->h_stage, g->h_stage_bytes, bytes)) != HSB_OK) return s;
@@ -2600,15 +2625,15 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   float2* s_lo = reinterpret_cast<float2*>(hs + o_lo);
   double* s_tf = reinterpret_cast<double*>(hs + o_tf);
   const char* d_in = ds + o_pts;
-  memcpy(hs, in.hints, (size_t)M * 12);
-  memcpy(hs + o_off, offsets, (size_t)(M + 1) * 4);
+  memcpy(hs, in.hints, (size_t)K * 12);
+  memcpy(hs + o_off, offsets, (size_t)(K + 1) * 4);
   if (total > 0) memcpy(hs + o_pts, in.pts, (size_t)total * pt_bytes);
   // a converted session's kept-endpoint count: in device memory for the map writer, in mapped host memory for the host
   int* kept_dev = reinterpret_cast<int*>(g->d_res + 4 * (size_t)M + 4);
   int* kept_mapped = reinterpret_cast<int*>(g->h_res_dev + 13 * (size_t)M + 4);
   int max_upd = 0;
-  for (int k = 0; k < M; ++k) {
-    hsb_handle* h = g->m[k];
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
     const int n = offsets[k + 1] - offsets[k];   // a cloud's size / a scan's beams: an upper bound of the endpoints kept
     const bool matched = !(map_without_matching && map_without_matching[k]);
     float og[2] = {0.f, 0.f};
@@ -2627,6 +2652,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     HsbGroupSessionDev& ss = s_sess[k];
     memset(&ss, 0, sizeof(ss));
     ss.gate_state = static_cast<float*>(h->d_gate.p);
+    ss.member = members[k];
     if (matched) {   // this scan becomes the last match's container (without matching the old one stays, :77-81)
       if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
       if (!conv) ss.last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
@@ -2656,7 +2682,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   // K1: (conversion +) match + gate, one session per CTA; the last session to finish publishes the step's sequence number
   HsbMatchParams P;
   fill_match_params(h0, P);
-  P.B = M;
+  P.B = K;
   P.hints = reinterpret_cast<const float*>(ds);
   // (a converted session converts with its own descriptor, HsbGroupSessionDev::conv)
   fill_scan(h0, {in.kind, reinterpret_cast<const float*>(d_in), reinterpret_cast<const int*>(ds + o_off), 0, max_n,
@@ -2682,14 +2708,14 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
   // one-wave grids are shared out among the sessions (a cloud's size or a scan's beam count bounds its endpoints: the
-  // grids are sized by it)
+  // grids are sized by it).  Mark is order-free and apply has one owner per cell, so the bits do not depend on the grid.
   HsbGroupUpdateParams U;
   U.lv = reinterpret_cast<const HsbUpdateLevelDev*>(ds + o_upd);
   U.log_odds = reinterpret_cast<const float2*>(ds + o_lo);
   U.res = g->d_res;
   U.levels = levels;
   constexpr int TEAM = 2;
-  const int slots = M * levels;
+  const int slots = K * levels;
   const int blocks = std::max(1, std::min((max_upd * TEAM + 7) / 8, (h0->sm_count * 6 + slots - 1) / slots));
   static int apply_ctas_per_sm = 0;
   if (!apply_ctas_per_sm) {
@@ -2706,14 +2732,18 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
   cfg.stream = st;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cfg.gridDim = dim3(blocks, levels, M);
+  cfg.gridDim = dim3(blocks, levels, K);
   HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_mark_group_kernel<TEAM>, U));
-  cfg.gridDim = dim3(sweep, levels, M);
+  cfg.gridDim = dim3(sweep, levels, K);
   HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_apply_group_kernel, U));
   h0->launches += 2;
   HSB_CUDA(h0, cudaGetLastError());
   HSB_CUDA(h0, cudaEventRecord(g->ev, st));
-  for (hsb_handle* h : g->m) {   // every later operation of a member waits for this step (HandleScope)
+  // every later operation of a stepped member waits for this step (HandleScope).  A member left out keeps its own
+  // group_ev: a map write still pending from an earlier nowait step of this group is waited for through the event,
+  // now recorded behind this step on the same stream.
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
     h->group_ev = nowait ? g->ev : nullptr;
     h->map_write_pending = nowait != 0;
   }
@@ -2722,10 +2752,10 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(g->h_res + 13 * (size_t)M);
     if ((s = wait_published(h0, seq, P.seq_value, st, "group step finished without publishing its poses")) != HSB_OK) return s;
   } else {
-    HSB_CUDA(h0, cudaStreamSynchronize(st));   // :93 onMapUpdated for every member
+    HSB_CUDA(h0, cudaStreamSynchronize(st));   // :93 onMapUpdated for every stepped member
   }
   const int* kept_host = reinterpret_cast<const int*>(g->h_res + 13 * (size_t)M + 4);
-  for (int k = 0; k < M; ++k) {
+  for (int k = 0; k < K; ++k) {
     const float* r = g->h_res + 4 * (size_t)k;
     memcpy(out_poses + 3 * (size_t)k, r, 3 * sizeof(float));
     if (map_updated) map_updated[k] = r[3] != 0.f;
@@ -2733,7 +2763,7 @@ int group_step(hsb_group* g, const GroupInput& in, const int* map_without_matchi
     const int n = conv ? kept_host[k] : offsets[k + 1] - offsets[k];   // the endpoints the session had
     if (conv) {
       if (out_kept) out_kept[k] = n;
-      if (matched) g->m[k]->last_n = n;   // the last match's container holds exactly these (as the single fused step)
+      if (matched) g->m[members[k]]->last_n = n;   // the last match's container holds exactly these (as the single fused step)
     }
     if (cov_inout && matched && n > 0)
       memcpy(cov_inout + 9 * (size_t)k, g->h_res + 4 * (size_t)M + 9 * (size_t)k, 9 * sizeof(float));
@@ -2749,7 +2779,8 @@ int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_
                           const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {HSB_IN_ENDPOINTS, "hsb_group_slam_update", hints, points_xy, offsets, origo, nullptr};
-  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, nullptr);
+  return group_step(g, in, (int)g->m.size(), g->all.data(), map_without_matching, nowait, out_poses, cov_inout,
+                    map_updated, nullptr);
 }
 
 int hsb_group_slam_update_cloud(hsb_group* g, const float* hints, const float* points_xyz, const int* offsets,
@@ -2757,7 +2788,8 @@ int hsb_group_slam_update_cloud(hsb_group* g, const float* hints, const float* p
                                 float* cov_inout, int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {HSB_IN_CLOUD, "hsb_group_slam_update_cloud", hints, points_xyz, offsets, nullptr, transforms};
-  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+  return group_step(g, in, (int)g->m.size(), g->all.data(), map_without_matching, nowait, out_poses, cov_inout,
+                    map_updated, out_kept);
 }
 
 int hsb_group_slam_update_ranges(hsb_group* g, const float* hints, const float* ranges, const int* offsets,
@@ -2765,7 +2797,8 @@ int hsb_group_slam_update_ranges(hsb_group* g, const float* hints, const float* 
                                  int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {HSB_IN_RANGES, "hsb_group_slam_update_ranges", hints, ranges, offsets, nullptr, nullptr};
-  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+  return group_step(g, in, (int)g->m.size(), g->all.data(), map_without_matching, nowait, out_poses, cov_inout,
+                    map_updated, out_kept);
 }
 
 int hsb_group_slam_update_projected(hsb_group* g, const float* hints, const float* ranges, const int* offsets,
@@ -2773,7 +2806,44 @@ int hsb_group_slam_update_projected(hsb_group* g, const float* hints, const floa
                                     float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
   if (!g) return HSB_ERR_INVALID_ARG;
   const GroupInput in = {HSB_IN_PROJECTED, "hsb_group_slam_update_projected", hints, ranges, offsets, nullptr, transforms};
-  return group_step(g, in, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+  return group_step(g, in, (int)g->m.size(), g->all.data(), map_without_matching, nowait, out_poses, cov_inout,
+                    map_updated, out_kept);
+}
+
+int hsb_group_slam_update_subset(hsb_group* g, int K, const int* members, const float* hints, const float* points_xy,
+                                 const int* offsets, const float* origo, const int* map_without_matching, int nowait,
+                                 float* out_poses, float* cov_inout, int* map_updated) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {HSB_IN_ENDPOINTS, "hsb_group_slam_update_subset", hints, points_xy, offsets, origo, nullptr};
+  return group_step(g, in, K, members, map_without_matching, nowait, out_poses, cov_inout, map_updated, nullptr);
+}
+
+int hsb_group_slam_update_cloud_subset(hsb_group* g, int K, const int* members, const float* hints,
+                                       const float* points_xyz, const int* offsets, const double* transforms,
+                                       const int* map_without_matching, int nowait, float* out_poses, float* cov_inout,
+                                       int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {HSB_IN_CLOUD, "hsb_group_slam_update_cloud_subset", hints, points_xyz, offsets, nullptr,
+                         transforms};
+  return group_step(g, in, K, members, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+}
+
+int hsb_group_slam_update_ranges_subset(hsb_group* g, int K, const int* members, const float* hints, const float* ranges,
+                                        const int* offsets, const int* map_without_matching, int nowait,
+                                        float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {HSB_IN_RANGES, "hsb_group_slam_update_ranges_subset", hints, ranges, offsets, nullptr, nullptr};
+  return group_step(g, in, K, members, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+}
+
+int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* members, const float* hints,
+                                           const float* ranges, const int* offsets, const double* transforms,
+                                           const int* map_without_matching, int nowait, float* out_poses,
+                                           float* cov_inout, int* map_updated, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  const GroupInput in = {HSB_IN_PROJECTED, "hsb_group_slam_update_projected_subset", hints, ranges, offsets, nullptr,
+                         transforms};
+  return group_step(g, in, K, members, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
 }
 
 }  // extern "C"

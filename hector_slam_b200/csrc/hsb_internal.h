@@ -48,14 +48,17 @@ struct HsbConvDev {
   int* out_n_host;
 };
 
-// One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges / _projected): the member handle's state
-// the match kernel touches.
+// One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges / _projected and their _subset forms): the
+// member handle's state the match kernel touches.
 struct HsbGroupSessionDev {
   float* gate_state;   // the member's lastMapUpdatePose[3] and write flag (hsb_handle::d_gate)
   float2* last_pts;    // the member's "containers of the last match": a matched scan's endpoints are copied here
   // converted input: the member's format; the sink is its last-match container when the session matches, its
   // update-scan buffer when not
   HsbConvDev conv;
+  // the member's position in the group (its row of HsbMatchParams::group_lv).  Kept here rather than in HsbMatchParams
+  // so that the parameter block, and with it every other instantiation of the match kernel, is unchanged.
+  int member;
 };
 
 struct HsbMatchParams {
@@ -106,8 +109,9 @@ struct HsbMatchParams {
   // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.
   float* record;
   int record_floats;
-  // group SLAM step (match_kernel<..., GRP = true>): scan b is session b of the group.  Its level descriptors are
-  // group_lv[b * levels ..] (built once per group) instead of lv[], its gate thresholds and map_without_matching flag
+  // group SLAM step (match_kernel<..., GRP = true>): scan b is session b of the step, which steps member
+  // group_sess[b].member of the group.  Its level descriptors are group_lv[member * levels ..] (built once per group)
+  // instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done
   // counts the sessions that have finished: the last one publishes seq_value to seq_host.  A converted session converts

@@ -750,10 +750,10 @@ struct MatchBounds {
 };
 
 // Level descriptors of scan `scan`: the kernel parameters' (one map for the whole batch), or — group SLAM step, every
-// session steps its own map — the session's row of the group's device array.
+// session steps its own map — the row of the group's device array that belongs to the session's member.
 template <bool GRP>
 __device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P, int scan, int lvl) {
-  if constexpr (GRP) return P.group_lv[(size_t)scan * P.levels + lvl];
+  if constexpr (GRP) return P.group_lv[(size_t)P.group_sess[scan].member * P.levels + lvl];
   else return P.lv[lvl];
 }
 

@@ -71,9 +71,25 @@ class SlamProcessor {
   // have left it.  The group is kept by ps[0] for as long as the same processors are stepped together in the same order.
   static void updateMany(SlamProcessor* const* ps, int M, const float* points_xy, const int* offsets, const float* origo,
                          const Pose* poseHintsWorld, const int* map_without_matching = 0) {
-    stepMany(ps, M, poseHintsWorld, "updateMany", [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
-      return hsb_group_slam_update(g, hints, points_xy, offsets, origo, map_without_matching, 0, poses, cov, updated);
-    });
+    stepMany(ps, M, 0, M, poseHintsWorld, "updateMany",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update(g, hints, points_xy, offsets, origo, map_without_matching, 0, poses, cov,
+                                            updated);
+             });
+  }
+
+  // updateMany() for the K processors ps[members[0..K)] of ps[0..M) that have a new scan (hsb_group_slam_update_subset):
+  // processor ps[members[k]] takes the scan points_xy[offsets[k] .. offsets[k+1]), origo[2k..], poseHintsWorld[k] and
+  // map_without_matching[k].  The cached group stays the one of ps[0..M), so steps over changing subsets reuse it; the
+  // processors not listed are left exactly as they are.
+  static void updateMany(SlamProcessor* const* ps, int M, const int* members, int K, const float* points_xy,
+                         const int* offsets, const float* origo, const Pose* poseHintsWorld,
+                         const int* map_without_matching = 0) {
+    stepMany(ps, M, members, K, poseHintsWorld, "updateMany",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_subset(g, K, members, hints, points_xy, offsets, origo, map_without_matching,
+                                                   0, poses, cov, updated);
+             });
   }
 
   // The node's default input (use_tf_scan_transformation, HectorMappingRos.cpp:283, 509-542): update() from the projected
@@ -99,10 +115,22 @@ class SlamProcessor {
   static void updateManyCloud(SlamProcessor* const* ps, int M, const float* points_xyz, const int* offsets,
                               const double* transforms, const Pose* poseHintsWorld, const int* map_without_matching = 0,
                               int* kept = 0) {
-    stepMany(ps, M, poseHintsWorld, "updateManyCloud",
+    stepMany(ps, M, 0, M, poseHintsWorld, "updateManyCloud",
              [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
                return hsb_group_slam_update_cloud(g, hints, points_xyz, offsets, transforms, map_without_matching, 0,
                                                   poses, cov, updated, kept);
+             });
+  }
+
+  // updateManyCloud() for the processors ps[members[0..K)] (hsb_group_slam_update_cloud_subset); every per-session
+  // array has K entries, as in the subset form of updateMany.
+  static void updateManyCloud(SlamProcessor* const* ps, int M, const int* members, int K, const float* points_xyz,
+                              const int* offsets, const double* transforms, const Pose* poseHintsWorld,
+                              const int* map_without_matching = 0, int* kept = 0) {
+    stepMany(ps, M, members, K, poseHintsWorld, "updateManyCloud",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_cloud_subset(g, K, members, hints, points_xyz, offsets, transforms,
+                                                         map_without_matching, 0, poses, cov, updated, kept);
              });
   }
 
@@ -129,10 +157,22 @@ class SlamProcessor {
   // group cache and end state as updateMany.
   static void updateManyRanges(SlamProcessor* const* ps, int M, const float* ranges, const int* offsets,
                                const Pose* poseHintsWorld, const int* map_without_matching = 0, int* kept = 0) {
-    stepMany(ps, M, poseHintsWorld, "updateManyRanges",
+    stepMany(ps, M, 0, M, poseHintsWorld, "updateManyRanges",
              [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
                return hsb_group_slam_update_ranges(g, hints, ranges, offsets, map_without_matching, 0, poses, cov,
                                                    updated, kept);
+             });
+  }
+
+  // updateManyRanges() for the processors ps[members[0..K)] (hsb_group_slam_update_ranges_subset); every per-session
+  // array has K entries, as in the subset form of updateMany.
+  static void updateManyRanges(SlamProcessor* const* ps, int M, const int* members, int K, const float* ranges,
+                               const int* offsets, const Pose* poseHintsWorld, const int* map_without_matching = 0,
+                               int* kept = 0) {
+    stepMany(ps, M, members, K, poseHintsWorld, "updateManyRanges",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_ranges_subset(g, K, members, hints, ranges, offsets, map_without_matching, 0,
+                                                          poses, cov, updated, kept);
              });
   }
 
@@ -162,10 +202,22 @@ class SlamProcessor {
   static void updateManyProjected(SlamProcessor* const* ps, int M, const float* ranges, const int* offsets,
                                   const double* transforms, const Pose* poseHintsWorld, const int* map_without_matching = 0,
                                   int* kept = 0) {
-    stepMany(ps, M, poseHintsWorld, "updateManyProjected",
+    stepMany(ps, M, 0, M, poseHintsWorld, "updateManyProjected",
              [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
                return hsb_group_slam_update_projected(g, hints, ranges, offsets, transforms, map_without_matching, 0,
                                                       poses, cov, updated, kept);
+             });
+  }
+
+  // updateManyProjected() for the processors ps[members[0..K)] (hsb_group_slam_update_projected_subset); every
+  // per-session array has K entries, as in the subset form of updateMany.
+  static void updateManyProjected(SlamProcessor* const* ps, int M, const int* members, int K, const float* ranges,
+                                  const int* offsets, const double* transforms, const Pose* poseHintsWorld,
+                                  const int* map_without_matching = 0, int* kept = 0) {
+    stepMany(ps, M, members, K, poseHintsWorld, "updateManyProjected",
+             [&](hsb_group* g, const float* hints, float* poses, float* cov, int* updated) {
+               return hsb_group_slam_update_projected_subset(g, K, members, hints, ranges, offsets, transforms,
+                                                             map_without_matching, 0, poses, cov, updated, kept);
              });
   }
 
@@ -238,25 +290,33 @@ class SlamProcessor {
   void check(int st) const {
     if (st != HSB_OK) throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(h_));
   }
-  // One group step for M processors: `step(group, hints, poses, cov, updated)` makes the C-ABI call; the processors'
-  // poses and covariances are kept as update() keeps them.
+  // One group step of the group of ps[0..M) over the K processors ps[members[k]] (members null: all M, in order):
+  // `step(group, hints, poses, cov, updated)` makes the C-ABI call; the stepped processors' poses and covariances are
+  // kept as update() keeps them.
   template <class Step>
-  static void stepMany(SlamProcessor* const* ps, int M, const Pose* poseHintsWorld, const char* what, Step step) {
+  static void stepMany(SlamProcessor* const* ps, int M, const int* members, int K, const Pose* poseHintsWorld,
+                       const char* what, Step step) {
     if (!ps || M < 1 || !ps[0])
       throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs M >= 1 processors");
+    if (K < 0 || K > M || (K > 0 && !members && K != M))
+      throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs 0 <= K <= M and a member list");
+    for (int k = 0; members && k < K; ++k)
+      if (members[k] < 0 || members[k] >= M)
+        throw std::invalid_argument(std::string("hector_slam_b200: ") + what + ": a member index is outside [0, M)");
     SlamProcessor& owner = *ps[0];
     hsb_group* g = owner.groupFor(ps, M);
-    std::vector<float> hints(3 * (size_t)M), poses(3 * (size_t)M), cov(9 * (size_t)M);
-    std::vector<int> updated(M);
-    for (int s = 0; s < M; ++s) {
+    std::vector<float> hints(3 * (size_t)K), poses(3 * (size_t)K), cov(9 * (size_t)K);
+    std::vector<int> updated(K);
+    for (int s = 0; s < K; ++s) {
+      const SlamProcessor& p = *ps[members ? members[s] : s];
       hints[3 * s] = poseHintsWorld[s].x;
       hints[3 * s + 1] = poseHintsWorld[s].y;
       hints[3 * s + 2] = poseHintsWorld[s].psi;
-      std::memcpy(&cov[9 * s], ps[s]->lastScanMatchCov_, sizeof(ps[s]->lastScanMatchCov_));   // untouched where unmatched
+      std::memcpy(&cov[9 * s], p.lastScanMatchCov_, sizeof(p.lastScanMatchCov_));   // untouched where unmatched
     }
     owner.check(step(g, hints.data(), poses.data(), cov.data(), updated.data()));
-    for (int s = 0; s < M; ++s) {
-      SlamProcessor& p = *ps[s];
+    for (int s = 0; s < K; ++s) {
+      SlamProcessor& p = *ps[members ? members[s] : s];
       p.lastScanMatchPose_ = Pose{poses[3 * s], poses[3 * s + 1], poses[3 * s + 2]};  // :83
       if (updated[s]) p.lastMapUpdatePose_ = p.lastScanMatchPose_;                    // :94
       std::memcpy(p.lastScanMatchCov_, &cov[9 * s], sizeof(p.lastScanMatchCov_));

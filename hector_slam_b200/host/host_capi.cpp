@@ -171,6 +171,66 @@ int hsbp_update_many_projected(void* const* ps, int M, const float* ranges, cons
   }
   return 0;
 }
+// The subset overloads: processor ps[members[k]] takes session k; hints and every per-session array have K entries.
+int hsbp_update_many_subset(void* const* ps, int M, const int* members, int K, const float* pts, const int* offsets,
+                            const float* origo, const float* hints, const int* map_without_matching) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(K > 0 ? K : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  for (int k = 0; k < K; ++k) poses[k] = hsb200::Pose{hints[3 * k], hints[3 * k + 1], hints[3 * k + 2]};
+  try {
+    hsb200::SlamProcessor::updateMany(procs.data(), M, members, K, pts, offsets, origo, poses.data(),
+                                      map_without_matching);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_many_cloud_subset(void* const* ps, int M, const int* members, int K, const float* points_xyz,
+                                  const int* offsets, const double* transforms, const float* hints,
+                                  const int* map_without_matching, int* out_kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(K > 0 ? K : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  for (int k = 0; k < K; ++k) poses[k] = hsb200::Pose{hints[3 * k], hints[3 * k + 1], hints[3 * k + 2]};
+  try {
+    hsb200::SlamProcessor::updateManyCloud(procs.data(), M, members, K, points_xyz, offsets, transforms, poses.data(),
+                                           map_without_matching, out_kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_many_ranges_subset(void* const* ps, int M, const int* members, int K, const float* ranges,
+                                   const int* offsets, const float* hints, const int* map_without_matching,
+                                   int* out_kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(K > 0 ? K : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  for (int k = 0; k < K; ++k) poses[k] = hsb200::Pose{hints[3 * k], hints[3 * k + 1], hints[3 * k + 2]};
+  try {
+    hsb200::SlamProcessor::updateManyRanges(procs.data(), M, members, K, ranges, offsets, poses.data(),
+                                            map_without_matching, out_kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_update_many_projected_subset(void* const* ps, int M, const int* members, int K, const float* ranges,
+                                      const int* offsets, const double* transforms, const float* hints,
+                                      const int* map_without_matching, int* out_kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  std::vector<hsb200::Pose> poses(K > 0 ? K : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  for (int k = 0; k < K; ++k) poses[k] = hsb200::Pose{hints[3 * k], hints[3 * k + 1], hints[3 * k + 2]};
+  try {
+    hsb200::SlamProcessor::updateManyProjected(procs.data(), M, members, K, ranges, offsets, transforms, poses.data(),
+                                               map_without_matching, out_kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

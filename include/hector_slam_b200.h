@@ -444,6 +444,39 @@ int hsb_group_slam_update_ranges(hsb_group* g, const float* hints_world, const f
 int hsb_group_slam_update_projected(hsb_group* g, const float* hints_world, const float* ranges, const int* offsets,
                                     const double* transforms, const int* map_without_matching, int nowait,
                                     float* out_poses_world, float* cov_inout, int* map_updated, int* out_kept);
+/* The four group steps above for K of the group's members, for robots whose scans do not arrive in step: session k
+ * steps members[k], an index into the handles given to hsb_group_create, in any order.  Every per-session array
+ * (hints_world, offsets (K + 1), origo, transforms, map_without_matching, out_poses_world, cov_inout, map_updated,
+ * out_kept) has K entries in session order; otherwise each call takes the arguments of its full form.
+ * Each session's pose, covariance, gate decision and kept count are bit-identical to the single-handle call on its
+ * member (hsb_slam_update / _cloud / _ranges / _projected) with the same inputs, and each stepped member is left in the
+ * state that call leaves.  A member not listed is neither read nor changed: its planes, texture twin, stamps, dirty
+ * rectangles, gate pose and last match's container stay as they are, its formats are not checked (a member without a
+ * cloud format may be left out of a cloud step), and work queued on its own stream does not delay the step.
+ * Ordering: the step runs after everything queued on the listed members and after any pending group step that
+ * involves them; every later call on a listed member runs after it.  Later calls on a member left out keep the
+ * ordering they had (they may also be ordered behind this step), so a map write still pending from an earlier nowait
+ * step of that member is still waited for.
+ * Rejected with HSB_ERR_INVALID_ARG before any member changes: K < 0 or K > M; members == NULL with K > 0; an index
+ * outside [0, M) or listed twice (the message names the session); and every rejection of the full form, applied to the
+ * listed members.  K = 0 returns HSB_OK, reads no other argument and queues nothing.  A step of K >= 1 is one
+ * host-to-device copy and three launches, counted on handles[0] whether or not it is listed. */
+int hsb_group_slam_update_subset(hsb_group* g, int K, const int* members, const float* hints_world,
+                                 const float* points_xy, const int* offsets, const float* origo,
+                                 const int* map_without_matching, int nowait, float* out_poses_world, float* cov_inout,
+                                 int* map_updated);
+int hsb_group_slam_update_cloud_subset(hsb_group* g, int K, const int* members, const float* hints_world,
+                                       const float* points_xyz, const int* offsets, const double* transforms,
+                                       const int* map_without_matching, int nowait, float* out_poses_world,
+                                       float* cov_inout, int* map_updated, int* out_kept);
+int hsb_group_slam_update_ranges_subset(hsb_group* g, int K, const int* members, const float* hints_world,
+                                        const float* ranges, const int* offsets, const int* map_without_matching,
+                                        int nowait, float* out_poses_world, float* cov_inout, int* map_updated,
+                                        int* out_kept);
+int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* members, const float* hints_world,
+                                           const float* ranges, const int* offsets, const double* transforms,
+                                           const int* map_without_matching, int nowait, float* out_poses_world,
+                                           float* cov_inout, int* map_updated, int* out_kept);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
