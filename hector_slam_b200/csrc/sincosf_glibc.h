@@ -24,8 +24,14 @@
 // (Grace) glibc's generic build uses the same algorithm with compiler-chosen contraction, so a
 // reference running there may differ in the last bit and the table below would need re-pinning.
 //
-// Arguments with |y| >= 120 (glibc's table-driven large-argument reduction) fall back to a
-// correctly rounded evaluation; pose angles are normalised to (-pi, pi] once per level.
+// Arguments with |y| >= 120 take glibc's large-argument reduction (reduce_large): the float's
+// 24-bit mantissa times a 96-bit window of 4/pi chosen by the exponent, the quadrant from the top
+// two bits and the remainder converted to double and scaled by pi/2^62; then the same
+// polynomials.  A correctly rounded sin/cos differs from glibc there on ~1.3 % of the arguments,
+// and pose angles reach it unnormalised (the hint of a match's coarsest level, the pose given to
+// the map writer, the poses of the likelihood / covariance entry points).  The 4/pi table
+// (glibc's __inv_pio4) is overlapping 32-bit windows of 4/pi's binary expansion at 8-bit steps;
+// tests/test_sincosf_glibc.py derives it from a computed pi.  +-inf and NaN return NaN.
 #ifndef HSB_SINCOSF_GLIBC_H
 #define HSB_SINCOSF_GLIBC_H
 
@@ -98,6 +104,54 @@ HSB_HD double sc_reduce(double x, int* np) {
   return HSB_DFMA(-(double)n, HSB_SC_HPI, x);
 }
 
+// __inv_pio4: word i = floor(4/pi * 2^(8i+7)) mod 2^32
+#define HSB_INV_PIO4_TABLE \
+    0x000000a2u, 0x0000a2f9u, 0x00a2f983u, 0xa2f9836eu, 0xf9836e4eu, 0x836e4e44u, 0x6e4e4415u, 0x4e441529u, \
+    0x441529fcu, 0x1529fc27u, 0x29fc2757u, 0xfc2757d1u, 0x2757d1f5u, 0x57d1f534u, 0xd1f534ddu, 0xf534ddc0u, \
+    0x34ddc0dbu, 0xddc0db62u, 0xc0db6295u, 0xdb629599u, 0x6295993cu, 0x95993c43u, 0x993c4390u, 0x3c439041u,
+static const uint32_t hsb_inv_pio4_host[24] = {HSB_INV_PIO4_TABLE};
+#if defined(__CUDACC__)
+__device__ const uint32_t hsb_inv_pio4_dev[24] = {HSB_INV_PIO4_TABLE};
+#endif
+
+// reduce_large, for 120 <= |y| < inf given the float's bits: returns x - n*pi/2 for the quadrant n (of |y|; the caller
+// folds the sign in), from a 96-bit slice of 4/pi selected by the exponent
+HSB_HD double sc_reduce_large(uint32_t xi, int* np) {
+#if defined(__CUDA_ARCH__)
+  const uint32_t* arr = &hsb_inv_pio4_dev[(xi >> 26) & 15];
+#else
+  const uint32_t* arr = &hsb_inv_pio4_host[(xi >> 26) & 15];
+#endif
+  const int shift = (xi >> 23) & 7;
+  xi = ((xi & 0xffffffu) | 0x800000u) << shift;
+  uint64_t res0 = (uint64_t)(uint32_t)(xi * arr[0]);   // a 32-bit product: wraps before it is widened
+  const uint64_t res1 = (uint64_t)xi * arr[4];
+  const uint64_t res2 = (uint64_t)xi * arr[8];
+  res0 = (res2 >> 32) | (res0 << 32);
+  res0 += res1;
+  const uint64_t n = (res0 + (1ull << 61)) >> 62;
+  res0 -= n << 62;
+  *np = (int)n;
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(__ll2double_rn((long long)res0), 0x1.921FB54442D18p-62);
+#else
+  return (double)(int64_t)res0 * 0x1.921FB54442D18p-62;
+#endif
+}
+
+// sin (want_cos false) or cos of 120 <= |y| < inf as glibc: the sign bit joins the quadrant for the sign and table
+// choice, the quadrant's parity (flipped for cos) picks the polynomial
+HSB_HD float sc_large(float y, bool want_cos) {
+  const uint32_t xi = f32_bits(y);
+  int n;
+  const double xr = sc_reduce_large(xi, &n);
+  const int q = (n + (int)(xi >> 31)) & 3;
+  const double sign = (q == 1 || q == 2) ? -1.0 : 1.0;
+  const double xs = HSB_DMUL(xr, sign), x2 = HSB_DMUL(xr, xr);
+  if (((n ^ (want_cos ? 1 : 0)) & 1) == 0) return (float)sc_sin_poly(xs, x2);
+  return (float)sc_cos_poly(x2, (q & 2) != 0);
+}
+
 HSB_HD float sinf_glibc(float y) {
   const double x = (double)y;
   const uint32_t top = (f32_bits(y) >> 20) & 0x7ffu;
@@ -115,7 +169,8 @@ HSB_HD float sinf_glibc(float y) {
     }
     return (float)sc_cos_poly(x2, (n & 2) != 0);
   }
-  return (float)sin(x);
+  if (top < 0x7f8u) return sc_large(y, false);
+  return y - y;                        // +-inf, NaN
 }
 
 HSB_HD float cosf_glibc(float y) {
@@ -135,7 +190,8 @@ HSB_HD float cosf_glibc(float y) {
     }
     return (float)sc_cos_poly(x2, (n & 2) != 0);
   }
-  return (float)cos(x);
+  if (top < 0x7f8u) return sc_large(y, true);
+  return y - y;
 }
 
 // sinf_glibc and cosf_glibc of the same argument with ONE argument reduction: the two polynomials are the ones the
@@ -167,8 +223,21 @@ HSB_HD void sincosf_glibc(float y, float* sp, float* cp) {
     *cp = even ? b : a;
     return;
   }
-  *sp = (float)sin(x);
-  *cp = (float)cos(x);
+  if (top < 0x7f8u) {
+    const uint32_t xi = f32_bits(y);
+    int n;
+    const double xr = sc_reduce_large(xi, &n);
+    const int q = (n + (int)(xi >> 31)) & 3;
+    const double sign = (q == 1 || q == 2) ? -1.0 : 1.0;
+    const double x2 = HSB_DMUL(xr, xr);
+    const float a = (float)sc_sin_poly(HSB_DMUL(xr, sign), x2);
+    const float b = (float)sc_cos_poly(x2, (q & 2) != 0);
+    const bool even = (n & 1) == 0;
+    *sp = even ? a : b;
+    *cp = even ? b : a;
+    return;
+  }
+  *sp = *cp = y - y;
 }
 
 // ---- expf as glibc 2.39's x86-64 FMA build evaluates it (sysdeps/ieee754/flt-32/e_expf.c, exp2f_data.c) -----------------

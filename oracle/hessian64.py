@@ -67,7 +67,7 @@ class Eval64:
                          self.dTr[0], self.dTr[1], self.dTr[2]])
 
 
-def evaluate(prob, pts, pose_map, pt_scale=1.0) -> Eval64:
+def evaluate(prob, pts, pose_map, pt_scale=1.0, cs=None) -> Eval64:
     """getCompleteHessianDerivs of one scan.  prob: (S_y, S_x) float32 probability plane of the level; pts: (n, 2)
     float32 endpoints in level-0 cells (the container's units); pose_map: (3,) float32 in the level's cells;
     pt_scale: the level's 2^-k (MapRepMultiMap.h:127)."""
@@ -77,7 +77,7 @@ def evaluate(prob, pts, pose_map, pt_scale=1.0) -> Eval64:
     n = pts.shape[0]
     pose = np.asarray(pose_map, np.float32).reshape(3)
     f32 = np.float32
-    s, c = sinf(pose[2]), cosf(pose[2])
+    s, c = (sinf(pose[2]), cosf(pose[2])) if cs is None else (np.float32(cs[1]), np.float32(cs[0]))   # cs: (c, s) in place of libm's
     x, y = pose[0], pose[1]
     with np.errstate(invalid="ignore", over="ignore"):
         px = pts[:, 0] * f32(pt_scale)                      # DataPointContainer setFrom: exact (power of two)

@@ -177,7 +177,9 @@ static float cached_prob(level_t* L, int index) {
 
 /* OccGridMapUtil.h:287-347 interpMapValueWithDerivatives; bounds MapDimensionProperties.h:65-68 */
 static void interp_with_derivs(level_t* L, float cx, float cy, float out[3]) {
-  if ((cx < 0.0f) || (cx > L->limit_x) || (cy < 0.0f) || (cy > L->limit_y)) {
+  /* a NaN coordinate (a NaN pose or endpoint) passes the reference's four comparisons and indexes the grid with
+   * (int)NaN; here it is out of the map, as on the device, so that a NaN step can be followed */
+  if (!((cx >= 0.0f) && (cx <= L->limit_x) && (cy >= 0.0f) && (cy <= L->limit_y))) {
     out[0] = out[1] = out[2] = 0.0f;
     return;
   }
@@ -448,6 +450,15 @@ static int pose_difference_larger_than(const float p1[3], const float p2[3], flo
   return 0;
 }
 
+/* the two util:: functions on their own, n at a time (oracle/pose32.py is tied to them) */
+void hso_normalize_angle(const float* in, int n, float* out) {
+  for (int i = 0; i < n; ++i) out[i] = normalize_angle(in[i]);
+}
+void hso_pose_difference_larger_than(const float* p1, const float* p2, const float* dist, const float* ang, int n,
+                                     int* out) {
+  for (int i = 0; i < n; ++i) out[i] = pose_difference_larger_than(p1 + 3 * i, p2 + 3 * i, dist[i], ang[i]);
+}
+
 /* MapRepMultiMap.h:134-147 updateByScan (coarse levels use the containers left by matchData) */
 static void maprep_update_by_scan(hso_t* h, const container_t* dc, const float pose[3]) {
   for (int i = 0; i < h->levels; ++i) {
@@ -646,7 +657,7 @@ void hso_update_level(void* hv, int level, const float* pts_level, int n, const 
 
 /* OccGridMapUtil.h:233-285 interpMapValue */
 static float interp_value(level_t* L, float cx, float cy) {
-  if ((cx < 0.0f) || (cx > L->limit_x) || (cy < 0.0f) || (cy > L->limit_y)) return 0.0f;
+  if (!((cx >= 0.0f) && (cx <= L->limit_x) && (cy >= 0.0f) && (cy <= L->limit_y))) return 0.0f;   /* NaN: out */
   int ix = (int)cx, iy = (int)cy;
   float fx = cx - (float)ix, fy = cy - (float)iy;
   int size_x = L->size_x;

@@ -45,14 +45,15 @@ class Lh64:
         return 1.01 * ((k + 1) * U32 * self.R64 / self.n + U32 * abs(self.lh64)) if self.n else 0.0
 
 
-def endpoint_funval(prob, pts, pose_map, pt_scale=1.0):
+def endpoint_funval(prob, pts, pose_map, pt_scale=1.0, cs=None):
     """-> (funval (n,) float32, inside (n,) bool).  prob: (S_y, S_x) float32 probability plane of the level; pts: (n, 2)
-    float32 endpoints in level-0 cells; pose_map: (3,) float32 state in the level's cells; pt_scale: the level's 2^-k."""
+    float32 endpoints in level-0 cells; pose_map: (3,) float32 state in the level's cells; pt_scale: the level's 2^-k;
+    cs: (cos, sin) to use instead of libm's (a test's check that one ulp of them shows)."""
     prob = np.ascontiguousarray(prob, dtype=F32)
     sy, sx = prob.shape
     pts = np.ascontiguousarray(pts, dtype=F32).reshape(-1, 2)
     pose = np.asarray(pose_map, F32).reshape(3)
-    s, c = sinf(pose[2]), cosf(pose[2])
+    s, c = (sinf(pose[2]), cosf(pose[2])) if cs is None else (F32(cs[1]), F32(cs[0]))   # cs: (c, s) in place of libm's
     x, y = pose[0], pose[1]
     with np.errstate(invalid="ignore", over="ignore"):
         px = pts[:, 0] * F32(pt_scale)                      # exact (power of two)

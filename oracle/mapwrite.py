@@ -112,12 +112,13 @@ class Beams:
     ref_defined: bool
 
 
-def beams(L: Level, pts, pose_world, origo=(0.0, 0.0), pt_scale: float = 1.0) -> Beams:
-    """Start and end cells of a scan (container points in level-0 cells, scaled by pt_scale as setFrom does)."""
+def beams(L: Level, pts, pose_world, origo=(0.0, 0.0), pt_scale: float = 1.0, cs=None) -> Beams:
+    """Start and end cells of a scan (container points in level-0 cells, scaled by pt_scale as setFrom does).  cs:
+    (cos, sin) to use instead of libm's (a test's check that one ulp of them shows)."""
     pts = np.asarray(pts, np.float32).reshape(-1, 2)
     pw = np.asarray(pose_world, np.float32).reshape(3)
     mx, my = _affine(L.mtw, pw[0], pw[1])                        # getMapCoordsPose :127
-    c, s = cosf(pw[2]), sinf(pw[2])                              # Rotation2Df :130-131
+    c, s = (cosf(pw[2]), sinf(pw[2])) if cs is None else (f32(cs[0]), f32(cs[1]))   # Rotation2Df :130-131
     ps = f32(pt_scale)
     with np.errstate(invalid="ignore", over="ignore"):
         ox, oy = f32(origo[0]) * ps, f32(origo[1]) * ps          # DataPointContainer setFrom (MapRepMultiMap.h:127)

@@ -20,6 +20,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_LIB = os.path.join(_HERE, "_ref", "libhsref.so")
 PORT_LIB = os.path.join(_HERE, "_build", "libhsoracle.so")
+REF_UTIL_LIB = os.path.join(_HERE, "_ref", "libhsref_util.so")   # the reference's util:: functions
 
 _f32p = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 _i32p = np.ctypeslib.ndpointer(dtype=np.int32, flags="C_CONTIGUOUS")
@@ -286,6 +287,43 @@ def _conv_lib(kind: str):
     if kind == "reference":
         return C.CDLL(REF_LIB), "hsref_"
     return C.CDLL(PORT_LIB), "hso_"
+
+
+def _util_lib(kind: str):
+    if kind == "reference":
+        return C.CDLL(REF_UTIL_LIB), "hsref_"
+    return C.CDLL(PORT_LIB), "hso_"
+
+
+def util_available(kind: str) -> bool:
+    """the library behind normalize_angle / pose_difference_larger_than of `kind` is built"""
+    return os.path.exists(REF_UTIL_LIB if kind == "reference" else PORT_LIB)
+
+
+def normalize_angle(angles, kind: str = "port") -> np.ndarray:
+    """util::normalize_angle of each float of `angles` (the reference's own, or the C port's) -> float32 array"""
+    lib, p = _util_lib(kind)
+    fn = getattr(lib, p + "normalize_angle")
+    fn.restype = None
+    fn.argtypes = [_f32p, C.c_int, _f32p]
+    a = _f32(angles).reshape(-1)
+    out = np.zeros_like(a)
+    fn(a, a.size, out)
+    return out
+
+
+def pose_difference_larger_than(p1, p2, dist, ang, kind: str = "port") -> np.ndarray:
+    """util::poseDifferenceLargerThan of each row pair of p1 / p2 (n, 3) with per-row thresholds -> bool array"""
+    lib, p = _util_lib(kind)
+    fn = getattr(lib, p + "pose_difference_larger_than")
+    fn.restype = None
+    fn.argtypes = [_f32p, _f32p, _f32p, _f32p, C.c_int, _i32p]
+    a, b = _f32(p1).reshape(-1, 3), _f32(p2).reshape(-1, 3)
+    n = a.shape[0]
+    d, g = np.broadcast_to(_f32(dist), (n,)).copy(), np.broadcast_to(_f32(ang), (n,)).copy()
+    out = np.zeros(n, np.int32)
+    fn(a, b, d, g, n, out)
+    return out != 0
 
 
 def scan_to_points(ranges, angle_min, angle_increment, range_min, range_max, scale_to_map, kind: str = "port"):

@@ -22,7 +22,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, angle_diff, golden_planes, load_golden, report
-from oracle import hessian64, record_oracle
+from oracle import hessian64, pose32, record_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -31,15 +31,6 @@ CASES = [(1, 1, 4), (1, 2, 4), (2, 1, 4), (2, 2, 4), (4, 1, 4), (8, 1, 4), (16, 
          (1, 32, 4), (1, 1, 8), (2, 1, 8), (8, 1, 5), (16, 1, 3)]
 RESET = dict(warps_per_scan=0, scans_per_block=0, unroll=0, stage_smem=1, partial=1, packed=0, seq=0, inline_scan=0,
              host_out=1)
-
-
-def normalize_angle(a):
-    """util::normalize_angle (UtilFunctions.h:37-49), double arithmetic narrowed to float like the kernel"""
-    r = math.fmod(math.fmod(float(a), 2 * math.pi) + 2 * math.pi, 2 * math.pi)
-    r = float(np.float32(r))
-    if r > math.pi:
-        r = float(np.float32(r - 2 * math.pi))
-    return np.float32(r)
 
 
 class Golden:
@@ -186,7 +177,7 @@ def test_record_consistency(G3):
                 assert np.all(r["H"][b] == 0) and np.all(r["dTr"][b] == 0) and np.all(r["est"][b] == 0), (b, l)
                 continue
             last = r["est"][b, -1]
-            nxt = rep.world_coords_pose(l, np.float32([last[0], last[1], normalize_angle(last[2])]))
+            nxt = rep.world_coords_pose(l, np.float32([last[0], last[1], pose32.normalize_angle(last[2])]))
         assert np.array_equal(bits(P[b]), bits(nxt)), b
         if n:
             assert np.array_equal(bits(C[b]), bits(recs[0]["H"][b, -1])), b

@@ -6,23 +6,9 @@ import numpy as np
 import pytest
 
 from conftest import load_golden, pose_err
+from oracle import pose32
 
 pytestmark = pytest.mark.gpu
-
-
-def host_gate(p1, p2, dist, ang):
-    """util::poseDifferenceLargerThan (UtilFunctions.h:73-92) in fp32 / double pi, as the façade has it."""
-    f = np.float32
-    with np.errstate(over="ignore", invalid="ignore"):
-        dx, dy = f(p1[0]) - f(p2[0]), f(p1[1]) - f(p2[1])
-        if np.sqrt(f(dx * dx) + f(dy * dy), dtype=f) > f(dist):
-            return True
-        a = f(f(p1[2]) - f(p2[2]))
-    if float(a) > np.pi:
-        a = f(float(a) - np.pi * 2.0)
-    elif float(a) < -np.pi:
-        a = f(float(a) + np.pi * 2.0)
-    return abs(a) > f(ang)
 
 
 @pytest.mark.parametrize("thresholds", [(0.0, 0.0), (0.35, 0.05)])
@@ -45,7 +31,7 @@ def test_fused_equals_host_driven_step(hsb_lib, thresholds):
         scan = g["scans"][k]
         pf, cf, uf = fused.slam_update(hint_f, scan)
         pp, cp = plain.matchData(hint_p, scan)
-        up = host_gate(pp, last, dist, ang)
+        up = pose32.pose_difference_larger_than(pp, last, dist, ang)
         if up:
             plain.updateByScan(scan, pp)
             plain.onMapUpdated()

@@ -13,27 +13,49 @@ from conftest import ROOT
 SRC = r'''
 #include <cstdio>
 #include <cmath>
+#include <cstring>
+#include <cstdint>
+#include <cfloat>
 #include "sincosf_glibc.h"
+static bool same(float a, float b) { uint32_t x, y; memcpy(&x, &a, 4); memcpy(&y, &b, 4); return x == y || (a != a && b != b); }
+static long n = 0, bad = 0, bad_large = 0;
+static void check(float x) {
+  ++n;
+  float sc, cc; hsb::sincosf_glibc(x, &sc, &cc);
+  const float s = sinf(x), c = cosf(x);
+  const long b = !same(hsb::sinf_glibc(x), s) + !same(hsb::cosf_glibc(x), c) + (!same(sc, s) || !same(cc, c));
+  bad += b;
+  if (!(fabsf(x) < 120.f)) bad_large += b;
+}
+static float from_bits(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 int main() {
-  long bad = 0, n = 0; unsigned s = 2463534242u;
+  unsigned s = 2463534242u;
   for (long i = 0; i < 12000000; ++i) {
     s = s * 1664525u + 1013904223u;
     float u = (float)(s >> 8) / 16777216.0f * 2.f - 1.f;
-    float x = (i % 3 == 0) ? u * 3.1415927f : (i % 3 == 1) ? u * 119.9f : ldexpf(u, -(int)(i % 40));
-    ++n;
-    if (hsb::sinf_glibc(x) != sinf(x)) ++bad;
-    if (hsb::cosf_glibc(x) != cosf(x)) ++bad;
-    float sc, cc; hsb::sincosf_glibc(x, &sc, &cc);
-    if (sc != sinf(x) || cc != cosf(x)) ++bad;
+    check((i % 3 == 0) ? u * 3.1415927f : (i % 3 == 1) ? u * 119.9f : ldexpf(u, -(int)(i % 40)));
   }
   const float edge[] = {0.f, -0.f, 0.78539816f, 0.785398185f, 0.78539822f, 1.5707963f, 3.1415927f, -3.1415927f, 6.2831855f,
-                        2.4414062e-4f, 2.4414065e-4f, 119.99999f};
-  for (float x : edge) {
-    if (hsb::sinf_glibc(x) != sinf(x)) ++bad; if (hsb::cosf_glibc(x) != cosf(x)) ++bad;
-    float sc, cc; hsb::sincosf_glibc(x, &sc, &cc);
-    if (sc != sinf(x) || cc != cosf(x)) ++bad;
+                        2.4414062e-4f, 2.4414065e-4f, 119.99999f, 120.f, -120.f, FLT_MAX, -FLT_MAX, INFINITY, -INFINITY, NAN,
+                        -NAN, 3.4e38f, -3.4e38f};
+  for (float x : edge) check(x);
+  // glibc's large-argument reduction: random bit patterns with 120 <= |y| < inf, every exponent, both signs
+  uint64_t r = 88172645463325252ull;
+  for (long i = 0; i < 6000000; ++i) {
+    r ^= r << 13; r ^= r >> 7; r ^= r << 17;
+    const uint32_t lo = 0x42f00000u, hi = 0x7f800000u;   // 120.f .. inf
+    check(from_bits((uint32_t)(lo + (r >> 8) % (hi - lo)) | (uint32_t)(r & 1) << 31));
   }
-  std::printf("%ld %ld\n", n, bad);
+  // every float in [119.99, 120.01], both signs: the switch between the two reductions
+  for (float x = 119.99f; x <= 120.01f; x = nextafterf(x, 1e9f)) { check(x); check(-x); }
+  // multiples of pi/2 up to 1e6, +-2 ulp: the largest reduced arguments relative to the result
+  for (long k = 1; k <= 636620; ++k) {
+    const float m = (float)(k * 1.5707963267948966);
+    float lo = m, hi = m;
+    for (int j = 0; j < 2; ++j) { lo = nextafterf(lo, 0.f); hi = nextafterf(hi, 1e9f); }
+    for (float x = lo; x <= hi; x = nextafterf(x, 1e9f)) { check(x); check(-x); }
+  }
+  std::printf("%ld %ld %ld\n", n, bad, bad_large);
   return bad ? 1 : 0;
 }
 '''
@@ -52,8 +74,52 @@ def test_sincosf_matches_libm(tmp_path):
     subprocess.run([cxx, "-O2", "-I", os.path.join(ROOT, "hector_slam_b200", "csrc"), str(src), "-o", str(exe), "-lm"],
                    check=True)
     out = subprocess.run([str(exe)], capture_output=True, text=True)
-    n, bad = (int(v) for v in out.stdout.split())
-    assert bad == 0 and n == 12000000, out.stdout
+    n, bad, bad_large = (int(v) for v in out.stdout.split())
+    assert bad == 0 and n > 12000000 + 6000000 + 5 * 636620, f"{n} arguments, {bad} mismatches ({bad_large} at |x| >= 120)"
+
+
+def _pi_fixed(bits):
+    """floor(pi * 2^bits), Machin's formula in integers (20 guard bits)"""
+    one = 1 << (bits + 20)
+
+    def arctan_inv(x):
+        s = t = one // x
+        k, x2, sign = 1, x * x, -1
+        while t:
+            t //= x2
+            s += sign * (t // (2 * k + 1))
+            k, sign = k + 1, -sign
+        return s
+
+    return (16 * arctan_inv(5) - 4 * arctan_inv(239)) >> 20
+
+
+def _inv_pio4_words():
+    """word i = floor(4/pi * 2^(8i+7)) mod 2^32: overlapping 32-bit windows of 4/pi at 8-bit steps"""
+    B = 400
+    inv = (4 << (2 * B)) // _pi_fixed(B)   # 4/pi * 2^B, exact in far more bits than the 24 words need
+    return [((inv << (8 * i + 7)) >> B) & 0xffffffff for i in range(24)]
+
+
+def test_inv_pio4_table():
+    """the header's 4/pi table is 4/pi's binary expansion, computed here from pi; where the running libm is a glibc
+    shared object, the same 96 bytes are in it (its __inv_pio4)"""
+    import ctypes.util
+    import re
+    import struct
+
+    want = _inv_pio4_words()
+    assert want[:4] == [0xa2, 0xa2f9, 0xa2f983, 0xa2f9836e]
+    text = open(os.path.join(ROOT, "hector_slam_b200", "csrc", "sincosf_glibc.h")).read()
+    body = re.search(r"#define HSB_INV_PIO4_TABLE((?:.*\\\n)*.*)", text).group(1)
+    got = [int(w, 16) for w in re.findall(r"0x([0-9a-f]{8})u", body)]
+    assert got == want
+    libm = ctypes.util.find_library("m")
+    path = next((os.path.join(d, libm) for d in ("/lib/x86_64-linux-gnu", "/usr/lib/x86_64-linux-gnu", "/lib64", "/usr/lib64")
+                 if libm and os.path.exists(os.path.join(d, libm))), None)
+    if path is None:
+        pytest.skip("no libm shared object found to cross-check against")
+    assert struct.pack("<24I", *want) in open(path, "rb").read()
 
 
 EXP_SRC = r'''
