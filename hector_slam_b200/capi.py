@@ -41,7 +41,7 @@ EXPORTED = [
     "hsb_group_slam_update_projected", "hsb_match_batch_projected", "hsb_match_batch_projected_submit",
     "hsb_match_batch_projected_device",
     "hsb_group_slam_update_subset", "hsb_group_slam_update_cloud_subset", "hsb_group_slam_update_ranges_subset",
-    "hsb_group_slam_update_projected_subset",
+    "hsb_group_slam_update_projected_subset", "hsb_group_sync_occupancy", "hsb_group_sync_occupancy_subset",
 ]
 
 
@@ -196,6 +196,8 @@ def load_library() -> C.CDLL:
     sig("hsb_group_slam_update_cloud_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_slam_update_ranges_subset", i, vp, i, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_slam_update_projected_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
+    sig("hsb_group_sync_occupancy", i, vp, i, vp, vp, i)
+    sig("hsb_group_sync_occupancy_subset", i, vp, i, vp, i, vp, vp, i)
     _lib = L
     return L
 
@@ -1018,6 +1020,30 @@ class SlamGroup:
         else:
             self._check(self.lib.hsb_group_slam_update_projected_subset(self.g, K, _ptr(mem), *args))
         return poses, cov.reshape(K, 3, 3), upd.astype(bool), kept.astype(int)
+
+    def sync_occupancy(self, level: int, grids, members=None, reset: bool = True):
+        """publishMap for the members in one pass (hsb_group_sync_occupancy): grids are one C-contiguous int8
+        (size_y, size_x) array per session, kept by the caller between calls; the cells of each member's mirror
+        rectangle are rewritten in place, no other byte is touched.  members as in slam_update
+        (hsb_group_sync_occupancy_subset).  -> one (x0, y0, x1, y1) per session, or None where the map did not change."""
+        K, mem = self._sessions(members)
+        assert len(grids) == K, (len(grids), K)
+        shape = None
+        if 0 <= level < self.reps[0].levels:   # (an invalid level is the C call's rejection)
+            sx, sy, _ = self.reps[0].level_info(level)
+            shape = (sy, sx)
+        for a in grids:
+            assert isinstance(a, np.ndarray) and a.dtype == np.int8 and a.flags.c_contiguous, "grids: C-contiguous int8"
+            assert shape is None or a.shape == shape, (a.shape, shape)
+        arr = (C.c_void_p * max(1, K))(*[a.ctypes.data for a in grids])
+        rects = np.zeros((max(1, K), 4), np.int32)
+        if mem is None:
+            self._check(self.lib.hsb_group_sync_occupancy(self.g, int(level), C.cast(arr, C.c_void_p), rects.ctypes.data,
+                                                          int(bool(reset))))
+        else:
+            self._check(self.lib.hsb_group_sync_occupancy_subset(self.g, K, _ptr(mem), int(level), C.cast(arr, C.c_void_p),
+                                                                 rects.ctypes.data, int(bool(reset))))
+        return [None if r[2] < r[0] else tuple(int(v) for v in r) for r in rects[:K]]
 
     def _sessions(self, members):
         """-> (sessions of the step, the member list as int32, or None for a step of every member)"""

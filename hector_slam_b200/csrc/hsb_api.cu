@@ -100,6 +100,7 @@ struct hsb_handle {
   float min_dist = 0.4f, min_angle = 0.13f;   // HectorSlamProcessor.h:62-63 defaults
   // tuning
   int tune_warps_per_scan = 0, tune_scans_per_block = 0, tune_stage_smem = 1, tune_chunk = 0, tune_unroll = 0, tune_packed = 0, tune_seq = 0, tune_partial = 1, tune_prefetch = 0, tune_trace = 0, tune_pace = 0, tune_pdl = 1, tune_auto_group = 1, tune_stagger = 0, tune_fixpoint = 1;
+  int tune_occ_chunk = 0;   // > 0: staging bytes per chunk of a group occupancy sync whose handles[0] this is
   DevBuf d_trace;
   DevBuf d_best;   // arg-max accumulator of hsb_best_hypothesis_device
   DevBuf d_record; // per-evaluation record of hsb_match_data_record
@@ -885,6 +886,7 @@ int hsb_set_tuning(hsb_handle* h, const char* key, int value) {
   else if (!strcmp(key, "auto_group")) h->tune_auto_group = value;
   else if (!strcmp(key, "stagger")) h->tune_stagger = value;
   else if (!strcmp(key, "fixpoint")) h->tune_fixpoint = value;
+  else if (!strcmp(key, "occupancy_chunk")) h->tune_occ_chunk = value;
   else return fail(h, HSB_ERR_INVALID_ARG, "hsb_set_tuning: unknown key '%s'", key);
   return HSB_OK;
 }
@@ -2415,6 +2417,15 @@ struct hsb_group {
   size_t h_stage_bytes = 0;
   DevBuf d_stage;
   unsigned seq = 0;
+  // occupancy sync (hsb_group_sync_occupancy): M x levels pointers to the members' mirror rectangles (Level::dirty + 4),
+  // member-major like d_lv; the call's member list, gathered rectangles and row table (device and pinned twin, sized
+  // for M sessions); the packed rows of one chunk (device and pinned staging)
+  int** d_mirror = nullptr;
+  char* d_occ_meta = nullptr;
+  char* h_occ_meta = nullptr;
+  DevBuf d_occ_rows;
+  int8_t* h_occ_rows = nullptr;
+  size_t h_occ_rows_bytes = 0;
 };
 
 namespace {
@@ -2431,6 +2442,16 @@ int group_fail(hsb_handle* h, int code, const char* fmt, ...) {
   return code;
 }
 
+// Layout of hsb_group::d_occ_meta / h_occ_meta for up to K sessions: member list | gathered rectangles | row table
+struct OccMeta {
+  size_t members = 0, rects, rows, bytes;
+  explicit OccMeta(int K) {
+    rects = ((size_t)K * sizeof(int) + 15) & ~(size_t)15;
+    rows = rects + (size_t)K * sizeof(int4);
+    bytes = rows + (size_t)K * sizeof(HsbOccRowsDev);
+  }
+};
+
 }  // namespace
 
 extern "C" {
@@ -2442,6 +2463,11 @@ int hsb_group_destroy(hsb_group* g) {
   for (hsb_handle* h : g->m)
     if (h->group_ev == g->ev) h->group_ev = nullptr;   // the step it would wait for is complete
   if (g->d_lv) cudaFree(g->d_lv);
+  if (g->d_mirror) cudaFree(g->d_mirror);
+  if (g->d_occ_meta) cudaFree(g->d_occ_meta);
+  if (g->d_occ_rows.p) cudaFree(g->d_occ_rows.p);
+  if (g->h_occ_meta) cudaFreeHost(g->h_occ_meta);
+  if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
   if (g->d_res) cudaFree(g->d_res);
   if (g->d_stage.p) cudaFree(g->d_stage.p);
   if (g->h_res) cudaFreeHost(g->h_res);
@@ -2519,6 +2545,13 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
       for (int l = 0; l < g->levels; ++l) fill_level_dev(g->m[s], l, lv[(size_t)s * g->levels + l]);
     HSB_GROUP_CUDA(cudaMalloc(&g->d_lv, lv.size() * sizeof(HsbLevelDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_lv, lv.data(), lv.size() * sizeof(HsbLevelDev), cudaMemcpyHostToDevice));
+    std::vector<int*> mirror((size_t)M * g->levels);
+    for (int s = 0; s < M; ++s)
+      for (int l = 0; l < g->levels; ++l) mirror[(size_t)s * g->levels + l] = g->m[s]->lv[l].dirty + 4;
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_mirror, mirror.size() * sizeof(int*)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_mirror, mirror.data(), mirror.size() * sizeof(int*), cudaMemcpyHostToDevice));
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
+    HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
   }
   HSB_GROUP_CUDA(cudaMalloc(&g->d_res, ((size_t)M * 5 + 4) * sizeof(float)));
   HSB_GROUP_CUDA(cudaMemset(g->d_res, 0, ((size_t)M * 5 + 4) * sizeof(float)));
@@ -2554,26 +2587,50 @@ constexpr int kGroupW = 8;
 // One group step of any input kind over K of the group's members: session k steps member members[k] (a step of every
 // member passes K = M and g->all).  Members not listed are neither read nor changed.  Everything that can reject the
 // step is checked before any member's state moves.
-int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, const int* map_without_matching,
-               int nowait, float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
-  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is stepped
-  const int M = (int)g->m.size(), levels = g->levels;
-  if (K < 0 || K > M) return fail(h0, HSB_ERR_INVALID_ARG, "%s: K is %d, must be in [0, %d]", in.fn, K, M);
+// The member list of a group call over K sessions: 0 <= K <= M, and with K > 0 a list of distinct indices in [0, M).
+int check_members(hsb_group* g, const char* fn, int K, const int* members) {
+  hsb_handle* h0 = g->m[0];
+  const int M = (int)g->m.size();
+  if (K < 0 || K > M) return fail(h0, HSB_ERR_INVALID_ARG, "%s: K is %d, must be in [0, %d]", fn, K, M);
   if (K == 0) return HSB_OK;
-  if (!members) return fail(h0, HSB_ERR_INVALID_ARG, "%s: members is NULL with K = %d", in.fn, K);
+  if (!members) return fail(h0, HSB_ERR_INVALID_ARG, "%s: members is NULL with K = %d", fn, K);
   std::fill(g->listed.begin(), g->listed.end(), 0);
   for (int k = 0; k < K; ++k) {
     const int j = members[k];
     if (j < 0 || j >= M)
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is outside [0, %d)", in.fn, k, j, M);
-    if (g->listed[j]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is listed twice", in.fn, k, j);
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is outside [0, %d)", fn, k, j, M);
+    if (g->listed[j]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is listed twice", fn, k, j);
     g->listed[j] = 1;
   }
+  return HSB_OK;
+}
+
+// Orders the group's stream behind everything queued for the listed members: the work they queued themselves, and a
+// pending step of another group they belong to.
+int order_members(hsb_group* g, int K, const int* members) {
+  hsb_handle* h0 = g->m[0];
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
+    if (h->group_ev && h->group_ev != g->ev) HSB_CUDA(h0, cudaStreamWaitEvent(g->stream, h->group_ev, 0));
+    if (h->queued) {
+      const int s = order_before(h, g->stream, true);
+      if (s != HSB_OK) return s;
+      h->queued = false;
+    }
+  }
+  return HSB_OK;
+}
+
+int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, const int* map_without_matching,
+               int nowait, float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is stepped
+  const int M = (int)g->m.size(), levels = g->levels;
+  int s = check_members(g, in.fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
   const bool cloud = in.kind == HSB_IN_CLOUD;
   const bool conv = in.kind != HSB_IN_ENDPOINTS;   // converted on the device: the kept count decides what the session had
   const bool tf = cloud || in.kind == HSB_IN_PROJECTED;   // with a laser transform per session
   const int* offsets = in.offsets;
-  int s;
   if (!in.hints || !offsets || !out_poses)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
   if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", in.fn, offsets[0]);
@@ -2596,15 +2653,7 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   if (conv && !staging_fits<kGroupW, 1>(whole_scan_slots(max_n), 1)) return fail_fused_too_long(h0, max_n);
   DeviceGuard guard(g->device);
   cudaStream_t st = g->stream;
-  // not before the work the members queued themselves, nor before a pending step of another group they belong to
-  for (int k = 0; k < K; ++k) {
-    hsb_handle* h = g->m[members[k]];
-    if (h->group_ev && h->group_ev != g->ev) HSB_CUDA(h0, cudaStreamWaitEvent(st, h->group_ev, 0));
-    if (h->queued) {
-      if ((s = order_before(h, st, true)) != HSB_OK) return s;
-      h->queued = false;
-    }
-  }
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
 
   // staging: hints | gate inputs | offsets | session descriptors | map-writer descriptors | increments |
   // laser transforms (cloud, projected) | scans
@@ -2771,9 +2820,136 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   return HSB_OK;
 }
 
+// Packed bytes of one device-to-host copy of a group occupancy sync (pinned staging owned by the group).  A larger total
+// goes in chunks split at row boundaries; hsb_set_tuning(handles[0], "occupancy_chunk", bytes) overrides it.  A chunk
+// always holds at least one row.
+constexpr size_t kOccChunkBytes = 32u << 20;
+
+// publishMap's grid for K members in one pass: gather (and clear) their mirror rectangles of `level` with one launch,
+// one synchronise to size the payload, then per chunk one threshold launch, one device-to-host copy and one synchronise,
+// and the rows scattered into grids[k] on the host.
+int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members, int level, int8_t* const* grids,
+                         int* out_rects, int reset) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (level < 0 || level >= g->levels)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if (!grids) return fail(h0, HSB_ERR_INVALID_ARG, "%s: grids is NULL", fn);
+  for (int k = 0; k < K; ++k)
+    if (!grids[k]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: grid is NULL", fn, k);
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
+
+  // pass 1: the rectangles, gathered and (reset) cleared in order behind the members' queued map writes
+  const OccMeta lay(K);
+  const int sx = h0->lv[level].sx;
+  memcpy(g->h_occ_meta, members, (size_t)K * sizeof(int));
+  HSB_CUDA(h0, cudaMemcpyAsync(g->d_occ_meta, g->h_occ_meta, (size_t)K * sizeof(int), cudaMemcpyHostToDevice, st));
+  hsb::gather_mirror_rects_kernel<<<(K + 127) / 128, 128, 0, st>>>(
+      g->d_mirror, g->levels, level, reinterpret_cast<const int*>(g->d_occ_meta), K, reset,
+      reinterpret_cast<int4*>(g->d_occ_meta + lay.rects));
+  h0->launches++;
+  HSB_CUDA(h0, cudaGetLastError());
+  HSB_CUDA(h0, cudaMemcpyAsync(g->h_occ_meta + lay.rects, g->d_occ_meta + lay.rects, (size_t)K * sizeof(int4),
+                               cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h0, cudaStreamSynchronize(st));
+  const int* rects = reinterpret_cast<const int*>(g->h_occ_meta + lay.rects);
+  if (out_rects) memcpy(out_rects, rects, (size_t)K * 4 * sizeof(int));
+
+  // the row table of the non-empty rectangles, in session order
+  HsbOccRowsDev* rows = reinterpret_cast<HsbOccRowsDev*>(g->h_occ_meta + lay.rows);
+  std::vector<int> sess;   // session of each row-table entry
+  int n_rows = 0, total_rows = 0;
+  size_t total = 0;
+  for (int k = 0; k < K; ++k) {
+    const int* r = rects + 4 * k;
+    if (r[2] < r[0] || r[3] < r[1]) continue;   // clean: the map did not change
+    hsb_handle* h = g->m[members[k]];
+    HsbOccRowsDev& e = rows[n_rows++];
+    e.logodds = h->lv[level].logodds;
+    e.sx = sx;
+    e.x0 = r[0];
+    e.y0 = r[1];
+    e.w = r[2] - r[0] + 1;
+    e.row0 = total_rows;
+    e.off = total;
+    const int hgt = r[3] - r[1] + 1;
+    total_rows += hgt;
+    total += (size_t)e.w * hgt;
+    h->d2h_bytes += (size_t)e.w * hgt;
+    sess.push_back(k);
+  }
+  if (n_rows == 0) return HSB_OK;
+  HSB_CUDA(h0, cudaMemcpyAsync(g->d_occ_meta + lay.rows, rows, (size_t)n_rows * sizeof(HsbOccRowsDev),
+                               cudaMemcpyHostToDevice, st));
+
+  // pass 2: chunks of whole rows
+  const size_t cap = std::max<size_t>(h0->tune_occ_chunk > 0 ? (size_t)h0->tune_occ_chunk : kOccChunkBytes, (size_t)sx);
+  if (std::min(cap, total) > g->h_occ_rows_bytes) {   // grown geometrically: dirty areas creep up from call to call
+    const size_t stage = std::min(cap, std::max(total, 2 * g->h_occ_rows_bytes));
+    if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
+    g->h_occ_rows = nullptr;
+    g->h_occ_rows_bytes = 0;
+    HSB_CUDA(h0, cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_rows), stage));
+    g->h_occ_rows_bytes = stage;
+    if ((s = ensure(h0, g->d_occ_rows, stage)) != HSB_OK) return s;
+  }
+  int8_t* d_out = static_cast<int8_t*>(g->d_occ_rows.p);
+  int e = 0, y = 0;   // the chunk starts at row y of row-table entry e
+  while (e < n_rows) {
+    const int e_begin = e, y_begin = y;
+    const size_t base = rows[e].off + (size_t)y * rows[e].w;
+    size_t bytes = 0;
+    while (e < n_rows) {   // whole rectangles while they fit, then as many rows of the next one as fit
+      const int w = rows[e].w, left = rects[4 * sess[e] + 3] - rects[4 * sess[e] + 1] + 1 - y;
+      const size_t fit = (cap - bytes) / (size_t)w;
+      if (fit >= (size_t)left) {
+        bytes += (size_t)left * w;
+        ++e;
+        y = 0;
+      } else {
+        bytes += fit * w;
+        y += (int)fit;
+        break;
+      }
+    }
+    const int r_begin = rows[e_begin].row0 + y_begin, r_end = (e < n_rows ? rows[e].row0 + y : total_rows);
+    const int blocks = (int)std::min<long>(((long)(r_end - r_begin) + 7) / 8, (long)h0->sm_count * 16);
+    hsb::occupancy_rows_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const HsbOccRowsDev*>(g->d_occ_meta + lay.rows),
+                                                       n_rows, r_begin, r_end, base, d_out);
+    h0->launches++;
+    HSB_CUDA(h0, cudaGetLastError());
+    HSB_CUDA(h0, cudaMemcpyAsync(g->h_occ_rows, d_out, bytes, cudaMemcpyDeviceToHost, st));
+    HSB_CUDA(h0, cudaStreamSynchronize(st));
+    // scatter the chunk's rows into the callers' grids
+    const int8_t* src = g->h_occ_rows;
+    for (int ee = e_begin, yy = y_begin; src < g->h_occ_rows + bytes; ++ee, yy = 0) {
+      const HsbOccRowsDev& d = rows[ee];
+      const int hgt = rects[4 * sess[ee] + 3] - d.y0 + 1;
+      for (; yy < hgt && src < g->h_occ_rows + bytes; ++yy, src += d.w)
+        memcpy(grids[sess[ee]] + (size_t)(d.y0 + yy) * sx + d.x0, src, (size_t)d.w);
+    }
+  }
+  return HSB_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int hsb_group_sync_occupancy(hsb_group* g, int level, int8_t* const* grids, int* out_rects, int reset) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_sync_occupancy(g, "hsb_group_sync_occupancy", (int)g->m.size(), g->all.data(), level, grids, out_rects,
+                              reset);
+}
+
+int hsb_group_sync_occupancy_subset(hsb_group* g, int K, const int* members, int level, int8_t* const* grids,
+                                    int* out_rects, int reset) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_sync_occupancy(g, "hsb_group_sync_occupancy_subset", K, members, level, grids, out_rects, reset);
+}
 
 int hsb_group_slam_update(hsb_group* g, const float* hints, const float* points_xy, const int* offsets, const float* origo,
                           const int* map_without_matching, int nowait, float* out_poses, float* cov_inout, int* map_updated) {

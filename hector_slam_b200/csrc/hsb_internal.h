@@ -175,6 +175,16 @@ struct HsbUpdateParams {
   const float* gate_flag;    // if set, *gate_flag == 0 turns the launch into a no-op (slam_gate_kernel in update_kernel.cuh)
 };
 
+// One non-empty rectangle of a group occupancy sync (hsb_group_sync_occupancy): the rows of all the call's rectangles are
+// numbered consecutively in session order; this one owns rows [row0, row0 + its height) and the packed bytes from off on
+// (w bytes per row).
+struct HsbOccRowsDev {
+  const float* logodds;   // the member's log-odds plane of the level
+  int sx, x0, y0, w;
+  int row0;
+  size_t off;
+};
+
 // Map write of a group SLAM step (update_mark_group_kernel / update_apply_group_kernel): blockIdx.z = session,
 // blockIdx.y = level.  Everything per session lives in device memory, uploaded with the step's scans.
 struct HsbGroupUpdateParams {

@@ -69,12 +69,15 @@ __global__ void clear_level_kernel(float* __restrict__ logodds, float* __restric
 }
 
 // N1: nav_msgs/OccupancyGrid values as HectorMappingRos::publishMap derives them
-// (hector_mapping/src/HectorMappingRos.cpp:448-468; isFree / isOccupied GridMapLogOdds.h:76-84).
+// (hector_mapping/src/HectorMappingRos.cpp:448-468; isFree / isOccupied GridMapLogOdds.h:76-84): 0 where l < 0, 100
+// where l > 0, -1 otherwise (+-0 and NaN).  Every occupancy export thresholds with this one expression.
+__device__ __forceinline__ int8_t occupancy_value(float l) {
+  return l < 0.0f ? (int8_t)0 : (l > 0.0f ? (int8_t)100 : (int8_t)-1);
+}
+
 __global__ void occupancy_kernel(const float* __restrict__ logodds, int8_t* __restrict__ out, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float l = logodds[i];
-    out[i] = l < 0.0f ? (int8_t)0 : (l > 0.0f ? (int8_t)100 : (int8_t)-1);
-  }
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = occupancy_value(logodds[i]);
 }
 
 // N1 on a rectangle: the cells of {x0, y0, w, hgt} thresholded into a packed w x hgt buffer (dirty-rectangle publishing).
@@ -83,8 +86,44 @@ __global__ void occupancy_rect_kernel(const float* __restrict__ logodds, int sx,
   const size_t n = (size_t)w * hgt;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int r = (int)(i / (size_t)w), c = (int)(i - (size_t)r * w);
-    const float l = logodds[(size_t)(y0 + r) * sx + (x0 + c)];
-    out[i] = l < 0.0f ? (int8_t)0 : (l > 0.0f ? (int8_t)100 : (int8_t)-1);
+    out[i] = occupancy_value(logodds[(size_t)(y0 + r) * sx + (x0 + c)]);
+  }
+}
+
+// Group occupancy sync, pass 1: session k's mirror rectangle of `level` (member members[k]'s, found through the group's
+// table mirror[member * levels + level]) into rects[4k ..], then, with reset, the rectangle cleared.
+__global__ void gather_mirror_rects_kernel(int* const* __restrict__ mirror, int levels, int level,
+                                           const int* __restrict__ members, int K, int reset, int4* __restrict__ rects) {
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < K; k += gridDim.x * blockDim.x) {
+    int* r = mirror[(size_t)members[k] * levels + level];
+    rects[k] = make_int4(r[0], r[1], r[2], r[3]);
+    if (reset) {
+      r[0] = INT_MAX;
+      r[1] = INT_MAX;
+      r[2] = -1;
+      r[3] = -1;
+    }
+  }
+}
+
+// Group occupancy sync, pass 2: rows [r_begin, r_end) of the call's stacked rectangles (HsbOccRowsDev) thresholded into
+// the packed chunk `out`, whose first byte is the call's packed byte `out_base`.  One warp per row, lanes along the row:
+// coalesced reads, each cell read once.  n_rows: the entries of `rows` (non-empty rectangles only).
+__global__ void occupancy_rows_kernel(const HsbOccRowsDev* __restrict__ rows, int n_rows, int r_begin, int r_end,
+                                      size_t out_base, int8_t* __restrict__ out) {
+  const int warps = blockDim.x >> 5, lane = threadIdx.x & 31;
+  for (int r = r_begin + blockIdx.x * warps + (threadIdx.x >> 5); r < r_end; r += gridDim.x * warps) {
+    int lo = 0, hi = n_rows - 1;   // the last rectangle that starts at or before row r
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (rows[mid].row0 <= r) lo = mid;
+      else hi = mid - 1;
+    }
+    const HsbOccRowsDev s = rows[lo];
+    const int y = r - s.row0;
+    const float* src = s.logodds + (size_t)(s.y0 + y) * s.sx + s.x0;
+    int8_t* dst = out + (s.off + (size_t)y * s.w - out_base);
+    for (int x = lane; x < s.w; x += 32) dst[x] = occupancy_value(src[x]);
   }
 }
 

@@ -271,6 +271,39 @@ class SlamProcessor {
   }
   // getGridMap(level): the log-odds plane, row-major [sizeY][sizeX]
   void getGridMap(int level, float* logodds_out) const { check(hsb_download_level(h_, level, logodds_out)); }
+
+  // HectorMappingRos::publishMap's grid kept up to date (HectorMappingRos.cpp:435-481): grid is this processor's whole
+  // level, sizeY x sizeX int8 row-major, kept between calls as the node keeps map_.map.data.  The cells written since the
+  // last call (the mirror rectangle, which this consumes) get publishMap's values (0 free, 100 occupied, -1 unknown); no
+  // other byte is touched.  rect (may be null) receives {x0, y0, x1, y1}; x1 < x0: nothing changed, nothing to publish.
+  void syncOccupancy(int level, int8_t* grid, int rect[4] = 0) {
+    int r[4];
+    check(hsb_get_mirror_dirty_rect(h_, level, r, 1));
+    if (rect) std::memcpy(rect, r, sizeof(r));
+    if (r[2] < r[0] || r[3] < r[1]) return;
+    int sx = 0, sy = 0;
+    float cl = 0.f;
+    check(hsb_get_level_info(h_, level, &sx, &sy, &cl));
+    const int w = r[2] - r[0] + 1, hgt = r[3] - r[1] + 1;
+    std::vector<int8_t> rows((size_t)w * hgt);
+    check(hsb_download_occupancy_rect(h_, level, r, rows.data()));
+    for (int y = 0; y < hgt; ++y) std::memcpy(grid + (size_t)(r[1] + y) * sx + r[0], &rows[(size_t)y * w], (size_t)w);
+  }
+
+  // syncOccupancy() for M processors in one pass (hsb_group_sync_occupancy, through the group updateMany keeps):
+  // grids[s] is processor s's grid, rects (4M ints, may be null) receives each rectangle.
+  static void syncOccupancyMany(SlamProcessor* const* ps, int M, int level, int8_t* const* grids, int* rects = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "syncOccupancyMany");
+    owner.check(hsb_group_sync_occupancy(owner.groupFor(ps, M), level, grids, rects, 1));
+  }
+
+  // syncOccupancyMany() for the processors ps[members[0..K)] (hsb_group_sync_occupancy_subset): grids[k] and
+  // rects[4k..] belong to ps[members[k]]; the processors not listed are left as they are.
+  static void syncOccupancyMany(SlamProcessor* const* ps, int M, const int* members, int K, int level,
+                                int8_t* const* grids, int* rects = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "syncOccupancyMany");
+    owner.check(hsb_group_sync_occupancy_subset(owner.groupFor(ps, M), K, members, level, grids, rects, 1));
+  }
   hsb_handle* handle() { return h_; }
 
   // util::poseDifferenceLargerThan, util/UtilFunctions.h:73-92 (float norm, double pi arithmetic)
@@ -296,14 +329,12 @@ class SlamProcessor {
   template <class Step>
   static void stepMany(SlamProcessor* const* ps, int M, const int* members, int K, const Pose* poseHintsWorld,
                        const char* what, Step step) {
-    if (!ps || M < 1 || !ps[0])
-      throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs M >= 1 processors");
+    SlamProcessor& owner = groupOwnerOf(ps, M, what);
     if (K < 0 || K > M || (K > 0 && !members && K != M))
       throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs 0 <= K <= M and a member list");
     for (int k = 0; members && k < K; ++k)
       if (members[k] < 0 || members[k] >= M)
         throw std::invalid_argument(std::string("hector_slam_b200: ") + what + ": a member index is outside [0, M)");
-    SlamProcessor& owner = *ps[0];
     hsb_group* g = owner.groupFor(ps, M);
     std::vector<float> hints(3 * (size_t)K), poses(3 * (size_t)K), cov(9 * (size_t)K);
     std::vector<int> updated(K);
@@ -321,6 +352,12 @@ class SlamProcessor {
       if (updated[s]) p.lastMapUpdatePose_ = p.lastScanMatchPose_;                    // :94
       std::memcpy(p.lastScanMatchCov_, &cov[9 * s], sizeof(p.lastScanMatchCov_));
     }
+  }
+  // ps[0], which keeps the group of ps[0..M)
+  static SlamProcessor& groupOwnerOf(SlamProcessor* const* ps, int M, const char* what) {
+    if (!ps || M < 1 || !ps[0])
+      throw std::invalid_argument(std::string("hector_slam_b200: ") + what + " needs M >= 1 processors");
+    return *ps[0];
   }
   // the cached group of updateMany: rebuilt only when the member list changes.  A processor belongs to at most one
   // cached group (its groupOwner_), so that destroying any member destroys that group first.

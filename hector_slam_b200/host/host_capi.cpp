@@ -231,6 +231,35 @@ int hsbp_update_many_projected_subset(void* const* ps, int M, const int* members
   }
   return 0;
 }
+int hsbp_sync_occupancy(void* p, int level, int8_t* grid, int* rect) {
+  try {
+    static_cast<hsb200::SlamProcessor*>(p)->syncOccupancy(level, grid, rect);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_sync_occupancy_many(void* const* ps, int M, int level, int8_t* const* grids, int* rects) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::syncOccupancyMany(procs.data(), M, level, grids, rects);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_sync_occupancy_many_subset(void* const* ps, int M, const int* members, int K, int level, int8_t* const* grids,
+                                    int* rects) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::syncOccupancyMany(procs.data(), M, members, K, level, grids, rects);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

@@ -477,6 +477,30 @@ int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* membe
                                            const float* ranges, const int* offsets, const double* transforms,
                                            const int* map_without_matching, int nowait, float* out_poses_world,
                                            float* cov_inout, int* map_updated, int* out_kept);
+/* HectorMappingRos::publishMap (hector_mapping/src/HectorMappingRos.cpp:435-481) for K of the group's members in one
+ * pass.  Session k is member members[k] (the full form: every member, in order).  grids[k] is the caller's whole-level
+ * grid of that member, size_y x size_x int8 row-major, kept between calls as the node keeps map_.map.data (:445-448).
+ * Let r be member k's mirror rectangle of `level` (hsb_get_mirror_dirty_rect) after all work already queued for it:
+ * out_rects[4k .. 4k+3] = r (out_rects may be NULL); x1 < x0 means the map did not change, so the caller skips
+ * publishing that robot (:440).  Every cell of r gets publishMap's value in grids[k][y * size_x + x] (0 where the
+ * log-odds l < 0, 100 where l > 0, -1 otherwise: +-0 and NaN), bit-identical to hsb_get_mirror_dirty_rect +
+ * hsb_download_occupancy_rect + a row-by-row copy; no other byte of grids[k] is read or written.  reset != 0 clears the
+ * mirror rectangle as hsb_get_mirror_dirty_rect(..., 1) does (the replication rectangle is untouched).  This call
+ * consumes the same rectangle that hsb_get_mirror_dirty_rect and MapRepB200::getGridMap consume: one consumer per
+ * handle.  A member not listed is neither read nor changed.
+ * Ordering: the call runs on the group's stream after everything queued on the listed members (their own work and a
+ * pending step of any group they belong to), and returns when every grid is written, so every later call on a member —
+ * its next step included, whose map write grows the rectangle this call cleared — runs after it.
+ * Cost: one launch gathers the K rectangles (one synchronise sizes the payload), then per chunk of at most 32 MiB of
+ * packed rows (rectangles are split at row boundaries) one threshold launch, one device-to-host copy into the group's
+ * pinned staging and one synchronise.  Launches are counted on handles[0]; hsb_get_d2h_bytes of each listed member
+ * grows by the area of its rectangle.
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued or cleared: K < 0 or K > M; members == NULL with K > 0;
+ * an index outside [0, M) or listed twice; level outside [0, levels); grids == NULL or a NULL grids[k] (the message
+ * names the session).  K = 0 returns HSB_OK, reads no other argument and queues nothing. */
+int hsb_group_sync_occupancy(hsb_group* g, int level, int8_t* const* grids, int* out_rects, int reset);
+int hsb_group_sync_occupancy_subset(hsb_group* g, int K, const int* members, int level, int8_t* const* grids,
+                                    int* out_rects, int reset);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
@@ -616,7 +640,8 @@ int hsb_get_gather_mode(const hsb_handle* h);
  * "prefetch" (1 = L2 bulk prefetch of the unstaged part of a scan), "unroll", "trace" (see hsb_read_trace),
  * "inline_scan" (1: hsb_match_data / hsb_slam_update send scans of up to 1280 endpoints inside the kernel launch
  * instead of through a host-to-device copy — slower per step in measurement, higher back-to-back rate; default 0),
- * "host_out".  Results never depend on them beyond summation order. */
+ * "host_out", "occupancy_chunk" (bytes of packed rows per chunk of a group occupancy sync whose handles[0] this handle
+ * is, 0 = 32 MiB; at least one row).  Results never depend on them beyond summation order. */
 int hsb_set_tuning(hsb_handle* h, const char* key, int value);
 /* Shape of the last match-kernel launch of this handle: {warps per scan, scans per CTA, gather batch (unroll),
  * endpoints of each scan staged in shared memory (0 = read through L1), grid size, resident CTAs per SM}.
