@@ -42,6 +42,7 @@ EXPORTED = [
     "hsb_match_batch_projected_device",
     "hsb_group_slam_update_subset", "hsb_group_slam_update_cloud_subset", "hsb_group_slam_update_ranges_subset",
     "hsb_group_slam_update_projected_subset", "hsb_group_sync_occupancy", "hsb_group_sync_occupancy_subset",
+    "hsb_group_get_dist", "hsb_group_get_dist_subset", "hsb_group_raycast", "hsb_group_raycast_subset",
 ]
 
 
@@ -198,6 +199,10 @@ def load_library() -> C.CDLL:
     sig("hsb_group_slam_update_projected_subset", i, vp, i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
     sig("hsb_group_sync_occupancy", i, vp, i, vp, vp, i)
     sig("hsb_group_sync_occupancy_subset", i, vp, i, vp, i, vp, vp, i)
+    sig("hsb_group_get_dist", i, vp, i, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_get_dist_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_raycast", i, vp, i, vp, vp, vp, vp, vp)
+    sig("hsb_group_raycast_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -1045,6 +1050,44 @@ class SlamGroup:
                                                                  rects.ctypes.data, int(bool(reset))))
         return [None if r[2] < r[0] else tuple(int(v) for v in r) for r in rects[:K]]
 
+    def get_dist(self, level: int, begin_world, end_world, members=None):
+        """DistanceMeasurementProvider::getDist for the members' rays in one pass (hsb_group_get_dist): begin_world and
+        end_world are one (n_s, 2) array of world points per session, or a tuple (points (Q, 2), offsets (K + 1,)).
+        members as in slam_update (hsb_group_get_dist_subset).  Each ray equals get_dist_batch on its member.
+        -> (dist [m] (Q,), hit_world (Q, 2), found (Q,) bool), in ray order"""
+        K, mem = self._sessions(members)
+        b, offsets = self._pack(begin_world, 2, K)
+        e, e_off = self._pack(end_world, 2, K)
+        assert np.array_equal(offsets, e_off), "begin_world and end_world hold different numbers of rays"
+        Q = b.shape[0]
+        dist, hit, found = np.zeros(Q, np.float32), np.zeros((Q, 2), np.float32), np.zeros(Q, np.int32)
+        args = (int(level), offsets.ctypes.data, _ptr(b if Q else None), _ptr(e if Q else None), dist.ctypes.data,
+                hit.ctypes.data, found.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_get_dist(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_get_dist_subset(self.g, K, _ptr(mem), *args))
+        return dist, hit, found.astype(bool)
+
+    def raycast(self, level: int, begin_cells, end_cells, members=None):
+        """checkOccupancyBresenhami for the members' rays in one pass (hsb_group_raycast): begin_cells and end_cells
+        are one (n_s, 2) int32 array of cells per session, or a tuple (cells (Q, 2), offsets (K + 1,)).  members as in
+        slam_update (hsb_group_raycast_subset).  Each ray equals raycast_batch on its member.
+        -> (dist (Q,) float32 [-1 = no hit], hit (Q, 2) int32), in ray order"""
+        K, mem = self._sessions(members)
+        b, offsets = self._pack(begin_cells, 2, K, np.int32)
+        e, e_off = self._pack(end_cells, 2, K, np.int32)
+        assert np.array_equal(offsets, e_off), "begin_cells and end_cells hold different numbers of rays"
+        Q = b.shape[0]
+        dist, hit = np.zeros(Q, np.float32), np.zeros((Q, 2), np.int32)
+        args = (int(level), offsets.ctypes.data, _ptr(b if Q else None), _ptr(e if Q else None), dist.ctypes.data,
+                hit.ctypes.data)
+        if mem is None:
+            self._check(self.lib.hsb_group_raycast(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_raycast_subset(self.g, K, _ptr(mem), *args))
+        return dist, hit
+
     def _sessions(self, members):
         """-> (sessions of the step, the member list as int32, or None for a step of every member)"""
         if members is None:
@@ -1052,15 +1095,17 @@ class SlamGroup:
         mem = np.ascontiguousarray(members, dtype=np.int32).reshape(-1)
         return mem.shape[0], mem
 
-    def _pack(self, scans, width, n):
+    def _pack(self, scans, width, n, dtype=np.float32):
         """n per-session arrays (n_s, width), or a tuple (points (N, width), offsets (n + 1,)) -> (points, offsets)."""
+        def arr(a):
+            return np.ascontiguousarray(a, dtype=dtype).reshape(-1, width)
         if isinstance(scans, tuple):
-            return _f32(scans[0]).reshape(-1, width), np.ascontiguousarray(scans[1], dtype=np.int32)
-        scans = [_f32(s).reshape(-1, width) for s in scans]
+            return arr(scans[0]), np.ascontiguousarray(scans[1], dtype=np.int32)
+        scans = [arr(s) for s in scans]
         assert len(scans) == n, (len(scans), n)
         offsets = np.zeros(n + 1, np.int32)
         offsets[1:] = np.cumsum([s.shape[0] for s in scans])
-        return (np.concatenate(scans) if offsets[-1] else np.zeros((0, width), np.float32)), offsets
+        return (np.concatenate(scans) if offsets[-1] else np.zeros((0, width), dtype)), offsets
 
     def close(self):
         if getattr(self, "g", None):

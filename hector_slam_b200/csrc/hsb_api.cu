@@ -2426,6 +2426,12 @@ struct hsb_group {
   DevBuf d_occ_rows;
   int8_t* h_occ_rows = nullptr;
   size_t h_occ_rows_bytes = 0;
+  // ray queries (hsb_group_raycast, hsb_group_get_dist): M x levels pointers to the members' log-odds planes,
+  // member-major like d_lv; the call's staging (member list, offsets and rays, then the results), pinned and on the device
+  float** d_planes = nullptr;
+  char* h_ray_stage = nullptr;
+  size_t h_ray_stage_bytes = 0;
+  DevBuf d_ray_stage;
 };
 
 namespace {
@@ -2468,6 +2474,9 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->d_occ_rows.p) cudaFree(g->d_occ_rows.p);
   if (g->h_occ_meta) cudaFreeHost(g->h_occ_meta);
   if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
+  if (g->d_planes) cudaFree(g->d_planes);
+  if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
+  if (g->h_ray_stage) cudaFreeHost(g->h_ray_stage);
   if (g->d_res) cudaFree(g->d_res);
   if (g->d_stage.p) cudaFree(g->d_stage.p);
   if (g->h_res) cudaFreeHost(g->h_res);
@@ -2550,6 +2559,11 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
       for (int l = 0; l < g->levels; ++l) mirror[(size_t)s * g->levels + l] = g->m[s]->lv[l].dirty + 4;
     HSB_GROUP_CUDA(cudaMalloc(&g->d_mirror, mirror.size() * sizeof(int*)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_mirror, mirror.data(), mirror.size() * sizeof(int*), cudaMemcpyHostToDevice));
+    std::vector<float*> planes((size_t)M * g->levels);
+    for (int s = 0; s < M; ++s)
+      for (int l = 0; l < g->levels; ++l) planes[(size_t)s * g->levels + l] = g->m[s]->lv[l].logodds;
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_planes, planes.size() * sizeof(float*)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_planes, planes.data(), planes.size() * sizeof(float*), cudaMemcpyHostToDevice));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
   }
@@ -2935,9 +2949,115 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
   return HSB_OK;
 }
 
+// hsb_raycast_batch (world: hsb_get_dist_batch) for K members in one pass: session k's rays [offsets[k], offsets[k+1])
+// on member members[k].  One host-to-device copy of member list, offsets and rays from the group's pinned staging, one
+// launch, one device-to-host copy of the results into the staging and one synchronise, whatever K is.  The results are
+// copied into the caller's arrays on the host.  No member's state changes.
+int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* members, int level, const int* offsets,
+               const void* begin, const void* end, float* out_dist, void* out_hit, int* out_found) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (level < 0 || level >= g->levels)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if (!offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets is NULL", fn);
+  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", fn, offsets[0]);
+  for (int k = 0; k < K; ++k)
+    if (offsets[k + 1] < offsets[k])
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets decrease at session %d (%d -> %d)", fn, k, offsets[k],
+                  offsets[k + 1]);
+  const int Q = offsets[K];
+  if (Q == 0) return HSB_OK;
+  if (!begin || !end || !out_dist)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s, %s and out_dist must not be NULL", fn,
+                world ? "begin_world" : "begin_cells", world ? "end_world" : "end_cells");
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
+
+  // staging: member list | offsets | begin | end, then the results: dist | hit | found (getDist)
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t o_off = al((size_t)K * 4), o_begin = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_end = o_begin + (size_t)Q * 8, o_dist = al(o_end + (size_t)Q * 8);
+  const size_t o_hit = al(o_dist + (size_t)Q * 4), o_found = o_hit + (size_t)Q * 8;
+  const size_t out_end = out_found ? o_found + (size_t)Q * 4 : out_hit ? o_found : o_dist + (size_t)Q * 4;
+  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
+  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
+  char* hs = g->h_ray_stage;
+  char* ds = static_cast<char*>(g->d_ray_stage.p);
+  memcpy(hs, members, (size_t)K * 4);
+  memcpy(hs + o_off, offsets, (size_t)(K + 1) * 4);
+  memcpy(hs + o_begin, begin, (size_t)Q * 8);
+  memcpy(hs + o_end, end, (size_t)Q * 8);
+  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, o_end + (size_t)Q * 8, cudaMemcpyHostToDevice, st));
+
+  HsbGroupRayParams P;
+  P.planes = g->d_planes;
+  P.members = reinterpret_cast<const int*>(ds);
+  P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.begin = ds + o_begin;
+  P.end = ds + o_end;
+  P.out_dist = reinterpret_cast<float*>(ds + o_dist);
+  P.out_hit = out_hit ? ds + o_hit : nullptr;
+  P.out_found = out_found ? reinterpret_cast<int*>(ds + o_found) : nullptr;
+  P.levels = g->levels;
+  P.level = level;
+  P.sx = h0->lv[level].sx;   // the members' geometry is one (hsb_group_create)
+  P.sy = h0->lv[level].sy;
+  P.K = K;
+  P.Q = Q;
+  float origo[2];   // getDist's transform, as hsb_get_dist_batch computes it
+  hsb_get_map_origin(h0, level, origo);
+  volatile float inv_scale = 1.0f / h0->lv[level].cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
+  P.origo_x = origo[0];
+  P.origo_y = origo[1];
+  P.scale = h0->lv[level].cell_length;
+  P.inv_scale = inv_scale;
+  const int blocks = std::min((Q + 7) / 8, h0->sm_count * 8);
+  if (world) hsb::group_ray_kernel<true><<<blocks, 256, 0, st>>>(P);
+  else hsb::group_ray_kernel<false><<<blocks, 256, 0, st>>>(P);
+  h0->launches++;
+  HSB_CUDA(h0, cudaGetLastError());
+  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_dist, ds + o_dist, out_end - o_dist, cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h0, cudaStreamSynchronize(st));
+  memcpy(out_dist, hs + o_dist, (size_t)Q * 4);
+  if (out_hit) memcpy(out_hit, hs + o_hit, (size_t)Q * 8);
+  if (out_found) memcpy(out_found, hs + o_found, (size_t)Q * 4);
+  return HSB_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,
+                      float* out_dist, int* out_hit) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_rays(g, "hsb_group_raycast", false, (int)g->m.size(), g->all.data(), level, offsets, begin_cells,
+                    end_cells, out_dist, out_hit, nullptr);
+}
+
+int hsb_group_raycast_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
+                             const int* begin_cells, const int* end_cells, float* out_dist, int* out_hit) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_rays(g, "hsb_group_raycast_subset", false, K, members, level, offsets, begin_cells, end_cells, out_dist,
+                    out_hit, nullptr);
+}
+
+int hsb_group_get_dist(hsb_group* g, int level, const int* offsets, const float* begin_world, const float* end_world,
+                       float* out_dist, float* out_hit_world, int* out_found) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_rays(g, "hsb_group_get_dist", true, (int)g->m.size(), g->all.data(), level, offsets, begin_world,
+                    end_world, out_dist, out_hit_world, out_found);
+}
+
+int hsb_group_get_dist_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
+                              const float* begin_world, const float* end_world, float* out_dist, float* out_hit_world,
+                              int* out_found) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_rays(g, "hsb_group_get_dist_subset", true, K, members, level, offsets, begin_world, end_world, out_dist,
+                    out_hit_world, out_found);
+}
 
 int hsb_group_sync_occupancy(hsb_group* g, int level, int8_t* const* grids, int* out_rects, int reset) {
   if (!g) return HSB_ERR_INVALID_ARG;

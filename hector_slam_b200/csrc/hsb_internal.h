@@ -185,6 +185,21 @@ struct HsbOccRowsDev {
   size_t off;
 };
 
+// A group ray query (group_ray_kernel: hsb_group_raycast, hsb_group_get_dist): Q rays of K sessions, session k's rays
+// [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`.  Arrays in device memory, in ray order.
+struct HsbGroupRayParams {
+  const float* const* planes;   // M x levels log-odds planes, member-major
+  const int* members;           // K
+  const int* offsets;           // K + 1
+  const void* begin;            // Q: int2 cells (ray cast) or float2 world points (getDist)
+  const void* end;
+  float* out_dist;              // Q
+  void* out_hit;                // Q int2 hit cells / float2 hit points, or null
+  int* out_found;               // Q (getDist), or null
+  int levels, level, sx, sy, K, Q;
+  float origo_x, origo_y, scale, inv_scale;   // getDist: the level's map origin and cell length, 1 / cell length
+};
+
 // Map write of a group SLAM step (update_mark_group_kernel / update_apply_group_kernel): blockIdx.z = session,
 // blockIdx.y = level.  Everything per session lives in device memory, uploaded with the step's scans.
 struct HsbGroupUpdateParams {

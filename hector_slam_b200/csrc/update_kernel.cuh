@@ -184,11 +184,35 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// N4: DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147) for B world-frame rays: world -> cell with
-// CoordinateTransformer<float>::getC2Coords ((w - origo) * inv_scale, :93-96) truncated by cast<int> (:136-137; a
-// non-finite or absurd coordinate is treated as outside the map), the ray cast, the hit cell back to the world with
-// getC1Coords (origo + cell * scale, :88-91) and the distance scaled by getC1Scale (scale * dist, :98-101; nothing hit:
-// scale * -1 as in the reference, hit_world = (0, 0) and found = 0 where the reference leaves hitCoords undefined).
+// N4: DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147) for the world-frame ray bw -> ew, one warp, its
+// results at index b: world -> cell with CoordinateTransformer<float>::getC2Coords ((w - origo) * inv_scale, :93-96)
+// truncated by cast<int> (:136-137; a non-finite or absurd coordinate is treated as outside the map), the ray cast, the
+// hit cell back to the world with getC1Coords (origo + cell * scale, :88-91) and the distance scaled by getC1Scale
+// (scale * dist, :98-101; nothing hit: scale * -1 as in the reference, hit_world = (0, 0) and found = 0 where the
+// reference leaves hitCoords undefined).  Every getDist kernel casts its rays with this one function.
+__device__ __forceinline__ void warp_getdist(const float* __restrict__ logodds, int sx, int sy, float origo_x,
+                                             float origo_y, float scale, float inv_scale, float2 bw, float2 ew, int lane,
+                                             int b, float* __restrict__ out_dist, float2* __restrict__ out_hit_world,
+                                             int* __restrict__ out_found) {
+  const float bx = __fmul_rn(__fsub_rn(bw.x, origo_x), inv_scale), by = __fmul_rn(__fsub_rn(bw.y, origo_y), inv_scale);
+  const float ex = __fmul_rn(__fsub_rn(ew.x, origo_x), inv_scale), ey = __fmul_rn(__fsub_rn(ew.y, origo_y), inv_scale);
+  const bool sane = fabsf(bx) < 1.0e9f && fabsf(by) < 1.0e9f && fabsf(ex) < 1.0e9f && fabsf(ey) < 1.0e9f;
+  const int2 p0 = sane ? make_int2((int)bx, (int)by) : make_int2(-1, -1);
+  const int2 p1 = sane ? make_int2((int)ex, (int)ey) : make_int2(-1, -1);
+  int2 hit;
+  const float dist = warp_raycast(logodds, sx, sy, p0, p1, lane, hit);
+  if (lane == 0) {
+    out_dist[b] = __fmul_rn(scale, dist);
+    const bool found = dist >= 0.0f;
+    if (out_found) out_found[b] = found ? 1 : 0;
+    if (out_hit_world)
+      out_hit_world[b] = found ? make_float2(__fadd_rn(origo_x, __fmul_rn((float)hit.x, scale)),
+                                             __fadd_rn(origo_y, __fmul_rn((float)hit.y, scale)))
+                               : make_float2(0.0f, 0.0f);
+  }
+}
+
+// N4 getDist for B world-frame rays on one plane (warp_getdist)
 __global__ void __launch_bounds__(256)
     getdist_kernel(const float* __restrict__ logodds, int sx, int sy, int B, float origo_x, float origo_y, float scale,
                    float inv_scale, const float2* __restrict__ begin_world, const float2* __restrict__ end_world,
@@ -196,23 +220,40 @@ __global__ void __launch_bounds__(256)
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int b = warp; b < B; b += nwarps) {
-    const float2 bw = begin_world[b], ew = end_world[b];
-    const float bx = __fmul_rn(__fsub_rn(bw.x, origo_x), inv_scale), by = __fmul_rn(__fsub_rn(bw.y, origo_y), inv_scale);
-    const float ex = __fmul_rn(__fsub_rn(ew.x, origo_x), inv_scale), ey = __fmul_rn(__fsub_rn(ew.y, origo_y), inv_scale);
-    const bool sane = fabsf(bx) < 1.0e9f && fabsf(by) < 1.0e9f && fabsf(ex) < 1.0e9f && fabsf(ey) < 1.0e9f;
-    const int2 p0 = sane ? make_int2((int)bx, (int)by) : make_int2(-1, -1);
-    const int2 p1 = sane ? make_int2((int)ex, (int)ey) : make_int2(-1, -1);
-    int2 hit;
-    const float dist = warp_raycast(logodds, sx, sy, p0, p1, lane, hit);
-    if (lane == 0) {
-      out_dist[b] = __fmul_rn(scale, dist);
-      const bool found = dist >= 0.0f;
-      if (out_found) out_found[b] = found ? 1 : 0;
-      if (out_hit_world)
-        out_hit_world[b] = found ? make_float2(__fadd_rn(origo_x, __fmul_rn((float)hit.x, scale)),
-                                               __fadd_rn(origo_y, __fmul_rn((float)hit.y, scale)))
-                                 : make_float2(0.0f, 0.0f);
+  for (int b = warp; b < B; b += nwarps)
+    warp_getdist(logodds, sx, sy, origo_x, origo_y, scale, inv_scale, begin_world[b], end_world[b], lane, b, out_dist,
+                 out_hit_world, out_found);
+}
+
+// N4 for a group (hsb_group_raycast / hsb_group_get_dist): ray q of the call belongs to the session k whose rays are
+// [offsets[k], offsets[k+1]) and is cast on member members[k]'s plane of the level, found through the group's table
+// planes[member * levels + level].  One warp per ray, grid-stride, as raycast_kernel / getdist_kernel; each ray's results
+// are theirs bit for bit.  kWorld: getDist rays (float2 world points); otherwise ray-cast rays (int2 cells).
+template <bool kWorld>
+__global__ void __launch_bounds__(256) group_ray_kernel(const HsbGroupRayParams P) {
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int q = warp; q < P.Q; q += nwarps) {
+    int lo = 0, hi = P.K - 1;   // the last session whose rays start at or before ray q (empty sessions are passed over)
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (P.offsets[mid] <= q) lo = mid;
+      else hi = mid - 1;
+    }
+    const float* logodds = P.planes[(size_t)P.members[lo] * P.levels + P.level];
+    if (kWorld) {
+      warp_getdist(logodds, P.sx, P.sy, P.origo_x, P.origo_y, P.scale, P.inv_scale,
+                   static_cast<const float2*>(P.begin)[q], static_cast<const float2*>(P.end)[q], lane, q, P.out_dist,
+                   static_cast<float2*>(P.out_hit), P.out_found);
+    } else {
+      int2 hit;
+      const float dist = warp_raycast(logodds, P.sx, P.sy, static_cast<const int2*>(P.begin)[q],
+                                      static_cast<const int2*>(P.end)[q], lane, hit);
+      if (lane == 0) {
+        P.out_dist[q] = dist;
+        if (P.out_hit) static_cast<int2*>(P.out_hit)[q] = hit;
+      }
     }
   }
 }

@@ -304,6 +304,33 @@ class SlamProcessor {
     SlamProcessor& owner = groupOwnerOf(ps, M, "syncOccupancyMany");
     owner.check(hsb_group_sync_occupancy_subset(owner.groupFor(ps, M), K, members, level, grids, rects, 1));
   }
+
+  // hector_map_tools' DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147) for n world-frame rays on this
+  // processor's level, as hector_map_server's get_distance_to_obstacle calls it (hector_map_server.cpp:123):
+  // dist[i] = distance to the first occupied cell in metres (-cell length: nothing hit), hitWorld[2i..] (may be null)
+  // the hit point ((0, 0) if none), found[i] (may be null) whether something was hit.  beginWorld / endWorld: n x 2.
+  void getDist(int level, int n, const float* beginWorld, const float* endWorld, float* dist, float* hitWorld = 0,
+               int* found = 0) {
+    check(hsb_get_dist_batch(h_, level, n, beginWorld, endWorld, dist, hitWorld, found));
+  }
+
+  // getDist() for M processors in one pass (hsb_group_get_dist, through the group updateMany keeps): processor s casts
+  // the rays [offsets[s], offsets[s+1]) of beginWorld / endWorld; the outputs are in ray order.
+  static void getDistMany(SlamProcessor* const* ps, int M, int level, const int* offsets, const float* beginWorld,
+                          const float* endWorld, float* dist, float* hitWorld = 0, int* found = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "getDistMany");
+    owner.check(hsb_group_get_dist(owner.groupFor(ps, M), level, offsets, beginWorld, endWorld, dist, hitWorld, found));
+  }
+
+  // getDistMany() for the processors ps[members[0..K)] (hsb_group_get_dist_subset): the rays [offsets[k],
+  // offsets[k+1]) belong to ps[members[k]]; the processors not listed are neither read nor waited for.
+  static void getDistMany(SlamProcessor* const* ps, int M, const int* members, int K, int level, const int* offsets,
+                          const float* beginWorld, const float* endWorld, float* dist, float* hitWorld = 0,
+                          int* found = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "getDistMany");
+    owner.check(hsb_group_get_dist_subset(owner.groupFor(ps, M), K, members, level, offsets, beginWorld, endWorld, dist,
+                                          hitWorld, found));
+  }
   hsb_handle* handle() { return h_; }
 
   // util::poseDifferenceLargerThan, util/UtilFunctions.h:73-92 (float norm, double pi arithmetic)

@@ -260,6 +260,39 @@ int hsbp_sync_occupancy_many_subset(void* const* ps, int M, const int* members, 
   }
   return 0;
 }
+int hsbp_get_dist(void* p, int level, int n, const float* begin_world, const float* end_world, float* dist,
+                  float* hit_world, int* found) {
+  try {
+    static_cast<hsb200::SlamProcessor*>(p)->getDist(level, n, begin_world, end_world, dist, hit_world, found);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_get_dist_many(void* const* ps, int M, int level, const int* offsets, const float* begin_world,
+                       const float* end_world, float* dist, float* hit_world, int* found) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::getDistMany(procs.data(), M, level, offsets, begin_world, end_world, dist, hit_world, found);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_get_dist_many_subset(void* const* ps, int M, const int* members, int K, int level, const int* offsets,
+                              const float* begin_world, const float* end_world, float* dist, float* hit_world,
+                              int* found) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::getDistMany(procs.data(), M, members, K, level, offsets, begin_world, end_world, dist,
+                                       hit_world, found);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

@@ -501,6 +501,33 @@ int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* membe
 int hsb_group_sync_occupancy(hsb_group* g, int level, int8_t* const* grids, int* out_rects, int reset);
 int hsb_group_sync_occupancy_subset(hsb_group* g, int K, const int* members, int level, int8_t* const* grids,
                                     int* out_rects, int reset);
+/* hector_map_server's get_distance_to_obstacle queries (hector_map_server.cpp:91-165, getDist at :123) for K of the
+ * group's members in one pass: hsb_group_get_dist is hsb_get_dist_batch, hsb_group_raycast is hsb_raycast_batch.
+ * Session k is member members[k] (the full form: every member, in order); its rays are [offsets[k], offsets[k+1]) of
+ * begin_* / end_* (Q x 2 each, Q = offsets[K]; a session may hold none).  The outputs are in ray order: out_dist Q,
+ * out_hit_world / out_hit Q x 2, out_found Q; the ones the single calls let be NULL may be NULL here.  Every ray's
+ * distance, hit and found flag are bit-identical to the single call on its member with the same ray (misses, edges,
+ * NaN and absurd world coordinates and the 5000-step cap included).  No member's state changes; a member not listed
+ * is neither read nor waited for.
+ * Ordering: the call runs on the group's stream after everything queued on the listed members (their own work and a
+ * pending step of any group they belong to, so a query right after a nowait step sees that step's map write), and
+ * returns when the results are in the caller's arrays.
+ * Cost: one host-to-device copy of member list, offsets and rays from the group's pinned staging (grown geometrically),
+ * one launch, one device-to-host copy of the results and one synchronise, whatever K is.  The launch is counted on
+ * handles[0].
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued: K < 0 or K > M; members == NULL with K > 0; an index
+ * outside [0, M) or listed twice (the message names the session); level outside [0, levels); offsets == NULL,
+ * offsets[0] != 0 or decreasing offsets (the message names the session); begin, end or out_dist NULL with Q > 0.
+ * K = 0 returns HSB_OK and reads no other argument; Q = 0 returns HSB_OK and queues nothing. */
+int hsb_group_get_dist(hsb_group* g, int level, const int* offsets, const float* begin_world, const float* end_world,
+                       float* out_dist, float* out_hit_world, int* out_found);
+int hsb_group_get_dist_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
+                              const float* begin_world, const float* end_world, float* out_dist, float* out_hit_world,
+                              int* out_found);
+int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,
+                      float* out_dist, int* out_hit);
+int hsb_group_raycast_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
+                             const int* begin_cells, const int* end_cells, float* out_dist, int* out_hit);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
