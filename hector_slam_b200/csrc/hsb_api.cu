@@ -2019,19 +2019,8 @@ int hsb_download_prob(hsb_handle* h, int level, float* out) {
 
 int hsb_download_occupancy(hsb_handle* h, int level, int8_t* out) {
   if (!h || level < 0 || level >= h->levels || !out) return HSB_ERR_INVALID_ARG;
-  HandleScope guard(h);
-  Level& L = h->lv[level];
-  const size_t n = (size_t)L.sx * L.sy;
-  int s = ensure(h, h->d_occ, n);
-  if (s != HSB_OK) return s;
-  int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)h->sm_count * 16);
-  hsb::occupancy_kernel<<<blocks, 256, 0, h->stream>>>(L.logodds, static_cast<int8_t*>(h->d_occ.p), n);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(out, h->d_occ.p, n, cudaMemcpyDeviceToHost, h->stream));
-  HSB_CUDA(h, cudaStreamSynchronize(h->stream));
-  h->d2h_bytes += n;
-  return HSB_OK;
+  const int rect[4] = {0, 0, h->lv[level].sx - 1, h->lv[level].sy - 1};
+  return hsb_download_occupancy_rect(h, level, rect, out);
 }
 
 // the likelihood launch on device pointers; `st` may be a caller's stream (ordered behind a pending map write)
@@ -2297,30 +2286,83 @@ int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset) {
   return HSB_OK;
 }
 
+// Every ray query's host body (hsb_raycast_batch, hsb_get_dist_batch and their group forms): Q = offsets[K] rays of K
+// sessions, session k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`, found in the device
+// table planes[member * levels + level] — or, with planes NULL, h's own plane of `level`, staged with the rays as a
+// one-entry table.  One host-to-device copy of member list, offsets, (plane) and rays from the pinned staging hs, one
+// launch on `st`, one device-to-host copy of the results into the staging and one synchronise; the results are then
+// copied into the caller's arrays on the host.  The launch and any error are counted on h, whose level gives the
+// geometry and getDist's transform (every member's geometry is h's).  world: getDist rays, otherwise ray-cast rays.
+static int ray_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage,
+                     const float* const* planes, int levels, int level, bool world, int K, const int* members,
+                     const int* offsets, const void* begin, const void* end, float* out_dist, void* out_hit,
+                     int* out_found) {
+  const int Q = offsets[K];
+  // staging: member list | offsets | (plane) | begin | end, then the results: dist | hit | found (getDist)
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t o_off = al((size_t)K * 4), o_plane = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_begin = planes ? o_plane : o_plane + 16;
+  const size_t o_end = o_begin + (size_t)Q * 8, o_dist = al(o_end + (size_t)Q * 8);
+  const size_t o_hit = al(o_dist + (size_t)Q * 4), o_found = o_hit + (size_t)Q * 8;
+  const size_t out_end = out_found ? o_found + (size_t)Q * 4 : out_hit ? o_found : o_dist + (size_t)Q * 4;
+  int s;
+  if ((s = ensure_pinned(h, hs_buf, hs_bytes, out_end)) != HSB_OK) return s;
+  if ((s = ensure(h, d_stage, out_end)) != HSB_OK) return s;
+  char* hs = reinterpret_cast<char*>(hs_buf);
+  char* ds = static_cast<char*>(d_stage.p);
+  memcpy(hs, members, (size_t)K * 4);
+  memcpy(hs + o_off, offsets, (size_t)(K + 1) * 4);
+  if (!planes) memcpy(hs + o_plane, &h->lv[level].logodds, sizeof(float*));
+  memcpy(hs + o_begin, begin, (size_t)Q * 8);
+  memcpy(hs + o_end, end, (size_t)Q * 8);
+  HSB_CUDA(h, cudaMemcpyAsync(ds, hs, o_end + (size_t)Q * 8, cudaMemcpyHostToDevice, st));
+
+  const Level& L = h->lv[level];
+  HsbRayParams P;
+  P.planes = planes ? planes : reinterpret_cast<const float* const*>(ds + o_plane);
+  P.members = reinterpret_cast<const int*>(ds);
+  P.offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.begin = ds + o_begin;
+  P.end = ds + o_end;
+  P.out_dist = reinterpret_cast<float*>(ds + o_dist);
+  P.out_hit = out_hit ? ds + o_hit : nullptr;
+  P.out_found = out_found ? reinterpret_cast<int*>(ds + o_found) : nullptr;
+  P.levels = planes ? levels : 1;
+  P.level = planes ? level : 0;
+  P.sx = L.sx;
+  P.sy = L.sy;
+  P.K = K;
+  P.Q = Q;
+  float origo[2];
+  hsb_get_map_origin(h, level, origo);
+  volatile float inv_scale = 1.0f / L.cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
+  P.origo_x = origo[0];
+  P.origo_y = origo[1];
+  P.scale = L.cell_length;
+  P.inv_scale = inv_scale;
+  const int blocks = std::min((Q + 7) / 8, h->sm_count * 8);
+  if (world) hsb::ray_kernel<true><<<blocks, 256, 0, st>>>(P);
+  else hsb::ray_kernel<false><<<blocks, 256, 0, st>>>(P);
+  h->launches++;
+  HSB_CUDA(h, cudaGetLastError());
+  HSB_CUDA(h, cudaMemcpyAsync(hs + o_dist, ds + o_dist, out_end - o_dist, cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaStreamSynchronize(st));
+  memcpy(out_dist, hs + o_dist, (size_t)Q * 4);
+  if (out_hit) memcpy(out_hit, hs + o_hit, (size_t)Q * 8);
+  if (out_found) memcpy(out_found, hs + o_found, (size_t)Q * 4);
+  return HSB_OK;
+}
+
+// The single calls stage through the handle's scan staging: every call that fills h_stage either synchronises or, a
+// nowait SLAM step, returns once its pose is published, which comes after the staging's host-to-device copy.
 int hsb_raycast_batch(hsb_handle* h, int level, int B, const int* begin_cells, const int* end_cells, float* out_dist,
                       int* out_hit) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !begin_cells || !end_cells || !out_dist) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  Level& L = h->lv[level];
-  int s;
-  if ((s = ensure(h, h->d_pts, (size_t)B * 16 + 16)) != HSB_OK) return s;      // begin | end
-  if ((s = ensure(h, h->d_poses, (size_t)B * 12 + 16)) != HSB_OK) return s;    // dist | hit
-  cudaStream_t st = h->stream;
-  int2* d_begin = static_cast<int2*>(h->d_pts.p);
-  int2* d_end = d_begin + B;
-  float* d_dist = static_cast<float*>(h->d_poses.p);
-  int2* d_hit = reinterpret_cast<int2*>(d_dist + ((B + 1) & ~1));
-  HSB_CUDA(h, cudaMemcpyAsync(d_begin, begin_cells, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  HSB_CUDA(h, cudaMemcpyAsync(d_end, end_cells, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  int blocks = std::min((B + 7) / 8, h->sm_count * 8);
-  hsb::raycast_kernel<<<blocks, 256, 0, st>>>(L.logodds, L.sx, L.sy, B, d_begin, d_end, d_dist, out_hit ? d_hit : nullptr);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(out_dist, d_dist, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  if (out_hit) HSB_CUDA(h, cudaMemcpyAsync(out_hit, d_hit, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  return HSB_OK;
+  const int members[1] = {0}, offsets[2] = {0, B};
+  return ray_query(h, h->stream, h->h_stage, h->h_stage_bytes, h->d_pts, nullptr, 1, level, false, 1, members, offsets,
+                   begin_cells, end_cells, out_dist, out_hit, nullptr);
 }
 
 int hsb_get_map_origin(const hsb_handle* h, int level, float out[2]) {
@@ -2340,31 +2382,9 @@ int hsb_get_dist_batch(hsb_handle* h, int level, int B, const float* begin_world
   if (!h || level < 0 || level >= h->levels || B < 0 || !begin_world || !end_world || !out_dist) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  Level& L = h->lv[level];
-  int s;
-  if ((s = ensure(h, h->d_pts, (size_t)B * 16 + 16)) != HSB_OK) return s;      // begin | end
-  if ((s = ensure(h, h->d_poses, (size_t)B * 16 + 16)) != HSB_OK) return s;    // dist | hit (2) | found
-  cudaStream_t st = h->stream;
-  float2* d_begin = static_cast<float2*>(h->d_pts.p);
-  float2* d_end = d_begin + B;
-  float2* d_hit = static_cast<float2*>(h->d_poses.p);
-  float* d_dist = reinterpret_cast<float*>(d_hit + B);
-  int* d_found = reinterpret_cast<int*>(d_dist + B);
-  HSB_CUDA(h, cudaMemcpyAsync(d_begin, begin_world, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  HSB_CUDA(h, cudaMemcpyAsync(d_end, end_world, (size_t)B * 8, cudaMemcpyHostToDevice, st));
-  float origo[2];
-  hsb_get_map_origin(h, level, origo);
-  volatile float inv_scale = 1.0f / L.cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
-  int blocks = std::min((B + 7) / 8, h->sm_count * 8);
-  hsb::getdist_kernel<<<blocks, 256, 0, st>>>(L.logodds, L.sx, L.sy, B, origo[0], origo[1], L.cell_length, inv_scale, d_begin, d_end,
-                                              d_dist, out_hit_world ? d_hit : nullptr, out_found ? d_found : nullptr);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(out_dist, d_dist, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  if (out_hit_world) HSB_CUDA(h, cudaMemcpyAsync(out_hit_world, d_hit, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
-  if (out_found) HSB_CUDA(h, cudaMemcpyAsync(out_found, d_found, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  return HSB_OK;
+  const int members[1] = {0}, offsets[2] = {0, B};
+  return ray_query(h, h->stream, h->h_stage, h->h_stage_bytes, h->d_pts, nullptr, 1, level, true, 1, members, offsets,
+                   begin_world, end_world, out_dist, out_hit_world, out_found);
 }
 
 void* hsb_level_logodds_device_ptr(hsb_handle* h, int level) {
@@ -2429,7 +2449,7 @@ struct hsb_group {
   // ray queries (hsb_group_raycast, hsb_group_get_dist): M x levels pointers to the members' log-odds planes,
   // member-major like d_lv; the call's staging (member list, offsets and rays, then the results), pinned and on the device
   float** d_planes = nullptr;
-  char* h_ray_stage = nullptr;
+  float* h_ray_stage = nullptr;
   size_t h_ray_stage_bytes = 0;
   DevBuf d_ray_stage;
 };
@@ -2950,9 +2970,8 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
 }
 
 // hsb_raycast_batch (world: hsb_get_dist_batch) for K members in one pass: session k's rays [offsets[k], offsets[k+1])
-// on member members[k].  One host-to-device copy of member list, offsets and rays from the group's pinned staging, one
-// launch, one device-to-host copy of the results into the staging and one synchronise, whatever K is.  The results are
-// copied into the caller's arrays on the host.  No member's state changes.
+// on member members[k], behind the members' queued work, through the group's pinned staging and plane table (ray_query:
+// one copy each way and one synchronise, whatever K is).  No member's state changes.
 int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* members, int level, const int* offsets,
                const void* begin, const void* end, float* out_dist, void* out_hit, int* out_found) {
   hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
@@ -2972,58 +2991,9 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s, %s and out_dist must not be NULL", fn,
                 world ? "begin_world" : "begin_cells", world ? "end_world" : "end_cells");
   DeviceGuard guard(g->device);
-  cudaStream_t st = g->stream;
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-
-  // staging: member list | offsets | begin | end, then the results: dist | hit | found (getDist)
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_off = al((size_t)K * 4), o_begin = al(o_off + (size_t)(K + 1) * 4);
-  const size_t o_end = o_begin + (size_t)Q * 8, o_dist = al(o_end + (size_t)Q * 8);
-  const size_t o_hit = al(o_dist + (size_t)Q * 4), o_found = o_hit + (size_t)Q * 8;
-  const size_t out_end = out_found ? o_found + (size_t)Q * 4 : out_hit ? o_found : o_dist + (size_t)Q * 4;
-  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
-  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
-  char* hs = g->h_ray_stage;
-  char* ds = static_cast<char*>(g->d_ray_stage.p);
-  memcpy(hs, members, (size_t)K * 4);
-  memcpy(hs + o_off, offsets, (size_t)(K + 1) * 4);
-  memcpy(hs + o_begin, begin, (size_t)Q * 8);
-  memcpy(hs + o_end, end, (size_t)Q * 8);
-  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, o_end + (size_t)Q * 8, cudaMemcpyHostToDevice, st));
-
-  HsbGroupRayParams P;
-  P.planes = g->d_planes;
-  P.members = reinterpret_cast<const int*>(ds);
-  P.offsets = reinterpret_cast<const int*>(ds + o_off);
-  P.begin = ds + o_begin;
-  P.end = ds + o_end;
-  P.out_dist = reinterpret_cast<float*>(ds + o_dist);
-  P.out_hit = out_hit ? ds + o_hit : nullptr;
-  P.out_found = out_found ? reinterpret_cast<int*>(ds + o_found) : nullptr;
-  P.levels = g->levels;
-  P.level = level;
-  P.sx = h0->lv[level].sx;   // the members' geometry is one (hsb_group_create)
-  P.sy = h0->lv[level].sy;
-  P.K = K;
-  P.Q = Q;
-  float origo[2];   // getDist's transform, as hsb_get_dist_batch computes it
-  hsb_get_map_origin(h0, level, origo);
-  volatile float inv_scale = 1.0f / h0->lv[level].cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
-  P.origo_x = origo[0];
-  P.origo_y = origo[1];
-  P.scale = h0->lv[level].cell_length;
-  P.inv_scale = inv_scale;
-  const int blocks = std::min((Q + 7) / 8, h0->sm_count * 8);
-  if (world) hsb::group_ray_kernel<true><<<blocks, 256, 0, st>>>(P);
-  else hsb::group_ray_kernel<false><<<blocks, 256, 0, st>>>(P);
-  h0->launches++;
-  HSB_CUDA(h0, cudaGetLastError());
-  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_dist, ds + o_dist, out_end - o_dist, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h0, cudaStreamSynchronize(st));
-  memcpy(out_dist, hs + o_dist, (size_t)Q * 4);
-  if (out_hit) memcpy(out_hit, hs + o_hit, (size_t)Q * 8);
-  if (out_found) memcpy(out_found, hs + o_found, (size_t)Q * 4);
-  return HSB_OK;
+  return ray_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_planes, g->levels, level,
+                   world, K, members, offsets, begin, end, out_dist, out_hit, out_found);
 }
 
 }  // namespace

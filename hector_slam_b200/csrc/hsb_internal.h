@@ -185,10 +185,10 @@ struct HsbOccRowsDev {
   size_t off;
 };
 
-// A group ray query (group_ray_kernel: hsb_group_raycast, hsb_group_get_dist): Q rays of K sessions, session k's rays
-// [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`.  Arrays in device memory, in ray order.
-struct HsbGroupRayParams {
-  const float* const* planes;   // M x levels log-odds planes, member-major
+// A ray query (ray_kernel: hsb_raycast_batch, hsb_get_dist_batch and their group forms): Q rays of K sessions, session
+// k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`.  Arrays in device memory, in ray order.
+struct HsbRayParams {
+  const float* const* planes;   // members x levels log-odds planes, member-major
   const int* members;           // K
   const int* offsets;           // K + 1
   const void* begin;            // Q: int2 cells (ray cast) or float2 world points (getDist)

@@ -75,12 +75,8 @@ __device__ __forceinline__ int8_t occupancy_value(float l) {
   return l < 0.0f ? (int8_t)0 : (l > 0.0f ? (int8_t)100 : (int8_t)-1);
 }
 
-__global__ void occupancy_kernel(const float* __restrict__ logodds, int8_t* __restrict__ out, size_t n) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = occupancy_value(logodds[i]);
-}
-
-// N1 on a rectangle: the cells of {x0, y0, w, hgt} thresholded into a packed w x hgt buffer (dirty-rectangle publishing).
+// N1 on a rectangle: the cells of {x0, y0, w, hgt} thresholded into a packed w x hgt buffer (dirty-rectangle publishing,
+// and the whole level's export as the rectangle of every cell).
 __global__ void occupancy_rect_kernel(const float* __restrict__ logodds, int sx, int x0, int y0, int w, int hgt,
                                       int8_t* __restrict__ out) {
   const size_t n = (size_t)w * hgt;
@@ -168,69 +164,12 @@ __device__ __forceinline__ float warp_raycast(const float* __restrict__ logodds,
   return dist;
 }
 
-__global__ void __launch_bounds__(256)
-    raycast_kernel(const float* __restrict__ logodds, int sx, int sy, int B, const int2* __restrict__ begin,
-                   const int2* __restrict__ end, float* __restrict__ out_dist, int2* __restrict__ out_hit) {
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int b = warp; b < B; b += nwarps) {
-    int2 hit;
-    const float dist = warp_raycast(logodds, sx, sy, begin[b], end[b], lane, hit);
-    if (lane == 0) {
-      out_dist[b] = dist;
-      if (out_hit) out_hit[b] = hit;
-    }
-  }
-}
-
-// N4: DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147) for the world-frame ray bw -> ew, one warp, its
-// results at index b: world -> cell with CoordinateTransformer<float>::getC2Coords ((w - origo) * inv_scale, :93-96)
-// truncated by cast<int> (:136-137; a non-finite or absurd coordinate is treated as outside the map), the ray cast, the
-// hit cell back to the world with getC1Coords (origo + cell * scale, :88-91) and the distance scaled by getC1Scale
-// (scale * dist, :98-101; nothing hit: scale * -1 as in the reference, hit_world = (0, 0) and found = 0 where the
-// reference leaves hitCoords undefined).  Every getDist kernel casts its rays with this one function.
-__device__ __forceinline__ void warp_getdist(const float* __restrict__ logodds, int sx, int sy, float origo_x,
-                                             float origo_y, float scale, float inv_scale, float2 bw, float2 ew, int lane,
-                                             int b, float* __restrict__ out_dist, float2* __restrict__ out_hit_world,
-                                             int* __restrict__ out_found) {
-  const float bx = __fmul_rn(__fsub_rn(bw.x, origo_x), inv_scale), by = __fmul_rn(__fsub_rn(bw.y, origo_y), inv_scale);
-  const float ex = __fmul_rn(__fsub_rn(ew.x, origo_x), inv_scale), ey = __fmul_rn(__fsub_rn(ew.y, origo_y), inv_scale);
-  const bool sane = fabsf(bx) < 1.0e9f && fabsf(by) < 1.0e9f && fabsf(ex) < 1.0e9f && fabsf(ey) < 1.0e9f;
-  const int2 p0 = sane ? make_int2((int)bx, (int)by) : make_int2(-1, -1);
-  const int2 p1 = sane ? make_int2((int)ex, (int)ey) : make_int2(-1, -1);
-  int2 hit;
-  const float dist = warp_raycast(logodds, sx, sy, p0, p1, lane, hit);
-  if (lane == 0) {
-    out_dist[b] = __fmul_rn(scale, dist);
-    const bool found = dist >= 0.0f;
-    if (out_found) out_found[b] = found ? 1 : 0;
-    if (out_hit_world)
-      out_hit_world[b] = found ? make_float2(__fadd_rn(origo_x, __fmul_rn((float)hit.x, scale)),
-                                             __fadd_rn(origo_y, __fmul_rn((float)hit.y, scale)))
-                               : make_float2(0.0f, 0.0f);
-  }
-}
-
-// N4 getDist for B world-frame rays on one plane (warp_getdist)
-__global__ void __launch_bounds__(256)
-    getdist_kernel(const float* __restrict__ logodds, int sx, int sy, int B, float origo_x, float origo_y, float scale,
-                   float inv_scale, const float2* __restrict__ begin_world, const float2* __restrict__ end_world,
-                   float* __restrict__ out_dist, float2* __restrict__ out_hit_world, int* __restrict__ out_found) {
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int b = warp; b < B; b += nwarps)
-    warp_getdist(logodds, sx, sy, origo_x, origo_y, scale, inv_scale, begin_world[b], end_world[b], lane, b, out_dist,
-                 out_hit_world, out_found);
-}
-
-// N4 for a group (hsb_group_raycast / hsb_group_get_dist): ray q of the call belongs to the session k whose rays are
-// [offsets[k], offsets[k+1]) and is cast on member members[k]'s plane of the level, found through the group's table
-// planes[member * levels + level].  One warp per ray, grid-stride, as raycast_kernel / getdist_kernel; each ray's results
-// are theirs bit for bit.  kWorld: getDist rays (float2 world points); otherwise ray-cast rays (int2 cells).
+// N4 (hsb_raycast_batch, hsb_get_dist_batch and their group forms): ray q of the call belongs to the session k whose
+// rays are [offsets[k], offsets[k+1]) and is cast on member members[k]'s plane of the level, found through the table
+// planes[member * levels + level] (a single handle's call: one session and a one-entry table).  One warp per ray,
+// grid-stride.  kWorld: getDist rays (float2 world points); otherwise ray-cast rays (int2 cells).
 template <bool kWorld>
-__global__ void __launch_bounds__(256) group_ray_kernel(const HsbGroupRayParams P) {
+__global__ void __launch_bounds__(256) ray_kernel(const HsbRayParams P) {
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -243,9 +182,32 @@ __global__ void __launch_bounds__(256) group_ray_kernel(const HsbGroupRayParams 
     }
     const float* logodds = P.planes[(size_t)P.members[lo] * P.levels + P.level];
     if (kWorld) {
-      warp_getdist(logodds, P.sx, P.sy, P.origo_x, P.origo_y, P.scale, P.inv_scale,
-                   static_cast<const float2*>(P.begin)[q], static_cast<const float2*>(P.end)[q], lane, q, P.out_dist,
-                   static_cast<float2*>(P.out_hit), P.out_found);
+      // DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147): world -> cell with
+      // CoordinateTransformer<float>::getC2Coords ((w - origo) * inv_scale, :93-96) truncated by cast<int> (:136-137; a
+      // non-finite or absurd coordinate is treated as outside the map), the ray cast, the hit cell back to the world with
+      // getC1Coords (origo + cell * scale, :88-91) and the distance scaled by getC1Scale (scale * dist, :98-101; nothing
+      // hit: scale * -1 as in the reference, hit_world = (0, 0) and found = 0 where the reference leaves hitCoords
+      // undefined).
+      const float2 bw = static_cast<const float2*>(P.begin)[q], ew = static_cast<const float2*>(P.end)[q];
+      const float bx = __fmul_rn(__fsub_rn(bw.x, P.origo_x), P.inv_scale);
+      const float by = __fmul_rn(__fsub_rn(bw.y, P.origo_y), P.inv_scale);
+      const float ex = __fmul_rn(__fsub_rn(ew.x, P.origo_x), P.inv_scale);
+      const float ey = __fmul_rn(__fsub_rn(ew.y, P.origo_y), P.inv_scale);
+      const bool sane = fabsf(bx) < 1.0e9f && fabsf(by) < 1.0e9f && fabsf(ex) < 1.0e9f && fabsf(ey) < 1.0e9f;
+      const int2 p0 = sane ? make_int2((int)bx, (int)by) : make_int2(-1, -1);
+      const int2 p1 = sane ? make_int2((int)ex, (int)ey) : make_int2(-1, -1);
+      int2 hit;
+      const float dist = warp_raycast(logodds, P.sx, P.sy, p0, p1, lane, hit);
+      if (lane == 0) {
+        P.out_dist[q] = __fmul_rn(P.scale, dist);
+        const bool found = dist >= 0.0f;
+        if (P.out_found) P.out_found[q] = found ? 1 : 0;
+        if (P.out_hit)
+          static_cast<float2*>(P.out_hit)[q] =
+              found ? make_float2(__fadd_rn(P.origo_x, __fmul_rn((float)hit.x, P.scale)),
+                                  __fadd_rn(P.origo_y, __fmul_rn((float)hit.y, P.scale)))
+                    : make_float2(0.0f, 0.0f);
+      }
     } else {
       int2 hit;
       const float dist = warp_raycast(logodds, P.sx, P.sy, static_cast<const int2*>(P.begin)[q],

@@ -184,7 +184,7 @@ def test_untouched_bytes_and_clean_members(hsb_lib, mode):
 @pytest.mark.parametrize("geom", mc.GEOMS, ids=mc.geom_id)
 def test_threshold_edge_values(hsb_lib, geom, mode):
     """Planes carrying -0, +0, the smallest denormals, +-inf, NaN and 50 at the corners, along the last row and column
-    and at random cells, planted by hsb_upload_level on every level: the synced grid equals occupancy_kernel's export
+    and at random cells, planted by hsb_upload_level on every level: the synced grid equals the whole-level export
     (hsb_download_occupancy) and the numpy threshold."""
     from hector_slam_b200 import capi
 

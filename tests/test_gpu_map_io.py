@@ -1,10 +1,10 @@
 """GPU: the kernels that read whole cells out of a level plane or move cells between planes, held bit for bit on
 non-square levels, long rays and plane edges, in both gather modes (LDG and TEX handles).
 
-  N1  occupancy export and rectangle downloads (occupancy_kernel, occupancy_rect_kernel, hsb_download_level_rect) against
-      a numpy publishMap threshold of the uploaded plane, with -0, +0, +-min denormal, +-inf, NaN and 50 planted;
-  N4  ray cast and getDist (warp_raycast, raycast_kernel, getdist_kernel) against HectorMapTools.h compiled unmodified
-      (oracle/_ref; the C port where it is absent) on the rays of tests/maptools_cases.py;
+  N1  occupancy export and rectangle downloads (occupancy_rect_kernel, hsb_download_level_rect) against a numpy
+      publishMap threshold of the uploaded plane, with -0, +0, +-min denormal, +-inf, NaN and 50 planted;
+  N4  ray cast and getDist (warp_raycast, ray_kernel) against HectorMapTools.h compiled unmodified (oracle/_ref; the C
+      port where it is absent) on the rays of tests/maptools_cases.py, and right after a nowait SLAM step;
   §6  tile replication between an owner and a replica on one device, both protocols (pack_rect / unpack_rect and
       pack_dirty / reset_dirty / unpack_dirty): log-odds, probabilities, texture twin, mirror and replication
       rectangles, the buffer header and the overflow boundary;
@@ -175,7 +175,49 @@ def test_constructed_long_rays(hsb_lib, geom, mode):
     rep.close()
 
 
-# ---- §6 ------------------------------------------------------------------------------------------------------------
+@MODES
+@pytest.mark.parametrize("kind", ["endpoints", "ranges"])
+def test_rays_right_after_a_nowait_step(hsb_lib, mode, kind):
+    """hsb_get_dist_batch and hsb_raycast_batch issued right after a nowait SLAM step see the step's map write and leave
+    the step's input alone (the scan and the rays go through the handle's one pinned staging): the rays, the poses and
+    every level's plane equal those of a twin stepped synchronously.  The rays start around the robot."""
+    from hector_slam_b200 import capi
+    from test_gpu_group_subset import geometry, session_data
+
+    fmt = geometry(0)
+    ticks = 8
+    data = session_data(40 + mode, ticks, fmt)
+    twins = [capi.MapRepB200(0.05, 512, 512, levels=3, update_factor_free=0.4, update_factor_occupied=0.9,
+                             gather_mode=mode) for _ in range(2)]
+    for rep in twins:
+        rep.set_scan_format(**fmt)
+    rng = np.random.default_rng(7 + mode)
+    ang = np.linspace(-np.pi, np.pi, 48, endpoint=False, dtype=np.float32)
+    for t in range(ticks):
+        level = t % 3
+        sx, sy, _ = twins[0].level_info(level)
+        p = data["truth"][t]
+        wb = np.repeat(p[None, :2], ang.size, axis=0).astype(np.float32)
+        we = (wb + np.float32(5.0) * np.stack([np.cos(ang), np.sin(ang)], axis=1)).astype(np.float32)
+        cb = np.int32([sx // 2, sy // 2]) + rng.integers(-(sx // 5), sx // 5 + 1, (64, 2)).astype(np.int32)
+        ce = np.stack([rng.integers(0, sx, 64), rng.integers(0, sy, 64)], axis=1).astype(np.int32)
+        out = []
+        for rep, nowait in zip(twins, (True, False)):
+            if kind == "endpoints":
+                pose = rep.slam_update(data["hints"][t], data["scans"][t], nowait=nowait)[0]
+            else:
+                pose = rep.slam_update_ranges(data["hints"][t], data["ranges"][t], nowait=nowait)[0]
+            out.append((pose,) + rep.get_dist_batch(level, wb, we) + rep.raycast_batch(level, cb, ce))
+        for i, (x, y) in enumerate(zip(*out)):
+            assert np.array_equal(bits(x) if x.dtype == np.float32 else x, bits(y) if y.dtype == np.float32 else y), (t, i)
+        assert out[0][3].sum() > 0, t   # some world ray hits a wall
+    for l in range(3):
+        assert same(twins[0].download_level(l), twins[1].download_level(l)), l
+    for rep in twins:
+        rep.close()
+
+
+# ---- §6 -----------------------------------------------------------------------------------------------------------
 
 REPL_MAPS = [(404, 300, 3, (0.5, 0.5)), (257, 131, 2, (0.3, 0.7))]
 
