@@ -43,6 +43,8 @@ EXPORTED = [
     "hsb_group_slam_update_subset", "hsb_group_slam_update_cloud_subset", "hsb_group_slam_update_ranges_subset",
     "hsb_group_slam_update_projected_subset", "hsb_group_sync_occupancy", "hsb_group_sync_occupancy_subset",
     "hsb_group_get_dist", "hsb_group_get_dist_subset", "hsb_group_raycast", "hsb_group_raycast_subset",
+    "hsb_group_likelihood", "hsb_group_likelihood_subset", "hsb_group_covariance", "hsb_group_covariance_subset",
+    "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
 ]
 
 
@@ -203,6 +205,12 @@ def load_library() -> C.CDLL:
     sig("hsb_group_get_dist_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_raycast", i, vp, i, vp, vp, vp, vp, vp)
     sig("hsb_group_raycast_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp)
+    sig("hsb_group_likelihood", i, vp, i, vp, vp, vp, vp, vp)
+    sig("hsb_group_likelihood_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp)
+    sig("hsb_group_covariance", i, vp, i, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_covariance_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_best_hypothesis", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_best_hypothesis_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -1087,6 +1095,61 @@ class SlamGroup:
         else:
             self._check(self.lib.hsb_group_raycast_subset(self.g, K, _ptr(mem), *args))
         return dist, hit
+
+    def _score_args(self, level, poses_world, points, members):
+        """the arguments the three pose-scoring calls share -> (K, mem, Q, args, arrays kept alive)"""
+        K, mem = self._sessions(members)
+        poses, pose_off = self._pack(poses_world, 3, K)
+        if points is None:
+            pts, scan_off, pp, op = None, None, None, None
+        else:
+            pts, scan_off = self._pack(points, 2, K)
+            if pts.shape[0] == 0:
+                pts = np.zeros((1, 2), np.float32)   # (a pointer for the C call: points and offsets come together)
+            pp, op = pts.ctypes.data, scan_off.ctypes.data
+        Q = poses.shape[0]
+        return K, mem, Q, (int(level), pose_off.ctypes.data, _ptr(poses if Q else None), pp, op), (poses, pose_off, pts, scan_off)
+
+    def likelihood(self, level: int, poses_world, points=None, members=None) -> np.ndarray:
+        """getLikelihoodForState of the members' poses in one pass (hsb_group_likelihood): poses_world is one (q_s, 3)
+        array of world poses per session, or a tuple (poses (Q, 3), offsets (K + 1,)); every pose of a session is
+        scored against that session's one scan on its member's map.  points: one (n_s, 2) endpoint array per session
+        (level-0 cells), or a tuple (points, offsets); None = each member's last matched scan as it is on the device.
+        members as in slam_update (hsb_group_likelihood_subset).  Each value equals likelihood_batch on its member.
+        -> likelihood (Q,), in pose order"""
+        K, mem, Q, args, keep = self._score_args(level, poses_world, points, members)
+        out = np.zeros(Q, np.float32)
+        if mem is None:
+            self._check(self.lib.hsb_group_likelihood(self.g, *args, out.ctypes.data))
+        else:
+            self._check(self.lib.hsb_group_likelihood_subset(self.g, K, _ptr(mem), *args, out.ctypes.data))
+        return out
+
+    def covariance(self, level: int, poses_world, points=None, members=None):
+        """getCovarianceForPose (+ getCovMatrixWorldCoords) of the members' poses in one pass (hsb_group_covariance);
+        arguments as in likelihood (hsb_group_covariance_subset with members).  Each matrix equals covariance_batch on
+        its member.  -> (cov_map (Q, 3, 3), cov_world (Q, 3, 3)), in pose order"""
+        K, mem, Q, args, keep = self._score_args(level, poses_world, points, members)
+        cm, cw = np.zeros((Q, 9), np.float32), np.zeros((Q, 9), np.float32)
+        if mem is None:
+            self._check(self.lib.hsb_group_covariance(self.g, *args, cm.ctypes.data, cw.ctypes.data))
+        else:
+            self._check(self.lib.hsb_group_covariance_subset(self.g, K, _ptr(mem), *args, cm.ctypes.data, cw.ctypes.data))
+        return cm.reshape(Q, 3, 3), cw.reshape(Q, 3, 3)
+
+    def best_hypothesis(self, level: int, poses_world, points=None, members=None):
+        """The most likely of each session's poses in one pass (hsb_group_best_hypothesis): relocalisation of several
+        robots at once; arguments as in likelihood (hsb_group_best_hypothesis_subset with members).  Each session's
+        winner equals best_hypothesis_device on its member: the highest likelihood, the lowest index among equals.
+        -> (likelihood (Q,), best4 (K, 4) {likelihood, x, y, psi}, index (K,) within the session, -1 where it is empty)"""
+        K, mem, Q, args, keep = self._score_args(level, poses_world, points, members)
+        out, best4, index = np.zeros(Q, np.float32), np.zeros((K, 4), np.float32), np.zeros(K, np.int32)
+        tail = (out.ctypes.data, best4.ctypes.data if K else None, index.ctypes.data if K else None)
+        if mem is None:
+            self._check(self.lib.hsb_group_best_hypothesis(self.g, *args, *tail))
+        else:
+            self._check(self.lib.hsb_group_best_hypothesis_subset(self.g, K, _ptr(mem), *args, *tail))
+        return out, best4, index
 
     def _sessions(self, members):
         """-> (sessions of the step, the member list as int32, or None for a step of every member)"""

@@ -2452,6 +2452,10 @@ struct hsb_group {
   float* h_ray_stage = nullptr;
   size_t h_ray_stage_bytes = 0;
   DevBuf d_ray_stage;
+  // pose scoring (hsb_group_likelihood, hsb_group_covariance, hsb_group_best_hypothesis) stages through the ray queries'
+  // staging above (every call that fills it returns synchronised); M arg-max accumulators of the best hypothesis,
+  // zeroed once (every call re-arms the ones it used)
+  unsigned long long* d_best = nullptr;
 };
 
 namespace {
@@ -2495,6 +2499,7 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->h_occ_meta) cudaFreeHost(g->h_occ_meta);
   if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
   if (g->d_planes) cudaFree(g->d_planes);
+  if (g->d_best) cudaFree(g->d_best);
   if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
   if (g->h_ray_stage) cudaFreeHost(g->h_ray_stage);
   if (g->d_res) cudaFree(g->d_res);
@@ -2584,6 +2589,8 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
       for (int l = 0; l < g->levels; ++l) planes[(size_t)s * g->levels + l] = g->m[s]->lv[l].logodds;
     HSB_GROUP_CUDA(cudaMalloc(&g->d_planes, planes.size() * sizeof(float*)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_planes, planes.data(), planes.size() * sizeof(float*), cudaMemcpyHostToDevice));
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_best, (size_t)M * sizeof(unsigned long long)));
+    HSB_GROUP_CUDA(cudaMemset(g->d_best, 0, (size_t)M * sizeof(unsigned long long)));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
   }
@@ -2996,9 +3003,197 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
                    world, K, members, offsets, begin, end, out_dist, out_hit, out_found);
 }
 
+
+// What a group pose-scoring call computes for every pose (hsb_group_likelihood, hsb_group_covariance) or session
+// (hsb_group_best_hypothesis).
+enum ScoreKind { SCORE_LIKELIHOOD, SCORE_COVARIANCE, SCORE_BEST };
+
+// hsb_likelihood_batch / hsb_covariance_batch / hsb_best_hypothesis_device for K members in one pass: session k's poses
+// [pose_offsets[k], pose_offsets[k+1]) scored on member members[k]'s map of `level` against the session's scan
+// (pts[scan_offsets[k] ..), or, with pts and scan_offsets NULL, the member's last-match container as it is on the device
+// when the call runs).  Behind the members' queued work, through the group's pinned query staging: one copy each way, one
+// launch (two for the best hypothesis) and one synchronise, whatever K is.  No member's state changes.
+int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* members, int level, const int* pose_offsets,
+                const float* poses, const float* pts, const int* scan_offsets, float* out_lh, float* out_map,
+                float* out_world, float* out_best4, int* out_best_index) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (level < 0 || level >= g->levels)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if (!pose_offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets is NULL", fn);
+  if (pose_offsets[0] != 0)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets[0] is %d, must be 0", fn, pose_offsets[0]);
+  for (int k = 0; k < K; ++k)
+    if (pose_offsets[k + 1] < pose_offsets[k])
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets decrease at session %d (%d -> %d)", fn, k, pose_offsets[k],
+                  pose_offsets[k + 1]);
+  if (!pts != !scan_offsets)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: points_xy and scan_offsets must both be given or both be NULL", fn);
+  const bool last = !pts;   // every session's scan is its member's last-match container
+  if (!last) {
+    if (scan_offsets[0] != 0)
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets[0] is %d, must be 0", fn, scan_offsets[0]);
+    for (int k = 0; k < K; ++k)
+      if (scan_offsets[k + 1] < scan_offsets[k])
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets decrease at session %d (%d -> %d)", fn, k, scan_offsets[k],
+                    scan_offsets[k + 1]);
+  }
+  const int Q = pose_offsets[K];
+  if (Q == 0) {   // nothing to score: every session's best hypothesis is the empty batch's
+    for (int k = 0; kind == SCORE_BEST && out_best4 && k < K; ++k) {
+      out_best4[4 * k] = -1.0f;
+      out_best4[4 * k + 1] = out_best4[4 * k + 2] = out_best4[4 * k + 3] = 0.0f;
+      if (out_best_index) out_best_index[k] = -1;
+    }
+    return HSB_OK;
+  }
+  if (!poses) return fail(h0, HSB_ERR_INVALID_ARG, "%s: poses_world is NULL", fn);
+  if (kind == SCORE_LIKELIHOOD && !out_lh) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_likelihood is NULL", fn);
+  if (kind == SCORE_COVARIANCE && !out_map && !out_world)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_cov_map and out_cov_world are both NULL", fn);
+  if (kind == SCORE_BEST && !out_best4) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_best4 is NULL", fn);
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
+
+  // staging: sessions | pose offsets | poses | (scans), then the results: likelihoods | best4 | best index, or
+  // covariance (map) | covariance (world), each only if asked for
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t total = last ? 0 : (size_t)scan_offsets[K];
+  const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_poses = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_pts = al(o_poses + (size_t)Q * 12), in_end = o_pts + total * 8, o_out = al(in_end);
+  size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, out_end = o_out;
+  if (kind == SCORE_COVARIANCE) {
+    o_world = o_map + (out_map ? (size_t)Q * 36 : 0);
+    out_end = o_world + (out_world ? (size_t)Q * 36 : 0);
+  } else {
+    o_best4 = al(o_lh + (size_t)Q * 4);
+    o_index = o_best4 + (kind == SCORE_BEST ? (size_t)K * 16 : 0);
+    out_end = kind == SCORE_BEST ? o_index + (size_t)K * 4 : o_lh + (size_t)Q * 4;
+  }
+  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
+  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
+  char* hs = reinterpret_cast<char*>(g->h_ray_stage);
+  char* ds = static_cast<char*>(g->d_ray_stage.p);
+  HsbScoreSessionDev* sess = reinterpret_cast<HsbScoreSessionDev*>(hs);
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
+    sess[k].member = members[k];
+    if (last) {   // (a member that never matched has no container: n = 0)
+      sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+      sess[k].n = h->d_last_pts.p ? h->last_n : 0;
+    } else {
+      sess[k].pts = reinterpret_cast<const float2*>(ds + o_pts) + scan_offsets[k];
+      sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
+    }
+  }
+  memcpy(hs + o_off, pose_offsets, (size_t)(K + 1) * 4);
+  memcpy(hs + o_poses, poses, (size_t)Q * 12);
+  if (total > 0) memcpy(hs + o_pts, pts, total * 8);
+  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, in_end, cudaMemcpyHostToDevice, st));
+
+  HsbScoreParams P;
+  memset(&P, 0, sizeof(P));
+  P.lv = g->d_lv;
+  P.sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
+  P.pose_offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.poses = reinterpret_cast<const float*>(ds + o_poses);
+  P.cell_length = h0->lv[level].cell_length;
+  P.levels = g->levels;
+  P.level = level;
+  P.K = K;
+  P.Q = Q;
+  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create checked)
+  if (kind == SCORE_COVARIANCE) {
+    P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
+    P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
+    const int blocks = std::min(Q, h0->sm_count * 8);
+    if (tex) hsb::covariance_group_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
+    else hsb::covariance_group_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(P);
+    h0->launches++;
+  } else {
+    P.out = reinterpret_cast<float*>(ds + o_lh);
+    if (kind == SCORE_BEST) {
+      P.best = g->d_best;
+      P.out_best4 = reinterpret_cast<float*>(ds + o_best4);
+      P.out_best_index = reinterpret_cast<int*>(ds + o_index);
+    }
+    const int blocks = std::min((Q + 3) / 4, h0->sm_count * 16);
+    if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
+    else hsb::likelihood_group_kernel<hsb::MODE_LDG><<<blocks, 128, 0, st>>>(P);
+    h0->launches++;
+    if (kind == SCORE_BEST) {
+      HSB_CUDA(h0, cudaGetLastError());
+      hsb::best_group_finish_kernel<<<(K + 127) / 128, 128, 0, st>>>(P);
+      h0->launches++;
+    }
+  }
+  HSB_CUDA(h0, cudaGetLastError());
+  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_out, ds + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h0, cudaStreamSynchronize(st));
+  if (kind == SCORE_COVARIANCE) {
+    if (out_map) memcpy(out_map, hs + o_map, (size_t)Q * 36);
+    if (out_world) memcpy(out_world, hs + o_world, (size_t)Q * 36);
+  } else {
+    if (out_lh) memcpy(out_lh, hs + o_lh, (size_t)Q * 4);
+    if (kind == SCORE_BEST) {
+      memcpy(out_best4, hs + o_best4, (size_t)K * 16);
+      if (out_best_index) memcpy(out_best_index, hs + o_index, (size_t)K * 4);
+    }
+  }
+  return HSB_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int hsb_group_likelihood(hsb_group* g, int level, const int* pose_offsets, const float* poses_world, const float* points_xy,
+                         const int* scan_offsets, float* out_likelihood) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_likelihood", SCORE_LIKELIHOOD, (int)g->m.size(), g->all.data(), level, pose_offsets,
+                     poses_world, points_xy, scan_offsets, out_likelihood, nullptr, nullptr, nullptr, nullptr);
+}
+
+int hsb_group_likelihood_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                float* out_likelihood) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_likelihood_subset", SCORE_LIKELIHOOD, K, members, level, pose_offsets, poses_world,
+                     points_xy, scan_offsets, out_likelihood, nullptr, nullptr, nullptr, nullptr);
+}
+
+int hsb_group_covariance(hsb_group* g, int level, const int* pose_offsets, const float* poses_world, const float* points_xy,
+                         const int* scan_offsets, float* out_cov_map, float* out_cov_world) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_covariance", SCORE_COVARIANCE, (int)g->m.size(), g->all.data(), level, pose_offsets,
+                     poses_world, points_xy, scan_offsets, nullptr, out_cov_map, out_cov_world, nullptr, nullptr);
+}
+
+int hsb_group_covariance_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                float* out_cov_map, float* out_cov_world) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_covariance_subset", SCORE_COVARIANCE, K, members, level, pose_offsets, poses_world,
+                     points_xy, scan_offsets, nullptr, out_cov_map, out_cov_world, nullptr, nullptr);
+}
+
+int hsb_group_best_hypothesis(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
+                              const float* points_xy, const int* scan_offsets, float* out_likelihood, float* out_best4,
+                              int* out_best_index) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_best_hypothesis", SCORE_BEST, (int)g->m.size(), g->all.data(), level, pose_offsets,
+                     poses_world, points_xy, scan_offsets, out_likelihood, nullptr, nullptr, out_best4, out_best_index);
+}
+
+int hsb_group_best_hypothesis_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                     const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                     float* out_likelihood, float* out_best4, int* out_best_index) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_score(g, "hsb_group_best_hypothesis_subset", SCORE_BEST, K, members, level, pose_offsets, poses_world,
+                     points_xy, scan_offsets, out_likelihood, nullptr, nullptr, out_best4, out_best_index);
+}
 
 int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,
                       float* out_dist, int* out_hit) {

@@ -200,6 +200,32 @@ struct HsbRayParams {
   float origo_x, origo_y, scale, inv_scale;   // getDist: the level's map origin and cell length, 1 / cell length
 };
 
+// One session of a group pose-scoring call: the scan its poses are scored against and the member whose map they are
+// scored on.
+struct HsbScoreSessionDev {
+  const float2* pts;   // the session's slice of the staged scans, or the member's last-match container
+  int n;
+  int member;
+};
+
+// A group pose-scoring call (likelihood_group_kernel, best_group_finish_kernel, covariance_group_kernel:
+// hsb_group_likelihood, hsb_group_best_hypothesis, hsb_group_covariance): Q poses of K sessions, session k's poses
+// [pose_offsets[k], pose_offsets[k+1]).  Arrays in device memory; outputs in pose order.
+struct HsbScoreParams {
+  const HsbLevelDev* lv;            // members x levels, member-major (hsb_group::d_lv)
+  const HsbScoreSessionDev* sess;   // K
+  const int* pose_offsets;          // K + 1
+  const float* poses;               // Q x 3, world
+  float* out;                       // Q likelihoods, or null
+  unsigned long long* best;         // K arg-max accumulators (best hypothesis), or null
+  float* out_best4;                 // K x 4 (best hypothesis)
+  int* out_best_index;              // K (best hypothesis)
+  float* out_map;                   // Q x 9 (covariance), or null
+  float* out_world;                 // Q x 9 (covariance), or null
+  float cell_length;                // of the level (covariance: the world matrix)
+  int levels, level, K, Q;
+};
+
 // Map write of a group SLAM step (update_mark_group_kernel / update_apply_group_kernel): blockIdx.z = session,
 // blockIdx.y = level.  Everything per session lives in device memory, uploaded with the step's scans.
 struct HsbGroupUpdateParams {

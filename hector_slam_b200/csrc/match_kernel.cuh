@@ -1187,6 +1187,35 @@ __device__ __forceinline__ float warp_likelihood(const LevelRegs& LR, float pt_s
   return 1.0f - residual / (float)n;  // getLikelihoodForResidual :203-209
 }
 
+// One pose of a likelihood batch, by one warp: the world pose to the level's map coordinates (getMapCoordsPose), then
+// warp_likelihood.  Shared by likelihood_kernel and likelihood_group_kernel.
+template <int MODE>
+__device__ __forceinline__ float pose_likelihood(const HsbLevelDev& L, const LevelRegs& LR, const float* __restrict__ pose_world,
+                                                 const float2* __restrict__ pts, int n, int lane) {
+  float ex, ey;
+  affine_apply_exact(L.mtw, pose_world[0], pose_world[1], ex, ey);
+  return warp_likelihood<MODE>(LR, L.pt_scale, pts, n, ex, ey, pose_world[2], lane);
+}
+
+// arg-max over a batch (relocalisation: the most likely hypothesis): (score, index) packed so that one 64-bit atomicMax
+// keeps the highest score and, among equals, the LOWEST index; a non-finite pose scores -1, and so does a NaN
+// likelihood (an empty scan: 1 - 0/0), whose bits would otherwise pack above every score
+__device__ __forceinline__ unsigned long long best_pack(float lh, const float* __restrict__ pose_world, unsigned index) {
+  const float px = pose_world[0], py = pose_world[1], pp = pose_world[2];
+  const bool finite = fabsf(px) <= 3.4e38f && fabsf(py) <= 3.4e38f && fabsf(pp) <= 3.4e38f;
+  const float sc = (finite && lh == lh) ? lh : -1.0f;
+  unsigned u = __float_as_uint(sc);
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)u << 32) | (unsigned long long)(0xffffffffu - index);
+}
+// ... and back: the winner's score and index (v != 0: an accumulator no pose reached stays 0)
+__device__ __forceinline__ float best_unpack(unsigned long long v, unsigned& index) {
+  unsigned u = (unsigned)(v >> 32);
+  u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+  index = 0xffffffffu - (unsigned)(v & 0xffffffffull);
+  return __uint_as_float(u);
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(128)
     likelihood_kernel(const HsbLevelDev L, int B, const float* __restrict__ poses_world, const float2* __restrict__ pts_all,
@@ -1202,22 +1231,10 @@ __global__ void __launch_bounds__(128)
       beg = offsets[b];
       n = offsets[b + 1] - beg;
     }
-    float ex, ey;
-    affine_apply_exact(L.mtw, poses_world[3 * b], poses_world[3 * b + 1], ex, ey);
-    const float lh = warp_likelihood<MODE>(LR, L.pt_scale, pts_all + beg, n, ex, ey, poses_world[3 * b + 2], lane);
+    const float lh = pose_likelihood<MODE>(L, LR, poses_world + 3 * b, pts_all + beg, n, lane);
     if (lane == 0) {
       if (out) out[b] = lh;
-      if (best) {
-        // arg-max over the batch (relocalisation: the most likely hypothesis): (score, index) packed so that one
-        // 64-bit atomicMax keeps the highest score and, among equals, the LOWEST index; a non-finite pose scores -1,
-        // and so does a NaN likelihood (an empty scan: 1 - 0/0), whose bits would otherwise pack above every score
-        const float px = poses_world[3 * b], py = poses_world[3 * b + 1], pp = poses_world[3 * b + 2];
-        const bool finite = fabsf(px) <= 3.4e38f && fabsf(py) <= 3.4e38f && fabsf(pp) <= 3.4e38f;
-        const float sc = (finite && lh == lh) ? lh : -1.0f;
-        unsigned u = __float_as_uint(sc);
-        u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-        atomicMax(best, ((unsigned long long)u << 32) | (unsigned long long)(0xffffffffu - (unsigned)b));
-      }
+      if (best) atomicMax(best, best_pack(lh, poses_world + 3 * b, (unsigned)b));
     }
   }
 }
@@ -1231,25 +1248,141 @@ __global__ void best_hypothesis_finish_kernel(unsigned long long* __restrict__ b
     out4[0] = -1.0f; out4[1] = 0.0f; out4[2] = 0.0f; out4[3] = 0.0f;
     return;
   }
-  unsigned u = (unsigned)(v >> 32);
-  u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-  const unsigned b = 0xffffffffu - (unsigned)(v & 0xffffffffull);
-  out4[0] = __uint_as_float(u);
+  unsigned b;
+  out4[0] = best_unpack(v, b);
   out4[1] = poses_world[3 * b]; out4[2] = poses_world[3 * b + 1]; out4[3] = poses_world[3 * b + 2];
 }
 
+// The session of entry q of a group query: the last session whose entries start at or before q (empty sessions are
+// passed over), as ray_kernel finds a ray's.
+__device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K, int q) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offsets[mid] <= q) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// N3 for a group (hsb_group_likelihood, hsb_group_best_hypothesis): pose q of the call belongs to the session k whose
+// poses are [pose_offsets[k], pose_offsets[k+1]) and is scored against that session's scan on its member's map of the
+// level (the group's descriptor table).  One warp per pose, grid-stride; the value is likelihood_kernel's.  With `best`,
+// session k's arg-max goes to best[k], the index being the pose's index in its session.
+template <int MODE>
+__global__ void __launch_bounds__(128) likelihood_group_kernel(const HsbScoreParams P) {
+  const int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int q = warp; q < P.Q; q += nwarps) {
+    const int k = session_of(P.pose_offsets, P.K, q);
+    const HsbScoreSessionDev s = P.sess[k];
+    const HsbLevelDev& L = P.lv[(size_t)s.member * P.levels + P.level];
+    const LevelRegs LR = level_regs(L);   // (all 32 lanes are here: a warp's lanes share q)
+    const float lh = pose_likelihood<MODE>(L, LR, P.poses + 3 * (size_t)q, s.pts, s.n, lane);
+    if (lane == 0) {
+      if (P.out) P.out[q] = lh;
+      if (P.best) atomicMax(P.best + k, best_pack(lh, P.poses + 3 * (size_t)q, (unsigned)(q - P.pose_offsets[k])));
+    }
+  }
+}
+// second launch of hsb_group_best_hypothesis: thread k unpacks session k's winner and re-arms its accumulator
+__global__ void __launch_bounds__(128) best_group_finish_kernel(const HsbScoreParams P) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= P.K) return;
+  const unsigned long long v = P.best[k];
+  P.best[k] = 0ull;
+  float* out4 = P.out_best4 + 4 * (size_t)k;
+  if (v == 0ull) {   // empty session
+    out4[0] = -1.0f; out4[1] = 0.0f; out4[2] = 0.0f; out4[3] = 0.0f;
+    P.out_best_index[k] = -1;
+    return;
+  }
+  unsigned b;
+  out4[0] = best_unpack(v, b);
+  const float* pose = P.poses + 3 * ((size_t)P.pose_offsets[k] + b);
+  out4[1] = pose[0]; out4[2] = pose[1]; out4[3] = pose[2];
+  P.out_best_index[k] = (int)b;
+}
+
+// getCovarianceForPose's sigma points (OccGridMapUtil.h:109-135): +-1.5 cells in x and y, +-0.05 rad, the pose itself
+constexpr float kSigmaCells = 1.5f, kSigmaAngle = 0.05f;
+// sigma point k of the pose (x, y, ang) in map coordinates
+__device__ __forceinline__ void sigma_point(int k, float x, float y, float ang, float& sx, float& sy, float& sa) {
+  sx = x; sy = y; sa = ang;
+  if (k == 0) sx = __fadd_rn(x, kSigmaCells);
+  else if (k == 1) sx = __fsub_rn(x, kSigmaCells);
+  else if (k == 2) sy = __fadd_rn(y, kSigmaCells);
+  else if (k == 3) sy = __fsub_rn(y, kSigmaCells);
+  else if (k == 4) sa = __fadd_rn(ang, kSigmaAngle);
+  else if (k == 5) sa = __fsub_rn(ang, kSigmaAngle);
+}
+// The likelihood-weighted mean and covariance of the seven sigma points (:137-154) with the fixed-size Eigen operations
+// in the order oracle/shim fixes: likelihoods.sum() by recursive halving, mean += point * lh, mean *= 1/sum,
+// cov += (lh * inv) * (d * d^T), every operation rounded separately; then getCovMatrixWorldCoords (:162-187).  One thread;
+// the matrices of pose b go to out_map / out_world + 9 b (either may be null).
+__device__ __forceinline__ void sigma_covariance(const float* lhs, float x, float y, float ang, float cell_length, int b,
+                                                 float* __restrict__ out_map, float* __restrict__ out_world) {
+  const float dt = kSigmaCells, da = kSigmaAngle;
+  const float sp[7][3] = {{__fadd_rn(x, dt), y, ang}, {__fsub_rn(x, dt), y, ang}, {x, __fadd_rn(y, dt), ang},
+                          {x, __fsub_rn(y, dt), ang}, {x, y, __fadd_rn(ang, da)}, {x, y, __fsub_rn(ang, da)}, {x, y, ang}};
+  const float sum = __fadd_rn(__fadd_rn(lhs[0], __fadd_rn(lhs[1], lhs[2])),
+                              __fadd_rn(__fadd_rn(lhs[3], lhs[4]), __fadd_rn(lhs[5], lhs[6])));
+  const float inv = __fdiv_rn(1.0f, sum);                                       // :137
+  float mean[3] = {0.f, 0.f, 0.f};
+  for (int i = 0; i < 7; ++i)
+    for (int c = 0; c < 3; ++c) mean[c] = __fadd_rn(mean[c], __fmul_rn(sp[i][c], lhs[i]));   // :144
+  for (int c = 0; c < 3; ++c) mean[c] = __fmul_rn(mean[c], inv);                             // :147
+  float cov[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int i = 0; i < 7; ++i) {                                                               // :151-154
+    const float d[3] = {__fsub_rn(sp[i][0], mean[0]), __fsub_rn(sp[i][1], mean[1]), __fsub_rn(sp[i][2], mean[2])};
+    const float wgt = __fmul_rn(lhs[i], inv);
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) cov[3 * r + c] = __fadd_rn(cov[3 * r + c], __fmul_rn(wgt, __fmul_rn(d[r], d[c])));
+  }
+  if (out_map)
+    for (int c = 0; c < 9; ++c) out_map[9 * (size_t)b + c] = cov[c];
+  if (out_world) {                                                                            // :162-187
+    float* w = out_world + 9 * (size_t)b;
+    const float st = cell_length, st2 = __fmul_rn(st, st);
+    w[0] = __fmul_rn(cov[0], st2);
+    w[4] = __fmul_rn(cov[4], st2);
+    w[3] = __fmul_rn(cov[3], st2);
+    w[1] = w[3];
+    w[6] = __fmul_rn(cov[6], st);
+    w[2] = w[6];
+    w[7] = __fmul_rn(cov[7], st);
+    w[5] = w[7];
+    w[8] = cov[8];
+  }
+}
+// Pose b of a covariance batch, by one CTA of 7 warps: warp k evaluates the likelihood of sigma point k, thread 0 forms
+// the matrices.  Ends with a barrier, so the caller may loop.  Shared by covariance_kernel and covariance_group_kernel.
+template <int MODE>
+__device__ __forceinline__ void pose_covariance(const HsbLevelDev& L, const LevelRegs& LR, const float* __restrict__ poses_world,
+                                                int b, const float2* __restrict__ pts, int n, float cell_length,
+                                                float* __restrict__ out_map, float* __restrict__ out_world) {
+  __shared__ float lhs[7];
+  const int lane = threadIdx.x & 31, k = threadIdx.x >> 5;
+  float x, y;
+  affine_apply_exact(L.mtw, poses_world[3 * b], poses_world[3 * b + 1], x, y);   // getMapCoordsPose
+  const float ang = poses_world[3 * b + 2];
+  float sx, sy, sa;
+  sigma_point(k, x, y, ang, sx, sy, sa);
+  const float lh = warp_likelihood<MODE>(LR, L.pt_scale, pts, n, sx, sy, sa, lane);
+  if (lane == 0) lhs[k] = lh;
+  __syncthreads();
+  if (threadIdx.x == 0) sigma_covariance(lhs, x, y, ang, cell_length, b, out_map, out_world);
+  __syncthreads();
+}
+
 // N3: OccGridMapUtil::getCovarianceForPose (OccGridMapUtil.h:106-160) + getCovMatrixWorldCoords (:162-187) for a batch of
-// poses: one CTA of 7 warps per pose, warp k evaluates the likelihood of sigma point k (:119-135: +-1.5 cells in x and
-// y, +-0.05 rad, the pose itself), thread 0 forms the likelihood-weighted mean and covariance with the fixed-size
-// Eigen operations in the order oracle/shim fixes: likelihoods.sum() by recursive halving, mean += point * lh,
-// mean *= 1/sum, cov += (lh * inv) * (d * d^T), every operation rounded separately.
+// poses: one CTA of 7 warps per pose (pose_covariance).
 template <int MODE>
 __global__ void __launch_bounds__(224)
     covariance_kernel(const HsbLevelDev L, int B, const float* __restrict__ poses_world, const float2* __restrict__ pts_all,
                       const int* __restrict__ offsets, int n_shared, float cell_length, float* __restrict__ out_map,
                       float* __restrict__ out_world) {
-  __shared__ float lhs[7];
-  const int lane = threadIdx.x & 31, k = threadIdx.x >> 5;
   const LevelRegs LR = level_regs(L);
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
     int beg = 0, n = n_shared;
@@ -1257,54 +1390,19 @@ __global__ void __launch_bounds__(224)
       beg = offsets[b];
       n = offsets[b + 1] - beg;
     }
-    float x, y;
-    affine_apply_exact(L.mtw, poses_world[3 * b], poses_world[3 * b + 1], x, y);   // getMapCoordsPose
-    const float ang = poses_world[3 * b + 2];
-    const float dt = 1.5f, da = 0.05f;                                             // :109-111
-    float sx = x, sy = y, sa = ang;
-    if (k == 0) sx = __fadd_rn(x, dt);
-    else if (k == 1) sx = __fsub_rn(x, dt);
-    else if (k == 2) sy = __fadd_rn(y, dt);
-    else if (k == 3) sy = __fsub_rn(y, dt);
-    else if (k == 4) sa = __fadd_rn(ang, da);
-    else if (k == 5) sa = __fsub_rn(ang, da);
-    const float lh = warp_likelihood<MODE>(LR, L.pt_scale, pts_all + beg, n, sx, sy, sa, lane);
-    if (lane == 0) lhs[k] = lh;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const float sp[7][3] = {{__fadd_rn(x, dt), y, ang}, {__fsub_rn(x, dt), y, ang}, {x, __fadd_rn(y, dt), ang},
-                              {x, __fsub_rn(y, dt), ang}, {x, y, __fadd_rn(ang, da)}, {x, y, __fsub_rn(ang, da)}, {x, y, ang}};
-      const float sum = __fadd_rn(__fadd_rn(lhs[0], __fadd_rn(lhs[1], lhs[2])),
-                                  __fadd_rn(__fadd_rn(lhs[3], lhs[4]), __fadd_rn(lhs[5], lhs[6])));
-      const float inv = __fdiv_rn(1.0f, sum);                                       // :137
-      float mean[3] = {0.f, 0.f, 0.f};
-      for (int i = 0; i < 7; ++i)
-        for (int c = 0; c < 3; ++c) mean[c] = __fadd_rn(mean[c], __fmul_rn(sp[i][c], lhs[i]));   // :144
-      for (int c = 0; c < 3; ++c) mean[c] = __fmul_rn(mean[c], inv);                             // :147
-      float cov[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      for (int i = 0; i < 7; ++i) {                                                               // :151-154
-        const float d[3] = {__fsub_rn(sp[i][0], mean[0]), __fsub_rn(sp[i][1], mean[1]), __fsub_rn(sp[i][2], mean[2])};
-        const float wgt = __fmul_rn(lhs[i], inv);
-        for (int r = 0; r < 3; ++r)
-          for (int c = 0; c < 3; ++c) cov[3 * r + c] = __fadd_rn(cov[3 * r + c], __fmul_rn(wgt, __fmul_rn(d[r], d[c])));
-      }
-      if (out_map)
-        for (int c = 0; c < 9; ++c) out_map[9 * (size_t)b + c] = cov[c];
-      if (out_world) {                                                                            // :162-187
-        float* w = out_world + 9 * (size_t)b;
-        const float st = cell_length, st2 = __fmul_rn(st, st);
-        w[0] = __fmul_rn(cov[0], st2);
-        w[4] = __fmul_rn(cov[4], st2);
-        w[3] = __fmul_rn(cov[3], st2);
-        w[1] = w[3];
-        w[6] = __fmul_rn(cov[6], st);
-        w[2] = w[6];
-        w[7] = __fmul_rn(cov[7], st);
-        w[5] = w[7];
-        w[8] = cov[8];
-      }
-    }
-    __syncthreads();
+    pose_covariance<MODE>(L, LR, poses_world, b, pts_all + beg, n, cell_length, out_map, out_world);
+  }
+}
+
+// N3 for a group (hsb_group_covariance): covariance_kernel's CTA per pose, the pose's session, scan and member map
+// found as likelihood_group_kernel finds them; every member's cell length is the group's (one geometry).
+template <int MODE>
+__global__ void __launch_bounds__(224) covariance_group_kernel(const HsbScoreParams P) {
+  for (int q = blockIdx.x; q < P.Q; q += gridDim.x) {
+    const HsbScoreSessionDev s = P.sess[session_of(P.pose_offsets, P.K, q)];
+    const HsbLevelDev& L = P.lv[(size_t)s.member * P.levels + P.level];
+    const LevelRegs LR = level_regs(L);   // (every warp is whole here: a CTA's threads share q)
+    pose_covariance<MODE>(L, LR, P.poses, q, s.pts, s.n, P.cell_length, P.out_map, P.out_world);
   }
 }
 

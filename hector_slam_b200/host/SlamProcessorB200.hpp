@@ -331,6 +331,67 @@ class SlamProcessor {
     owner.check(hsb_group_get_dist_subset(owner.groupFor(ps, M), K, members, level, offsets, beginWorld, endWorld, dist,
                                           hitWorld, found));
   }
+  // getLikelihoodForState (OccGridMapUtil.h:189-221) for M processors in one pass (hsb_group_likelihood, through the
+  // group updateMany keeps): processor s's world poses [poseOffsets[s], poseOffsets[s+1]) of posesWorld (x, y, psi) are
+  // scored on its map of `level` against its scan pointsXY[scanOffsets[s] .. scanOffsets[s+1]) (level-0 cells), or,
+  // with pointsXY and scanOffsets null, against the scan of its last matched update as it is on the device.
+  // likelihood: one per pose, in pose order.
+  static void likelihoodMany(SlamProcessor* const* ps, int M, int level, const int* poseOffsets, const float* posesWorld,
+                             const float* pointsXY, const int* scanOffsets, float* likelihood) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "likelihoodMany");
+    owner.check(hsb_group_likelihood(owner.groupFor(ps, M), level, poseOffsets, posesWorld, pointsXY, scanOffsets,
+                                     likelihood));
+  }
+
+  // likelihoodMany() for the processors ps[members[0..K)] (hsb_group_likelihood_subset): session k's poses and scan
+  // belong to ps[members[k]]; the processors not listed are neither read nor waited for.
+  static void likelihoodMany(SlamProcessor* const* ps, int M, const int* members, int K, int level,
+                             const int* poseOffsets, const float* posesWorld, const float* pointsXY,
+                             const int* scanOffsets, float* likelihood) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "likelihoodMany");
+    owner.check(hsb_group_likelihood_subset(owner.groupFor(ps, M), K, members, level, poseOffsets, posesWorld, pointsXY,
+                                            scanOffsets, likelihood));
+  }
+
+  // getCovarianceForPose and getCovMatrixWorldCoords (OccGridMapUtil.h:106-187) for M processors in one pass
+  // (hsb_group_covariance); poses and scans as in likelihoodMany.  covMap / covWorld: 9 floats per pose, row-major;
+  // either may be null, not both.
+  static void covarianceMany(SlamProcessor* const* ps, int M, int level, const int* poseOffsets, const float* posesWorld,
+                             const float* pointsXY, const int* scanOffsets, float* covMap, float* covWorld) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "covarianceMany");
+    owner.check(hsb_group_covariance(owner.groupFor(ps, M), level, poseOffsets, posesWorld, pointsXY, scanOffsets, covMap,
+                                     covWorld));
+  }
+
+  // covarianceMany() for the processors ps[members[0..K)] (hsb_group_covariance_subset).
+  static void covarianceMany(SlamProcessor* const* ps, int M, const int* members, int K, int level,
+                             const int* poseOffsets, const float* posesWorld, const float* pointsXY,
+                             const int* scanOffsets, float* covMap, float* covWorld) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "covarianceMany");
+    owner.check(hsb_group_covariance_subset(owner.groupFor(ps, M), K, members, level, poseOffsets, posesWorld, pointsXY,
+                                            scanOffsets, covMap, covWorld));
+  }
+
+  // The most likely of each processor's pose hypotheses in one pass (hsb_group_best_hypothesis): relocalising several
+  // lost robots at once; poses and scans as in likelihoodMany.  best4: per processor {likelihood, x, y, psi} of its
+  // winner (the lowest index among equals; likelihood -1 without hypotheses); bestIndex (may be null): the winner's
+  // index among the processor's poses, -1 without hypotheses; likelihood (may be null): one per pose.
+  static void bestHypothesisMany(SlamProcessor* const* ps, int M, int level, const int* poseOffsets,
+                                 const float* posesWorld, const float* pointsXY, const int* scanOffsets, float* best4,
+                                 int* bestIndex = 0, float* likelihood = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "bestHypothesisMany");
+    owner.check(hsb_group_best_hypothesis(owner.groupFor(ps, M), level, poseOffsets, posesWorld, pointsXY, scanOffsets,
+                                          likelihood, best4, bestIndex));
+  }
+
+  // bestHypothesisMany() for the processors ps[members[0..K)] (hsb_group_best_hypothesis_subset).
+  static void bestHypothesisMany(SlamProcessor* const* ps, int M, const int* members, int K, int level,
+                                 const int* poseOffsets, const float* posesWorld, const float* pointsXY,
+                                 const int* scanOffsets, float* best4, int* bestIndex = 0, float* likelihood = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "bestHypothesisMany");
+    owner.check(hsb_group_best_hypothesis_subset(owner.groupFor(ps, M), K, members, level, poseOffsets, posesWorld,
+                                                 pointsXY, scanOffsets, likelihood, best4, bestIndex));
+  }
   hsb_handle* handle() { return h_; }
 
   // util::poseDifferenceLargerThan, util/UtilFunctions.h:73-92 (float norm, double pi arithmetic)

@@ -293,6 +293,82 @@ int hsbp_get_dist_many_subset(void* const* ps, int M, const int* members, int K,
   }
   return 0;
 }
+int hsbp_likelihood_many(void* const* ps, int M, int level, const int* pose_offsets, const float* poses_world,
+                         const float* points_xy, const int* scan_offsets, float* likelihood) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::likelihoodMany(procs.data(), M, level, pose_offsets, poses_world, points_xy, scan_offsets,
+                                          likelihood);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_likelihood_many_subset(void* const* ps, int M, const int* members, int K, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                float* likelihood) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::likelihoodMany(procs.data(), M, members, K, level, pose_offsets, poses_world, points_xy,
+                                          scan_offsets, likelihood);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_covariance_many(void* const* ps, int M, int level, const int* pose_offsets, const float* poses_world,
+                         const float* points_xy, const int* scan_offsets, float* cov_map, float* cov_world) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::covarianceMany(procs.data(), M, level, pose_offsets, poses_world, points_xy, scan_offsets,
+                                          cov_map, cov_world);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_covariance_many_subset(void* const* ps, int M, const int* members, int K, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets, float* cov_map,
+                                float* cov_world) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::covarianceMany(procs.data(), M, members, K, level, pose_offsets, poses_world, points_xy,
+                                          scan_offsets, cov_map, cov_world);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_best_hypothesis_many(void* const* ps, int M, int level, const int* pose_offsets, const float* poses_world,
+                              const float* points_xy, const int* scan_offsets, float* best4, int* best_index,
+                              float* likelihood) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::bestHypothesisMany(procs.data(), M, level, pose_offsets, poses_world, points_xy, scan_offsets,
+                                              best4, best_index, likelihood);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_best_hypothesis_many_subset(void* const* ps, int M, const int* members, int K, int level,
+                                     const int* pose_offsets, const float* poses_world, const float* points_xy,
+                                     const int* scan_offsets, float* best4, int* best_index, float* likelihood) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::bestHypothesisMany(procs.data(), M, members, K, level, pose_offsets, poses_world, points_xy,
+                                              scan_offsets, best4, best_index, likelihood);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

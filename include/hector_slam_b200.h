@@ -528,6 +528,61 @@ int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* be
                       float* out_dist, int* out_hit);
 int hsb_group_raycast_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
                              const int* begin_cells, const int* end_cells, float* out_dist, int* out_hit);
+/* Scoring poses for K of the group's members in one pass: hsb_group_likelihood is hsb_likelihood_batch
+ * (getLikelihoodForState, OccGridMapUtil.h:189-221), hsb_group_covariance is hsb_covariance_batch (getCovarianceForPose,
+ * :106-187) and hsb_group_best_hypothesis is hsb_best_hypothesis_device.  A server scores the poses a group step
+ * returned (the step's own "covariance" is the raw Hessian; the likelihood of the returned pose is the reference's measure
+ * of a match gone wrong) or picks the best of many hypotheses for each lost robot.
+ * Session k is member members[k] (the full form: every member, in order).  Its poses are [pose_offsets[k],
+ * pose_offsets[k+1]) of poses_world (Q x 3, Q = pose_offsets[K]; a session may hold none).  All of a session's poses are
+ * scored against that session's ONE scan, on that member's map, at `level`.  The outputs are in pose order:
+ * out_likelihood Q (may be NULL for the best hypothesis), out_cov_map / out_cov_world Q x 9 (either may be NULL, not
+ * both), out_best4 K x 4 {likelihood, x, y, psi} and out_best_index K (may be NULL; the winner's index within its
+ * session, -1 for an empty session).
+ * The scan of session k:
+ *  - points_xy and scan_offsets given: points_xy[scan_offsets[k] .. scan_offsets[k+1]), level-0 cell units, DataContainer
+ *    layout, as hsb_likelihood_batch takes them;
+ *  - points_xy == NULL and scan_offsets == NULL: the member's last-match container as it is on the device when the call
+ *    runs on the group's stream, that is the endpoints of the member's last matched step of any input kind (single or
+ *    group).  No scan crosses the bus.  A step with map_without_matching set does not replace the container: the scan of
+ *    the last MATCHED step stays in force.  A member that has never matched has n = 0, which gives the reference's
+ *    1 - 0/0 NaN as the single call does for an empty scan.
+ * Bits: every likelihood equals hsb_likelihood_batch(member, level, ...) on the same pose and scan bit for bit, every
+ * covariance equals hsb_covariance_batch bit for bit (NaN patterns included), and every session's out_best4 equals
+ * hsb_best_hypothesis_device on that member with the session's poses: the highest score, the lowest index among equals;
+ * a non-finite pose and a NaN likelihood score -1; an empty session gives {-1, 0, 0, 0}.  With the last-match container
+ * the scan is the one hsb_cloud_to_points / hsb_scan_to_points / hsb_projected_scan_to_points returns for the stepped
+ * input, or the endpoints given to an endpoint step.
+ * No member's state changes; a member not listed is neither read nor waited for.
+ * Ordering: the call runs on the group's stream after everything queued on the listed members (their own work and a
+ * pending step of any group they belong to, so a call right after a nowait step sees that step's map write and its
+ * last-match container), and returns when the results are in the caller's arrays.
+ * Cost, whatever K is: one host-to-device copy from the group's pinned staging (grown geometrically) of the sessions'
+ * descriptors (member, scan address and length), the pose offsets, the poses and, when given, the scans; one launch
+ * (two for the best hypothesis); one device-to-host copy of one result block; one synchronise.  Launches are counted on
+ * handles[0].
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued: K < 0 or K > M; members == NULL with K > 0; an index
+ * outside [0, M) or listed twice (the message names the session); level outside [0, levels); pose_offsets == NULL,
+ * pose_offsets[0] != 0 or decreasing (the message names the session); exactly one of points_xy / scan_offsets NULL;
+ * scan_offsets[0] != 0 or decreasing; poses_world, out_likelihood (likelihood), both covariance outputs or out_best4
+ * NULL with Q > 0.  K = 0 returns HSB_OK and reads no other argument; Q = 0 returns HSB_OK and queues nothing (the best
+ * hypothesis of every session is then the empty session's, written if out_best4 is given). */
+int hsb_group_likelihood(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
+                         const float* points_xy, const int* scan_offsets, float* out_likelihood);
+int hsb_group_likelihood_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                float* out_likelihood);
+int hsb_group_covariance(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
+                         const float* points_xy, const int* scan_offsets, float* out_cov_map, float* out_cov_world);
+int hsb_group_covariance_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                float* out_cov_map, float* out_cov_world);
+int hsb_group_best_hypothesis(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
+                              const float* points_xy, const int* scan_offsets, float* out_likelihood, float* out_best4,
+                              int* out_best_index);
+int hsb_group_best_hypothesis_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
+                                     const float* poses_world, const float* points_xy, const int* scan_offsets,
+                                     float* out_likelihood, float* out_best4, int* out_best_index);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
