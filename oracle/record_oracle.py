@@ -38,7 +38,8 @@ def level_iterations(levels: int, iters=None) -> list[int]:
 
 
 class RecordOracle(pyoracle.Oracle):
-    def __init__(self, kind: str, map_resolution: float, size: int, levels: int, start=(0.5, 0.5), silent: bool = True):
+    def __init__(self, kind: str, map_resolution: float, size: int, levels: int, start=(0.5, 0.5), silent: bool = True,
+                 *, size_y: int | None = None):
         path = REF_LIB if kind == "reference" else PORT_LIB
         if not os.path.exists(path):
             raise FileNotFoundError(f"record oracle missing: {path} (run `make -C oracle -f record.mk`)")
@@ -52,7 +53,8 @@ class RecordOracle(pyoracle.Oracle):
         fn.argtypes = [vp, _f32p, _f32p, i, _f32p, vp, _f32p, _f32p, _f32p] + ([_i32p] if kind == "reference" else [])
         if silent and kind == "reference":
             self._fn("silence")(1)
-        self.size_x = self.size_y = int(size)
+        self.size_x = int(size)
+        self.size_y = int(size if size_y is None else size_y)
         self.levels = int(levels)
         self.h = self._fn("create")(map_resolution, self.size_x, self.size_y, start[0], start[1], levels)
 

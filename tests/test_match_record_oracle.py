@@ -86,6 +86,80 @@ def test_port_record_equals_reference_hooks(rec_oracle):
             assert np.array_equal(bits(pp), bits(ro.match(hint, scan)[0])), name
 
 
+def geometry_cases(rec_oracle, kind, gi):
+    """tests/match_cases.py's geometry gi on the oracle `kind`: its finite scans and the edge scan, built with the
+    port as the matcher"""
+    import match_cases as mcs
+
+    g = (mcs.GEOMS + [mcs.companion(x) for x in mcs.GEOMS])[gi]
+    sx, sy, L, start, res = g
+    orcs = {}
+    for k in ("port", kind):
+        o = rec_oracle.RecordOracle(k, res, sx, L, start=start, size_y=sy)
+        for l, (a, b) in enumerate(mcs.level_sizes(g)):
+            o.set_logodds(l, mcs.field(a, b, l))
+        orcs[k] = o
+    po = orcs["port"]
+    cases = mcs.Cases(g, [po.get_prob(l) for l in range(L)], po, seed=100 + gi)
+    scans = []
+    for k, n in enumerate((33, 1081, 2049)):
+        h = cases.hint(k)
+        scans.append((h, cases.scan(n, h, nonfinite=False)))
+    if L > 1:
+        h = cases.hint(5)
+        scans.append((h, cases.strip_scan(700, h)))
+    h = cases.hint(3)
+    base = cases.scan(1081, h, nonfinite=False, slots=mcs.SLOTS)
+    it = mcs.edge_iterations(L)
+    h, pts, designed, rec = mcs.build_edge_scan(
+        cases, lambda hh, p: mcs.split_record(po.match_record(hh, p, it)[2], L, it), h, base, cases.slots)
+    mcs.check_edges(cases, rec, pts, designed)
+    scans.append((h, pts))
+    return orcs, scans
+
+
+def _geom_params():
+    import match_cases as mcs
+
+    allg = mcs.GEOMS + [mcs.companion(x) for x in mcs.GEOMS]
+    return list(range(len(allg))), [mcs.geom_id(g) + ("-corner" if g[3] is mcs.CORNER else "") for g in allg]
+
+
+@pytest.mark.parametrize("gi", _geom_params()[0], ids=_geom_params()[1])
+def test_geometry_port_record_equals_reference(rec_oracle, gi):
+    """Non-square, odd-sized and off-centre multi-level maps (tests/match_cases.py), edge endpoints built exactly: the
+    port's record reduced to the hooks' view equals the reference's hooks bit for bit, with the default iteration
+    schedule, [-1, 2, 4] and the edge scans' schedule, and its every evaluation equals getCompleteHessianDerivs at the recorded input pose on
+    every level."""
+    if not rec_oracle.available("reference"):
+        pytest.skip("compiled reference not built")
+    import match_cases as mcs
+
+    orcs, scans = geometry_cases(rec_oracle, "reference", gi)
+    po, ro = orcs["port"], orcs["reference"]
+    for iters in (None, [-1, 2, 4][:po.levels], mcs.edge_iterations(po.levels)):
+        for k, (hint, scan) in enumerate(scans):
+            pp, cp, rec = po.match_record(hint, scan, iters)
+            pr, cr, hooks, _ = ro.match_record(hint, scan, iters)
+            assert np.array_equal(bits(pp), bits(pr)) and np.array_equal(bits(cp), bits(cr)), (k, iters)
+            assert np.array_equal(bits(rec_oracle.port_hooks(po, rec, scan.shape[0], iters)), bits(hooks)), (k, iters)
+            mis = po.level_iterations(iters)
+            off = 0
+            for l in range(po.levels - 1, -1, -1):
+                E = mis[l] + 1
+                ev = rec[off + 3:off + 3 + 15 * E].reshape(E, 15)
+                pin = ro.map_coords_pose(l, rec[off:off + 3])
+                pl = (scan * np.float32(2.0 ** -l)).astype(np.float32)
+                for e in range(E):
+                    H, d = ro.hessian_derivs(l, pin, pl)
+                    assert np.array_equal(bits(H.reshape(9)), bits(ev[e, :9])), (k, l, e)
+                    assert np.array_equal(bits(d), bits(ev[e, 9:12])), (k, l, e)
+                    pin = ev[e, 12:15]
+                off += 3 + 15 * E
+    for o in orcs.values():
+        o.close()
+
+
 def test_port_record_sums_equal_reference_derivs(rec_oracle):
     if not rec_oracle.available("reference"):
         pytest.skip("compiled reference not built")
