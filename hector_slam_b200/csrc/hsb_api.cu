@@ -64,7 +64,7 @@ struct hsb_handle {
   cudaStream_t copy_stream[2] = {nullptr, nullptr};
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   // device staging for the host-buffer entry points
-  DevBuf d_hints, d_pts, d_offsets, d_poses, d_cov, d_scratch;
+  DevBuf d_pts, d_scratch;
   // "containers of the last match" (MapRepMultiMap::dataContainers) and the update scan
   DevBuf d_last_pts, d_upd_pts;   // single-scan buffers: 16 floats of header (hint, gate inputs), then the points
   float* h_stage = nullptr;       // pinned staging for the single-scan calls (header + points, one H2D per call)
@@ -775,7 +775,7 @@ int hsb_destroy(hsb_handle* h) {
   HandleScope guard(h);
   cudaDeviceSynchronize();
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
-  DevBuf* bufs[] = {&h->d_hints, &h->d_pts, &h->d_offsets, &h->d_poses, &h->d_cov, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
+  DevBuf* bufs[] = {&h->d_pts, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
                     &h->d_beam_cs, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
                     &h->d_conv_in, &h->d_cloud_tf, &h->d_fused_in, &h->d_proj_unit};
   for (DevBuf* b : bufs)
@@ -2074,30 +2074,148 @@ int hsb_best_hypothesis_device(hsb_handle* h, int level, int B, const float* d_p
   return HSB_OK;
 }
 
+}  // extern "C"
+
+namespace {
+
+// What a pose-scoring call computes for every pose (likelihood, covariance) or session (best hypothesis).
+enum ScoreKind { SCORE_LIKELIHOOD, SCORE_COVARIANCE, SCORE_BEST };
+constexpr size_t kScoreChunk = 1 << 20;   // most bytes of points score_query stages in its pinned copy
+
+// Every host-buffer pose-scoring body (hsb_likelihood_batch, hsb_covariance_batch and the group calls): Q poses of K
+// sessions, session k's poses [pose_offsets[k], pose_offsets[k+1]) scored on member sess[k].member's map of `level`,
+// whose descriptor is lv[member * levels + level] — or, with lv NULL, h's own level, staged with the poses as a one-entry
+// table.  sessions(sess, pose_offsets, staged) writes the K session descriptors and K + 1 pose offsets into the staging;
+// `staged` is where the n_pts points of `pts` will lie on the device, so a session's scan is a slice of them or any
+// other device scan the caller knows of.  One host-to-device copy from the pinned staging hs (points past kScoreChunk
+// bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K arg-max accumulators are
+// `best`), one device-to-host copy of the asked-for results and one synchronise.  The launches and any error are
+// counted on h, whose level gives the cell length (every member's geometry is h's).
+template <typename Sessions>
+int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage, const HsbLevelDev* lv,
+                int levels, int level, ScoreKind kind, int K, int Q, const float* poses, const float* pts, size_t n_pts,
+                const Sessions& sessions, unsigned long long* best, float* out_lh, float* out_map, float* out_world,
+                float* out_best4, int* out_best_index) {
+  // staging: sessions | pose offsets | (level descriptor) | poses | scans, then the results: likelihoods | best4 | best
+  // index, or covariance (map) | covariance (world), each only if asked for
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_lv = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_poses = lv ? o_lv : al(o_lv + sizeof(HsbLevelDev));
+  const size_t o_pts = al(o_poses + (size_t)Q * 12), in_end = o_pts + n_pts * 8, o_out = al(in_end);
+  size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, out_end = o_out;
+  if (kind == SCORE_COVARIANCE) {
+    o_world = o_map + (out_map ? (size_t)Q * 36 : 0);
+    out_end = o_world + (out_world ? (size_t)Q * 36 : 0);
+  } else {
+    o_best4 = al(o_lh + (size_t)Q * 4);
+    o_index = o_best4 + (kind == SCORE_BEST ? (size_t)K * 16 : 0);
+    out_end = kind == SCORE_BEST ? o_index + (size_t)K * 4 : o_lh + (size_t)Q * 4;
+  }
+  int s;
+  if ((s = ensure_pinned(h, hs_buf, hs_bytes, out_end)) != HSB_OK) return s;
+  if ((s = ensure(h, d_stage, out_end)) != HSB_OK) return s;
+  char* hs = reinterpret_cast<char*>(hs_buf);
+  char* ds = static_cast<char*>(d_stage.p);
+  sessions(reinterpret_cast<HsbScoreSessionDev*>(hs), reinterpret_cast<int*>(hs + o_off),
+           reinterpret_cast<const float2*>(ds + o_pts));
+  if (!lv) {
+    HsbLevelDev L = {};
+    fill_level_dev(h, level, L);
+    memcpy(hs + o_lv, &L, sizeof(L));
+  }
+  memcpy(hs + o_poses, poses, (size_t)Q * 12);
+  // More points than kScoreChunk bytes go straight from the caller's memory: the driver overlaps its host staging of a
+  // pageable copy with the transfer, where staging megabytes here first would serialise the two.
+  const bool inline_pts = n_pts * 8 <= kScoreChunk;
+  if (inline_pts && n_pts > 0) memcpy(hs + o_pts, pts, n_pts * 8);
+  HSB_CUDA(h, cudaMemcpyAsync(ds, hs, inline_pts ? in_end : o_pts, cudaMemcpyHostToDevice, st));
+  if (!inline_pts) HSB_CUDA(h, cudaMemcpyAsync(ds + o_pts, pts, n_pts * 8, cudaMemcpyHostToDevice, st));
+
+  HsbScoreParams P;
+  memset(&P, 0, sizeof(P));
+  P.lv = lv ? lv : reinterpret_cast<const HsbLevelDev*>(ds + o_lv);
+  P.sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
+  P.pose_offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.poses = reinterpret_cast<const float*>(ds + o_poses);
+  P.cell_length = h->lv[level].cell_length;
+  P.levels = lv ? levels : 1;
+  P.level = lv ? level : 0;
+  P.K = K;
+  P.Q = Q;
+  const bool tex = h->gather_mode == HSB_GATHER_TEX;
+  if (kind == SCORE_COVARIANCE) {
+    P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
+    P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
+    const int blocks = std::min(Q, h->sm_count * 8);
+    if (tex) hsb::covariance_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
+    else hsb::covariance_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(P);
+    h->launches++;
+  } else {
+    P.out = reinterpret_cast<float*>(ds + o_lh);
+    if (kind == SCORE_BEST) {
+      P.best = best;
+      P.out_best4 = reinterpret_cast<float*>(ds + o_best4);
+      P.out_best_index = reinterpret_cast<int*>(ds + o_index);
+    }
+    const int blocks = std::min((Q + 3) / 4, h->sm_count * 16);
+    if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
+    else hsb::likelihood_group_kernel<hsb::MODE_LDG><<<blocks, 128, 0, st>>>(P);
+    h->launches++;
+    if (kind == SCORE_BEST) {
+      HSB_CUDA(h, cudaGetLastError());
+      hsb::best_group_finish_kernel<<<(K + 127) / 128, 128, 0, st>>>(P);
+      h->launches++;
+    }
+  }
+  HSB_CUDA(h, cudaGetLastError());
+  HSB_CUDA(h, cudaMemcpyAsync(hs + o_out, ds + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaStreamSynchronize(st));
+  if (kind == SCORE_COVARIANCE) {
+    if (out_map) memcpy(out_map, hs + o_map, (size_t)Q * 36);
+    if (out_world) memcpy(out_world, hs + o_world, (size_t)Q * 36);
+  } else {
+    if (out_lh) memcpy(out_lh, hs + o_lh, (size_t)Q * 4);
+    if (out_best4) memcpy(out_best4, hs + o_best4, (size_t)K * 16);   // (given with SCORE_BEST only)
+    if (out_best_index) memcpy(out_best_index, hs + o_index, (size_t)K * 4);
+  }
+  return HSB_OK;
+}
+
+// hsb_likelihood_batch / hsb_covariance_batch on h's level, on h->stream, staged through the handle's scan staging as
+// the ray queries are (see hsb_raycast_batch).  Every session is on member 0.  Without offsets: one session of all B
+// poses whose scan is the shared one, n points long (none are staged if n < 0); with offsets: B sessions of one pose
+// each, session b's scan [offsets[b], offsets[b+1]) of the offsets[B] staged points.
+int single_score(hsb_handle* h, ScoreKind kind, int level, int B, const float* poses, const float* pts, const int* offsets,
+                 int n, float* out_lh, float* out_map, float* out_world) {
+  const size_t total = offsets ? (size_t)offsets[B] : (size_t)(n > 0 ? n : 0);
+  if (total > 0 && !pts) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
+  const int K = offsets ? B : 1;
+  auto sessions = [&](HsbScoreSessionDev* sess, int* pose_offsets, const float2* staged) {
+    for (int k = 0; k < K; ++k) {
+      sess[k].pts = staged + (offsets ? offsets[k] : 0);
+      sess[k].n = offsets ? offsets[k + 1] - offsets[k] : n;
+      sess[k].member = 0;
+      pose_offsets[k] = k;
+    }
+    pose_offsets[K] = B;
+  };
+  return score_query(h, h->stream, h->h_stage, h->h_stage_bytes, h->d_pts, nullptr, 1, level, kind, K, B, poses, pts,
+                     total, sessions, nullptr, out_lh, out_map, out_world, nullptr, nullptr);
+}
+
+}  // namespace
+
+extern "C" {
+
+// A negative n_shared scores against no points in both calls, but as the length of the scan the likelihood sees 0
+// (1 - 0/0: NaN) and the covariance's sigma points see n_shared itself (1 - 0/n_shared: 1).
 int hsb_likelihood_batch(hsb_handle* h, int level, int B, const float* poses, const float* pts, const int* offsets,
                          int n_shared, float* out) {
   if (!h || level < 0 || level >= h->levels || B < 0 || !poses || !out) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  size_t total = offsets ? (size_t)offsets[B] : (size_t)(n_shared > 0 ? n_shared : 0);
-  if (total > 0 && !pts) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  int s;
-  if ((s = ensure(h, h->d_hints, (size_t)B * 12)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_pts, total * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_offsets, (size_t)(B + 1) * 4)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_poses, (size_t)B * 12)) != HSB_OK) return s;
-  cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_hints.p, poses, (size_t)B * 12, cudaMemcpyHostToDevice, st));
-  if (total > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_pts.p, pts, total * 8, cudaMemcpyHostToDevice, st));
-  if (offsets) HSB_CUDA(h, cudaMemcpyAsync(h->d_offsets.p, offsets, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, st));
-  float* d_out = static_cast<float*>(h->d_poses.p);
-  s = likelihood_device(h, level, B, static_cast<const float*>(h->d_hints.p), static_cast<const float2*>(h->d_pts.p),
-                        offsets ? static_cast<const int*>(h->d_offsets.p) : nullptr, offsets ? 0 : (n_shared > 0 ? n_shared : 0),
-                        d_out, st);
-  if (s != HSB_OK) return s;
-  HSB_CUDA(h, cudaMemcpyAsync(out, d_out, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  return HSB_OK;
+  return single_score(h, SCORE_LIKELIHOOD, level, B, poses, pts, offsets, n_shared > 0 ? n_shared : 0, out, nullptr,
+                      nullptr);
 }
 
 int hsb_covariance_batch(hsb_handle* h, int level, int B, const float* poses, const float* pts, const int* offsets, int n_shared,
@@ -2105,37 +2223,7 @@ int hsb_covariance_batch(hsb_handle* h, int level, int B, const float* poses, co
   if (!h || level < 0 || level >= h->levels || B < 0 || !poses || (!out_cov_map && !out_cov_world)) return HSB_ERR_INVALID_ARG;
   if (B == 0) return HSB_OK;
   HandleScope guard(h);
-  size_t total = offsets ? (size_t)offsets[B] : (size_t)(n_shared > 0 ? n_shared : 0);
-  if (total > 0 && !pts) return fail(h, HSB_ERR_INVALID_ARG, "points pointer is NULL");
-  int s;
-  if ((s = ensure(h, h->d_hints, (size_t)B * 12)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_pts, total * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_offsets, (size_t)(B + 1) * 4)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_cov, (size_t)B * 72)) != HSB_OK) return s;
-  cudaStream_t st = h->stream;
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_hints.p, poses, (size_t)B * 12, cudaMemcpyHostToDevice, st));
-  if (total > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_pts.p, pts, total * 8, cudaMemcpyHostToDevice, st));
-  if (offsets) HSB_CUDA(h, cudaMemcpyAsync(h->d_offsets.p, offsets, (size_t)(B + 1) * 4, cudaMemcpyHostToDevice, st));
-  HsbLevelDev L;
-  fill_level_dev(h, level, L);
-  const int blocks = std::min(B, h->sm_count * 8);
-  const int* d_off = offsets ? static_cast<const int*>(h->d_offsets.p) : nullptr;
-  float* d_map = static_cast<float*>(h->d_cov.p);
-  float* d_world = d_map + 9 * (size_t)B;
-  if (h->gather_mode == HSB_GATHER_TEX)
-    hsb::covariance_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(L, B, static_cast<const float*>(h->d_hints.p),
-                                                                  static_cast<const float2*>(h->d_pts.p), d_off,
-                                                                  offsets ? 0 : n_shared, h->lv[level].cell_length, d_map, d_world);
-  else
-    hsb::covariance_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(L, B, static_cast<const float*>(h->d_hints.p),
-                                                                  static_cast<const float2*>(h->d_pts.p), d_off,
-                                                                  offsets ? 0 : n_shared, h->lv[level].cell_length, d_map, d_world);
-  h->launches++;
-  HSB_CUDA(h, cudaGetLastError());
-  if (out_cov_map) HSB_CUDA(h, cudaMemcpyAsync(out_cov_map, d_map, (size_t)B * 36, cudaMemcpyDeviceToHost, st));
-  if (out_cov_world) HSB_CUDA(h, cudaMemcpyAsync(out_cov_world, d_world, (size_t)B * 36, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h, cudaStreamSynchronize(st));
-  return HSB_OK;
+  return single_score(h, SCORE_COVARIANCE, level, B, poses, pts, offsets, n_shared, nullptr, out_cov_map, out_cov_world);
 }
 
 static int get_dirty(hsb_handle* h, int level, int which, int rect[4], int reset) {
@@ -3003,16 +3091,12 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
                    world, K, members, offsets, begin, end, out_dist, out_hit, out_found);
 }
 
-
-// What a group pose-scoring call computes for every pose (hsb_group_likelihood, hsb_group_covariance) or session
-// (hsb_group_best_hypothesis).
-enum ScoreKind { SCORE_LIKELIHOOD, SCORE_COVARIANCE, SCORE_BEST };
-
 // hsb_likelihood_batch / hsb_covariance_batch / hsb_best_hypothesis_device for K members in one pass: session k's poses
 // [pose_offsets[k], pose_offsets[k+1]) scored on member members[k]'s map of `level` against the session's scan
 // (pts[scan_offsets[k] ..), or, with pts and scan_offsets NULL, the member's last-match container as it is on the device
-// when the call runs).  Behind the members' queued work, through the group's pinned query staging: one copy each way, one
-// launch (two for the best hypothesis) and one synchronise, whatever K is.  No member's state changes.
+// when the call runs).  Behind the members' queued work, through the group's pinned query staging and descriptor table
+// (score_query: one copy each way, one launch, two for the best hypothesis, and one synchronise, whatever K is).  No
+// member's state changes.
 int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* members, int level, const int* pose_offsets,
                 const float* poses, const float* pts, const int* scan_offsets, float* out_lh, float* out_map,
                 float* out_world, float* out_best4, int* out_best_index) {
@@ -3054,95 +3138,25 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_cov_map and out_cov_world are both NULL", fn);
   if (kind == SCORE_BEST && !out_best4) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_best4 is NULL", fn);
   DeviceGuard guard(g->device);
-  cudaStream_t st = g->stream;
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-
-  // staging: sessions | pose offsets | poses | (scans), then the results: likelihoods | best4 | best index, or
-  // covariance (map) | covariance (world), each only if asked for
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t total = last ? 0 : (size_t)scan_offsets[K];
-  const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_poses = al(o_off + (size_t)(K + 1) * 4);
-  const size_t o_pts = al(o_poses + (size_t)Q * 12), in_end = o_pts + total * 8, o_out = al(in_end);
-  size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, out_end = o_out;
-  if (kind == SCORE_COVARIANCE) {
-    o_world = o_map + (out_map ? (size_t)Q * 36 : 0);
-    out_end = o_world + (out_world ? (size_t)Q * 36 : 0);
-  } else {
-    o_best4 = al(o_lh + (size_t)Q * 4);
-    o_index = o_best4 + (kind == SCORE_BEST ? (size_t)K * 16 : 0);
-    out_end = kind == SCORE_BEST ? o_index + (size_t)K * 4 : o_lh + (size_t)Q * 4;
-  }
-  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
-  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
-  char* hs = reinterpret_cast<char*>(g->h_ray_stage);
-  char* ds = static_cast<char*>(g->d_ray_stage.p);
-  HsbScoreSessionDev* sess = reinterpret_cast<HsbScoreSessionDev*>(hs);
-  for (int k = 0; k < K; ++k) {
-    hsb_handle* h = g->m[members[k]];
-    sess[k].member = members[k];
-    if (last) {   // (a member that never matched has no container: n = 0)
-      sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
-      sess[k].n = h->d_last_pts.p ? h->last_n : 0;
-    } else {
-      sess[k].pts = reinterpret_cast<const float2*>(ds + o_pts) + scan_offsets[k];
-      sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
+  auto sessions = [&](HsbScoreSessionDev* sess, int* offsets, const float2* staged) {
+    for (int k = 0; k < K; ++k) {
+      hsb_handle* h = g->m[members[k]];
+      sess[k].member = members[k];
+      if (last) {   // (a member that never matched has no container: n = 0)
+        sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+        sess[k].n = h->d_last_pts.p ? h->last_n : 0;
+      } else {
+        sess[k].pts = staged + scan_offsets[k];
+        sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
+      }
     }
-  }
-  memcpy(hs + o_off, pose_offsets, (size_t)(K + 1) * 4);
-  memcpy(hs + o_poses, poses, (size_t)Q * 12);
-  if (total > 0) memcpy(hs + o_pts, pts, total * 8);
-  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, in_end, cudaMemcpyHostToDevice, st));
-
-  HsbScoreParams P;
-  memset(&P, 0, sizeof(P));
-  P.lv = g->d_lv;
-  P.sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
-  P.pose_offsets = reinterpret_cast<const int*>(ds + o_off);
-  P.poses = reinterpret_cast<const float*>(ds + o_poses);
-  P.cell_length = h0->lv[level].cell_length;
-  P.levels = g->levels;
-  P.level = level;
-  P.K = K;
-  P.Q = Q;
-  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create checked)
-  if (kind == SCORE_COVARIANCE) {
-    P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
-    P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
-    const int blocks = std::min(Q, h0->sm_count * 8);
-    if (tex) hsb::covariance_group_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
-    else hsb::covariance_group_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(P);
-    h0->launches++;
-  } else {
-    P.out = reinterpret_cast<float*>(ds + o_lh);
-    if (kind == SCORE_BEST) {
-      P.best = g->d_best;
-      P.out_best4 = reinterpret_cast<float*>(ds + o_best4);
-      P.out_best_index = reinterpret_cast<int*>(ds + o_index);
-    }
-    const int blocks = std::min((Q + 3) / 4, h0->sm_count * 16);
-    if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
-    else hsb::likelihood_group_kernel<hsb::MODE_LDG><<<blocks, 128, 0, st>>>(P);
-    h0->launches++;
-    if (kind == SCORE_BEST) {
-      HSB_CUDA(h0, cudaGetLastError());
-      hsb::best_group_finish_kernel<<<(K + 127) / 128, 128, 0, st>>>(P);
-      h0->launches++;
-    }
-  }
-  HSB_CUDA(h0, cudaGetLastError());
-  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_out, ds + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h0, cudaStreamSynchronize(st));
-  if (kind == SCORE_COVARIANCE) {
-    if (out_map) memcpy(out_map, hs + o_map, (size_t)Q * 36);
-    if (out_world) memcpy(out_world, hs + o_world, (size_t)Q * 36);
-  } else {
-    if (out_lh) memcpy(out_lh, hs + o_lh, (size_t)Q * 4);
-    if (kind == SCORE_BEST) {
-      memcpy(out_best4, hs + o_best4, (size_t)K * 16);
-      if (out_best_index) memcpy(out_best_index, hs + o_index, (size_t)K * 4);
-    }
-  }
-  return HSB_OK;
+    memcpy(offsets, pose_offsets, (size_t)(K + 1) * 4);
+  };
+  // (h0's gather mode is every member's: hsb_group_create checked)
+  return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, level, kind,
+                     K, Q, poses, pts, last ? 0 : (size_t)scan_offsets[K], sessions, g->d_best, out_lh, out_map,
+                     out_world, out_best4, out_best_index);
 }
 
 }  // namespace

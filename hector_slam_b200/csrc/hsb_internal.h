@@ -200,19 +200,19 @@ struct HsbRayParams {
   float origo_x, origo_y, scale, inv_scale;   // getDist: the level's map origin and cell length, 1 / cell length
 };
 
-// One session of a group pose-scoring call: the scan its poses are scored against and the member whose map they are
-// scored on.
+// One session of a pose-scoring call: the scan its poses are scored against and the member whose map they are scored
+// on.
 struct HsbScoreSessionDev {
   const float2* pts;   // the session's slice of the staged scans, or the member's last-match container
   int n;
   int member;
 };
 
-// A group pose-scoring call (likelihood_group_kernel, best_group_finish_kernel, covariance_group_kernel:
-// hsb_group_likelihood, hsb_group_best_hypothesis, hsb_group_covariance): Q poses of K sessions, session k's poses
+// A pose-scoring call from host buffers (likelihood_group_kernel, best_group_finish_kernel, covariance_kernel:
+// hsb_likelihood_batch, hsb_covariance_batch and the group calls): Q poses of K sessions, session k's poses
 // [pose_offsets[k], pose_offsets[k+1]).  Arrays in device memory; outputs in pose order.
 struct HsbScoreParams {
-  const HsbLevelDev* lv;            // members x levels, member-major (hsb_group::d_lv)
+  const HsbLevelDev* lv;            // members x levels, member-major (hsb_group::d_lv; one entry for a single handle)
   const HsbScoreSessionDev* sess;   // K
   const int* pose_offsets;          // K + 1
   const float* poses;               // Q x 3, world

@@ -1188,7 +1188,8 @@ __device__ __forceinline__ float warp_likelihood(const LevelRegs& LR, float pt_s
 }
 
 // One pose of a likelihood batch, by one warp: the world pose to the level's map coordinates (getMapCoordsPose), then
-// warp_likelihood.  Shared by likelihood_kernel and likelihood_group_kernel.
+// warp_likelihood.  Shared by likelihood_kernel (poses and scans on the device) and likelihood_group_kernel (staged from
+// host buffers).
 template <int MODE>
 __device__ __forceinline__ float pose_likelihood(const HsbLevelDev& L, const LevelRegs& LR, const float* __restrict__ pose_world,
                                                  const float2* __restrict__ pts, int n, int lane) {
@@ -1253,7 +1254,7 @@ __global__ void best_hypothesis_finish_kernel(unsigned long long* __restrict__ b
   out4[1] = poses_world[3 * b]; out4[2] = poses_world[3 * b + 1]; out4[3] = poses_world[3 * b + 2];
 }
 
-// The session of entry q of a group query: the last session whose entries start at or before q (empty sessions are
+// The session of pose q of a scoring call: the last session whose poses start at or before q (empty sessions are
 // passed over), as ray_kernel finds a ray's.
 __device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K, int q) {
   int lo = 0, hi = K - 1;
@@ -1265,10 +1266,11 @@ __device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K
   return lo;
 }
 
-// N3 for a group (hsb_group_likelihood, hsb_group_best_hypothesis): pose q of the call belongs to the session k whose
-// poses are [pose_offsets[k], pose_offsets[k+1]) and is scored against that session's scan on its member's map of the
-// level (the group's descriptor table).  One warp per pose, grid-stride; the value is likelihood_kernel's.  With `best`,
-// session k's arg-max goes to best[k], the index being the pose's index in its session.
+// N3 from host buffers (hsb_likelihood_batch, hsb_group_likelihood, hsb_group_best_hypothesis): pose q of the call
+// belongs to the session k whose poses are [pose_offsets[k], pose_offsets[k+1]) and is scored against that session's
+// scan on its member's map of the level (the descriptor table).  One warp per pose, grid-stride; the value is
+// likelihood_kernel's.  With `best`, session k's arg-max goes to best[k], the index being the pose's index in its
+// session.
 template <int MODE>
 __global__ void __launch_bounds__(128) likelihood_group_kernel(const HsbScoreParams P) {
   const int lane = threadIdx.x & 31;
@@ -1357,7 +1359,7 @@ __device__ __forceinline__ void sigma_covariance(const float* lhs, float x, floa
   }
 }
 // Pose b of a covariance batch, by one CTA of 7 warps: warp k evaluates the likelihood of sigma point k, thread 0 forms
-// the matrices.  Ends with a barrier, so the caller may loop.  Shared by covariance_kernel and covariance_group_kernel.
+// the matrices.  Ends with a barrier, so the caller may loop.
 template <int MODE>
 __device__ __forceinline__ void pose_covariance(const HsbLevelDev& L, const LevelRegs& LR, const float* __restrict__ poses_world,
                                                 int b, const float2* __restrict__ pts, int n, float cell_length,
@@ -1376,28 +1378,11 @@ __device__ __forceinline__ void pose_covariance(const HsbLevelDev& L, const Leve
   __syncthreads();
 }
 
-// N3: OccGridMapUtil::getCovarianceForPose (OccGridMapUtil.h:106-160) + getCovMatrixWorldCoords (:162-187) for a batch of
-// poses: one CTA of 7 warps per pose (pose_covariance).
+// N3: OccGridMapUtil::getCovarianceForPose (OccGridMapUtil.h:106-160) + getCovMatrixWorldCoords (:162-187) for
+// hsb_covariance_batch and hsb_group_covariance: one CTA of 7 warps per pose (pose_covariance), the pose's session, scan
+// and member map found as likelihood_group_kernel finds them; every member's cell length is the call's (one geometry).
 template <int MODE>
-__global__ void __launch_bounds__(224)
-    covariance_kernel(const HsbLevelDev L, int B, const float* __restrict__ poses_world, const float2* __restrict__ pts_all,
-                      const int* __restrict__ offsets, int n_shared, float cell_length, float* __restrict__ out_map,
-                      float* __restrict__ out_world) {
-  const LevelRegs LR = level_regs(L);
-  for (int b = blockIdx.x; b < B; b += gridDim.x) {
-    int beg = 0, n = n_shared;
-    if (offsets) {
-      beg = offsets[b];
-      n = offsets[b + 1] - beg;
-    }
-    pose_covariance<MODE>(L, LR, poses_world, b, pts_all + beg, n, cell_length, out_map, out_world);
-  }
-}
-
-// N3 for a group (hsb_group_covariance): covariance_kernel's CTA per pose, the pose's session, scan and member map
-// found as likelihood_group_kernel finds them; every member's cell length is the group's (one geometry).
-template <int MODE>
-__global__ void __launch_bounds__(224) covariance_group_kernel(const HsbScoreParams P) {
+__global__ void __launch_bounds__(224) covariance_kernel(const HsbScoreParams P) {
   for (int q = blockIdx.x; q < P.Q; q += gridDim.x) {
     const HsbScoreSessionDev s = P.sess[session_of(P.pose_offsets, P.K, q)];
     const HsbLevelDev& L = P.lv[(size_t)s.member * P.levels + P.level];

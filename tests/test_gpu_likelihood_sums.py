@@ -1,4 +1,5 @@
-"""GPU: the N3 kernels — likelihood_kernel, covariance_kernel and the arg-max of hsb_best_hypothesis_device — against
+"""GPU: the N3 kernels — likelihood_kernel (the device entry points), likelihood_group_kernel and covariance_kernel (the
+host-buffer ones, hsb_likelihood_batch and hsb_covariance_batch) and the arg-max of hsb_best_hypothesis_device — against
 the float64 reference of the pose likelihood (oracle/likelihood64.py), tightly enough to see ONE endpoint lost or counted
 twice, in both scan layouts, both gather modes, around both grid caps and on the map's edges.
 
@@ -50,7 +51,8 @@ def sm_count():
 
 
 def lh_cap():
-    """poses the likelihood grid covers in one pass: sm_count * 16 CTAs of 4 warps (hsb_api.cu likelihood_device)"""
+    """poses the likelihood grid covers in one pass: sm_count * 16 CTAs of 4 warps (hsb_api.cu likelihood_device and
+    score_query)"""
     return sm_count() * 16 * 4
 
 

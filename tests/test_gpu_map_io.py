@@ -5,6 +5,8 @@ non-square levels, long rays and plane edges, in both gather modes (LDG and TEX 
       publishMap threshold of the uploaded plane, with -0, +0, +-min denormal, +-inf, NaN and 50 planted;
   N4  ray cast and getDist (warp_raycast, ray_kernel) against HectorMapTools.h compiled unmodified (oracle/_ref; the C
       port where it is absent) on the rays of tests/maptools_cases.py, and right after a nowait SLAM step;
+  N3  hsb_likelihood_batch and hsb_covariance_batch right after a nowait SLAM step, their launch count, and a negative
+      shared scan length;
   §6  tile replication between an owner and a replica on one device, both protocols (pack_rect / unpack_rect and
       pack_dirty / reset_dirty / unpack_dirty): log-odds, probabilities, texture twin, mirror and replication
       rectangles, the buffer header and the overflow boundary;
@@ -215,6 +217,97 @@ def test_rays_right_after_a_nowait_step(hsb_lib, mode, kind):
         assert same(twins[0].download_level(l), twins[1].download_level(l)), l
     for rep in twins:
         rep.close()
+
+
+# ---- N3 ------------------------------------------------------------------------------------------------------------
+
+@MODES
+@pytest.mark.parametrize("kind", ["endpoints", "ranges"])
+def test_scores_right_after_a_nowait_step(hsb_lib, mode, kind):
+    """hsb_likelihood_batch and hsb_covariance_batch issued right after a nowait SLAM step see the step's map write and
+    leave the step's input alone (the scan and the poses go through the handle's one pinned staging), with one shared
+    scan and with per-pose offsets: the likelihoods, both covariance matrices, the poses and every level's plane equal
+    those of a twin stepped synchronously.  The poses lie around the robot and are scored against the step's scan."""
+    from hector_slam_b200 import capi
+    from test_gpu_group_subset import geometry, session_data
+
+    fmt = geometry(1)
+    ticks = 8
+    data = session_data(50 + mode, ticks, fmt)
+    twins = [capi.MapRepB200(0.05, 512, 512, levels=3, update_factor_free=0.4, update_factor_occupied=0.9,
+                             gather_mode=mode) for _ in range(2)]
+    for rep in twins:
+        rep.set_scan_format(**fmt)
+    rng = np.random.default_rng(11 + mode)
+    for t in range(ticks):
+        level = t % 3
+        scan = data["scans"][t]
+        poses = (data["truth"][t] + rng.uniform(-1, 1, (6, 3)) * np.float32([0.1, 0.1, 0.05])).astype(np.float32)
+        offsets = np.int32([0] + sorted(rng.integers(0, scan.shape[0] + 1, 5)) + [scan.shape[0]])
+        out = []
+        for rep, nowait in zip(twins, (True, False)):
+            if kind == "endpoints":
+                pose = rep.slam_update(data["hints"][t], scan, nowait=nowait)[0]
+            else:
+                pose = rep.slam_update_ranges(data["hints"][t], data["ranges"][t], nowait=nowait)[0]
+            out.append((pose, rep.likelihood_batch(level, poses, scan), rep.likelihood_batch(level, poses, scan, offsets))
+                       + rep.covariance_batch(level, poses, scan) + rep.covariance_batch(level, poses, scan, offsets))
+        for i, (x, y) in enumerate(zip(*out)):
+            assert same(x, y), (t, i)
+        assert np.isfinite(out[0][1]).all(), t
+    for l in range(3):
+        assert same(twins[0].download_level(l), twins[1].download_level(l)), l
+    for rep in twins:
+        rep.close()
+
+
+def score_handle(mode):
+    """A 1-level 256^2 handle at resolution 0.25 from (0, 0), so that world = map cells x 0.25 exactly, and B = 5 map
+    poses with their world twins."""
+    from hector_slam_b200 import capi
+
+    rep = capi.MapRepB200(0.25, 256, 256, levels=1, start=(0.0, 0.0), gather_mode=mode)
+    rep.upload_level(0, mc.plane(256, 256, seed=3))
+    rng = np.random.default_rng(5 + mode)
+    pm = np.stack([rng.uniform(60, 200, 5), rng.uniform(60, 200, 5), rng.uniform(-3.1, 3.1, 5)], axis=1).astype(np.float32)
+    return rep, pm, (pm * np.float32([0.25, 0.25, 1.0])).astype(np.float32)
+
+
+@MODES
+def test_score_launch_count(hsb_lib, mode):
+    """Each hsb_likelihood_batch and hsb_covariance_batch call is one launch, in either scan layout."""
+    rep, _, world = score_handle(mode)
+    pts = np.random.default_rng(1).uniform(-40, 40, (300, 2)).astype(np.float32)
+    offsets = np.int32([0, 0, 1, 100, 299, 300])
+    calls = [lambda: rep.likelihood_batch(0, world, pts), lambda: rep.likelihood_batch(0, world, pts, offsets),
+             lambda: rep.covariance_batch(0, world, pts), lambda: rep.covariance_batch(0, world, pts, offsets)]
+    for i, call in enumerate(calls):
+        n = rep.launch_count
+        call()
+        assert rep.launch_count == n + 1, i
+    rep.close()
+
+
+@MODES
+def test_negative_shared_scan_length(hsb_lib, mode):
+    """A negative n_shared with offsets NULL, through the C-ABI: no points are read, the likelihood's scan length is 0
+    (1 - 0/0: NaN for every pose) and the covariance's is n_shared itself (each sigma point 1 - 0/n_shared = 1), so the
+    covariance is oracle/likelihood64.py's fp32 formula on seven likelihoods of 1.0."""
+    from oracle import likelihood64
+
+    rep, pm, world = score_handle(mode)
+    B = world.shape[0]
+    lh = np.zeros(B, np.float32)
+    assert hsb_lib.hsb_likelihood_batch(rep.h, 0, B, world.ctypes.data, None, None, -1, lh.ctypes.data) == 0
+    assert np.isnan(lh).all(), lh
+    cm, cw = np.zeros((B, 9), np.float32), np.zeros((B, 9), np.float32)
+    assert hsb_lib.hsb_covariance_batch(rep.h, 0, B, world.ctypes.data, None, None, -1, cm.ctypes.data,
+                                        cw.ctypes.data) == 0
+    assert np.isfinite(cm).all() and np.isfinite(cw).all()
+    for b in range(B):
+        wm, ww = likelihood64.covariance_fp32(np.ones(7, np.float32), pm[b], 0.25)
+        assert same(cm[b], wm.reshape(9)) and same(cw[b], ww.reshape(9)), (b, cm[b], wm, cw[b], ww)
+    rep.close()
 
 
 # ---- §6 -----------------------------------------------------------------------------------------------------------
