@@ -45,6 +45,7 @@ EXPORTED = [
     "hsb_group_get_dist", "hsb_group_get_dist_subset", "hsb_group_raycast", "hsb_group_raycast_subset",
     "hsb_group_likelihood", "hsb_group_likelihood_subset", "hsb_group_covariance", "hsb_group_covariance_subset",
     "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
+    "hsb_group_match_batch", "hsb_group_match_batch_subset",
 ]
 
 
@@ -211,6 +212,8 @@ def load_library() -> C.CDLL:
     sig("hsb_group_covariance_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_best_hypothesis", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_best_hypothesis_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch", i, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     _lib = L
     return L
 
@@ -1150,6 +1153,34 @@ class SlamGroup:
         else:
             self._check(self.lib.hsb_group_best_hypothesis_subset(self.g, K, _ptr(mem), *args, *tail))
         return out, best4, index
+
+    def match_batch(self, hints, points=None, members=None, want_cov: bool = True):
+        """matchData from many start poses for the members in one pass (hsb_group_match_batch): hints is one (q_s, 3)
+        array of world hints per session, or a tuple (hints (Q, 3), offsets (K + 1,)); every hint of a session is matched
+        over all levels with that session's one scan on its member's map.  points as in likelihood: one (n_s, 2) endpoint
+        array per session (level-0 cells), or a tuple (points, offsets); None = each member's last matched scan as it is
+        on the device.  members as in slam_update (hsb_group_match_batch_subset).  Each pose equals match_batch on its
+        member in shared-scan mode with the warps per scan the group call reports (handles[0]'s last_launch_shape).
+        -> (poses (Q, 3), cov (Q, 3, 3) | None), in hint order"""
+        K, mem = self._sessions(members)
+        h, hint_off = self._pack(hints, 3, K)
+        if points is None:
+            pp, op, keep = None, None, None
+        else:
+            pts, scan_off = self._pack(points, 2, K)
+            if pts.shape[0] == 0:
+                pts = np.zeros((1, 2), np.float32)   # (a pointer for the C call: points and offsets come together)
+            pp, op, keep = pts.ctypes.data, scan_off.ctypes.data, (pts, scan_off)
+        Q = h.shape[0]
+        poses = np.zeros((Q, 3), np.float32)
+        cov = np.zeros((Q, 9), np.float32) if want_cov else None
+        args = (hint_off.ctypes.data, _ptr(h if Q else None), pp, op, _ptr(poses if Q else None), _ptr(cov if Q else None))
+        if mem is None:
+            self._check(self.lib.hsb_group_match_batch(self.g, *args))
+        else:
+            self._check(self.lib.hsb_group_match_batch_subset(self.g, K, _ptr(mem), *args))
+        del keep
+        return poses, None if cov is None else cov.reshape(Q, 3, 3)
 
     def _sessions(self, members):
         """-> (sessions of the step, the member list as int32, or None for a step of every member)"""

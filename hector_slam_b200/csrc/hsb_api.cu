@@ -308,7 +308,7 @@ int fail_fused_too_long(hsb_handle* h, int max_n) {
   return fail(h, HSB_ERR_UNSUPPORTED, "scan too long for the fused conversion (%d points)", max_n);
 }
 
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, int GRP = hsb::GRP_NONE, bool PROJ = false>
 int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int Gr,
                    const hsb::InlineScan<INL>& S = hsb::InlineScan<INL>()) {
   if (Gr <= 0 || Gr > G) Gr = G;   // groups per CTA actually launched (a G-group kernel runs with fewer: see launch_match)
@@ -443,8 +443,8 @@ int launch_match_projected(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStre
     const bool tex = h->gather_mode == HSB_GATHER_TEX;
 #define HSB_PROJ_CASE(w)                                                                                     \
   if (W == w)                                                                                                \
-    return tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, false, true>(h, P, max_n, st, 1)      \
-               : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, false, true>(h, P, max_n, st, 1);
+    return tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_NONE, true>(h, P, max_n, st, 1) \
+               : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_NONE, true>(h, P, max_n, st, 1);
     HSB_PROJ_CASE(1);
     HSB_PROJ_CASE(2);
     HSB_PROJ_CASE(4);
@@ -455,6 +455,16 @@ int launch_match_projected(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStre
               W, G, U);
 }
 
+// Warps per scan of a batch of B scans under the default tuning: one warp per scan as soon as the batch fills the chip,
+// more warps per scan for small batches, never more than 8 (the per-evaluation reduction / barrier cost grows with the
+// group size).
+int auto_warps_per_scan(const hsb_handle* h, long B) {
+  const long want = ((long)h->sm_count * 24) / (B > 0 ? B : 1);
+  int W = 1;
+  while (W * 2 <= want && W < 8) W *= 2;
+  return W;
+}
+
 int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   if (h->map_write_pending && st != h->stream) {
     // hsb_slam_update_nowait left a map write running on the handle's stream: a match on another stream waits for it
@@ -463,15 +473,10 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   }
   int W = h->tune_warps_per_scan, G = h->tune_scans_per_block;
   if (W <= 0) {
-    // One warp per scan as soon as the batch fills the chip, more warps per scan for small batches,
-    // never more than 8 (the per-evaluation reduction / barrier cost grows with the group size).
     // (a pipelined host-batch call passes ONE size for all its chunks: a scan's result must not depend on the
     // chunk it happens to travel in — the reduction order follows the shape — so that results are invariant
     // under a permutation of the batch, as the reference's are)
-    const long Bs = h->shape_batch > 0 ? h->shape_batch : P.B;
-    long want = ((long)h->sm_count * 24) / (Bs > 0 ? Bs : 1);
-    W = 1;
-    while (W * 2 <= want && W < 8) W *= 2;
+    W = auto_warps_per_scan(h, h->shape_batch > 0 ? h->shape_batch : P.B);
   }
   int Gr = 0;   // 0: as many groups per CTA as the instantiation has
   if (G <= 0) {
@@ -2876,12 +2881,12 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
   if (in.kind == HSB_IN_PROJECTED)
     s = h0->gather_mode == HSB_GATHER_TEX
-            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true, true>(h0, P, max_n, st, 1)
-            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true, true>(h0, P, max_n, st, 1);
+            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_STEP, true>(h0, P, max_n, st, 1)
+            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP, true>(h0, P, max_n, st, 1);
   else
     s = h0->gather_mode == HSB_GATHER_TEX
-            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, true>(h0, P, max_n, st, 1)
-            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, true>(h0, P, max_n, st, 1);
+            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_STEP>(h0, P, max_n, st, 1)
+            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP>(h0, P, max_n, st, 1);
   if (s != HSB_OK) return s;
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
@@ -3159,6 +3164,113 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
                      out_world, out_best4, out_best_index);
 }
 
+// hsb_match_batch in shared-scan mode for K members in one pass: session k's hints [hint_offsets[k], hint_offsets[k+1])
+// each matched over all levels on member members[k]'s maps with the session's one scan (pts[scan_offsets[k] ..), or,
+// with pts and scan_offsets NULL, the member's last-match container as it is on the device when the call runs).  One
+// match-kernel launch (GRP_MATCH: one hint per scan) in the shape hsb_match_batch would take for Q hints, behind the
+// members' queued work, through the group's pinned query staging: one copy each way and one synchronise, whatever K is.
+// No member's state changes.
+int group_match(hsb_group* g, const char* fn, int K, const int* members, const int* hint_offsets, const float* hints,
+                const float* pts, const int* scan_offsets, float* out_poses, float* out_cov) {
+  hsb_handle* h0 = g->m[0];   // launches, launch shape and errors are accounted on handles[0], whether or not it is listed
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (!hint_offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets is NULL", fn);
+  if (hint_offsets[0] != 0)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets[0] is %d, must be 0", fn, hint_offsets[0]);
+  for (int k = 0; k < K; ++k)
+    if (hint_offsets[k + 1] < hint_offsets[k])
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets decrease at session %d (%d -> %d)", fn, k, hint_offsets[k],
+                  hint_offsets[k + 1]);
+  if (!pts != !scan_offsets)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: points_xy and scan_offsets must both be given or both be NULL", fn);
+  const bool last = !pts;   // every session's scan is its member's last-match container
+  if (!last) {
+    if (scan_offsets[0] != 0)
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets[0] is %d, must be 0", fn, scan_offsets[0]);
+    for (int k = 0; k < K; ++k)
+      if (scan_offsets[k + 1] < scan_offsets[k])
+        return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets decrease at session %d (%d -> %d)", fn, k, scan_offsets[k],
+                    scan_offsets[k + 1]);
+  }
+  const int Q = hint_offsets[K];
+  if (Q == 0) return HSB_OK;
+  if (!hints) return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints_world is NULL", fn);
+  if (!out_poses) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_poses_world is NULL", fn);
+  // the launch shape: hsb_match_batch's for Q hints (launch_match), among the shapes the group match is compiled for —
+  // W in {1, 2, 4, 8}, one scan per CTA, 4 gathers in flight, unpacked (with one warp per scan, grouping scans into
+  // CTAs does not change a bit, so the auto-group shapes need no twin)
+  const int W = h0->tune_warps_per_scan > 0 ? h0->tune_warps_per_scan : auto_warps_per_scan(h0, Q);
+  const int G = h0->tune_scans_per_block > 0 ? h0->tune_scans_per_block : 1;
+  const int U = h0->tune_unroll > 0 ? h0->tune_unroll : 4;
+  if (!has_projected_kernel(h0, W, G, U))   // (the same set of shapes)
+    return fail(h0, HSB_ERR_UNSUPPORTED, "%s: no group match kernel for tuning warps_per_scan=%d scans_per_block=%d "
+                "unroll=%d packed=%d", fn, W, G, U, h0->tune_packed);
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
+
+  // staging: sessions | hint offsets | hints | scans, then the results: poses | covariances
+  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const size_t n_pts = last ? 0 : (size_t)scan_offsets[K];
+  const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_hints = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_pts = al(o_hints + (size_t)Q * 12), in_end = o_pts + n_pts * 8, o_poses = al(in_end);
+  const size_t o_cov = o_poses + (size_t)Q * 12, out_end = o_cov + (out_cov ? (size_t)Q * 36 : 0);
+  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
+  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
+  char* hs = reinterpret_cast<char*>(g->h_ray_stage);
+  char* ds = static_cast<char*>(g->d_ray_stage.p);
+  HsbScoreSessionDev* sess = reinterpret_cast<HsbScoreSessionDev*>(hs);
+  const float2* staged = reinterpret_cast<const float2*>(ds + o_pts);
+  int max_n = 0;
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
+    sess[k].member = members[k];
+    if (last) {   // (a member that never matched has no container: n = 0)
+      sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+      sess[k].n = h->d_last_pts.p ? h->last_n : 0;
+    } else {
+      sess[k].pts = staged + scan_offsets[k];
+      sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
+    }
+    // (only a session with hints launches work: an unused long scan must not shrink the staging of the others)
+    if (hint_offsets[k + 1] > hint_offsets[k]) max_n = std::max(max_n, sess[k].n);
+  }
+  memcpy(hs + o_off, hint_offsets, (size_t)(K + 1) * 4);
+  memcpy(hs + o_hints, hints, (size_t)Q * 12);
+  if (n_pts > 0) memcpy(hs + o_pts, pts, n_pts * 8);
+  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, in_end, cudaMemcpyHostToDevice, st));
+
+  HsbMatchParams P;
+  fill_match_params(h0, P);   // (lv[] is unused: every hint reads its member's row of the group's table)
+  P.B = Q;
+  P.hints = reinterpret_cast<const float*>(ds + o_hints);
+  P.kind = HSB_IN_ENDPOINTS;
+  P.out_poses = reinterpret_cast<float*>(ds + o_poses);
+  P.out_cov = out_cov ? reinterpret_cast<float*>(ds + o_cov) : nullptr;
+  P.group_lv = g->d_lv;
+  P.match_sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
+  P.match_offsets = reinterpret_cast<const int*>(ds + o_off);
+  P.match_K = K;
+  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create checked)
+  s = HSB_ERR_UNSUPPORTED;
+#define HSB_GM_CASE(w)                                                                                                 \
+  if (W == w)                                                                                                          \
+    s = tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h0, P, max_n, st, 1)                \
+            : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h0, P, max_n, st, 1);
+  HSB_GM_CASE(1);
+  HSB_GM_CASE(2);
+  HSB_GM_CASE(4);
+  HSB_GM_CASE(8);
+#undef HSB_GM_CASE
+  if (s != HSB_OK) return s;
+  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_poses, ds + o_poses, out_end - o_poses, cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h0, cudaStreamSynchronize(st));
+  memcpy(out_poses, hs + o_poses, (size_t)Q * 12);
+  if (out_cov) memcpy(out_cov, hs + o_cov, (size_t)Q * 36);
+  return HSB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -3207,6 +3319,21 @@ int hsb_group_best_hypothesis_subset(hsb_group* g, int K, const int* members, in
   if (!g) return HSB_ERR_INVALID_ARG;
   return group_score(g, "hsb_group_best_hypothesis_subset", SCORE_BEST, K, members, level, pose_offsets, poses_world,
                      points_xy, scan_offsets, out_likelihood, nullptr, nullptr, out_best4, out_best_index);
+}
+
+int hsb_group_match_batch(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* points_xy,
+                          const int* scan_offsets, float* out_poses_world, float* out_cov) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch", (int)g->m.size(), g->all.data(), hint_offsets, hints_world, points_xy,
+                     scan_offsets, out_poses_world, out_cov);
+}
+
+int hsb_group_match_batch_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                 const float* hints_world, const float* points_xy, const int* scan_offsets,
+                                 float* out_poses_world, float* out_cov) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_subset", K, members, hint_offsets, hints_world, points_xy, scan_offsets,
+                     out_poses_world, out_cov);
 }
 
 int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,

@@ -61,6 +61,14 @@ struct HsbGroupSessionDev {
   int member;
 };
 
+// One session of a pose-scoring call or of a group batch match: the scan its poses are scored against (its hints are
+// matched with) and the member whose map they are scored (matched) on.
+struct HsbScoreSessionDev {
+  const float2* pts;   // the session's slice of the staged scans, or the member's last-match container
+  int n;
+  int member;
+};
+
 struct HsbMatchParams {
   HsbLevelDev lv[HSB_MAX_LEVELS];
   int levels;
@@ -109,7 +117,7 @@ struct HsbMatchParams {
   // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.
   float* record;
   int record_floats;
-  // group SLAM step (match_kernel<..., GRP = true>): scan b is session b of the step, which steps member
+  // group SLAM step (match_kernel<..., GRP = GRP_STEP>): scan b is session b of the step, which steps member
   // group_sess[b].member of the group.  Its level descriptors are group_lv[member * levels ..] (built once per group)
   // instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
@@ -117,9 +125,23 @@ struct HsbMatchParams {
   // counts the sessions that have finished: the last one publishes seq_value to seq_host.  A converted session converts
   // with group_sess[b].conv (conv above is unused); a set map_without_matching flag still converts the scan for the map
   // writer: only the match is skipped.
+  // group batch match (match_kernel<..., GRP = GRP_MATCH>, hsb_group_match_batch): scan b is hint b of session k, the
+  // last one with match_offsets[k] <= b (match_offsets: match_K + 1 hint bounds).  The hint is matched with the
+  // session's scan match_sess[k].pts / .n (endpoints; offsets, n_shared and pts above are unused) on member
+  // match_sess[k].member's maps, group_lv[member * levels ..].  The epilogue is the plain batch one: pose and covariance
+  // out, no gate, no sequence number, no container copy.  match_K fills the padding after record_floats and the two
+  // arrays share storage with the step's, so the block keeps its size and layout: the inline-scan kernels' second
+  // parameter stays where it was.
+  int match_K;
   const HsbLevelDev* group_lv;
-  const HsbGroupSessionDev* group_sess;
-  unsigned* group_done;
+  union {
+    const HsbGroupSessionDev* group_sess;
+    const HsbScoreSessionDev* match_sess;
+  };
+  union {
+    unsigned* group_done;
+    const int* match_offsets;
+  };
 };
 
 struct HsbUpdateLevelDev {
@@ -198,14 +220,6 @@ struct HsbRayParams {
   int* out_found;               // Q (getDist), or null
   int levels, level, sx, sy, K, Q;
   float origo_x, origo_y, scale, inv_scale;   // getDist: the level's map origin and cell length, 1 / cell length
-};
-
-// One session of a pose-scoring call: the scan its poses are scored against and the member whose map they are scored
-// on.
-struct HsbScoreSessionDev {
-  const float2* pts;   // the session's slice of the staged scans, or the member's last-match container
-  int n;
-  int member;
 };
 
 // A pose-scoring call from host buffers (likelihood_group_kernel, best_group_finish_kernel, covariance_kernel:

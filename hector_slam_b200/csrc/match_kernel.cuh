@@ -749,26 +749,46 @@ struct MatchBounds {
   static constexpr int kMinBlocks = (W == 1 && 28 % G == 0) ? 28 / G : 1;
 };
 
-// Level descriptors of scan `scan`: the kernel parameters' (one map for the whole batch), or — group SLAM step, every
-// session steps its own map — the row of the group's device array that belongs to the session's member.
-template <bool GRP>
-__device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P, int scan, int lvl) {
-  if constexpr (GRP) return P.group_lv[(size_t)P.group_sess[scan].member * P.levels + lvl];
+// Which group a match kernel serves (its GRP template value): none (one handle's map for the whole batch), the group
+// SLAM step (one session per scan, hsb_group_slam_update) or the group batch match (one hint per scan,
+// hsb_group_match_batch).
+enum { GRP_NONE = 0, GRP_STEP = 1, GRP_MATCH = 2 };
+
+// The session of hint q of a group batch match or of pose q of a scoring call: the last session whose hints / poses
+// start at or before q (empty sessions are passed over), as ray_kernel finds a ray's.
+__device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K, int q) {
+  int lo = 0, hi = K - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (offsets[mid] <= q) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Level descriptors of scan `scan`: the kernel parameters' (one map for the whole batch), or — group SLAM step and group
+// batch match, every session works on its own member's map — the row of the group's device array that belongs to the
+// session's member (`member`: the group batch match's, looked up once per scan).
+template <int GRP>
+__device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P, int scan, int member, int lvl) {
+  if constexpr (GRP == GRP_STEP) return P.group_lv[(size_t)P.group_sess[scan].member * P.levels + lvl];
+  else if constexpr (GRP == GRP_MATCH) return P.group_lv[(size_t)member * P.levels + lvl];
   else return P.lv[lvl];
 }
 
 // Conversion descriptor of scan `scan`: the kernel parameters' (one handle), or the session's (group SLAM step).
-template <bool GRP>
+template <int GRP>
 __device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, int scan) {
-  if constexpr (GRP) return P.group_sess[scan].conv;
+  if constexpr (GRP == GRP_STEP) return P.group_sess[scan].conv;
   else return P.conv;
 }
 
-// GRP: the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv.
+// GRP: GRP_STEP, the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv;
+// GRP_MATCH, the group batch match (hsb_group_match_batch), one hint per scan — see HsbMatchParams::match_sess.
 // PROJ: converted input is HSB_IN_PROJECTED (laser_geometry's projection and the cloud rule, stage_from_projected); only
 // the instantiations the projected SLAM steps and batch matches launch carry that branch (hsb_api.cu
 // launch_match_projected).
-template <int W, int G, int MODE, int U, bool PACK, bool INL = false, bool GRP = false, bool PROJ = false>
+template <int W, int G, int MODE, int U, bool PACK, bool INL = false, int GRP = GRP_NONE, bool PROJ = false>
 __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -792,7 +812,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
 
   // fused SLAM step: let the map writer's CTAs (launched with programmatic stream serialisation, update_kernel.cuh)
   // become resident on the idle SMs while this single-scan match runs; they wait for this grid's completion
-  if (GRP || P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (GRP == GRP_STEP || P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (t == 0) mbar_init(mbar, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   // Pacing (G > 1, P.pace_slack > 0).  The per-scan timeline (tuning key trace) shows that the warps of an SM do NOT
@@ -834,10 +854,17 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       n = P.n_shared;
       beg = P.kind == HSB_IN_ENDPOINTS ? 0 : (size_t)scan * n;
     }
-    if constexpr (GRP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
+    if constexpr (GRP == GRP_STEP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
       if (P.kind == HSB_IN_ENDPOINTS && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a conversion runs first, below)
     }
     const float2* __restrict__ gpts = P.pts + beg;
+    int member = 0;
+    if constexpr (GRP == GRP_MATCH) {   // group batch match: the scan, its length and the map are the hint's session's
+      const HsbScoreSessionDev& s = P.match_sess[session_of(P.match_offsets, P.match_K, scan)];
+      gpts = s.pts;
+      n = s.n;
+      member = s.member;
+    }
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
     bool staged = false;
     int ns = 0;                      // points [0, ns) are read from shared memory, [ns, n) from global memory
@@ -853,7 +880,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       group_sync<W>(g);
       ns = n;
       staged = true;
-    } else if (P.kind != HSB_IN_ENDPOINTS) {
+    } else if (GRP != GRP_MATCH && P.kind != HSB_IN_ENDPOINTS) {
       // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
       const HsbConvDev& C = conv_desc<GRP>(P, scan);
       const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
@@ -886,7 +913,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
           if (C.out_n_host) *C.out_n_host = n;
         }
       }
-      if constexpr (GRP) {
+      if constexpr (GRP == GRP_STEP) {
         if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // map_without_matching: converted for the writer, not matched
       }
       ns = n;
@@ -945,7 +972,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     int evals_ran = 0;   // evaluations this scan actually ran (trace slot 5)
     if (n > 0) {
       for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
-        const HsbLevelDev& L = level_desc<GRP>(P, scan, lvl);
+        const HsbLevelDev& L = level_desc<GRP>(P, scan, member, lvl);
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
         if (recording) {
@@ -1090,7 +1117,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       P.trace[8 * (size_t)scan + 6] = warp_id();
       P.trace[8 * (size_t)scan + 7] = sm_id();
     }
-    if (GRP && t == 0) {
+    if (GRP == GRP_STEP && t == 0) {
       // group SLAM step: the session's gate, against its own handle's state and thresholds
       slam_gate(P.group_sess[scan].gate_state, P.gate_in + 3 * scan, wx, wy, wpsi, P.out_poses + 4 * scan,
                 P.gate_out_host + 4 * scan);
@@ -1115,7 +1142,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
         c[6] = last.h02; c[7] = last.h12; c[8] = last.h22;
       }
     }
-    if (GRP && t == 0) {
+    if (GRP == GRP_STEP && t == 0) {
       // group SLAM step: the LAST session to finish publishes the sequence number — every session's results (each made
       // visible system-wide before its count) are then in host memory
       __threadfence_system();
@@ -1128,7 +1155,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       __threadfence_system();
       *reinterpret_cast<volatile unsigned*>(P.seq_host) = P.seq_value;
     }
-    if constexpr (GRP) {
+    if constexpr (GRP == GRP_STEP) {
       // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
       // its later map writes without matching read it (after the pose is out: only the map writers wait for this).
       // A converted scan is already there (the conversion's sink, above).
@@ -1252,18 +1279,6 @@ __global__ void best_hypothesis_finish_kernel(unsigned long long* __restrict__ b
   unsigned b;
   out4[0] = best_unpack(v, b);
   out4[1] = poses_world[3 * b]; out4[2] = poses_world[3 * b + 1]; out4[3] = poses_world[3 * b + 2];
-}
-
-// The session of pose q of a scoring call: the last session whose poses start at or before q (empty sessions are
-// passed over), as ray_kernel finds a ray's.
-__device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K, int q) {
-  int lo = 0, hi = K - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (offsets[mid] <= q) lo = mid;
-    else hi = mid - 1;
-  }
-  return lo;
 }
 
 // N3 from host buffers (hsb_likelihood_batch, hsb_group_likelihood, hsb_group_best_hypothesis): pose q of the call

@@ -392,6 +392,29 @@ class SlamProcessor {
     owner.check(hsb_group_best_hypothesis_subset(owner.groupFor(ps, M), K, members, level, poseOffsets, posesWorld,
                                                  pointsXY, scanOffsets, likelihood, best4, bestIndex));
   }
+
+  // MapRepMultiMap::matchData (MapRepMultiMap.h:116-132) from many start poses for M processors in one pass
+  // (hsb_group_match_batch, through the group updateMany keeps): processor s's world hints [hintOffsets[s],
+  // hintOffsets[s+1]) of hintsWorld (x, y, psi) are each matched over all levels on its map with its scan
+  // pointsXY[scanOffsets[s] .. scanOffsets[s+1]) (level-0 cells), or, with pointsXY and scanOffsets null, with the scan
+  // of its last matched update as it is on the device.  posesWorld: one pose per hint, in hint order; cov (may be null):
+  // the Hessian of each hint's last evaluation, 9 floats row-major.  No processor's state changes.
+  static void matchMany(SlamProcessor* const* ps, int M, const int* hintOffsets, const float* hintsWorld,
+                        const float* pointsXY, const int* scanOffsets, float* posesWorld, float* cov = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchMany");
+    owner.check(hsb_group_match_batch(owner.groupFor(ps, M), hintOffsets, hintsWorld, pointsXY, scanOffsets, posesWorld,
+                                      cov));
+  }
+
+  // matchMany() for the processors ps[members[0..K)] (hsb_group_match_batch_subset): session k's hints and scan
+  // belong to ps[members[k]]; the processors not listed are neither read nor waited for.
+  static void matchMany(SlamProcessor* const* ps, int M, const int* members, int K, const int* hintOffsets,
+                        const float* hintsWorld, const float* pointsXY, const int* scanOffsets, float* posesWorld,
+                        float* cov = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchMany");
+    owner.check(hsb_group_match_batch_subset(owner.groupFor(ps, M), K, members, hintOffsets, hintsWorld, pointsXY,
+                                             scanOffsets, posesWorld, cov));
+  }
   hsb_handle* handle() { return h_; }
 
   // util::poseDifferenceLargerThan, util/UtilFunctions.h:73-92 (float norm, double pi arithmetic)

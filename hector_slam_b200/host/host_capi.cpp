@@ -369,6 +369,31 @@ int hsbp_best_hypothesis_many_subset(void* const* ps, int M, const int* members,
   }
   return 0;
 }
+int hsbp_match_many(void* const* ps, int M, const int* hint_offsets, const float* hints_world, const float* points_xy,
+                    const int* scan_offsets, float* out_poses_world, float* out_cov) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::matchMany(procs.data(), M, hint_offsets, hints_world, points_xy, scan_offsets,
+                                     out_poses_world, out_cov);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
+int hsbp_match_many_subset(void* const* ps, int M, const int* members, int K, const int* hint_offsets,
+                           const float* hints_world, const float* points_xy, const int* scan_offsets,
+                           float* out_poses_world, float* out_cov) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::matchMany(procs.data(), M, members, K, hint_offsets, hints_world, points_xy, scan_offsets,
+                                     out_poses_world, out_cov);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

@@ -583,6 +583,44 @@ int hsb_group_best_hypothesis(hsb_group* g, int level, const int* pose_offsets, 
 int hsb_group_best_hypothesis_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
                                      const float* poses_world, const float* points_xy, const int* scan_offsets,
                                      float* out_likelihood, float* out_best4, int* out_best_index);
+/* MapRepMultiMap::matchData (MapRepMultiMap.h:116-132) from many start poses for K of the group's members in one pass:
+ * hsb_match_batch in shared-scan mode for each member.  A server re-matches a lost robot's last scan from a spread of
+ * hints on that robot's own map, then picks the winner with hsb_group_best_hypothesis on the returned poses.
+ * Session k is member members[k] (the full form: every member, in order).  Its hints are [hint_offsets[k],
+ * hint_offsets[k+1]) of hints_world (Q x 3, Q = hint_offsets[K]; a session may hold none).  Each hint runs the full
+ * coarse-to-fine matchData over all levels, on that member's current map, with the session's ONE scan.
+ * The scan of session k:
+ *  - points_xy and scan_offsets given: points_xy[scan_offsets[k] .. scan_offsets[k+1]), level-0 cell units, DataContainer
+ *    layout, as hsb_match_batch takes them;
+ *  - points_xy == NULL and scan_offsets == NULL: the member's last-match container as it is on the device when the call
+ *    runs, by the rule hsb_group_likelihood documents (the endpoints of the last MATCHED step of any input kind; n = 0
+ *    for a member that has never matched).  No scan crosses the bus.
+ * The outputs are in hint order: out_poses_world Q x 3, out_cov Q x 9 (may be NULL), the Hessian of the last evaluation
+ * (ScanMatcher.h:184).  An empty scan returns the hint and an all-zero covariance, as hsb_match_batch does.
+ * Bits: every pose and covariance equals hsb_match_batch(member, B = the session's hint count, its hints, its scan,
+ * offsets = NULL, n_shared = n) run with the same warps per scan W, bit for bit.  The reduction order follows W, and the
+ * call takes W as hsb_match_batch would for ONE batch of Q hints (or handles[0]'s tuning warps_per_scan), so it may
+ * differ from what each member's own call would take; hsb_get_last_launch_shape(handles[0]) reports it.
+ * No member's state changes: no planes, stamps, dirty rectangles or gate pose, and the last-match container is not
+ * replaced.  A member not listed is neither read nor waited for.
+ * Ordering: the call runs on the group's stream after everything queued on the listed members (their own work and a
+ * pending step of any group they belong to, so a call right after a nowait step sees that step's map write and its
+ * last-match container), and returns when the results are in the caller's arrays.
+ * Cost, whatever K is: one host-to-device copy from the group's pinned staging (grown geometrically) of the sessions'
+ * descriptors (member, scan address and length), the hint offsets, the hints and, when given, the scans; one match
+ * launch, counted on handles[0]; one device-to-host copy of the poses (and covariances, if asked for); one synchronise.
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued, no output byte written: K < 0 or K > M; members == NULL
+ * with K > 0; an index outside [0, M) or listed twice (the message names the session); hint_offsets == NULL,
+ * hint_offsets[0] != 0 or decreasing (the message names the session); exactly one of points_xy / scan_offsets NULL;
+ * scan_offsets[0] != 0 or decreasing; hints_world or out_poses_world NULL with Q > 0.  Rejected with
+ * HSB_ERR_UNSUPPORTED: a handles[0] tuning whose launch shape has no group match kernel (the shapes are W in {1, 2, 4,
+ * 8}, one scan per CTA, 4 gathers in flight, unpacked; the message names the tuning).  K = 0 returns HSB_OK and reads no
+ * other argument; Q = 0 returns HSB_OK and queues nothing. */
+int hsb_group_match_batch(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* points_xy,
+                          const int* scan_offsets, float* out_poses_world, float* out_cov);
+int hsb_group_match_batch_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                 const float* hints_world, const float* points_xy, const int* scan_offsets,
+                                 float* out_poses_world, float* out_cov);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
