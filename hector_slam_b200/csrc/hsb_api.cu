@@ -379,7 +379,9 @@ int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st,
     HSB_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
   }
   P.trace = nullptr;
-  if (h->tune_trace) {
+  // (hsb_set_tuning refuses the key above HSB_TRACE_MAX_LEVELS; a launch with more levels, whichever handle's tuning
+  // it runs under, gets no trace pointer, so the kernel's stores cannot leave a scan's 8 slots)
+  if (h->tune_trace && P.levels <= HSB_TRACE_MAX_LEVELS) {
     int s = ensure(h, h->d_trace, (size_t)P.B * 64);
     if (s != HSB_OK) return s;
     P.trace = static_cast<unsigned long long*>(h->d_trace.p);
@@ -884,7 +886,13 @@ int hsb_set_tuning(hsb_handle* h, const char* key, int value) {
   else if (!strcmp(key, "inline_scan")) h->tune_inline_scan = value;
   else if (!strcmp(key, "partial")) h->tune_partial = value;
   else if (!strcmp(key, "prefetch")) h->tune_prefetch = value;
-  else if (!strcmp(key, "trace")) h->tune_trace = value;
+  else if (!strcmp(key, "trace")) {
+    // a scan's 8-slot record holds the start, one time per level and the end only up to HSB_TRACE_MAX_LEVELS levels
+    if (value && h->levels > HSB_TRACE_MAX_LEVELS)
+      return fail(h, HSB_ERR_UNSUPPORTED, "hsb_set_tuning: trace records at most %d levels, the handle has %d",
+                  HSB_TRACE_MAX_LEVELS, h->levels);
+    h->tune_trace = value;
+  }
   else if (!strcmp(key, "pace")) h->tune_pace = value;
   else if (!strcmp(key, "time_update")) h->tune_time_update = value;
   else if (!strcmp(key, "pdl")) h->tune_pdl = value;

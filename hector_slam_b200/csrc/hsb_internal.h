@@ -107,6 +107,8 @@ struct HsbMatchParams {
   // diagnostics (hsb_set_tuning "trace"): per scan 8 x u64 =
   //   [0] start, [1 .. levels] after each level (coarsest first), [1 + levels] end,
   //   [5] evaluations the scan actually ran (written with <= 3 levels, where slot 5 is free), [6] %warpid, [7] %smid
+  // The layout holds up to HSB_TRACE_MAX_LEVELS levels (the end time then sits in slot 5); with more the host leaves
+  // the pointer null (hsb_api.cu launch_match), so no store of the kernel can land outside a scan's 8 slots.
   unsigned long long* trace;
   // per-evaluation record (hsb_match_data_record / hsb_match_batch_record_device), nullptr = none.  Scan b owns
   // record[b * record_floats ..], record_floats = R = sum over levels of (3 + 15 * evals).  Per level, coarsest first:

@@ -43,6 +43,8 @@ extern "C" {
 #endif
 
 #define HSB_MAX_LEVELS 8
+/* the most levels a scan's 8-slot trace record can describe (tuning key "trace", hsb_read_trace) */
+#define HSB_TRACE_MAX_LEVELS 4
 
 typedef struct hsb_handle hsb_handle;
 
@@ -70,7 +72,8 @@ typedef struct hsb_config {
   int   map_size_y;
   float start_x;          /* startCoords: where world (0,0) sits in the map, as a fraction  */
   float start_y;
-  int   levels;           /* multi_res_size, 1..HSB_MAX_LEVELS                              */
+  int   levels;           /* multi_res_size, 1..HSB_MAX_LEVELS: every depth 1..8 is tested   */
+                          /* (4..8: tests/deep_cases.py); the coarsest level has >= 4 cells   */
   int   device;           /* CUDA device ordinal                                            */
   /* maxIterations handed to ScanMatcher::matchData per level (the matcher then runs
    * maxIterations + 1 evaluations, ScanMatcher.h:74,94).  A zero entry selects the reference's
@@ -761,7 +764,9 @@ int hsb_get_gather_mode(const hsb_handle* h);
  * "inline_scan" (1: hsb_match_data / hsb_slam_update send scans of up to 1280 endpoints inside the kernel launch
  * instead of through a host-to-device copy — slower per step in measurement, higher back-to-back rate; default 0),
  * "host_out", "occupancy_chunk" (bytes of packed rows per chunk of a group occupancy sync whose handles[0] this handle
- * is, 0 = 32 MiB; at least one row).  Results never depend on them beyond summation order. */
+ * is, 0 = 32 MiB; at least one row).  Results never depend on them beyond summation order.
+ * "trace" is refused with HSB_ERR_UNSUPPORTED on a handle of more than HSB_TRACE_MAX_LEVELS levels: the 8-slot
+ * record has no room for their level times. */
 int hsb_set_tuning(hsb_handle* h, const char* key, int value);
 /* Shape of the last match-kernel launch of this handle: {warps per scan, scans per CTA, gather batch (unroll),
  * endpoints of each scan staged in shared memory (0 = read through L1), grid size, resident CTAs per SM}.
@@ -771,7 +776,9 @@ int hsb_get_last_launch_shape(const hsb_handle* h, int out[6]);
  * the tuning key "time_update" was set before the write — bench.py's K2 roofline. */
 int hsb_get_last_update_device_ms(hsb_handle* h, float* ms);
 /* Timeline of the last match launch when the tuning key "trace" is set: per scan 8 x uint64 =
- * {%globaltimer at start, after each level (coarsest first), at the end (slot 1 + levels), ..., %smid (slot 7)}.
+ * {%globaltimer at start, after each level (coarsest first), at the end (slot 1 + levels), ..., %warpid (slot 6),
+ * %smid (slot 7)}; with up to 3 levels slot 5 holds the evaluations the scan ran.  Handles of at most
+ * HSB_TRACE_MAX_LEVELS levels only (with 4 the end time is slot 5); deeper ones cannot set the key and record nothing.
  * Synchronises the device; returns the number of scans copied (<= max_scans) or a negative status. */
 int hsb_read_trace(hsb_handle* h, uint64_t* out, int max_scans);
 /* library build identification, e.g. "hector_slam_b200 0.1 (sm_90a)" */

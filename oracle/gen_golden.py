@@ -3,6 +3,7 @@
 TEST INFRASTRUCTURE.  Run in the build container, where /root/reference exists:
 
     make -C oracle && python oracle/gen_golden.py
+    make -C oracle -f record.mk && python oracle/gen_golden.py deep      (deep.npz: 8- and 5-level maps)
 
 The reference ships no golden vectors (SURVEY.md §4/§8c), so these fixtures are produced by the
 unmodified reference headers themselves (compiled against oracle/shim).  They pin
@@ -303,8 +304,92 @@ def gen_next(kind="reference"):
     np.savez_compressed(os.path.join(OUT, "next.npz"), **out)
 
 
+# ---------------- deep pyramids: 8 and 5 levels (tests/deep_cases.py) ------------------------------------------------
+# (sx, sy, levels, start, resolution): the 8-level map whose coarse widths take every residue mod 4, and the node's
+# default size with two more levels than its default 3
+DEEP_GEOMS = {"g8": (1000, 640, 8, (0.3, 0.7), 0.05), "g5": (2048, 2048, 5, (0.5, 0.5), 0.025)}
+# maxIterations per level, level 0 first, in every encoding of hsb_config::max_iterations (0: the reference's literal,
+# -1: none, n: n), truncated to the depth
+DEEP_SCHEDULES = {"default": None, "mixed": [0, -1, 2, 7, -1, 1, 0, 4], "single": [-1] * 8}
+DEEP_STEPS, DEEP_MWM, DEEP_MATCHES = 14, (6, 7, 11), 12
+
+
+def deep_run(g):
+    """A short SLAM run for geometry g: 1081-beam scans along a path in the one-room world, and which steps are
+    map_without_matching (two in a row and one later, none first: the coarse levels then write from the container of
+    the last matched scan).  Every step's hint is the path's pose, as when odometry supplies the start estimate: on
+    the 8-level map the coarsest levels (6.4 m cells, 7 x 5 of them) send the reference's own matcher tens of metres
+    off on a map of one or two scans, and a run that fed its estimates back would leave the map at the second step.
+    -> (scans (K, 1081, 2), mwm (K,) bool, hints (K, 3), the path (K, 3) float64)"""
+    world = synth.World(1, seed=1234)
+    rng = np.random.default_rng(4242)
+    traj = np.array([-3.0, -2.0, 0.2]) + np.arange(DEEP_STEPS)[:, None] * np.array([0.12, 0.05, 0.025])
+    scans = np.stack([synth.make_scan(world, p, rng, 1.0 / g[4]) for p in traj]).astype(np.float32)
+    mwm = np.zeros(DEEP_STEPS, bool)
+    mwm[list(DEEP_MWM)] = True
+    return scans, mwm, traj.astype(np.float32), traj
+
+
+def deep_matches(g, traj):
+    """DEEP_MATCHES scans from poses around the path, with perturbed hints, an empty one last"""
+    world = synth.World(1, seed=1234)
+    rng = np.random.default_rng(777)
+    poses = traj[rng.integers(0, len(traj), DEEP_MATCHES)] + rng.uniform(-0.3, 0.3, (DEEP_MATCHES, 3)) * [1, 1, 0.3]
+    scans = np.stack([synth.make_scan(world, p, rng, 1.0 / g[4]) for p in poses]).astype(np.float32)
+    return scans, synth.perturb_hints(poses, seed=5, dxy=0.08, dpsi=0.04).astype(np.float32)
+
+
+def deep_arrays(kind="reference"):
+    """The arrays of deep.npz from the compiled reference or (kind="port") the C port: per geometry the run's poses,
+    covariances and final planes, then matchData on the final map under the default and the mixed schedule with what
+    the matcher reports to its hooks (oracle/record_oracle.py)."""
+    from oracle.record_oracle import RecordOracle, port_hooks
+
+    out = {}
+    for tag, g in DEEP_GEOMS.items():
+        sx, sy, L, start, res = g
+        orc = RecordOracle(kind, res, sx, L, start=start, size_y=sy)
+        orc.set_update_factors(0.4, 0.9)
+        orc.set_map_update_thresholds(0.0, 0.0)
+        scans, mwm, hints, traj = deep_run(g)
+        est, cov = [], []
+        for k in range(DEEP_STEPS):
+            p, c = orc.update(scans[k], hints[k], map_without_matching=bool(mwm[k]))
+            est.append(p)
+            cov.append(c.reshape(9))
+        out.update({f"{tag}_geom": np.float64([sx, sy, L, start[0], start[1], res]), f"{tag}_run_scans": scans,
+                    f"{tag}_run_mwm": mwm, f"{tag}_run_hints": hints,
+                    f"{tag}_run_est": np.float32(est), f"{tag}_run_cov": np.float32(cov)})
+        for l in range(L):
+            out[f"{tag}_final{l}"] = orc.get_logodds(l)
+        mscans, mhints = deep_matches(g, traj)
+        out[f"{tag}_match_scans"], out[f"{tag}_match_hints"] = mscans, mhints
+        for name in ("default", "mixed"):
+            iters = None if DEEP_SCHEDULES[name] is None else DEEP_SCHEDULES[name][:L]
+            P, Cv, Hk = [], [], []
+            for k in range(DEEP_MATCHES):
+                if kind == "reference":
+                    p, c, hooks, _ = orc.match_record(mhints[k], mscans[k], iters)
+                else:
+                    p, c, rec = orc.match_record(mhints[k], mscans[k], iters)
+                    hooks = port_hooks(orc, rec, mscans[k].shape[0], iters)
+                P.append(p)
+                Cv.append(c.reshape(9))
+                Hk.append(hooks)
+            out[f"{tag}_{name}_poses"], out[f"{tag}_{name}_cov"] = np.float32(P), np.float32(Cv)
+            out[f"{tag}_{name}_hooks"] = np.float32(Hk)
+        orc.close()
+    return out
+
+
+def gen_deep(kind="reference"):
+    np.savez_compressed(os.path.join(OUT, "deep.npz"), **deep_arrays(kind))
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "next":
         gen_next()
+    elif len(sys.argv) > 1 and sys.argv[1] == "deep":
+        gen_deep()
     else:
         main()

@@ -274,3 +274,35 @@ def test_next_rows_goldens_bit_exact(pyoracle):
         d, hw, f = o.get_dist(0, g["gd_begin"][i], g["gd_end"][i])
         assert np.float32(d) == g["gd_dist"][i] and f == bool(g["gd_found"][i]) and np.array_equal(hw, g["gd_hit"][i])
     o.close()
+
+
+def test_deep_golden_bit_exact(pyoracle):
+    """tests/golden/deep.npz (oracle/gen_golden.py deep, from the compiled reference): a 14-step SLAM run with three
+    map_without_matching steps on a 1000 x 640 x 8 and a 2048 x 2048 x 5 map, then matchData on the final maps under the
+    default and the mixed iteration schedule with the matcher's hook reports.  The C port reproduces every array bit
+    for bit on any machine: run poses and covariances, all 13 planes, match poses, covariances and hooks."""
+    import subprocess
+
+    from conftest import ROOT
+    from oracle import gen_golden, record_oracle
+
+    if not record_oracle.available("port"):
+        subprocess.run(["make", "-C", f"{ROOT}/oracle", "-f", "record.mk", "port"], check=True, capture_output=True)
+    want, got = load_golden("deep.npz"), gen_golden.deep_arrays("port")
+    assert sorted(want.files) == sorted(got)
+    for k in want.files:
+        a, b = want[k], np.asarray(got[k])
+        assert a.shape == b.shape and a.dtype == b.dtype, k
+        if a.dtype == np.float32:
+            assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), k
+        else:
+            assert np.array_equal(a, b), k
+    for tag, g in gen_golden.DEEP_GEOMS.items():
+        L = g[2]
+        assert all(np.any(want[f"{tag}_final{l}"] != 0) for l in range(L)), tag       # every level was written
+        assert not np.array_equal(want[f"{tag}_default_poses"], want[f"{tag}_mixed_poses"]), tag
+    # the 5-level run tracks the path it was simulated on (noise sigma 1 cm).  (The 8-level one does not: its coarsest
+    # levels, 7 x 5 cells of 6.4 m, throw the reference's matcher off: see oracle/gen_golden.py deep_run.)
+    traj = gen_golden.deep_run(gen_golden.DEEP_GEOMS["g5"])[3]
+    assert np.abs(want["g5_run_est"][:, :2] - traj[:, :2]).max() < 0.02
+    assert np.abs(want["g5_default_poses"] - want["g5_match_hints"]).max() < 0.15
