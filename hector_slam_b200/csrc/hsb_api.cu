@@ -311,6 +311,8 @@ int fail_fused_too_long(hsb_handle* h, int max_n) {
 template <int W, int G, int MODE, int U, bool PACK, bool INL = false, int GRP = hsb::GRP_NONE, bool PROJ = false>
 int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st, int Gr,
                    const hsb::InlineScan<INL>& S = hsb::InlineScan<INL>()) {
+  // launch_match's one-wave path passes its group count to a G > 1 kernel: one CTA per SM, one warp per scan
+  const bool one_wave_groups = G > 1 && Gr > 0;
   if (Gr <= 0 || Gr > G) Gr = G;   // groups per CTA actually launched (a G-group kernel runs with fewer: see launch_match)
   const size_t header = hsb::MatchSmem<W, G>::kHeaderBytes;
   auto kern = hsb::match_kernel<W, G, MODE, U, PACK, INL, GRP, PROJ>;
@@ -341,7 +343,11 @@ int launch_match_t(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st,
     pts = (pts - 2) / gt * gt;
     return pts >= 4 * gt ? pts + 2 : 0;
   };
-  const bool may_split = h->tune_partial && !PACK && !fused;   // a staged PREFIX is allowed
+  // A staged PREFIX is allowed — except on the one-wave path: there the CTA's scans, when they do not fit whole, are not
+  // staged at all.  A prefix of each of ~32 scans fills the SM's shared memory and leaves L1 about 28 KB for the map
+  // gathers of all of them; unstaged, L1 keeps nearly all 256 KB, and the gathers that miss it and the endpoints read
+  // through it cost less than the prefix saves (DESIGN.md §4, scan staging).
+  const bool may_split = h->tune_partial && !PACK && !fused && !one_wave_groups;
   if (cap > 0 && !staging_fits<W, G>(cap, Gr)) {        // the CTA's scans do not fit whole
     if (fused) return fail_fused_too_long(h, max_n);
     cap = may_split ? cap_for(1) : 0;
@@ -484,8 +490,9 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   if (G <= 0) {
     G = 1;
     // One-wave batches of one-warp scans (tuning "auto_group", on by default): ONE CTA per SM holding ceil(B / SMs) <= 32
-    // scans instead of one-warp CTAs.  One CTA pays the 1 KB per-CTA shared-memory reservation once, so more of each
-    // scan can be staged at full residency, and its warps start and end together.  Up to 28 scans per SM the 28-group
+    // scans instead of one-warp CTAs.  One CTA pays the 1 KB per-CTA shared-memory reservation once, so up to 26 scans
+    // per SM can be staged whole at full residency (more are not staged: launch_match_t), and its warps start and end
+    // together.  Up to 28 scans per SM the 28-group
     // kernel runs (72 registers, the one-warp kernel's budget); up to 32 the 32-group kernel (1024 threads, 64 registers),
     // which keeps the benchmark's 4096 scans in one wave on a 132-SM H100 where 28 per SM would leave a second wave.
     // Larger batches keep one scan per CTA: finished warps are replaced at once there, which a CTA-wide drain would

@@ -10,11 +10,15 @@
 //   ldg64x2   2 x ld.global.v2 from a pair plane;  ldg32x4: 4 x ld.global.f32 from the plain plane (K1's MODE_LDG)
 //   tld4+128 / tld4+64: every other gather through the texture path, the others through the LSU path — do they overlap?
 // Output: ns and SM cycles (at the clock measured in the kernel) per warp-level gather per SM, 28 warps per SM.
-// Build: make -C scripts/ubench bin/tex_rate     Run: bin/tex_rate [map size, default 2048]
+// `resident`: each warp keeps coming back to a fixed set of scan-like footprints; sweeps the per-SM working set,
+// warps per SM and the L1 size (a K1-sized shared-memory request against none) — what an L1 hit saves a scan gather.
+// Build: make -C scripts/ubench bin/tex_rate     Run: bin/tex_rate [resident] [map size, default 2048]
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e)); exit(1);} } while (0)
@@ -113,6 +117,84 @@ __global__ void __launch_bounds__(896, 1) rate_kernel(const Args A) {
   if (threadIdx.x == 0) A.clocks[blockIdx.x] = (unsigned long long)(c1 - c0);
 }
 
+// Resident footprints: warp w of an SM cycles through F scan-like footprints of its own (the "scan" pattern's shape,
+// bases drawn once per footprint), so from the second pass on every gather finds its cells in L1 when the SM's
+// working set (warps x F footprints) fits there.  F at least the number of gathers a warp issues = every footprint
+// new, the "scan" pattern under the same code.  The dynamic shared-memory request only sets the carve-out.
+template <int U>
+__global__ void __launch_bounds__(1024, 1) resident_kernel(const Args A, int F) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned seed = (blockIdx.x * 977u + warp * 131u + 7u) * 2654435761u;
+  const unsigned m = (unsigned)A.mask;
+  const unsigned step = (lane * 3u) >> 1, row = (unsigned)lane >> 3;
+  float acc = 0.f;
+  int k = 0;
+  const long long c0 = clock64();
+  for (int it = 0; it < A.iters; ++it) {
+    float xs[U], ys[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const unsigned s = (seed ^ ((unsigned)k * 0x9E3779B9u)) * 1664525u + 1013904223u;
+      const unsigned bx = (s >> 7) & m, by = (s >> 19) & m, dir = (s >> 3) & 1u;
+      unsigned x = (bx + (dir ? step : row)) & m, y = (by + (dir ? row : step)) & m;
+      if (x >= m) x = m - 1;
+      if (y >= m) y = m - 1;
+      xs[u] = u2f(x);
+      ys[u] = u2f(y);
+      k = (k + 1 == F) ? 0 : k + 1;
+    }
+    float r[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) r[u] = gather<OP_TLD4>(A, xs[u], ys[u]);
+#pragma unroll
+    for (int u = 0; u < U; ++u) acc += r[u];
+  }
+  const long long c1 = clock64();
+  if (acc == 123.456f) A.out[0] = acc;
+  if (threadIdx.x == 0) A.clocks[blockIdx.x] = (unsigned long long)(c1 - c0);
+}
+
+// Cycles per warp-level tld4 per SM for resident footprints, against L1 size (dynamic shared memory request) x
+// warps per SM x per-SM working set.  A footprint is counted as 16 sectors (512 B): lanes 1.5 cells apart on 4 rows
+// of a 2x2 footprint each, ~100 distinct fp32 cells in a block-linear layout.
+static void resident_sweep(Args A, int sms) {
+  constexpr int U = 4;
+  constexpr int kFootprintBytes = 512;
+  const int big_smem = 227 * 1024;   // leaves 28 KB of the 256 KB for L1, as a fully staged one-wave K1 CTA does
+  CK(cudaFuncSetAttribute(resident_kernel<U>, cudaFuncAttributeMaxDynamicSharedMemorySize, big_smem));
+  std::vector<unsigned long long> clk(sms);
+  const int warps_list[4] = {8, 16, 28, 32};
+  const int ws_kb[5] = {16, 64, 128, 480, 0};   // 0: no reuse (every footprint new)
+  printf("resident tld4 footprints: cycles per warp-level gather per SM (%d SMs, %d gathers per warp)\n", sms, A.iters * U);
+  for (int cfg = 0; cfg < 2; ++cfg) {
+    const int smem = cfg == 0 ? big_smem : 0;
+    CK(cudaFuncSetAttribute(resident_kernel<U>, cudaFuncAttributePreferredSharedMemoryCarveout, cfg == 0 ? 100 : 0));
+    printf("%s\n", cfg == 0 ? "L1 ~28 KB (227 KB dynamic shared memory)" : "L1 maximal (no shared memory, carve-out 0)");
+    printf("  warps/SM");
+    for (int w : ws_kb) w ? printf("  %6d KB", w) : printf("  no reuse");
+    printf("   no-reuse / best\n");
+    for (int warps : warps_list) {
+      printf("  %8d", warps);
+      double best = 1e30, none = 0;
+      for (int w : ws_kb) {
+        const int F = w ? std::max(1, (w * 1024) / (warps * kFootprintBytes)) : A.iters * U;
+        resident_kernel<U><<<sms, warps * 32, smem>>>(A, F);
+        CK(cudaGetLastError());
+        CK(cudaDeviceSynchronize());
+        resident_kernel<U><<<sms, warps * 32, smem>>>(A, F);
+        CK(cudaDeviceSynchronize());
+        CK(cudaMemcpy(clk.data(), A.clocks, sizeof(unsigned long long) * sms, cudaMemcpyDeviceToHost));
+        double cyc = 0;
+        for (int i = 0; i < sms; ++i) cyc += (double)clk[i];
+        cyc /= (double)sms * A.iters * U * warps;
+        printf("  %9.2f", cyc);
+        if (w) best = std::min(best, cyc); else none = cyc;
+      }
+      printf("   %6.2fx\n", none / best);
+    }
+  }
+}
+
 template <int OP>
 static void run(const char* name, Args A, int sms, int warps, const char* const* pat_names) {
   constexpr int U = 4;
@@ -143,6 +225,8 @@ static void run(const char* name, Args A, int sms, int warps, const char* const*
 }
 
 int main(int argc, char** argv) {
+  const bool resident = argc > 1 && strcmp(argv[1], "resident") == 0;
+  if (resident) { --argc; ++argv; }
   const int size = argc > 1 ? atoi(argv[1]) : 2048;
   const int warps = argc > 2 ? atoi(argv[2]) : 28;
   int dev = 0, sms = 0;
@@ -184,6 +268,11 @@ int main(int argc, char** argv) {
   CK(cudaMalloc(&A.out, 16));
   CK(cudaMalloc(&A.clocks, sizeof(unsigned long long) * sms));
   const char* pats[5] = {"same", "consec", "win64", "random", "scan"};
+  if (resident) {
+    A.tex = t1;
+    resident_sweep(A, sms);
+    return 0;
+  }
   A.tex = t1;
   run<OP_TLD4>("tld4", A, sms, warps, pats);
   A.tex = t4;
