@@ -46,6 +46,7 @@ EXPORTED = [
     "hsb_group_likelihood", "hsb_group_likelihood_subset", "hsb_group_covariance", "hsb_group_covariance_subset",
     "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
     "hsb_group_match_batch", "hsb_group_match_batch_subset",
+    "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
 ]
 
 
@@ -214,6 +215,9 @@ def load_library() -> C.CDLL:
     sig("hsb_group_best_hypothesis_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_match_batch", i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_match_batch_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_pack_dirty_device", i, vp, vp, C.c_size_t, i, vp)
+    sig("hsb_group_pack_dirty_device_subset", i, vp, i, vp, vp, C.c_size_t, i, vp)
+    sig("hsb_group_unpack_dirty_device", i, vp, vp, C.c_size_t, vp)
     _lib = L
     return L
 
@@ -1060,6 +1064,24 @@ class SlamGroup:
             self._check(self.lib.hsb_group_sync_occupancy_subset(self.g, K, _ptr(mem), int(level), C.cast(arr, C.c_void_p),
                                                                  rects.ctypes.data, int(bool(reset))))
         return [None if r[2] < r[0] else tuple(int(v) for v in r) for r in rects[:K]]
+
+    def pack_dirty_device(self, d_buf: int, capacity: int, reset: bool = True, stream: int = 0, members=None):
+        """Every member's dirty tiles into one device buffer of `capacity` bytes (hsb_group_pack_dirty_device): a group
+        header, then per session the buffer MapRepB200.pack_dirty_device writes for that member alone; rows placed
+        first-fit in session order, a block that does not fit is deferred and keeps its rectangles.  members as in
+        slam_update (hsb_group_pack_dirty_device_subset).  Asynchronous on `stream`."""
+        K, mem = self._sessions(members)
+        if mem is None:
+            self._check(self.lib.hsb_group_pack_dirty_device(self.g, d_buf, int(capacity), int(bool(reset)), stream))
+        else:
+            self._check(self.lib.hsb_group_pack_dirty_device_subset(self.g, K, _ptr(mem), d_buf, int(capacity),
+                                                                    int(bool(reset)), stream))
+
+    def unpack_dirty_device(self, d_buf: int, capacity: int, stream: int = 0):
+        """Apply a buffer pack_dirty_device wrote on an owner group listing its handles in this group's order
+        (hsb_group_unpack_dirty_device).  Deferred blocks count on their member's replication_overflows(), a buffer that
+        does not fit this group on reps[0]'s.  Asynchronous on `stream`."""
+        self._check(self.lib.hsb_group_unpack_dirty_device(self.g, d_buf, int(capacity), stream))
 
     def get_dist(self, level: int, begin_world, end_world, members=None):
         """DistanceMeasurementProvider::getDist for the members' rays in one pass (hsb_group_get_dist): begin_world and

@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <vector>
@@ -2352,8 +2353,10 @@ static void fill_tile_params(hsb_handle* h, HsbTileParams& T, float* d_buf, size
     T.lv[l].dirty = L.dirty;
   }
   T.buf = d_buf;
-  T.capacity_words = (unsigned)std::min<size_t>(capacity_bytes / 4, 0xffffffffu);
+  T.capacity_words = std::min<size_t>(capacity_bytes / 4, 0xffffffffu);
   T.error_count = h->d_dirty_all + HSB_MAX_LEVELS * 8;
+  T.K = 1;
+  T.M = 1;
 }
 
 int hsb_pack_dirty_device(hsb_handle* h, float* d_buf, size_t capacity_bytes, int reset, void* stream) {
@@ -2564,6 +2567,12 @@ struct hsb_group {
   // staging above (every call that fills it returns synchronised); M arg-max accumulators of the best hypothesis,
   // zeroed once (every call re-arms the ones it used)
   unsigned long long* d_best = nullptr;
+  // map replication (hsb_group_pack_dirty_device, hsb_group_unpack_dirty_device): M x levels tile descriptors,
+  // member-major like d_lv, and the members' replication-overflow counters; two events ordering the caller's stream
+  // against the group's
+  HsbTileLevelDev* d_tile_lv = nullptr;
+  int** d_tile_counters = nullptr;
+  cudaEvent_t ev_tile[2] = {nullptr, nullptr};
 };
 
 namespace {
@@ -2608,6 +2617,10 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
   if (g->d_planes) cudaFree(g->d_planes);
   if (g->d_best) cudaFree(g->d_best);
+  if (g->d_tile_lv) cudaFree(g->d_tile_lv);
+  if (g->d_tile_counters) cudaFree(g->d_tile_counters);
+  for (cudaEvent_t e : g->ev_tile)
+    if (e) cudaEventDestroy(e);
   if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
   if (g->h_ray_stage) cudaFreeHost(g->h_ray_stage);
   if (g->d_res) cudaFree(g->d_res);
@@ -2699,6 +2712,19 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
     HSB_GROUP_CUDA(cudaMemcpy(g->d_planes, planes.data(), planes.size() * sizeof(float*), cudaMemcpyHostToDevice));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_best, (size_t)M * sizeof(unsigned long long)));
     HSB_GROUP_CUDA(cudaMemset(g->d_best, 0, (size_t)M * sizeof(unsigned long long)));
+    std::vector<HsbTileLevelDev> tile((size_t)M * g->levels);
+    std::vector<int*> counters(M);
+    for (int s = 0; s < M; ++s) {
+      HsbTileParams T;
+      fill_tile_params(g->m[s], T, nullptr, 0);
+      for (int l = 0; l < g->levels; ++l) tile[(size_t)s * g->levels + l] = T.lv[l];
+      counters[s] = T.error_count;
+    }
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_tile_lv, tile.size() * sizeof(HsbTileLevelDev)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_tile_lv, tile.data(), tile.size() * sizeof(HsbTileLevelDev), cudaMemcpyHostToDevice));
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_tile_counters, counters.size() * sizeof(int*)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_tile_counters, counters.data(), counters.size() * sizeof(int*), cudaMemcpyHostToDevice));
+    for (cudaEvent_t& e : g->ev_tile) HSB_GROUP_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
   }
@@ -3461,6 +3487,147 @@ int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* membe
   const GroupInput in = {HSB_IN_PROJECTED, "hsb_group_slam_update_projected_subset", hints, ranges, offsets, nullptr,
                          transforms};
   return group_step(g, in, K, members, map_without_matching, nowait, out_poses, cov_inout, map_updated, out_kept);
+}
+
+}  // extern "C"
+
+// ---- group map replication: every session's dirty tiles in one buffer, one pack launch and one unpack launch --------
+namespace {
+
+// A subset pack lists its sessions' members in the launch parameters (no host-to-device copy whose pinned source a later
+// call could overwrite before it runs): up to 128 in a 512-byte block, up to 4096 in a 16 KB one.
+constexpr int kTileSubsetSmall = 128, kTileSubsetMax = 4096;
+
+// The caller's stream behind everything queued on the sessions' members (members == nullptr: all M in order): a pending
+// step of any group they belong to, and, for a member that queued work of its own since, its stream (all_streams: its
+// copy streams too).  group_stream: also behind everything queued on this group's stream.
+int tile_order_before(hsb_group* g, cudaStream_t user, int K, const int* members, bool all_streams, bool group_stream) {
+  hsb_handle* h0 = g->m[0];
+  if (group_stream) {
+    HSB_CUDA(h0, cudaEventRecord(g->ev_tile[0], g->stream));
+    HSB_CUDA(h0, cudaStreamWaitEvent(user, g->ev_tile[0], 0));
+  }
+  std::vector<cudaEvent_t> waited;
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members ? members[k] : k];
+    if (h->group_ev && std::find(waited.begin(), waited.end(), h->group_ev) == waited.end()) {
+      HSB_CUDA(h0, cudaStreamWaitEvent(user, h->group_ev, 0));
+      waited.push_back(h->group_ev);
+    }
+    if (h->queued) {
+      const int s = order_before(h, user, all_streams);
+      if (s != HSB_OK) return s;
+    }
+  }
+  return HSB_OK;
+}
+
+// Everything the sessions' members queue after the call waits for it: the group's stream waits for the caller's, and the
+// members take the group's event, recorded behind that wait, as they take a nowait step's (HandleScope, order_members).
+// map_write: the members' planes were written (a match on a copy stream waits for the handle's stream, launch_match).
+int tile_order_after(hsb_group* g, cudaStream_t user, int K, const int* members, bool map_write) {
+  hsb_handle* h0 = g->m[0];
+  HSB_CUDA(h0, cudaEventRecord(g->ev_tile[1], user));
+  HSB_CUDA(h0, cudaStreamWaitEvent(g->stream, g->ev_tile[1], 0));
+  HSB_CUDA(h0, cudaEventRecord(g->ev, g->stream));
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members ? members[k] : k];
+    h->group_ev = g->ev;
+    if (map_write) h->map_write_pending = true;
+  }
+  return HSB_OK;
+}
+
+void fill_group_tile_params(hsb_group* g, HsbTileParams& T, float* d_buf, size_t capacity_bytes, int K) {
+  memset(&T, 0, sizeof(T));
+  T.levels = g->levels;
+  T.buf = d_buf;
+  T.capacity_words = std::min<size_t>(capacity_bytes / 4, 0xffffffffu);
+  T.error_count = g->m[0]->d_dirty_all + HSB_MAX_LEVELS * 8;
+  T.table = g->d_tile_lv;
+  T.counters = g->d_tile_counters;
+  T.K = K;
+  T.M = (int)g->m.size();
+}
+
+// hsb_pack_dirty_device for K sessions (members == g->all: every member in order) into one buffer.
+int group_pack_dirty(hsb_group* g, const char* fn, int K, const int* members, float* d_buf, size_t capacity_bytes,
+                     int reset, cudaStream_t user) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
+  const bool all = members == g->all.data();   // the full form: session k is member k, no list in the launch
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (all) members = nullptr;
+  if (!d_buf) return fail(h0, HSB_ERR_INVALID_ARG, "%s: d_buf is NULL", fn);
+  const size_t min_bytes = 4 * (size_t)(hsb_tile_group_header_words(K) + (unsigned long long)HSB_TILE_HEADER_WORDS * K);
+  if (capacity_bytes < min_bytes)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: capacity_bytes is %zu, below the minimum of %zu bytes for K = %d", fn,
+                capacity_bytes, min_bytes, K);
+  if (members && K > kTileSubsetMax)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: K is %d, a subset pack lists at most %d sessions", fn, K, kTileSubsetMax);
+  DeviceGuard guard(g->device);
+  if ((s = tile_order_before(g, user, K, members, false, false)) != HSB_OK) return s;
+  HsbTileParams T;
+  fill_group_tile_params(g, T, d_buf, capacity_bytes, K);
+  T.reset = reset;
+  const int blocks = h0->sm_count * 4;
+  if (!members) {
+    hsb::pack_dirty_group_kernel<<<blocks, 256, 0, user>>>(T);
+  } else if (K <= kTileSubsetSmall) {
+    hsb::TileMembers<kTileSubsetSmall> S;
+    memcpy(S.idx, members, (size_t)K * sizeof(int));
+    hsb::pack_dirty_subset_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S);
+  } else {
+    std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
+    memcpy(S->idx, members, (size_t)K * sizeof(int));
+    hsb::pack_dirty_subset_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S);
+  }
+  if (reset) {
+    const int threads = K * 4 * g->levels;
+    hsb::reset_dirty_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T);
+  }
+  h0->launches += reset ? 2 : 1;
+  HSB_CUDA(h0, cudaGetLastError());
+  return tile_order_after(g, user, K, members, false);
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_group_pack_dirty_device(hsb_group* g, float* d_buf, size_t capacity_bytes, int reset, void* stream) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_pack_dirty(g, "hsb_group_pack_dirty_device", (int)g->m.size(), g->all.data(), d_buf, capacity_bytes,
+                          reset, (cudaStream_t)stream);
+}
+
+int hsb_group_pack_dirty_device_subset(hsb_group* g, int K, const int* members, float* d_buf, size_t capacity_bytes,
+                                       int reset, void* stream) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_pack_dirty(g, "hsb_group_pack_dirty_device_subset", K, members, d_buf, capacity_bytes, reset,
+                          (cudaStream_t)stream);
+}
+
+int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capacity_bytes, void* stream) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  hsb_handle* h0 = g->m[0];
+  const char* fn = "hsb_group_unpack_dirty_device";
+  if (!d_buf) return fail(h0, HSB_ERR_INVALID_ARG, "%s: d_buf is NULL", fn);
+  const size_t min_bytes = 4 * (size_t)(hsb_tile_group_header_words(1) + HSB_TILE_HEADER_WORDS);
+  if (capacity_bytes < min_bytes)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: capacity_bytes is %zu, below the minimum of %zu bytes (one block)", fn,
+                capacity_bytes, min_bytes);
+  DeviceGuard guard(g->device);
+  const int M = (int)g->m.size();
+  cudaStream_t user = (cudaStream_t)stream;
+  int s;
+  if ((s = tile_order_before(g, user, M, nullptr, true, true)) != HSB_OK) return s;
+  HsbTileParams T;
+  fill_group_tile_params(g, T, const_cast<float*>(d_buf), capacity_bytes, 0);
+  hsb::unpack_dirty_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T);
+  h0->launches++;
+  HSB_CUDA(h0, cudaGetLastError());
+  return tile_order_after(g, user, M, nullptr, true);
 }
 
 }  // extern "C"

@@ -174,6 +174,17 @@ struct HsbUpdateLevelDev {
 // level 0's rectangle, then level 1's, ...
 #define HSB_TILE_HEADER_WORDS 64
 #define HSB_TILE_MAGIC 0x48534254
+// A group's buffer (hsb_group_pack_dirty_device / hsb_group_unpack_dirty_device): a group header of G words —
+// [0] HSB_TILE_GROUP_MAGIC, [1] K, [2] levels, [3] deferred blocks, [4] words used (G + 64 K + shipped cells),
+// [5 + 2k], [6 + 2k] session k's {member index in the group, word offset of its block}, zeros up to G = 5 + 2K rounded
+// up to a multiple of 4 — then K blocks in session order, each exactly the buffer hsb_pack_dirty_device writes for that
+// member alone (HSB_TILE_HEADER_WORDS of header, then its rows).  A deferred block (overflow = 1) has no rows.  The
+// blocks' rows are placed first-fit in session order: a block whose rows fit behind those already placed is shipped.
+#define HSB_TILE_GROUP_MAGIC 0x48534247
+#define HSB_TILE_GROUP_FIXED_WORDS 5
+__host__ __device__ inline unsigned long long hsb_tile_group_header_words(int K) {
+  return (HSB_TILE_GROUP_FIXED_WORDS + 2ull * (unsigned long long)K + 3ull) & ~3ull;
+}
 struct HsbTileLevelDev {
   float* logodds;
   float* prob;
@@ -182,12 +193,19 @@ struct HsbTileLevelDev {
   int* dirty;   // [0..3] replication rectangle, [4..7] host-mirror rectangle
 };
 struct HsbTileParams {
-  HsbTileLevelDev lv[HSB_MAX_LEVELS];
+  HsbTileLevelDev lv[HSB_MAX_LEVELS];   // a single handle's levels (table == nullptr)
   int levels;
   float* buf;
-  unsigned capacity_words;   // whole buffer, header included
+  unsigned long long capacity_words;    // whole buffer, headers included
   int reset;                 // pack: clear the replication rectangles afterwards (unless overflowed)
-  int* error_count;          // unpack: incremented when an overflowed buffer arrives
+  int* error_count;          // unpack: incremented once when a buffer arrives that does not fit (a single handle's
+                             // counter also takes its overflowed buffers)
+  // group form: M x levels descriptors, member-major (hsb_group::d_tile_lv), each member's overflow counter (a deferred
+  // block is counted there), the sessions of a pack (K) and the group's size; a single handle passes table = nullptr
+  // and K = 1
+  const HsbTileLevelDev* table;
+  int* const* counters;
+  int K, M;
 };
 
 struct HsbUpdateParams {

@@ -566,87 +566,319 @@ __global__ void unpack_rect_kernel(float* __restrict__ logodds, float* __restric
 // header and the rectangles' log-odds rows behind it; the replicas' unpack kernel reads the header from the buffer the
 // collective delivered.  No size ever travels through a host, so the whole replication step is stream-ordered: pack ->
 // ONE fixed-size ncclBroadcast -> unpack (DESIGN.md §6).
-struct TileLayout {
-  int x0[HSB_MAX_LEVELS], y0[HSB_MAX_LEVELS], w[HSB_MAX_LEVELS], h[HSB_MAX_LEVELS];
-  unsigned off[HSB_MAX_LEVELS + 1];   // cells before level l
+//
+// One body serves a single handle and a group (hsb_group_pack_dirty_device / hsb_group_unpack_dirty_device).  It walks
+// a table of blocks, one per session: the block's member, its level descriptors (P.table's member-major row, or the
+// single handle's P.lv) and the word where the block starts.  A single handle's buffer is one block at word 0 and no
+// group header.  Sessions are laid out kTileChunk at a time in shared memory (every CTA lays out every chunk: the
+// layout of a block depends on all blocks before it), then the chunk's rows go one warp per row over the grid.
+
+constexpr int kTileChunk = 128;   // sessions laid out per pass (threads 0 .. kTileChunk-1 of the 256-thread CTA)
+
+struct TileChunk {
+  int4 rect[kTileChunk][HSB_MAX_LEVELS];   // the block's rectangles {x0, y0, x1, y1} (x1 < x0: clean)
+  unsigned long long start[kTileChunk];    // the block's first word in the buffer (its HSB_TILE_* header)
+  unsigned long long cells[kTileChunk];    // the block's row words (cells of all its rectangles)
+  unsigned row0[kTileChunk + 1];           // shipped rows of the chunk before the block's; row0[n]: all of them
+  int member[kTileChunk];
+  int ship[kTileChunk];                    // 1: rows shipped, 0: deferred
 };
-__device__ __forceinline__ void tile_layout_from(const int* rects, int levels, TileLayout& t) {
-  unsigned acc = 0;
-  for (int l = 0; l < levels; ++l) {
-    const int x0 = rects[4 * l], y0 = rects[4 * l + 1], x1 = rects[4 * l + 2], y1 = rects[4 * l + 3];
-    const bool dirty = x1 >= x0 && y1 >= y0;
-    t.x0[l] = x0; t.y0[l] = y0;
-    t.w[l] = dirty ? x1 - x0 + 1 : 0;
-    t.h[l] = dirty ? y1 - y0 + 1 : 0;
-    t.off[l] = acc;
-    acc += (unsigned)t.w[l] * (unsigned)t.h[l];
+
+__device__ __forceinline__ bool tile_dirty(int4 r) { return r.z >= r.x && r.w >= r.y; }
+// a rectangle's width / height as 64-bit counts (a foreign buffer's rectangles may be anything)
+__device__ __forceinline__ long long tile_w(int4 r) { return tile_dirty(r) ? (long long)r.z - r.x + 1 : 0; }
+__device__ __forceinline__ long long tile_h(int4 r) { return tile_dirty(r) ? (long long)r.w - r.y + 1 : 0; }
+
+__device__ __forceinline__ const HsbTileLevelDev* tile_levels(const HsbTileParams& P, int member) {
+  return P.table ? P.table + (size_t)member * P.levels : P.lv;
+}
+// where a block's deferral is counted: its member's overflow counter (a single handle: its own)
+__device__ __forceinline__ int* tile_counter(const HsbTileParams& P, int member) {
+  return P.table ? P.counters[member] : P.error_count;
+}
+
+// Warp 0: row0[1 .. n] hold each block's row count; turned into the exclusive prefix row0[0 .. n].
+__device__ __forceinline__ void tile_row_prefix(TileChunk& c, int n) {
+  const int lane = threadIdx.x;
+  unsigned carry = 0;
+  for (int b = 0; b < n; b += 32) {
+    unsigned v = b + lane < n ? c.row0[b + lane + 1] : 0u;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned y = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += y;
+    }
+    if (b + lane < n) c.row0[b + lane + 1] = carry + v;
+    carry += __shfl_sync(0xffffffffu, v, 31);
   }
-  t.off[levels] = acc;
+  if (lane == 0) c.row0[0] = 0u;
+}
+
+// The chunk's rows, one warp per row: row r belongs to the block whose rows [row0[j], row0[j+1]) hold it (blocks
+// without rows are passed over), then to the first of its dirty levels that still has rows left.  kPack: plane -> buffer;
+// otherwise buffer -> plane, probability and texture twin, with the per-cell bounds guard (a foreign geometry must not
+// write out of bounds).
+template <bool kPack>
+__device__ __forceinline__ void tile_rows(const HsbTileParams& P, const TileChunk& c, int n) {
+  const int lane = threadIdx.x & 31;
+  const unsigned total = c.row0[n];
+  const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (unsigned r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < total; r += nwarps) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (c.row0[mid] <= r) lo = mid;
+      else hi = mid - 1;
+    }
+    unsigned long long off = c.start[lo] + HSB_TILE_HEADER_WORDS;
+    long long rr = r - c.row0[lo];
+    int l = 0;
+    int4 q = c.rect[lo][0];
+    for (;; ++l) {
+      q = c.rect[lo][l];
+      const long long h = tile_h(q);
+      if (rr < h) break;
+      rr -= h;
+      off += (unsigned long long)(tile_w(q) * h);
+    }
+    const long long w = tile_w(q);
+    off += (unsigned long long)(rr * w);
+    const HsbTileLevelDev L = tile_levels(P, c.member[lo])[l];
+    const int y = q.y + (int)rr;
+    if (kPack) {
+      const float* src = L.logodds + (size_t)y * L.sx + q.x;
+      for (int x = lane; x < w; x += 32) P.buf[off + x] = src[x];
+    } else {
+      if (y < 0 || y >= L.sy) continue;
+      for (int x = lane; x < w; x += 32) {
+        const int cx = q.x + x;
+        if (cx < 0 || cx >= L.sx) continue;
+        const size_t o = (size_t)y * L.sx + cx;
+        const float v = P.buf[off + x];
+        L.logodds[o] = v;
+        const float p = prob_from_logodds(v);
+        L.prob[o] = p;
+        if (L.surf) surf2Dwrite(p, L.surf, cx * (int)sizeof(float), y);
+      }
+    }
+  }
+}
+
+// The sessions of a pack: a single handle (one block, member 0), every member of a group in order, or a subset listed
+// in the launch's parameters (N sessions at most).
+struct TileSingle {
+  __device__ int member(int) const { return 0; }
+};
+struct TileAll {
+  __device__ int member(int k) const { return k; }
+};
+template <int N>
+struct TileMembers {
+  int idx[N];
+  __device__ int member(int k) const { return idx[k]; }
+};
+
+// Pack: each session's block header, first-fit placement of its rows in session order (a block whose rows do not fit
+// behind those already placed is deferred: overflow = 1, no rows), the rows, and for a group the group header.
+template <class Sessions>
+__device__ __forceinline__ void pack_dirty_body(const HsbTileParams& P, const Sessions& S) {
+  __shared__ TileChunk c;
+  __shared__ unsigned long long s_used;   // row words placed before the current chunk
+  __shared__ int s_deferred;
+  const int K = P.K, levels = P.levels;
+  const bool group = P.table != nullptr;
+  const unsigned long long G = group ? hsb_tile_group_header_words(K) : 0ull;
+  const unsigned long long room = P.capacity_words - G - (unsigned long long)HSB_TILE_HEADER_WORDS * K;
+  if (threadIdx.x == 0) { s_used = 0ull; s_deferred = 0; }
+  for (int k0 = 0; k0 < K; k0 += kTileChunk) {
+    const int n = min(kTileChunk, K - k0);
+    const int j = threadIdx.x;
+    if (j < n) {
+      const int m = S.member(k0 + j);
+      const HsbTileLevelDev* lv = tile_levels(P, m);
+      unsigned long long cells = 0;
+      unsigned rows = 0;
+      for (int l = 0; l < levels; ++l) {
+        const int* d = lv[l].dirty;
+        const int4 q = make_int4(d[0], d[1], d[2], d[3]);
+        c.rect[j][l] = q;
+        cells += (unsigned long long)(tile_w(q) * tile_h(q));
+        rows += (unsigned)tile_h(q);
+      }
+      c.member[j] = m;
+      c.cells[j] = cells;
+      c.row0[j + 1] = rows;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {   // first fit, 32 sessions at a time: ship the run of blocks that fits, defer the first that
+      const int lane = threadIdx.x;   // does not, repeat with the rest
+      unsigned long long used = s_used;
+      int deferred = 0;
+      for (int b = 0; b < n; b += 32) {
+        const int jj = b + lane;
+        const unsigned long long cj = jj < n ? c.cells[jj] : 0ull;
+        const unsigned long long base = G + (unsigned long long)HSB_TILE_HEADER_WORDS * (k0 + jj);
+        unsigned pending = __ballot_sync(0xffffffffu, jj < n);
+        while (pending) {
+          const bool mine = (pending >> lane) & 1u;
+          unsigned long long x = mine ? cj : 0ull;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+          }
+          const unsigned over = __ballot_sync(0xffffffffu, mine && used + x > room);
+          const unsigned ship = pending & (over ? (over & (0u - over)) - 1u : 0xffffffffu);
+          if ((ship >> lane) & 1u) { c.start[jj] = base + used + x - cj; c.ship[jj] = 1; }
+          const unsigned long long placed = ship ? __shfl_sync(0xffffffffu, x, 31 - __clz(ship)) : 0ull;
+          pending &= ~ship;
+          if (over) {
+            const int f = __ffs(over) - 1;
+            if (lane == f) { c.start[jj] = base + used + placed; c.ship[jj] = 0; c.row0[jj + 1] = 0u; }
+            pending &= ~(1u << f);
+            ++deferred;
+          }
+          used += placed;
+        }
+      }
+      __syncwarp();
+      tile_row_prefix(c, n);
+      if (lane == 0) { s_used = used; s_deferred += deferred; }
+    }
+    __syncthreads();
+    if (blockIdx.x == 0 && j < n) {   // the block's header, exactly hsb_pack_dirty_device's for this member alone
+      int* hdr = reinterpret_cast<int*>(P.buf + c.start[j]);
+      hdr[0] = HSB_TILE_MAGIC; hdr[1] = levels; hdr[2] = c.ship[j] ? 0 : 1; hdr[3] = (int)c.cells[j];
+      for (int l = 0; l < levels; ++l) {
+        const int4 q = c.rect[j][l];
+        hdr[4 + 4 * l] = q.x; hdr[5 + 4 * l] = q.y; hdr[6 + 4 * l] = q.z; hdr[7 + 4 * l] = q.w;
+      }
+      if (group) {
+        int* gh = reinterpret_cast<int*>(P.buf);
+        gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * (k0 + j)] = c.member[j];
+        gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * (k0 + j) + 1] = (int)(unsigned)c.start[j];
+      }
+    }
+    tile_rows<true>(P, c, n);
+    __syncthreads();   // the next chunk reuses c
+  }
+  if (group && blockIdx.x == 0 && threadIdx.x == 0) {
+    int* gh = reinterpret_cast<int*>(P.buf);
+    gh[0] = HSB_TILE_GROUP_MAGIC; gh[1] = K; gh[2] = levels; gh[3] = s_deferred;
+    gh[4] = (int)(unsigned)(G + (unsigned long long)HSB_TILE_HEADER_WORDS * K + s_used);
+    for (unsigned long long w = HSB_TILE_GROUP_FIXED_WORDS + 2ull * K; w < G; ++w) gh[w] = 0;
+  }
 }
 
 __global__ void __launch_bounds__(256) pack_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  __shared__ int rects[4 * HSB_MAX_LEVELS];
-  if (threadIdx.x < 4 * P.levels) rects[threadIdx.x] = P.lv[threadIdx.x >> 2].dirty[threadIdx.x & 3];
-  __syncthreads();
-  TileLayout t;
-  tile_layout_from(rects, P.levels, t);
-  const unsigned total = t.off[P.levels];
-  const bool overflow = (unsigned long long)total + HSB_TILE_HEADER_WORDS > P.capacity_words;
-  int* hdr = reinterpret_cast<int*>(P.buf);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    hdr[0] = HSB_TILE_MAGIC; hdr[1] = P.levels; hdr[2] = overflow ? 1 : 0; hdr[3] = (int)total;
-  }
-  if (blockIdx.x == 0 && threadIdx.x < 4 * P.levels) hdr[4 + threadIdx.x] = rects[threadIdx.x];
-  if (overflow) return;
-  float* out = P.buf + HSB_TILE_HEADER_WORDS;
-  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= t.off[l + 1]) ++l;
-    const unsigned k = i - t.off[l];
-    const unsigned r = k / (unsigned)t.w[l], c = k - r * (unsigned)t.w[l];
-    out[i] = P.lv[l].logodds[(size_t)(t.y0[l] + (int)r) * P.lv[l].sx + (t.x0[l] + (int)c)];
-  }
+  pack_dirty_body(P, TileSingle());
 }
-// after pack (stream order): the shipped rectangles are forgotten — unless the buffer overflowed and nothing was shipped
+__global__ void __launch_bounds__(256) pack_dirty_group_kernel(const __grid_constant__ HsbTileParams P) {
+  pack_dirty_body(P, TileAll());
+}
+template <int N>
+__global__ void __launch_bounds__(256) pack_dirty_subset_kernel(const __grid_constant__ HsbTileParams P,
+                                                                const __grid_constant__ TileMembers<N> S) {
+  pack_dirty_body(P, S);
+}
+
+// after pack (stream order): the shipped blocks' rectangles are forgotten, a deferred block's are kept.  One thread per
+// (block, level, coordinate); the block's member and start come from the group header (a single handle: member 0, 0).
 __global__ void reset_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  const int* hdr = reinterpret_cast<const int*>(P.buf);
-  if (hdr[2] != 0) return;
-  const int l = threadIdx.x >> 2, k = threadIdx.x & 3;
-  if (l < P.levels) P.lv[l].dirty[k] = (k < 2) ? INT_MAX : -1;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int per = 4 * P.levels, k = i / per;
+  if (k >= P.K) return;
+  const int* gh = reinterpret_cast<const int*>(P.buf);
+  const int member = P.table ? gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k] : 0;
+  const unsigned long long start = P.table ? (unsigned)gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k + 1] : 0u;
+  if (reinterpret_cast<const int*>(P.buf + start)[2] != 0) return;
+  const int l = (i - k * per) >> 2, q = i & 3;
+  tile_levels(P, member)[l].dirty[q] = (q < 2) ? INT_MAX : -1;
 }
+
+// Unpack, pass 1: the buffer fits the replica (group header and every block's header inside the capacity, every shipped
+// block's rows too), evaluated identically by every CTA.  Reads block j of the chunk into c (rectangles, start, member,
+// ship, cells).  A deferred block carries no rows: its rectangles may be larger than the whole buffer (that is why it
+// was deferred) and are not checked against it.
+__device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChunk& c, int k, int j) {
+  const int* gh = reinterpret_cast<const int*>(P.buf);
+  int member = 0;
+  unsigned long long start = 0;
+  if (P.table) {
+    member = gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k];
+    start = (unsigned)gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k + 1];
+    if (member < 0 || member >= P.M) return false;
+  }
+  if (start + HSB_TILE_HEADER_WORDS > P.capacity_words) return false;
+  const int* hdr = reinterpret_cast<const int*>(P.buf + start);
+  if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != P.levels) return false;
+  const bool ship = hdr[2] == 0;
+  unsigned long long cells = 0;
+  unsigned rows = 0;
+  for (int l = 0; l < P.levels; ++l) {
+    const int4 q = make_int4(hdr[4 + 4 * l], hdr[5 + 4 * l], hdr[6 + 4 * l], hdr[7 + 4 * l]);
+    c.rect[j][l] = q;
+    if (!ship) continue;
+    const long long w = tile_w(q), h = tile_h(q);
+    if (w > P.capacity_words || h > P.capacity_words) return false;   // (keeps w * h and the sums below in 64 bits)
+    cells += (unsigned long long)(w * h);
+    rows += (unsigned)h;
+  }
+  if (ship && start + HSB_TILE_HEADER_WORDS + cells > P.capacity_words) return false;
+  c.start[j] = start;
+  c.cells[j] = cells;
+  c.member[j] = member;
+  c.ship[j] = ship ? 1 : 0;
+  c.row0[j + 1] = ship ? rows : 0u;
+  return true;
+}
+
 __global__ void __launch_bounds__(256) unpack_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  const int* hdr = reinterpret_cast<const int*>(P.buf);
-  if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != P.levels || hdr[2] != 0) {
+  __shared__ TileChunk c;
+  const int* gh = reinterpret_cast<const int*>(P.buf);
+  int K = 1;
+  bool fits = true;
+  if (P.table) {
+    fits = P.capacity_words >= HSB_TILE_GROUP_FIXED_WORDS && gh[0] == HSB_TILE_GROUP_MAGIC && gh[2] == P.levels &&
+           gh[1] >= 0 && gh[1] <= P.M;
+    if (fits) {
+      K = gh[1];
+      fits = hsb_tile_group_header_words(K) <= P.capacity_words;
+    }
+  }
+  for (int k0 = 0; fits && k0 < K; k0 += kTileChunk) {
+    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
+    const bool ok = j >= n || tile_read_block(P, c, k0 + j, j);
+    fits = __syncthreads_and(ok);
+  }
+  if (!fits) {   // nothing from a buffer that does not fit is applied; counted once on handles[0]
     if (blockIdx.x == 0 && threadIdx.x == 0 && P.error_count) atomicAdd(P.error_count, 1);
     return;
   }
-  TileLayout t;
-  tile_layout_from(hdr + 4, P.levels, t);
-  const unsigned total = t.off[P.levels];
-  if ((unsigned long long)total + HSB_TILE_HEADER_WORDS > P.capacity_words) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && P.error_count) atomicAdd(P.error_count, 1);
-    return;
-  }
-  if (blockIdx.x == 0 && threadIdx.x < P.levels && t.w[threadIdx.x] > 0) {   // the replica's host mirror has to follow
-    const int l = threadIdx.x;
-    int* md = P.lv[l].dirty + 4;
-    atomicMin(md + 0, t.x0[l]); atomicMin(md + 1, t.y0[l]);
-    atomicMax(md + 2, t.x0[l] + t.w[l] - 1); atomicMax(md + 3, t.y0[l] + t.h[l] - 1);
-  }
-  const float* in = P.buf + HSB_TILE_HEADER_WORDS;
-  for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    int l = 0;
-    while (i >= t.off[l + 1]) ++l;
-    const unsigned k = i - t.off[l];
-    const unsigned r = k / (unsigned)t.w[l], c = k - r * (unsigned)t.w[l];
-    const int x = t.x0[l] + (int)c, y = t.y0[l] + (int)r;
-    if (x < 0 || y < 0 || x >= P.lv[l].sx || y >= P.lv[l].sy) continue;   // a foreign geometry must not write out of bounds
-    const size_t off = (size_t)y * P.lv[l].sx + x;
-    const float v = in[i];
-    P.lv[l].logodds[off] = v;
-    const float p = prob_from_logodds(v);
-    P.lv[l].prob[off] = p;
-    if (P.lv[l].surf) surf2Dwrite(p, P.lv[l].surf, x * (int)sizeof(float), y);
+  for (int k0 = 0; k0 < K; k0 += kTileChunk) {
+    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
+    if (j < n) tile_read_block(P, c, k0 + j, j);
+    __syncthreads();
+    if (threadIdx.x < 32) tile_row_prefix(c, n);
+    if (blockIdx.x == 0 && j < n) {
+      const int m = c.member[j];
+      if (!c.ship[j]) {   // a deferred block: counted once on its member's counter
+        int* cnt = tile_counter(P, m);
+        if (cnt) atomicAdd(cnt, 1);
+      } else {            // the replica's host mirror has to follow
+        const HsbTileLevelDev* lv = tile_levels(P, m);
+        for (int l = 0; l < P.levels; ++l) {
+          const int4 q = c.rect[j][l];
+          if (!tile_dirty(q)) continue;
+          int* md = lv[l].dirty + 4;
+          atomicMin(md + 0, q.x); atomicMin(md + 1, q.y);
+          atomicMax(md + 2, q.z); atomicMax(md + 3, q.w);
+        }
+      }
+    }
+    __syncthreads();
+    tile_rows<false>(P, c, n);
+    __syncthreads();
   }
 }
 

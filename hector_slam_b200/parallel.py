@@ -213,3 +213,22 @@ def broadcast_dirty_tiles_async(rep, buf: torch.Tensor, src: int = 0, group=None
     dist.broadcast(buf, src=src, group=group)
     if dist.get_rank(group) != src:
         rep.unpack_dirty_device(buf.data_ptr(), nbytes, stream)
+
+
+def broadcast_group_dirty_tiles_async(group, buf: torch.Tensor, src: int = 0, members=None, pg=None) -> None:
+    """The group form of broadcast_dirty_tiles_async: the owner rank packs every listed member's dirty tiles into `buf`
+    with one launch (SlamGroup.pack_dirty_device: a group header, then one block per session, rows placed first-fit),
+    ONE fixed-size broadcast moves it, and the replica ranks apply it to their group with one launch
+    (SlamGroup.unpack_dirty_device), which must list its handles in the owner group's order.  One collective per tick
+    whatever the number of robots, nothing read back, nothing synchronised.  A member whose rows did not fit is deferred:
+    it keeps its rectangles on the owner and ships with the next call; its replica counts it
+    (reps[k].replication_overflows()).  `members` (owner side): pack only these members, in session order."""
+    if not dist.is_initialized() or dist.get_world_size(pg) == 1:
+        return
+    nbytes = buf.numel() * 4
+    stream = torch.cuda.current_stream(buf.device).cuda_stream if buf.is_cuda else 0   # (CPU tensors: the gloo tests)
+    if dist.get_rank(pg) == src:
+        group.pack_dirty_device(buf.data_ptr(), nbytes, True, stream, members=members)
+    dist.broadcast(buf, src=src, group=pg)
+    if dist.get_rank(pg) != src:
+        group.unpack_dirty_device(buf.data_ptr(), nbytes, stream)

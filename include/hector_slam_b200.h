@@ -681,6 +681,37 @@ int hsb_pack_dirty_device(hsb_handle* h, float* d_buf, size_t capacity_bytes, in
 int hsb_unpack_dirty_device(hsb_handle* h, const float* d_buf, size_t capacity_bytes, void* stream);
 int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset);
 
+/* The same transport for a group: K sessions' dirty tiles in ONE buffer, one pack launch (plus one with `reset`) and one
+ * unpack launch, counted on handles[0], whatever K is; nothing is synchronised or copied to the host.  Session k packs
+ * member members[k] (hsb_group_pack_dirty_device: every member in order).
+ * Buffer, in 4-byte words: a group header of G words — [0] group magic 0x48534247, [1] K, [2] levels, [3] deferred
+ * blocks, [4] words used, then K pairs {member index in the group, word offset of its block}, zero-padded to
+ * G = 5 + 2K rounded up to a multiple of 4 — then K blocks in session order.  Each block is exactly the buffer
+ * hsb_pack_dirty_device writes for that member alone (256-byte header, then its rows), so one block can also be applied
+ * with hsb_unpack_dirty_device.  Every block's header is written; the words left (capacity - G - 64 K) go to the
+ * blocks' rows first-fit in session order: a block whose rows fit behind those already placed is shipped, one whose
+ * rows do not is deferred (overflow = 1, no rows) and later blocks may still ship.  A deferred member keeps its
+ * replication rectangles even with `reset` (the next pack ships the union); `reset` clears the shipped members' ones.
+ * Mirror rectangles on the owner are not touched.  Only a member larger than the whole buffer needs the two-step
+ * protocol.
+ * hsb_group_unpack_dirty_device applies every shipped block on member `member index` of g (a replica group listing its
+ * handles in the owner group's order) as hsb_unpack_dirty_device does (log-odds, probability, texture twin, mirror
+ * rectangle; the replication rectangle stays clean) and counts a deferred block once on that member's
+ * hsb_get_replication_overflows counter.  A buffer that does not fit g (wrong magic, another level count, a member index
+ * >= M, a block offset or size past the capacity) is counted once on handles[0]'s counter and nothing of it is applied.
+ * Ordering, with `stream` in the role hsb_pack_dirty_device gives it: pack runs after everything queued on the listed
+ * members (including a pending step of any group they belong to, so a pack right after a nowait step ships its map
+ * write) and their next map write waits for it; a member not listed is neither read nor changed.  Unpack runs after
+ * everything queued on every member of g (all their streams) and everything a member queues afterwards waits for it.
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued: K < 0 or K > M; members == NULL with K > 0; an index
+ * outside [0, M) or listed twice (the message names the session); a subset of more than 4096 sessions; d_buf == NULL; a
+ * capacity below 4 (G + 64 K) bytes (unpack: below one block's, 4 (8 + 64)); the message names the minimum.  K = 0
+ * returns HSB_OK and queues nothing. */
+int hsb_group_pack_dirty_device(hsb_group* g, float* d_buf, size_t capacity_bytes, int reset, void* stream);
+int hsb_group_pack_dirty_device_subset(hsb_group* g, int K, const int* members, float* d_buf, size_t capacity_bytes,
+                                       int reset, void* stream);
+int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capacity_bytes, void* stream);
+
 /* ---- after the path: what the node does with the results -------------------------------------*/
 /* nav_msgs/OccupancyGrid cell values of one level, as HectorMappingRos::publishMap derives them
  * (hector_mapping/src/HectorMappingRos.cpp:448-468): 0 where the cell is free (log-odds < 0,
