@@ -47,6 +47,7 @@ EXPORTED = [
     "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
     "hsb_group_match_batch", "hsb_group_match_batch_subset",
     "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
+    "hsb_group_create_mixed",
 ]
 
 
@@ -192,6 +193,7 @@ def load_library() -> C.CDLL:
     sig("hsb_pack_rect_device", i, vp, i, vp, vp, vp)
     sig("hsb_unpack_rect_device", i, vp, i, vp, vp, vp)
     sig("hsb_group_create", i, vp, i, C.POINTER(vp))
+    sig("hsb_group_create_mixed", i, vp, i, C.POINTER(vp))
     sig("hsb_group_destroy", i, vp)
     sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
     sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
@@ -931,15 +933,18 @@ class MapRepB200:
 class SlamGroup:
     """HectorSlamProcessor::update for several MapRepB200 handles — one SLAM session, one map each — in one device pass
     (hsb_group_slam_update).  Each session's results and its handle's state equal a slam_update() on that handle bit for
-    bit.  The group does not own the handles: close() it before closing any of them."""
+    bit.  The group does not own the handles: close() it before closing any of them.
+    mixed=True (hsb_group_create_mixed): the handles may differ in map size, resolution and start; every call then takes
+    each member's own sizes (grids, cell units, world-to-map transforms)."""
 
-    def __init__(self, reps):
+    def __init__(self, reps, mixed: bool = False):
         self.lib = load_library()
         self.reps = list(reps)
         self.M = len(self.reps)
         arr = (C.c_void_p * max(1, self.M))(*[None if r is None else r.h for r in self.reps])
         g = C.c_void_p()
-        st = self.lib.hsb_group_create(C.cast(arr, C.c_void_p), self.M, C.byref(g))
+        create = self.lib.hsb_group_create_mixed if mixed else self.lib.hsb_group_create
+        st = create(C.cast(arr, C.c_void_p), self.M, C.byref(g))
         if st != 0:
             raise HsbError(st, (self.lib.hsb_last_error(None) or b"").decode())
         self.g = g
@@ -1043,18 +1048,18 @@ class SlamGroup:
 
     def sync_occupancy(self, level: int, grids, members=None, reset: bool = True):
         """publishMap for the members in one pass (hsb_group_sync_occupancy): grids are one C-contiguous int8
-        (size_y, size_x) array per session, kept by the caller between calls; the cells of each member's mirror
-        rectangle are rewritten in place, no other byte is touched.  members as in slam_update
+        (size_y, size_x) array per session, its member's own level size, kept by the caller between calls; the cells of
+        each member's mirror rectangle are rewritten in place, no other byte is touched.  members as in slam_update
         (hsb_group_sync_occupancy_subset).  -> one (x0, y0, x1, y1) per session, or None where the map did not change."""
         K, mem = self._sessions(members)
         assert len(grids) == K, (len(grids), K)
-        shape = None
-        if 0 <= level < self.reps[0].levels:   # (an invalid level is the C call's rejection)
-            sx, sy, _ = self.reps[0].level_info(level)
-            shape = (sy, sx)
-        for a in grids:
+        sel = range(K) if mem is None else mem
+        for k, (m, a) in enumerate(zip(sel, grids)):
             assert isinstance(a, np.ndarray) and a.dtype == np.int8 and a.flags.c_contiguous, "grids: C-contiguous int8"
-            assert shape is None or a.shape == shape, (a.shape, shape)
+            rep = self.reps[m] if 0 <= m < self.M else None   # (a bad member or level is the C call's rejection)
+            if rep is not None and 0 <= level < rep.levels:
+                sx, sy, _ = rep.level_info(level)
+                assert a.shape == (sy, sx), (k, a.shape, (sy, sx))
         arr = (C.c_void_p * max(1, K))(*[a.ctypes.data for a in grids])
         rects = np.zeros((max(1, K), 4), np.int32)
         if mem is None:

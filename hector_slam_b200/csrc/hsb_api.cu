@@ -2111,7 +2111,7 @@ constexpr size_t kScoreChunk = 1 << 20;   // most bytes of points score_query st
 // other device scan the caller knows of.  One host-to-device copy from the pinned staging hs (points past kScoreChunk
 // bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K arg-max accumulators are
 // `best`), one device-to-host copy of the asked-for results and one synchronise.  The launches and any error are
-// counted on h, whose level gives the cell length (every member's geometry is h's).
+// counted on h.  sessions() also gives each session its member's cell length of `level` (the covariance's world matrix).
 template <typename Sessions>
 int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage, const HsbLevelDev* lv,
                 int levels, int level, ScoreKind kind, int K, int Q, const float* poses, const float* pts, size_t n_pts,
@@ -2158,7 +2158,6 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   P.sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
   P.pose_offsets = reinterpret_cast<const int*>(ds + o_off);
   P.poses = reinterpret_cast<const float*>(ds + o_poses);
-  P.cell_length = h->lv[level].cell_length;
   P.levels = lv ? levels : 1;
   P.level = lv ? level : 0;
   P.K = K;
@@ -2216,6 +2215,7 @@ int single_score(hsb_handle* h, ScoreKind kind, int level, int B, const float* p
       sess[k].pts = staged + (offsets ? offsets[k] : 0);
       sess[k].n = offsets ? offsets[k + 1] - offsets[k] : n;
       sess[k].member = 0;
+      sess[k].cell_length = h->lv[level].cell_length;
       pose_offsets[k] = k;
     }
     pose_offsets[K] = B;
@@ -2397,22 +2397,38 @@ int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset) {
   return HSB_OK;
 }
 
+// h's level as a ray query sees it (HsbRayLevelDev): getDist's transform computed exactly as the single calls have
+// always computed it.
+static void fill_ray_level(const hsb_handle* h, int level, HsbRayLevelDev& d) {
+  const Level& L = h->lv[level];
+  float origo[2];
+  hsb_get_map_origin(h, level, origo);
+  volatile float inv_scale = 1.0f / L.cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
+  d.plane = L.logodds;
+  d.sx = L.sx;
+  d.sy = L.sy;
+  d.origo_x = origo[0];
+  d.origo_y = origo[1];
+  d.scale = L.cell_length;
+  d.inv_scale = inv_scale;
+}
+
 // Every ray query's host body (hsb_raycast_batch, hsb_get_dist_batch and their group forms): Q = offsets[K] rays of K
-// sessions, session k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`, found in the device
-// table planes[member * levels + level] — or, with planes NULL, h's own plane of `level`, staged with the rays as a
-// one-entry table.  One host-to-device copy of member list, offsets, (plane) and rays from the pinned staging hs, one
-// launch on `st`, one device-to-host copy of the results into the staging and one synchronise; the results are then
-// copied into the caller's arrays on the host.  The launch and any error are counted on h, whose level gives the
-// geometry and getDist's transform (every member's geometry is h's).  world: getDist rays, otherwise ray-cast rays.
+// sessions, session k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s level `level`, described by the
+// device table lv[member * levels + level] (plane, size, getDist's transform) — or, with lv NULL, h's own level, staged
+// with the rays as a one-entry table.  One host-to-device copy of member list, offsets, (level) and rays from the pinned
+// staging hs, one launch on `st`, one device-to-host copy of the results into the staging and one synchronise; the
+// results are then copied into the caller's arrays on the host.  The launch and any error are counted on h.
+// world: getDist rays, otherwise ray-cast rays.
 static int ray_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage,
-                     const float* const* planes, int levels, int level, bool world, int K, const int* members,
+                     const HsbRayLevelDev* lv, int levels, int level, bool world, int K, const int* members,
                      const int* offsets, const void* begin, const void* end, float* out_dist, void* out_hit,
                      int* out_found) {
   const int Q = offsets[K];
-  // staging: member list | offsets | (plane) | begin | end, then the results: dist | hit | found (getDist)
+  // staging: member list | offsets | (level) | begin | end, then the results: dist | hit | found (getDist)
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_off = al((size_t)K * 4), o_plane = al(o_off + (size_t)(K + 1) * 4);
-  const size_t o_begin = planes ? o_plane : o_plane + 16;
+  const size_t o_off = al((size_t)K * 4), o_lv = al(o_off + (size_t)(K + 1) * 4);
+  const size_t o_begin = lv ? o_lv : al(o_lv + sizeof(HsbRayLevelDev));
   const size_t o_end = o_begin + (size_t)Q * 8, o_dist = al(o_end + (size_t)Q * 8);
   const size_t o_hit = al(o_dist + (size_t)Q * 4), o_found = o_hit + (size_t)Q * 8;
   const size_t out_end = out_found ? o_found + (size_t)Q * 4 : out_hit ? o_found : o_dist + (size_t)Q * 4;
@@ -2423,14 +2439,17 @@ static int ray_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_
   char* ds = static_cast<char*>(d_stage.p);
   memcpy(hs, members, (size_t)K * 4);
   memcpy(hs + o_off, offsets, (size_t)(K + 1) * 4);
-  if (!planes) memcpy(hs + o_plane, &h->lv[level].logodds, sizeof(float*));
+  if (!lv) {
+    HsbRayLevelDev R;
+    fill_ray_level(h, level, R);
+    memcpy(hs + o_lv, &R, sizeof(R));
+  }
   memcpy(hs + o_begin, begin, (size_t)Q * 8);
   memcpy(hs + o_end, end, (size_t)Q * 8);
   HSB_CUDA(h, cudaMemcpyAsync(ds, hs, o_end + (size_t)Q * 8, cudaMemcpyHostToDevice, st));
 
-  const Level& L = h->lv[level];
   HsbRayParams P;
-  P.planes = planes ? planes : reinterpret_cast<const float* const*>(ds + o_plane);
+  P.lv = lv ? lv : reinterpret_cast<const HsbRayLevelDev*>(ds + o_lv);
   P.members = reinterpret_cast<const int*>(ds);
   P.offsets = reinterpret_cast<const int*>(ds + o_off);
   P.begin = ds + o_begin;
@@ -2438,19 +2457,10 @@ static int ray_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_
   P.out_dist = reinterpret_cast<float*>(ds + o_dist);
   P.out_hit = out_hit ? ds + o_hit : nullptr;
   P.out_found = out_found ? reinterpret_cast<int*>(ds + o_found) : nullptr;
-  P.levels = planes ? levels : 1;
-  P.level = planes ? level : 0;
-  P.sx = L.sx;
-  P.sy = L.sy;
+  P.levels = lv ? levels : 1;
+  P.level = lv ? level : 0;
   P.K = K;
   P.Q = Q;
-  float origo[2];
-  hsb_get_map_origin(h, level, origo);
-  volatile float inv_scale = 1.0f / L.cell_length;   // CoordinateTransformer::setTransforms, HectorMapTools.h:64
-  P.origo_x = origo[0];
-  P.origo_y = origo[1];
-  P.scale = L.cell_length;
-  P.inv_scale = inv_scale;
   const int blocks = std::min((Q + 7) / 8, h->sm_count * 8);
   if (world) hsb::ray_kernel<true><<<blocks, 256, 0, st>>>(P);
   else hsb::ray_kernel<false><<<blocks, 256, 0, st>>>(P);
@@ -2528,7 +2538,7 @@ int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
 // (stamp bases, writer slots, the last match's container size and origo) is advanced here exactly as it advances there.
 
 struct hsb_group {
-  std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create was given them
+  std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create(_mixed) was given them
   std::vector<int> all;            // 0 .. M-1: the member list of a step of every member
   std::vector<unsigned char> listed;   // scratch of a step's member-list check, M flags
   int device = 0;
@@ -2557,9 +2567,10 @@ struct hsb_group {
   DevBuf d_occ_rows;
   int8_t* h_occ_rows = nullptr;
   size_t h_occ_rows_bytes = 0;
-  // ray queries (hsb_group_raycast, hsb_group_get_dist): M x levels pointers to the members' log-odds planes,
-  // member-major like d_lv; the call's staging (member list, offsets and rays, then the results), pinned and on the device
-  float** d_planes = nullptr;
+  // ray queries (hsb_group_raycast, hsb_group_get_dist): M x levels descriptors of the members' levels (plane, size,
+  // getDist's transform), member-major like d_lv; the call's staging (member list, offsets and rays, then the results),
+  // pinned and on the device
+  HsbRayLevelDev* d_ray_lv = nullptr;
   float* h_ray_stage = nullptr;
   size_t h_ray_stage_bytes = 0;
   DevBuf d_ray_stage;
@@ -2615,7 +2626,7 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->d_occ_rows.p) cudaFree(g->d_occ_rows.p);
   if (g->h_occ_meta) cudaFreeHost(g->h_occ_meta);
   if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
-  if (g->d_planes) cudaFree(g->d_planes);
+  if (g->d_ray_lv) cudaFree(g->d_ray_lv);
   if (g->d_best) cudaFree(g->d_best);
   if (g->d_tile_lv) cudaFree(g->d_tile_lv);
   if (g->d_tile_counters) cudaFree(g->d_tile_counters);
@@ -2633,36 +2644,58 @@ int hsb_group_destroy(hsb_group* g) {
   return HSB_OK;
 }
 
-int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
-  if (!out) return group_fail(nullptr, HSB_ERR_INVALID_ARG, "hsb_group_create: out is NULL");
+}  // extern "C"
+
+namespace {
+
+// hsb_group_create (mixed = false: every member has handles[0]'s geometry) and hsb_group_create_mixed (members may
+// differ in map size, resolution and start; everything a group launch shares must still agree).  fn names the entry
+// point in the error messages.
+int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed, const char* fn) {
+  if (!out) return group_fail(nullptr, HSB_ERR_INVALID_ARG, "%s: out is NULL", fn);
   *out = nullptr;
   hsb_handle* h0 = (handles && M > 0) ? handles[0] : nullptr;
-  if (!handles || M < 1) return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: a group needs M >= 1 handles (M = %d)", M);
+  if (!handles || M < 1) return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: a group needs M >= 1 handles (M = %d)", fn, M);
   for (int s = 0; s < M; ++s)
-    if (!handles[s]) return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: handle %d is NULL", s);
+    if (!handles[s]) return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: handle %d is NULL", fn, s);
   {
     std::vector<hsb_handle*> sorted(handles, handles + M);
     std::sort(sorted.begin(), sorted.end());
     if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
-      return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: a handle is listed twice");
+      return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: a handle is listed twice", fn);
   }
   for (int s = 1; s < M; ++s) {
     const hsb_handle* h = handles[s];
     if (h->device != h0->device)
-      return group_fail(h0, HSB_ERR_INVALID_ARG, "hsb_group_create: handle %d is on device %d, handle 0 on device %d", s,
+      return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: handle %d is on device %d, handle 0 on device %d", fn, s,
                         h->device, h0->device);
+    if (mixed) {   // what every group launch shares: the level count, the per-level iteration counts, the gather mode
+      if (h->levels != h0->levels)
+        return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: handle %d has %d levels, handle 0 has %d", fn, s, h->levels,
+                          h0->levels);
+      for (int l = 0; l < h0->levels; ++l)
+        if (h->lv[l].evals != h0->lv[l].evals)
+          return group_fail(h0, HSB_ERR_INVALID_ARG,
+                            "%s: handle %d differs from handle 0 in the resolved max_iterations of level %d (%d, %d)", fn,
+                            s, l, h->lv[l].evals - 1, h0->lv[l].evals - 1);
+      if (h->gather_mode != h0->gather_mode)
+        return group_fail(h0, HSB_ERR_INVALID_ARG,
+                          "%s: handle %d differs from handle 0 in the resolved gather mode (%d, %d)", fn, s,
+                          h->gather_mode, h0->gather_mode);
+      continue;
+    }
     bool same = h->levels == h0->levels && h->cfg.map_size_x == h0->cfg.map_size_x &&
                 h->cfg.map_size_y == h0->cfg.map_size_y && h->cfg.map_resolution == h0->cfg.map_resolution &&
                 h->cfg.start_x == h0->cfg.start_x && h->cfg.start_y == h0->cfg.start_y && h->gather_mode == h0->gather_mode;
     for (int l = 0; same && l < h0->levels; ++l) same = h->lv[l].evals == h0->lv[l].evals;
     if (!same)
       return group_fail(h0, HSB_ERR_INVALID_ARG,
-                        "hsb_group_create: handle %d differs from handle 0 in levels, map size, resolution, start, "
-                        "max_iterations or gather mode", s);
+                        "%s: handle %d differs from handle 0 in levels, map size, resolution, start, "
+                        "max_iterations or gather mode", fn, s);
   }
   DeviceGuard guard(h0->device);
   hsb_group* g = new (std::nothrow) hsb_group();
-  if (!g) return group_fail(h0, HSB_ERR_OUT_OF_MEMORY, "hsb_group_create: out of host memory");
+  if (!g) return group_fail(h0, HSB_ERR_OUT_OF_MEMORY, "%s: out of host memory", fn);
   g->m.assign(handles, handles + M);
   g->all.resize(M);
   for (int s = 0; s < M; ++s) g->all[s] = s;
@@ -2674,7 +2707,7 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
     cudaError_t _e = (expr);                                                                                 \
     if (_e != cudaSuccess) {                                                                                 \
       const int _code = _e == cudaErrorMemoryAllocation ? HSB_ERR_OUT_OF_MEMORY : HSB_ERR_CUDA;              \
-      group_fail(h0, _code, "hsb_group_create: %s failed: %s", #expr, cudaGetErrorString(_e));               \
+      group_fail(h0, _code, "%s: %s failed: %s", fn, #expr, cudaGetErrorString(_e));                         \
       hsb_group_destroy(g);                                                                                  \
       return _code;                                                                                          \
     }                                                                                                        \
@@ -2685,7 +2718,7 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
     HandleScope scope(h);
     const int s = reset_gate(h);
     if (s != HSB_OK) {
-      group_fail(h0, s, "hsb_group_create: %s", h->err.c_str());
+      group_fail(h0, s, "%s: %s", fn, h->err.c_str());
       hsb_group_destroy(g);
       return s;
     }
@@ -2705,11 +2738,11 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
       for (int l = 0; l < g->levels; ++l) mirror[(size_t)s * g->levels + l] = g->m[s]->lv[l].dirty + 4;
     HSB_GROUP_CUDA(cudaMalloc(&g->d_mirror, mirror.size() * sizeof(int*)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_mirror, mirror.data(), mirror.size() * sizeof(int*), cudaMemcpyHostToDevice));
-    std::vector<float*> planes((size_t)M * g->levels);
+    std::vector<HsbRayLevelDev> ray((size_t)M * g->levels);
     for (int s = 0; s < M; ++s)
-      for (int l = 0; l < g->levels; ++l) planes[(size_t)s * g->levels + l] = g->m[s]->lv[l].logodds;
-    HSB_GROUP_CUDA(cudaMalloc(&g->d_planes, planes.size() * sizeof(float*)));
-    HSB_GROUP_CUDA(cudaMemcpy(g->d_planes, planes.data(), planes.size() * sizeof(float*), cudaMemcpyHostToDevice));
+      for (int l = 0; l < g->levels; ++l) fill_ray_level(g->m[s], l, ray[(size_t)s * g->levels + l]);
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_ray_lv, ray.size() * sizeof(HsbRayLevelDev)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_ray_lv, ray.data(), ray.size() * sizeof(HsbRayLevelDev), cudaMemcpyHostToDevice));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_best, (size_t)M * sizeof(unsigned long long)));
     HSB_GROUP_CUDA(cudaMemset(g->d_best, 0, (size_t)M * sizeof(unsigned long long)));
     std::vector<HsbTileLevelDev> tile((size_t)M * g->levels);
@@ -2736,6 +2769,18 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
 #undef HSB_GROUP_CUDA
   *out = g;
   return HSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
+  return group_create(handles, M, out, false, "hsb_group_create");
+}
+
+int hsb_group_create_mixed(hsb_handle* const* handles, int M, hsb_group** out) {
+  return group_create(handles, M, out, true, "hsb_group_create_mixed");
 }
 
 }  // extern "C"
@@ -2997,7 +3042,8 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
 
 // Packed bytes of one device-to-host copy of a group occupancy sync (pinned staging owned by the group).  A larger total
 // goes in chunks split at row boundaries; hsb_set_tuning(handles[0], "occupancy_chunk", bytes) overrides it.  A chunk
-// always holds at least one row.
+// always holds at least one whole row of the widest level among the call's changed members (in a group of one geometry,
+// handles[0]'s row), so every rectangle's row fits one.
 constexpr size_t kOccChunkBytes = 32u << 20;
 
 // publishMap's grid for K members in one pass: gather (and clear) their mirror rectangles of `level` with one launch,
@@ -3019,7 +3065,6 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
 
   // pass 1: the rectangles, gathered and (reset) cleared in order behind the members' queued map writes
   const OccMeta lay(K);
-  const int sx = h0->lv[level].sx;
   memcpy(g->h_occ_meta, members, (size_t)K * sizeof(int));
   HSB_CUDA(h0, cudaMemcpyAsync(g->d_occ_meta, g->h_occ_meta, (size_t)K * sizeof(int), cudaMemcpyHostToDevice, st));
   hsb::gather_mirror_rects_kernel<<<(K + 127) / 128, 128, 0, st>>>(
@@ -3036,7 +3081,7 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
   // the row table of the non-empty rectangles, in session order
   HsbOccRowsDev* rows = reinterpret_cast<HsbOccRowsDev*>(g->h_occ_meta + lay.rows);
   std::vector<int> sess;   // session of each row-table entry
-  int n_rows = 0, total_rows = 0;
+  int n_rows = 0, total_rows = 0, max_sx = 0;
   size_t total = 0;
   for (int k = 0; k < K; ++k) {
     const int* r = rects + 4 * k;
@@ -3044,7 +3089,8 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
     hsb_handle* h = g->m[members[k]];
     HsbOccRowsDev& e = rows[n_rows++];
     e.logodds = h->lv[level].logodds;
-    e.sx = sx;
+    e.sx = h->lv[level].sx;   // (the member's own row pitch: members of a mixed group differ)
+    max_sx = std::max(max_sx, e.sx);
     e.x0 = r[0];
     e.y0 = r[1];
     e.w = r[2] - r[0] + 1;
@@ -3061,7 +3107,7 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
                                cudaMemcpyHostToDevice, st));
 
   // pass 2: chunks of whole rows
-  const size_t cap = std::max<size_t>(h0->tune_occ_chunk > 0 ? (size_t)h0->tune_occ_chunk : kOccChunkBytes, (size_t)sx);
+  const size_t cap = std::max<size_t>(h0->tune_occ_chunk > 0 ? (size_t)h0->tune_occ_chunk : kOccChunkBytes, (size_t)max_sx);
   if (std::min(cap, total) > g->h_occ_rows_bytes) {   // grown geometrically: dirty areas creep up from call to call
     const size_t stage = std::min(cap, std::max(total, 2 * g->h_occ_rows_bytes));
     if (g->h_occ_rows) cudaFreeHost(g->h_occ_rows);
@@ -3104,7 +3150,7 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
       const HsbOccRowsDev& d = rows[ee];
       const int hgt = rects[4 * sess[ee] + 3] - d.y0 + 1;
       for (; yy < hgt && src < g->h_occ_rows + bytes; ++yy, src += d.w)
-        memcpy(grids[sess[ee]] + (size_t)(d.y0 + yy) * sx + d.x0, src, (size_t)d.w);
+        memcpy(grids[sess[ee]] + (size_t)(d.y0 + yy) * d.sx + d.x0, src, (size_t)d.w);
     }
   }
   return HSB_OK;
@@ -3133,7 +3179,7 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
                 world ? "begin_world" : "begin_cells", world ? "end_world" : "end_cells");
   DeviceGuard guard(g->device);
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-  return ray_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_planes, g->levels, level,
+  return ray_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_ray_lv, g->levels, level,
                    world, K, members, offsets, begin, end, out_dist, out_hit, out_found);
 }
 
@@ -3189,6 +3235,7 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
     for (int k = 0; k < K; ++k) {
       hsb_handle* h = g->m[members[k]];
       sess[k].member = members[k];
+      sess[k].cell_length = h->lv[level].cell_length;
       if (last) {   // (a member that never matched has no container: n = 0)
         sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
         sess[k].n = h->d_last_pts.p ? h->last_n : 0;
@@ -3199,7 +3246,7 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
     }
     memcpy(offsets, pose_offsets, (size_t)(K + 1) * 4);
   };
-  // (h0's gather mode is every member's: hsb_group_create checked)
+  // (h0's gather mode is every member's: hsb_group_create(_mixed) checked)
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, level, kind,
                      K, Q, poses, pts, last ? 0 : (size_t)scan_offsets[K], sessions, g->d_best, out_lh, out_map,
                      out_world, out_best4, out_best_index);
@@ -3267,6 +3314,7 @@ int group_match(hsb_group* g, const char* fn, int K, const int* members, const i
   for (int k = 0; k < K; ++k) {
     hsb_handle* h = g->m[members[k]];
     sess[k].member = members[k];
+    sess[k].cell_length = 0.0f;   // (unused by the match)
     if (last) {   // (a member that never matched has no container: n = 0)
       sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
       sess[k].n = h->d_last_pts.p ? h->last_n : 0;
@@ -3293,7 +3341,7 @@ int group_match(hsb_group* g, const char* fn, int K, const int* members, const i
   P.match_sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
   P.match_offsets = reinterpret_cast<const int*>(ds + o_off);
   P.match_K = K;
-  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create checked)
+  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create(_mixed) checked)
   s = HSB_ERR_UNSUPPORTED;
 #define HSB_GM_CASE(w)                                                                                                 \
   if (W == w)                                                                                                          \

@@ -67,6 +67,7 @@ struct HsbScoreSessionDev {
   const float2* pts;   // the session's slice of the staged scans, or the member's last-match container
   int n;
   int member;
+  float cell_length;   // of the member's level of a scoring call (covariance: the world matrix); unused by the match
 };
 
 struct HsbMatchParams {
@@ -227,10 +228,18 @@ struct HsbOccRowsDev {
   size_t off;
 };
 
+// One member's level as a ray query sees it: the log-odds plane, its size, and getDist's transform — the map origin
+// (hsb_get_map_origin), the cell length and 1 / cell length, all computed on the host as the single calls compute them.
+struct HsbRayLevelDev {
+  const float* plane;
+  int sx, sy;
+  float origo_x, origo_y, scale, inv_scale;
+};
+
 // A ray query (ray_kernel: hsb_raycast_batch, hsb_get_dist_batch and their group forms): Q rays of K sessions, session
-// k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s plane of `level`.  Arrays in device memory, in ray order.
+// k's rays [offsets[k], offsets[k+1]) cast on member members[k]'s level `level`.  Arrays in device memory, in ray order.
 struct HsbRayParams {
-  const float* const* planes;   // members x levels log-odds planes, member-major
+  const HsbRayLevelDev* lv;     // members x levels, member-major (hsb_group::d_ray_lv; one entry for a single handle)
   const int* members;           // K
   const int* offsets;           // K + 1
   const void* begin;            // Q: int2 cells (ray cast) or float2 world points (getDist)
@@ -238,8 +247,7 @@ struct HsbRayParams {
   float* out_dist;              // Q
   void* out_hit;                // Q int2 hit cells / float2 hit points, or null
   int* out_found;               // Q (getDist), or null
-  int levels, level, sx, sy, K, Q;
-  float origo_x, origo_y, scale, inv_scale;   // getDist: the level's map origin and cell length, 1 / cell length
+  int levels, level, K, Q;
 };
 
 // A pose-scoring call from host buffers (likelihood_group_kernel, best_group_finish_kernel, covariance_kernel:
@@ -256,7 +264,6 @@ struct HsbScoreParams {
   int* out_best_index;              // K (best hypothesis)
   float* out_map;                   // Q x 9 (covariance), or null
   float* out_world;                 // Q x 9 (covariance), or null
-  float cell_length;                // of the level (covariance: the world matrix)
   int levels, level, K, Q;
 };
 

@@ -1395,14 +1395,14 @@ __device__ __forceinline__ void pose_covariance(const HsbLevelDev& L, const Leve
 
 // N3: OccGridMapUtil::getCovarianceForPose (OccGridMapUtil.h:106-160) + getCovMatrixWorldCoords (:162-187) for
 // hsb_covariance_batch and hsb_group_covariance: one CTA of 7 warps per pose (pose_covariance), the pose's session, scan
-// and member map found as likelihood_group_kernel finds them; every member's cell length is the call's (one geometry).
+// and member map found as likelihood_group_kernel finds them; the world matrix takes the session's member's cell length.
 template <int MODE>
 __global__ void __launch_bounds__(224) covariance_kernel(const HsbScoreParams P) {
   for (int q = blockIdx.x; q < P.Q; q += gridDim.x) {
     const HsbScoreSessionDev s = P.sess[session_of(P.pose_offsets, P.K, q)];
     const HsbLevelDev& L = P.lv[(size_t)s.member * P.levels + P.level];
     const LevelRegs LR = level_regs(L);   // (every warp is whole here: a CTA's threads share q)
-    pose_covariance<MODE>(L, LR, P.poses, q, s.pts, s.n, P.cell_length, P.out_map, P.out_world);
+    pose_covariance<MODE>(L, LR, P.poses, q, s.pts, s.n, s.cell_length, P.out_map, P.out_world);
   }
 }
 

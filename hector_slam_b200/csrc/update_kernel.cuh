@@ -165,9 +165,10 @@ __device__ __forceinline__ float warp_raycast(const float* __restrict__ logodds,
 }
 
 // N4 (hsb_raycast_batch, hsb_get_dist_batch and their group forms): ray q of the call belongs to the session k whose
-// rays are [offsets[k], offsets[k+1]) and is cast on member members[k]'s plane of the level, found through the table
-// planes[member * levels + level] (a single handle's call: one session and a one-entry table).  One warp per ray,
-// grid-stride.  kWorld: getDist rays (float2 world points); otherwise ray-cast rays (int2 cells).
+// rays are [offsets[k], offsets[k+1]) and is cast on member members[k]'s level, whose plane, size and getDist transform
+// are the table entry lv[member * levels + level] (a single handle's call: one session and a one-entry table), so the
+// members of a group may differ in map size, resolution and start.  One warp per ray, grid-stride.  kWorld: getDist rays
+// (float2 world points); otherwise ray-cast rays (int2 cells).
 template <bool kWorld>
 __global__ void __launch_bounds__(256) ray_kernel(const HsbRayParams P) {
   const int lane = threadIdx.x & 31;
@@ -180,7 +181,7 @@ __global__ void __launch_bounds__(256) ray_kernel(const HsbRayParams P) {
       if (P.offsets[mid] <= q) lo = mid;
       else hi = mid - 1;
     }
-    const float* logodds = P.planes[(size_t)P.members[lo] * P.levels + P.level];
+    const HsbRayLevelDev R = P.lv[(size_t)P.members[lo] * P.levels + P.level];
     if (kWorld) {
       // DistanceMeasurementProvider::getDist (HectorMapTools.h:133-147): world -> cell with
       // CoordinateTransformer<float>::getC2Coords ((w - origo) * inv_scale, :93-96) truncated by cast<int> (:136-137; a
@@ -189,28 +190,28 @@ __global__ void __launch_bounds__(256) ray_kernel(const HsbRayParams P) {
       // hit: scale * -1 as in the reference, hit_world = (0, 0) and found = 0 where the reference leaves hitCoords
       // undefined).
       const float2 bw = static_cast<const float2*>(P.begin)[q], ew = static_cast<const float2*>(P.end)[q];
-      const float bx = __fmul_rn(__fsub_rn(bw.x, P.origo_x), P.inv_scale);
-      const float by = __fmul_rn(__fsub_rn(bw.y, P.origo_y), P.inv_scale);
-      const float ex = __fmul_rn(__fsub_rn(ew.x, P.origo_x), P.inv_scale);
-      const float ey = __fmul_rn(__fsub_rn(ew.y, P.origo_y), P.inv_scale);
+      const float bx = __fmul_rn(__fsub_rn(bw.x, R.origo_x), R.inv_scale);
+      const float by = __fmul_rn(__fsub_rn(bw.y, R.origo_y), R.inv_scale);
+      const float ex = __fmul_rn(__fsub_rn(ew.x, R.origo_x), R.inv_scale);
+      const float ey = __fmul_rn(__fsub_rn(ew.y, R.origo_y), R.inv_scale);
       const bool sane = fabsf(bx) < 1.0e9f && fabsf(by) < 1.0e9f && fabsf(ex) < 1.0e9f && fabsf(ey) < 1.0e9f;
       const int2 p0 = sane ? make_int2((int)bx, (int)by) : make_int2(-1, -1);
       const int2 p1 = sane ? make_int2((int)ex, (int)ey) : make_int2(-1, -1);
       int2 hit;
-      const float dist = warp_raycast(logodds, P.sx, P.sy, p0, p1, lane, hit);
+      const float dist = warp_raycast(R.plane, R.sx, R.sy, p0, p1, lane, hit);
       if (lane == 0) {
-        P.out_dist[q] = __fmul_rn(P.scale, dist);
+        P.out_dist[q] = __fmul_rn(R.scale, dist);
         const bool found = dist >= 0.0f;
         if (P.out_found) P.out_found[q] = found ? 1 : 0;
         if (P.out_hit)
           static_cast<float2*>(P.out_hit)[q] =
-              found ? make_float2(__fadd_rn(P.origo_x, __fmul_rn((float)hit.x, P.scale)),
-                                  __fadd_rn(P.origo_y, __fmul_rn((float)hit.y, P.scale)))
+              found ? make_float2(__fadd_rn(R.origo_x, __fmul_rn((float)hit.x, R.scale)),
+                                  __fadd_rn(R.origo_y, __fmul_rn((float)hit.y, R.scale)))
                     : make_float2(0.0f, 0.0f);
       }
     } else {
       int2 hit;
-      const float dist = warp_raycast(logodds, P.sx, P.sy, static_cast<const int2*>(P.begin)[q],
+      const float dist = warp_raycast(R.plane, R.sx, R.sy, static_cast<const int2*>(P.begin)[q],
                                       static_cast<const int2*>(P.end)[q], lane, hit);
       if (lane == 0) {
         P.out_dist[q] = dist;
@@ -797,9 +798,11 @@ __global__ void reset_dirty_kernel(const __grid_constant__ HsbTileParams P) {
 }
 
 // Unpack, pass 1: the buffer fits the replica (group header and every block's header inside the capacity, every shipped
-// block's rows too), evaluated identically by every CTA.  Reads block j of the chunk into c (rectangles, start, member,
-// ship, cells).  A deferred block carries no rows: its rectangles may be larger than the whole buffer (that is why it
-// was deferred) and are not checked against it.
+// block's rows too, and every shipped rectangle inside its level of the member it lands on), evaluated identically by
+// every CTA.  Reads block j of the chunk into c (rectangles, start, member, ship, cells).  A deferred block carries no
+// rows: its rectangles may be larger than the whole buffer (that is why it was deferred) and are not checked.  The
+// level-size check keeps a block packed on a member of another size (an owner group listing its handles in another
+// order than a mixed replica group) from growing a mirror rectangle past the plane it lands on.
 __device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChunk& c, int k, int j) {
   const int* gh = reinterpret_cast<const int*>(P.buf);
   int member = 0;
@@ -813,12 +816,14 @@ __device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChun
   const int* hdr = reinterpret_cast<const int*>(P.buf + start);
   if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != P.levels) return false;
   const bool ship = hdr[2] == 0;
+  const HsbTileLevelDev* lv = tile_levels(P, member);
   unsigned long long cells = 0;
   unsigned rows = 0;
   for (int l = 0; l < P.levels; ++l) {
     const int4 q = make_int4(hdr[4 + 4 * l], hdr[5 + 4 * l], hdr[6 + 4 * l], hdr[7 + 4 * l]);
     c.rect[j][l] = q;
     if (!ship) continue;
+    if (tile_dirty(q) && (q.x < 0 || q.y < 0 || q.z >= lv[l].sx || q.w >= lv[l].sy)) return false;
     const long long w = tile_w(q), h = tile_h(q);
     if (w > P.capacity_words || h > P.capacity_words) return false;   // (keeps w * h and the sums below in 64 bits)
     cells += (unsigned long long)(w * h);

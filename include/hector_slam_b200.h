@@ -385,10 +385,25 @@ int hsb_slam_update_projected(hsb_handle* h, const float pose_hint_world[3], con
  * A group of existing handles stepped together.  The group does not own the handles.  Destroy the group before any of
  * its handles.  Members must have the same geometry: levels, map_size_x/y, map_resolution, start_x/y, the resolved
  * max_iterations of every level and the resolved gather mode, and sit on one device; update factors and the two gate
- * thresholds are per handle and may differ.  A handle may belong to several groups.  Errors of hsb_group_create:
- * hsb_last_error(NULL) and hsb_last_error(handles[0]); of the other group calls: hsb_last_error(handles[0]). */
+ * thresholds are per handle and may differ.  A group made by hsb_group_create_mixed may hold members that differ in
+ * map_size_x/y, map_resolution and start_x/y; every group call then takes each member's own sizes: grids[k] of the
+ * occupancy sync is member k's own size_y x size_x at `level`, session k's endpoints and scans are in member k's own
+ * level-0 cell units, and a world ray, pose or hint is mapped into each member's own grid.  A handle may belong to
+ * several groups.  Errors of hsb_group_create(_mixed): hsb_last_error(NULL) and hsb_last_error(handles[0]); of the other
+ * group calls: hsb_last_error(handles[0]). */
 typedef struct hsb_group hsb_group;
 int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out);
+/* hsb_group_create for members of different maps: robots at different sites, at different resolutions, started at
+ * different map_start_x/y.  Members may differ in map_size_x, map_size_y, map_resolution, start_x and start_y; they must
+ * still agree on the level count, the resolved max_iterations of every level and the resolved gather mode (an
+ * HSB_GATHER_AUTO member larger than the texture limit resolves to LDG), and sit on one device — a mismatch is rejected
+ * with HSB_ERR_INVALID_ARG, the message naming the member and the field.  Every other rejection and error rule of
+ * hsb_group_create applies.  Every group call on such a group has exactly the contract documented for it: each
+ * session's results and each stepped member's end state are bit-identical to the single-handle call on that member, and
+ * a step is still one host-to-device copy and three launches counted on handles[0].  hsb_group_unpack_dirty_device
+ * treats a shipped block whose rectangle on any level lies outside that level of the member it lands on as a buffer
+ * that does not fit the group: counted once on handles[0], nothing of it applied. */
+int hsb_group_create_mixed(hsb_handle* const* handles, int M, hsb_group** out);
 int hsb_group_destroy(hsb_group* g);
 /* HectorSlamProcessor::update for every member at once. Session s is handles[s] with hint hints[3s..], the scan
  * points_xy[offsets[s] .. offsets[s+1]) (level-0 cells, DataContainer layout), origo[2s..] (NULL = 0,0) and
@@ -698,7 +713,9 @@ int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset);
  * handles in the owner group's order) as hsb_unpack_dirty_device does (log-odds, probability, texture twin, mirror
  * rectangle; the replication rectangle stays clean) and counts a deferred block once on that member's
  * hsb_get_replication_overflows counter.  A buffer that does not fit g (wrong magic, another level count, a member index
- * >= M, a block offset or size past the capacity) is counted once on handles[0]'s counter and nothing of it is applied.
+ * >= M, a block offset or size past the capacity, a shipped rectangle outside its level of the member it lands on — in a
+ * mixed group, an owner that lists its handles in another order) is counted once on handles[0]'s counter and nothing of
+ * it is applied.  (The size check only guards bounds: it cannot tell apart two members whose rectangles both fit.)
  * Ordering, with `stream` in the role hsb_pack_dirty_device gives it: pack runs after everything queued on the listed
  * members (including a pending step of any group they belong to, so a pack right after a nowait step ships its map
  * write) and their next map write waits for it; a member not listed is neither read nor changed.  Unpack runs after
