@@ -136,10 +136,10 @@ def assert_same_session(out, i, ref, tag):
         assert K[i] == kept, (tag, i, K[i], kept)
 
 
-def assert_same_state(a, b, tag, probe=True):
+def assert_same_state(a, b, tag, probe=True, levels=LEVELS):
     """Every level's log-odds and probability, the texture twin (probe over the written area), both dirty rectangles
     (read without reset) and the gate pose."""
-    for l in range(LEVELS):
+    for l in range(levels):
         la = a.download_level(l)
         assert np.array_equal(bits(la), bits(b.download_level(l))), (tag, l)
         assert np.array_equal(bits(a.download_prob(l)), bits(b.download_prob(l))), (tag, l)
