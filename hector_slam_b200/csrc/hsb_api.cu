@@ -51,6 +51,35 @@ struct BatchSet {
   bool busy = false;
 };
 
+// Pose, write-the-map flag and covariance of a single-scan match or SLAM step, in the order one copy moves them
+struct PoseResult {
+  float pose[3];
+  float flag;     // the step's gate decision (unused by hsb_match_data)
+  float cov[9];
+};
+
+// The single-scan calls' mapped pinned block (hsb_handle::h_pin): what their kernels write, or their copies bring, for
+// the host.  Every slot is written and read by calls on the handle's stream.
+struct PinnedSlots {
+  PoseResult match;    // hsb_match_data
+  PoseResult step;     // the SLAM steps
+  unsigned step_seq;   // a nowait step's sequence number, published once `step` and step_kept are in place
+  int step_kept;       // a converted step's kept-endpoint count
+  int conv_kept;       // the stand-alone conversions' kept-endpoint count
+  float hessian[12];   // hsb_hessian_derivs: H row-major, then dTr
+  float gate[4];       // the gate state on its way to or from the device: lastMapUpdatePose, write flag
+  int rect[4];         // a dirty rectangle on its way to the host
+};
+
+// The single-scan calls' device block (hsb_handle::d_scratch)
+struct DeviceSlots {
+  PoseResult match;    // hsb_match_data with tuning host_out = 0
+  PoseResult step;     // a SLAM step's pose and flag, which its map write reads (with host_out = 0 also its covariance)
+  int step_kept;       // a converted step's kept-endpoint count, which its map write reads
+  int conv_kept;       // the stand-alone conversions' kept-endpoint count
+  float hessian[12];   // hsb_hessian_derivs
+};
+
 }  // namespace
 
 struct hsb_handle {
@@ -65,7 +94,8 @@ struct hsb_handle {
   cudaStream_t copy_stream[2] = {nullptr, nullptr};
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   // device staging for the host-buffer entry points
-  DevBuf d_pts, d_scratch;
+  DevBuf d_pts;
+  DeviceSlots* d_scratch = nullptr;
   // "containers of the last match" (MapRepMultiMap::dataContainers) and the update scan
   DevBuf d_last_pts, d_upd_pts;   // single-scan buffers: 16 floats of header (hint, gate inputs), then the points
   float* h_stage = nullptr;       // pinned staging for the single-scan calls (header + points, one H2D per call)
@@ -84,8 +114,8 @@ struct hsb_handle {
   int last_n = 0;
   float last_origo[2] = {0.f, 0.f};
   // pinned host scratch
-  float* h_pin = nullptr;  // 64 floats, mapped: kernels of the single-scan calls write their results here
-  float* h_pin_dev = nullptr;    // device alias of h_pin
+  PinnedSlots* h_pin = nullptr;       // mapped: kernels of the single-scan calls write their results here
+  PinnedSlots* h_pin_dev = nullptr;   // device alias of h_pin
   int shape_batch = 0;           // > 0: pick the launch shape for this batch size instead of the launch's own (pipelined host calls)
   int tune_host_out = 1;         // single-scan calls: kernels write results into mapped host memory (no D2H copy)
   int tune_inline_scan = 0;      // 1: single-scan calls send the scan in the kernel parameters (no H2D copy operation) — measured slower, see match_kernel.cuh
@@ -97,7 +127,7 @@ struct hsb_handle {
   int* d_dirty_all = nullptr;   // HSB_MAX_LEVELS x 8 ints, see Level::dirty
   uint64_t d2h_bytes = 0;       // bytes the plane / rectangle download entry points copied to the host (diagnostic)
   cudaEvent_t ev_sync[4] = {nullptr, nullptr, nullptr, nullptr};   // ordering of caller streams against the handle's own
-  DevBuf d_gate;           // fused SLAM step: lastMapUpdatePose[3], write-the-map flag
+  float* d_gate = nullptr;   // SLAM steps: lastMapUpdatePose[3], write-the-map flag
   float min_dist = 0.4f, min_angle = 0.13f;   // HectorSlamProcessor.h:62-63 defaults
   // tuning
   int tune_warps_per_scan = 0, tune_scans_per_block = 0, tune_stage_smem = 1, tune_chunk = 0, tune_unroll = 0, tune_packed = 0, tune_seq = 0, tune_partial = 1, tune_prefetch = 0, tune_trace = 0, tune_pace = 0, tune_pdl = 1, tune_auto_group = 1, tune_stagger = 0, tune_fixpoint = 1;
@@ -584,6 +614,14 @@ int destroy_level(hsb_handle* h, Level& L) {
   return HSB_OK;
 }
 
+// lastMapUpdatePose = FLT_MAX^3 (HectorSlamProcessor.h:117), write flag 0
+int reset_gate(hsb_handle* h) {
+  const float init[4] = {FLT_MAX, FLT_MAX, FLT_MAX, 0.f};
+  memcpy(h->h_pin->gate, init, sizeof(init));
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_gate, h->h_pin->gate, sizeof(init), cudaMemcpyHostToDevice, h->stream));
+  return HSB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -691,11 +729,13 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
   for (int i = 0; i < 2; ++i) HSB_CUDA_C(cudaEventCreate(&h->ev_time[i]));
   HSB_CUDA_C(cudaMalloc(&h->d_dirty_all, (HSB_MAX_LEVELS * 8 + 4) * sizeof(int)));   // + the replication error counter
   HSB_CUDA_C(cudaMemset(h->d_dirty_all, 0, (HSB_MAX_LEVELS * 8 + 4) * sizeof(int)));
-  HSB_CUDA_C(cudaHostAlloc(&h->h_pin, 64 * sizeof(float), cudaHostAllocMapped));
+  HSB_CUDA_C(cudaHostAlloc(&h->h_pin, sizeof(PinnedSlots), cudaHostAllocMapped));
   HSB_CUDA_C(cudaHostGetDevicePointer(&h->h_pin_dev, h->h_pin, 0));
-  // pinned memory comes back from earlier allocations with their contents: a nowait step polls h_pin[22] for its
+  // pinned memory comes back from earlier allocations with their contents: a nowait step polls step_seq for its
   // sequence number (1, 2, ...), which must not be there before the step publishes it
-  memset(h->h_pin, 0, 64 * sizeof(float));
+  memset(h->h_pin, 0, sizeof(PinnedSlots));
+  HSB_CUDA_C(cudaMalloc(&h->d_scratch, sizeof(DeviceSlots)));
+  HSB_CUDA_C(cudaMalloc(&h->d_gate, 4 * sizeof(float)));
 
   h->gather_mode = cfg->gather_mode == HSB_GATHER_LDG ? HSB_GATHER_LDG : HSB_GATHER_TEX;  // AUTO -> TEX (measured faster)
   // The texture twin is a CUDA array with texture gather, whose extent the device limits (maxTexture2DGather, 32768 x
@@ -778,6 +818,7 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
     for (int i = 0; i < HSB_MAX_LEVELS * 8; ++i) clean[i] = (i & 2) ? -1 : INT_MAX;
     HSB_CUDA_C(cudaMemcpyAsync(h->d_dirty_all, clean, sizeof(clean), cudaMemcpyHostToDevice, h->stream));
   }
+  HSB_TRY(reset_gate(h));
   HSB_CUDA_C(cudaStreamSynchronize(h->stream));
 #undef HSB_TRY
 #undef HSB_CUDA_C
@@ -790,7 +831,7 @@ int hsb_destroy(hsb_handle* h) {
   HandleScope guard(h);
   cudaDeviceSynchronize();
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
-  DevBuf* bufs[] = {&h->d_pts, &h->d_scratch, &h->d_gate, &h->d_last_pts, &h->d_upd_pts,
+  DevBuf* bufs[] = {&h->d_pts, &h->d_last_pts, &h->d_upd_pts,
                     &h->d_beam_cs, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
                     &h->d_conv_in, &h->d_cloud_tf, &h->d_fused_in, &h->d_proj_unit};
   for (DevBuf* b : bufs)
@@ -806,6 +847,8 @@ int hsb_destroy(hsb_handle* h) {
       if (S.chunk_ready[i]) cudaEventDestroy(S.chunk_ready[i]);
   }
   if (h->d_dirty_all) cudaFree(h->d_dirty_all);
+  if (h->d_scratch) cudaFree(h->d_scratch);
+  if (h->d_gate) cudaFree(h->d_gate);
   for (int i = 0; i < 2; ++i)
     if (h->ev_time[i]) cudaEventDestroy(h->ev_time[i]);
   for (int i = 0; i < 4; ++i)
@@ -838,16 +881,6 @@ static int upload_scan(hsb_handle* h, DevBuf& b, const float* header, int nh, co
   if (nh > 0) memcpy(h->h_stage, header, (size_t)nh * sizeof(float));
   if (n > 0) memcpy(h->h_stage + kScanHeaderFloats, pts, (size_t)n * 8);
   HSB_CUDA(h, cudaMemcpyAsync(b.p, h->h_stage, bytes, cudaMemcpyHostToDevice, st));
-  return HSB_OK;
-}
-
-// lastMapUpdatePose = FLT_MAX^3 (HectorSlamProcessor.h:117) for the fused step
-static int reset_gate(hsb_handle* h) {
-  int s = ensure(h, h->d_gate, 4 * sizeof(float));
-  if (s != HSB_OK) return s;
-  const float init[4] = {FLT_MAX, FLT_MAX, FLT_MAX, 0.f};
-  memcpy(h->h_pin + 56, init, sizeof(init));
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_gate.p, h->h_pin + 56, sizeof(init), cudaMemcpyHostToDevice, h->stream));
   return HSB_OK;
 }
 
@@ -981,6 +1014,62 @@ void fill_conv(const hsb_handle* h, HsbInputKind kind, HsbConvDev& c) {
   }
 }
 
+// The scan of n endpoints (converted input: an upper bound until the kept count is known) with container origo `origo`
+// (NULL = 0, 0) is the last match's container now (MapRepMultiMap::matchData, MapRepMultiMap.h:127): a later
+// updateByScan draws the coarse levels from it (:143).
+void record_match(hsb_handle* h, int n, const float origo[2]) {
+  h->last_n = n;
+  h->last_origo[0] = origo ? origo[0] : 0.f;
+  h->last_origo[1] = origo ? origo[1] : 0.f;
+}
+
+// One scan of a SLAM step (HectorSlamProcessor::update), as the single and the group steps take it.
+struct StepSession {
+  float origo[2];     // the container origo
+  float gate_in[3];   // minDist, minAngle, map_without_matching
+  // where the scan's endpoints go: the last match's container when the scan is matched; without matching the
+  // reference leaves that container alone (HectorSlamProcessor.h:77-81, MapRepMultiMap.h:143) and they go to the
+  // update-scan buffer
+  DevBuf* sink;
+  HsbConvDev conv;    // converted input: h's conversion into the sink; zero for endpoints
+};
+
+// The session of a step of h on a scan of `kind` with n inputs (converted: an upper bound of the endpoints kept), laser
+// transform T (cloud and projected) or caller origo (endpoints; NULL = 0, 0), matched or map_without_matching.  The
+// sink is grown to n endpoints; a converted scan's kept count goes to n_dev (device) and, if set, n_host (mapped host).
+int step_session(hsb_handle* h, HsbInputKind kind, int n, const double* T, const float origo[2], bool matched, int* n_dev,
+                 int* n_host, StepSession& ss) {
+  ss.origo[0] = ss.origo[1] = 0.f;
+  if (T) cloud_origo(h, T, ss.origo);   // (a LaserScan's origo is zero, HectorMappingRos.cpp:491)
+  else if (origo) memcpy(ss.origo, origo, sizeof(ss.origo));
+  ss.gate_in[0] = h->min_dist;
+  ss.gate_in[1] = h->min_angle;
+  ss.gate_in[2] = matched ? 0.f : 1.f;
+  ss.sink = matched ? &h->d_last_pts : &h->d_upd_pts;
+  const int s = ensure_scan_buf(h, *ss.sink, n);
+  if (s != HSB_OK) return s;
+  memset(&ss.conv, 0, sizeof(ss.conv));
+  if (kind != HSB_IN_ENDPOINTS) {
+    fill_conv(h, kind, ss.conv);
+    ss.conv.out_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));
+    ss.conv.out_n = n_dev;
+    ss.conv.out_n_host = n_host;
+  }
+  return HSB_OK;
+}
+
+// A finished session's results: pose and write flag from res (4 floats), the covariance from cov when the session
+// matched and had endpoints (`kept`: counted on the device for converted input), and the kept count.  A matched
+// scan's container holds exactly the kept endpoints.
+void step_results(hsb_handle* h, bool matched, int kept, const float* res, const float* cov, float* out_pose,
+                  int* map_updated, float* cov_inout, int* out_kept) {
+  memcpy(out_pose, res, 3 * sizeof(float));
+  if (map_updated) *map_updated = res[3] != 0.f;
+  if (cov_inout && matched && kept > 0) memcpy(cov_inout, cov, 9 * sizeof(float));
+  if (out_kept) *out_kept = kept;
+  if (matched) h->last_n = kept;
+}
+
 // A scan, or a batch of scans, of one input kind.
 struct ScanIn {
   HsbInputKind kind;
@@ -1066,20 +1155,15 @@ static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts,
                            float cov_inout[9], float* record_out) {
   if (!h || !hint || !out_pose || n < 0 || (n > 0 && !pts)) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  // MapRepMultiMap::matchData fills dataContainers[] from this scan (MapRepMultiMap.h:127) whenever
-  // there is a coarse level; hsb_update_by_scan reuses it for the coarse levels (:143).
-  int s = ensure(h, h->d_scratch, 64 * sizeof(float));
-  if (s != HSB_OK) return s;
-  float* d_s = static_cast<float*>(h->d_scratch.p);  // [4..6] pose, [8..16] cov
   cudaStream_t st = h->stream;
-  h->last_n = n;
-  h->last_origo[0] = origo ? origo[0] : 0.f;
-  h->last_origo[1] = origo ? origo[1] : 0.f;
+  record_match(h, n, origo);
   // the kernel writes pose + Hessian straight into mapped host memory: no device-to-host copy operation on the
   // critical path (reading the scan from host memory the same way was slower than copying it)
   const bool host_out = h->tune_host_out != 0;
+  PoseResult* res = host_out ? &h->h_pin_dev->match : &h->d_scratch->match;
   const int R = record_floats(h);
   float* d_rec = nullptr;
+  int s;
   if (record_out) {
     if ((s = ensure(h, h->d_record, (size_t)R * sizeof(float))) != HSB_OK) return s;
     d_rec = static_cast<float*>(h->d_record.p);
@@ -1093,16 +1177,16 @@ static int match_data_impl(hsb_handle* h, const float hint[3], const float* pts,
   P.B = 1;
   P.hints = scan_header(h->d_last_pts);
   fill_scan(h, {HSB_IN_ENDPOINTS, scan_points(h->d_last_pts), nullptr, n, n, nullptr}, P);
-  P.out_poses = host_out ? h->h_pin_dev + 4 : d_s + 4;
-  P.out_cov = host_out ? h->h_pin_dev + 8 : d_s + 8;
+  P.out_poses = res->pose;
+  P.out_cov = res->cov;
   P.record = d_rec;
   P.record_floats = R;
   if ((s = launch_match_single(h, P, inl, hint, 3, pts)) != HSB_OK) return s;
-  if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 4, d_s + 4, 13 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(&h->h_pin->match, res, sizeof(PoseResult), cudaMemcpyDeviceToHost, st));
   if (record_out) HSB_CUDA(h, cudaMemcpyAsync(record_out, d_rec, (size_t)R * sizeof(float), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
-  memcpy(out_pose, h->h_pin + 4, 3 * sizeof(float));
-  if (cov_inout && n > 0) memcpy(cov_inout, h->h_pin + 8, 9 * sizeof(float));
+  memcpy(out_pose, h->h_pin->match.pose, 3 * sizeof(float));
+  if (cov_inout && n > 0) memcpy(cov_inout, h->h_pin->match.cov, 9 * sizeof(float));
   return HSB_OK;
 }
 
@@ -1124,12 +1208,11 @@ int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const 
   HandleScope guard(h);
   int s;
   if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   cudaStream_t st = h->stream;
   if (n > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_pts.p, pts, (size_t)n * 8, cudaMemcpyHostToDevice, st));
   HsbLevelDev L;
   fill_level_dev(h, level, L);
-  float* d_out = static_cast<float*>(h->d_scratch.p) + 32;
+  float* d_out = h->d_scratch->hessian;
   if (h->gather_mode == HSB_GATHER_TEX)
     hsb::hessian_kernel<hsb::MODE_TEX><<<1, 256, 0, st>>>(L, static_cast<const float2*>(h->d_pts.p), n, pose_map[0],
                                                           pose_map[1], pose_map[2], d_out);
@@ -1138,10 +1221,10 @@ int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const 
                                                           pose_map[1], pose_map[2], d_out);
   h->launches++;
   HSB_CUDA(h, cudaGetLastError());
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 32, d_out, 12 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin->hessian, d_out, 12 * sizeof(float), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
-  memcpy(H_out, h->h_pin + 32, 9 * sizeof(float));
-  memcpy(dTr_out, h->h_pin + 41, 3 * sizeof(float));
+  memcpy(H_out, h->h_pin->hessian, 9 * sizeof(float));
+  memcpy(dTr_out, h->h_pin->hessian + 9, 3 * sizeof(float));
   return HSB_OK;
 }
 
@@ -1282,20 +1365,19 @@ int to_points(hsb_handle* h, HsbInputKind kind, const float* in, int n, const do
   if ((s = ensure(h, h->d_conv_in, in_bytes > 0 ? in_bytes : 12)) != HSB_OK) return s;
   if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
   if (T && (s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
   cudaStream_t st = h->stream;
   if (n > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_conv_in.p, in, in_bytes, cudaMemcpyHostToDevice, st));
   if (T) HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
   HsbConvDev c;
   fill_conv(h, kind, c);
   c.out_pts = static_cast<float2*>(h->d_pts.p);
-  c.out_n = reinterpret_cast<int*>(static_cast<float*>(h->d_scratch.p) + 48);
+  c.out_n = &h->d_scratch->conv_kept;
   if ((s = launch_conversion(h, kind, static_cast<const float*>(h->d_conv_in.p), n,
                              T ? static_cast<const double*>(h->d_cloud_tf.p) : nullptr, c, st)) != HSB_OK)
     return s;
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 48, c.out_n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  HSB_CUDA(h, cudaMemcpyAsync(&h->h_pin->conv_kept, c.out_n, sizeof(int), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
-  const int kept = *reinterpret_cast<int*>(h->h_pin + 48);
+  const int kept = h->h_pin->conv_kept;
   if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
   *out_n = kept;
   if (T && out_origo) cloud_origo(h, T, out_origo);
@@ -1574,52 +1656,58 @@ int hsb_free_pinned(void* p) {
 
 }  // extern "C"
 
-extern "C" {
-
 // ---- map writing -------------------------------------------------------------------------------
 
-static int run_update(hsb_handle* h, HsbUpdateParams& P, int max_n) {
-  if (max_n <= 0) return HSB_OK;
-  cudaStream_t st = h->stream;
-  // mark: two warps per beam, four beams per CTA; apply: a fixed one-wave grid sweeping each level's box
-  constexpr int TEAM = 2;
-  int blocks = (max_n * TEAM + 7) / 8;
-  int cap = (h->sm_count * 6) / (P.levels > 0 ? P.levels : 1);   // all levels' CTAs resident at once (6 per SM: its launch bounds)
-  if (cap < 1) cap = 1;
-  if (blocks > cap) blocks = cap;
-  if (h->tune_time_update) HSB_CUDA(h, cudaEventRecord(h->ev_time[0], st));
-  // (as many CTAs as are resident at once — the register count decides, asked from the occupancy API — so that the
-  // sweep is ONE wave)
+namespace {
+
+constexpr int kMarkTeam = 2;   // warps per beam of the mark phase
+
+// The map writer's two launches on st, Mark then Apply, over `levels` levels of `sessions` scans whose longest has
+// max_n endpoints (grid y = level, z = session).  Mark: kMarkTeam warps per beam, four beams per CTA, at most as many
+// CTAs as are resident at once (six per SM: its launch bounds), shared out among the (session, level) slots.  Apply: a
+// one-wave sweep of each level's box, its CTAs per SM asked once from the occupancy API (the register count decides).
+// Mark is order-free and apply has one owner per cell (update_kernel.cuh), so the bits do not depend on the grids.
+// pdl: programmatic dependent launch (pdl_wait() in update_kernel.cuh).
+template <auto Mark, auto Apply, typename Params>
+int launch_map_write(hsb_handle* h, cudaStream_t st, const Params& P, int levels, int sessions, int max_n, bool pdl) {
   static int apply_ctas_per_sm = 0;
   if (!apply_ctas_per_sm) {
     int nb = 0;
-    HSB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hsb::update_apply_kernel, 256, 0));
+    HSB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, Apply, 256, 0));
     apply_ctas_per_sm = nb > 0 ? nb : 4;
   }
-  int sweep = (h->sm_count * apply_ctas_per_sm) / (P.levels > 0 ? P.levels : 1);
-  if (sweep < 1) sweep = 1;
-  if (h->tune_pdl) {
-    // programmatic dependent launch: see pdl_wait() in update_kernel.cuh
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cfg.gridDim = dim3(blocks, P.levels);
-    HSB_CUDA(h, cudaLaunchKernelEx(&cfg, hsb::update_mark_kernel<TEAM>, P));
-    cfg.gridDim = dim3(sweep, P.levels);
-    HSB_CUDA(h, cudaLaunchKernelEx(&cfg, hsb::update_apply_kernel, P));
-  } else {
-    hsb::update_mark_kernel<TEAM><<<dim3(blocks, P.levels), 256, 0, st>>>(P);
-    hsb::update_apply_kernel<<<dim3(sweep, P.levels), 256, 0, st>>>(P);
-  }
-  if (h->tune_time_update) HSB_CUDA(h, cudaEventRecord(h->ev_time[1], st));
+  const int slots = levels * sessions;
+  const int blocks = std::max(1, std::min((max_n * kMarkTeam + 7) / 8, (h->sm_count * 6 + slots - 1) / slots));
+  const int sweep = std::max(1, (h->sm_count * apply_ctas_per_sm + slots - 1) / slots);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(256);
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl ? 1 : 0;
+  cfg.gridDim = dim3(blocks, levels, sessions);
+  HSB_CUDA(h, cudaLaunchKernelEx(&cfg, Mark, P));
+  cfg.gridDim = dim3(sweep, levels, sessions);
+  HSB_CUDA(h, cudaLaunchKernelEx(&cfg, Apply, P));
   h->launches += 2;
   HSB_CUDA(h, cudaGetLastError());
+  return HSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+static int run_update(hsb_handle* h, const HsbUpdateParams& P, int max_n) {
+  if (max_n <= 0) return HSB_OK;
+  cudaStream_t st = h->stream;
+  if (h->tune_time_update) HSB_CUDA(h, cudaEventRecord(h->ev_time[0], st));
+  const int s = launch_map_write<hsb::update_mark_kernel<kMarkTeam>, hsb::update_apply_kernel>(h, st, P, P.levels, 1,
+                                                                                             max_n, h->tune_pdl != 0);
+  if (s != HSB_OK) return s;
+  if (h->tune_time_update) HSB_CUDA(h, cudaEventRecord(h->ev_time[1], st));
   return HSB_OK;
 }
 
@@ -1636,7 +1724,11 @@ static int next_stamp_base(hsb_handle* h, int level, uint32_t* base, cudaStream_
   return HSB_OK;
 }
 
-static void fill_update_level(hsb_handle* h, int l, HsbUpdateLevelDev& d) {
+// Level l's map-writer descriptor d for a write of the scan `pts` (n endpoints; with n_dev the count the device holds
+// there, n an upper bound) from origo (NULL = 0, 0), both scaled by pt_scale.  A level with endpoints advances its stamp
+// base (a wrap clears the stamps on `st`) and writer slot, and raises *max_n to n.
+static int fill_update_level(hsb_handle* h, int l, float pt_scale, const float2* pts, int n, const int* n_dev,
+                             const float origo[2], cudaStream_t st, HsbUpdateLevelDev& d, int* max_n) {
   const Level& L = h->lv[l];
   memset(&d, 0, sizeof(d));
   d.logodds = L.logodds;
@@ -1649,37 +1741,32 @@ static void fill_update_level(hsb_handle* h, int l, HsbUpdateLevelDev& d) {
   d.dirty = L.dirty;
   d.scratch = L.scratch;
   d.slot = L.parity;
+  d.pt_scale = pt_scale;
+  d.pts = pts;
+  d.n = n;
+  d.n_dev = n_dev;
+  d.origo_x = origo ? origo[0] : 0.f;
+  d.origo_y = origo ? origo[1] : 0.f;
+  // an empty container still advances the stamps in the reference (OccGridMapBase.h:164-167); no-op here
+  d.active = n > 0;
+  if (!d.active) return HSB_OK;
+  *max_n = std::max(*max_n, n);
+  return next_stamp_base(h, l, &d.stamp_base, st);
 }
 
 // MapRepMultiMap::updateByScan (MapRepMultiMap.h:134-147) for one scan of h: its map-writer level descriptors
-// d[0 .. levels).  Level 0 reads this scan (`pts`, n; converted input: the kept count the device holds at n_dev, n is an
-// upper bound); the coarse levels read it too if it has just become the last match's container (`matched`), and
-// otherwise the container the last matchData left behind (:143).  Advances the stamp bases (a wrap clears the stamps on
-// `st`) and writer slots of the active levels, and raises *max_n to the longest active scan.
+// d[0 .. levels).  Level 0 reads this scan (`pts`, n, n_dev as fill_update_level takes them); the coarse levels read it
+// too if it has just become the last match's container (`matched`), and otherwise the container the last matchData
+// left behind (:143).
 static int fill_update_levels(hsb_handle* h, HsbUpdateLevelDev* d, const float2* pts, int n, const int* n_dev,
                               const float origo[2], bool matched, cudaStream_t st, int* max_n) {
+  const float2* last = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
   for (int l = 0; l < h->levels; ++l) {
-    fill_update_level(h, l, d[l]);
-    d[l].pt_scale = (float)(1.0 / pow(2.0, (double)l));
-    if (l == 0 || matched) {
-      d[l].pts = pts;
-      d[l].n = n;
-      d[l].n_dev = n_dev;
-      d[l].origo_x = origo ? origo[0] : 0.f;
-      d[l].origo_y = origo ? origo[1] : 0.f;
-    } else {
-      d[l].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
-      d[l].n = h->last_n;
-      d[l].origo_x = h->last_origo[0];
-      d[l].origo_y = h->last_origo[1];
-    }
-    // an empty container still advances the stamps in the reference (OccGridMapBase.h:164-167); no-op here
-    d[l].active = d[l].n > 0;
-    if (d[l].active) {
-      const int s = next_stamp_base(h, l, &d[l].stamp_base, st);
-      if (s != HSB_OK) return s;
-      *max_n = std::max(*max_n, d[l].n);
-    }
+    const float pt_scale = (float)(1.0 / pow(2.0, (double)l));
+    const int s = l == 0 || matched
+                      ? fill_update_level(h, l, pt_scale, pts, n, n_dev, origo, st, d[l], max_n)
+                      : fill_update_level(h, l, pt_scale, last, h->last_n, nullptr, h->last_origo, st, d[l], max_n);
+    if (s != HSB_OK) return s;
   }
   return HSB_OK;
 }
@@ -1739,40 +1826,34 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
   int s;
   const int n = in.n_shared;   // converted: a cloud's points or a scan's beams, an upper bound of the endpoints kept
   const bool conv = in.kind != HSB_IN_ENDPOINTS;
-  if ((s = ensure(h, h->d_scratch, 64 * sizeof(float))) != HSB_OK) return s;
-  if (!h->d_gate.p && (s = reset_gate(h)) != HSB_OK) return s;
-  // scratch: [8..10] pose, [11] flag, [12..20] cov, [40] the kept-endpoint count of converted input
-  float* d_s = static_cast<float*>(h->d_scratch.p);
-  float* d_gate = static_cast<float*>(h->d_gate.p);
-  int* n_dev = conv ? reinterpret_cast<int*>(d_s + 40) : nullptr;
+  const bool matched = !map_without_matching;
+  PoseResult* d_res = &h->d_scratch->step;
+  int* n_dev = conv ? &h->d_scratch->step_kept : nullptr;
   cudaStream_t st = h->stream;
   // results (pose, flag, Hessian, kept count) are written into mapped host memory by the kernels themselves: the step
   // is one host-to-device copy and three launches (match with the gate in its epilogue, mark, apply — the latter two
   // with programmatic dependent launch).  Endpoint steps only: tuning host_out = 0 copies them back instead.
   const bool host_out = conv || h->tune_host_out != 0;
   const bool poll = host_out && nowait;   // return when the pose has arrived; the map write continues on the stream
-  volatile unsigned* seq = reinterpret_cast<volatile unsigned*>(h->h_pin + 22);
-  unsigned* seq_dev = reinterpret_cast<unsigned*>(h->h_pin_dev + 22);
+  PoseResult* h_res = &h->h_pin_dev->step;
+  unsigned* seq_dev = &h->h_pin_dev->step_seq;
   const unsigned seq_value = ++h->step_seq;
-  int* kept_host = reinterpret_cast<int*>(h->h_pin + 24);
-  int* kept_dev = reinterpret_cast<int*>(h->h_pin_dev + 24);
-  // without matching the reference leaves the coarse containers alone (HectorSlamProcessor.h:77-81,
-  // MapRepMultiMap.h:143): only level 0 sees this scan
-  DevBuf& pbuf = map_without_matching ? h->d_upd_pts : h->d_last_pts;
-  const float header[6] = {hint[0], hint[1], hint[2], h->min_dist, h->min_angle, map_without_matching ? 1.f : 0.f};
-  const bool inl = !conv && !map_without_matching && inline_scan_applies(h, n);   // header + scan travel in the match launch
-  float origo[2] = {0.f, 0.f};
+  int* kept_dev = &h->h_pin_dev->step_kept;
+  // the match kernel publishes a converted scan's kept count itself; without matching publish_int_kernel does
+  StepSession ss;
+  if ((s = step_session(h, in.kind, n, in.tf, origo_in, matched, n_dev, matched ? kept_dev : nullptr, ss)) != HSB_OK) return s;
+  const float header[6] = {hint[0], hint[1], hint[2], ss.gate_in[0], ss.gate_in[1], ss.gate_in[2]};
+  const bool inl = !conv && matched && inline_scan_applies(h, n);   // header + scan travel in the match launch
   const float* d_hdr;   // the header on the device: [0..2] hint, [3..5] minDist / minAngle / force
   ScanIn dev;           // the scan on the device
   if (!conv) {
     // staging, endpoints: header + points straight into the container the map writer reads
-    if ((s = inl ? ensure_scan_buf(h, pbuf, n) : upload_scan(h, pbuf, header, 6, in.in, n, st)) != HSB_OK) return s;
-    d_hdr = scan_header(pbuf);
-    dev = {HSB_IN_ENDPOINTS, scan_points(pbuf), nullptr, n, n, nullptr};
-    if (origo_in) memcpy(origo, origo_in, sizeof(origo));
+    if (!inl && (s = upload_scan(h, *ss.sink, header, 6, in.in, n, st)) != HSB_OK) return s;
+    d_hdr = scan_header(*ss.sink);
+    dev = {HSB_IN_ENDPOINTS, scan_points(*ss.sink), nullptr, n, n, nullptr};
   } else {
     // staging, converted input (floats): [0..15] header; cloud / projected: [16..39] the laser transform (12 doubles),
-    // [40..] the cloud or the ranges; ranges: [16..] the ranges.  The conversion writes the endpoints into the container.
+    // [40..] the cloud or the ranges; ranges: [16..] the ranges.  The conversion writes the endpoints into the sink.
     const size_t kHdr = 16, kTf = in.tf ? 24 : 0, per_pt = in.kind == HSB_IN_CLOUD ? 3 : 1;
     const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
     if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
@@ -1783,77 +1864,60 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     if (in.tf) memcpy(hs + kHdr, in.tf, 12 * sizeof(double));
     if (n > 0) memcpy(hs + kHdr + kTf, in.in, (size_t)n * per_pt * sizeof(float));
     HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
-    if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
     const float* d_c = static_cast<const float*>(h->d_fused_in.p);
     d_hdr = d_c;
     dev = {in.kind, d_c + kHdr + kTf, nullptr, n, n, in.tf ? reinterpret_cast<const double*>(d_c + kHdr) : nullptr};
-    if (in.tf) cloud_origo(h, in.tf, origo);   // a LaserScan's origo is zero (HectorMappingRos.cpp:491)
   }
-  float2* d_pts = reinterpret_cast<float2*>(scan_points(pbuf));
-  if (!map_without_matching) {
+  float2* d_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));
+  if (matched) {
     // :78 match, and :83-89 the gate in the same kernel's epilogue (an empty scan still passes through it: pose = hint)
     HsbMatchParams P;
     fill_match_params(h, P);
     P.B = 1;
     P.hints = d_hdr;
     fill_scan(h, dev, P);
-    if (conv) {
-      P.conv.out_pts = d_pts;
-      P.conv.out_n = n_dev;
-      P.conv.out_n_host = kept_dev;
-    }
-    P.out_poses = d_s + 8;
-    P.out_cov = host_out ? h->h_pin_dev + 12 : d_s + 12;
-    P.gate_state = d_gate;
+    P.conv = ss.conv;
+    P.out_poses = d_res->pose;
+    P.out_cov = host_out ? h_res->cov : d_res->cov;
+    P.gate_state = h->d_gate;
     P.gate_in = d_hdr + 3;
-    P.gate_out_host = host_out ? h->h_pin_dev + 8 : nullptr;
+    P.gate_out_host = host_out ? h_res->pose : nullptr;
     P.seq_host = poll ? seq_dev : nullptr;
     P.seq_value = seq_value;
     // (a projected step takes the single step's default shape: hsb_slam_update_projected checked the tuning)
     s = launch_match_single(h, P, inl, header, 6, in.in);
-    // the scan is the last match's container now (endpoints: since the staging copy, whether or not the match launched)
-    if (s == HSB_OK || !conv) {
-      h->last_n = n;   // (converted: an upper bound until the kept count arrives; the writer reads the exact one on the device)
-      h->last_origo[0] = origo[0];
-      h->last_origo[1] = origo[1];
-    }
+    // (endpoints: the scan is in the container since the staging copy, whether or not the match launched)
+    if (s == HSB_OK || !conv) record_match(h, n, ss.origo);
     if (s != HSB_OK) return s;
   } else if (!conv) {
     // without matching, endpoints: the gate alone (:80, :89)
-    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, host_out ? h->h_pin_dev + 8 : nullptr,
+    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(h->d_gate, d_hdr + 3, d_hdr, d_res->pose, host_out ? h_res->pose : nullptr,
                                             poll ? seq_dev : nullptr, seq_value);
     h->launches += 1;
     HSB_CUDA(h, cudaGetLastError());
   } else {
     // without matching, converted input: the stand-alone conversion kernel, the gate, then the kept count's publication
-    HsbConvDev c;
-    fill_conv(h, in.kind, c);
-    c.out_pts = d_pts;
-    c.out_n = n_dev;
-    if ((s = launch_conversion(h, in.kind, dev.in, n, dev.tf, c, st)) != HSB_OK) return s;
-    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(d_gate, d_hdr + 3, d_hdr, d_s + 8, h->h_pin_dev + 8, nullptr, 0);
+    if ((s = launch_conversion(h, in.kind, dev.in, n, dev.tf, ss.conv, st)) != HSB_OK) return s;
+    hsb::slam_gate_kernel<<<1, 32, 0, st>>>(h->d_gate, d_hdr + 3, d_hdr, d_res->pose, h_res->pose, nullptr, 0);
     hsb::publish_int_kernel<<<1, 32, 0, st>>>(n_dev, kept_dev, poll ? seq_dev : nullptr, seq_value);
     h->launches += 2;
     HSB_CUDA(h, cudaGetLastError());
   }
-  if ((s = enqueue_update_by_scan(h, d_pts, n, n_dev, origo, !map_without_matching, nullptr, d_s + 8, d_gate + 3)) != HSB_OK)
+  if ((s = enqueue_update_by_scan(h, d_pts, n, n_dev, ss.origo, matched, nullptr, d_res->pose, h->d_gate + 3)) != HSB_OK)
     return s;   // :91
   if (poll) {
     // the pose is all the caller needs now; every later call on this handle is stream-ordered behind the map write
-    if ((s = wait_published(h, seq, seq_value, st, "fused step finished without publishing its pose")) != HSB_OK) return s;
+    s = wait_published(h, &h->h_pin->step_seq, seq_value, st, "fused step finished without publishing its pose");
+    if (s != HSB_OK) return s;
     h->map_write_pending = true;
   } else {
-    if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 8, d_s + 8, 13 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (!host_out) HSB_CUDA(h, cudaMemcpyAsync(&h->h_pin->step, d_res, sizeof(PoseResult), cudaMemcpyDeviceToHost, st));
     HSB_CUDA(h, cudaStreamSynchronize(st));  // :93 onMapUpdated — the probability plane is current
     h->map_write_pending = false;
   }
   // the endpoints the step had: known on the host for endpoints, counted on the device for converted input
-  const int kept = conv ? *kept_host : n;
-  if (conv && !map_without_matching) h->last_n = kept;
-  memcpy(out_pose, h->h_pin + 8, 3 * sizeof(float));
-  if (map_updated) *map_updated = h->h_pin[11] != 0.f;
-  if (cov_inout && kept > 0 && !map_without_matching) memcpy(cov_inout, h->h_pin + 12, 9 * sizeof(float));
-  if (out_kept) *out_kept = kept;
+  const PoseResult& r = h->h_pin->step;
+  step_results(h, matched, conv ? h->h_pin->step_kept : n, r.pose, r.cov, out_pose, map_updated, cov_inout, out_kept);
   return HSB_OK;
 }
 
@@ -1910,10 +1974,8 @@ int hsb_slam_update_projected(hsb_handle* h, const float hint[3], const float* r
 int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
   if (!h || !pose) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  int s = ensure(h, h->d_gate, 4 * sizeof(float));
-  if (s != HSB_OK) return s;
-  memcpy(h->h_pin + 56, pose, 3 * sizeof(float));
-  HSB_CUDA(h, cudaMemcpyAsync(h->d_gate.p, h->h_pin + 56, 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  memcpy(h->h_pin->gate, pose, 3 * sizeof(float));
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_gate, h->h_pin->gate, 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
   return HSB_OK;
 }
@@ -1921,13 +1983,9 @@ int hsb_set_last_map_update_pose(hsb_handle* h, const float pose[3]) {
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]) {
   if (!h || !out) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  if (!h->d_gate.p) {
-    int s = reset_gate(h);
-    if (s != HSB_OK) return s;
-  }
-  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin + 56, h->d_gate.p, 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  HSB_CUDA(h, cudaMemcpyAsync(h->h_pin->gate, h->d_gate, 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
-  memcpy(out, h->h_pin + 56, 3 * sizeof(float));
+  memcpy(out, h->h_pin->gate, 3 * sizeof(float));
   return HSB_OK;
 }
 
@@ -1943,16 +2001,11 @@ int hsb_update_level_by_scan(hsb_handle* h, int level, const float* pts, int n, 
   memcpy(P.pose_world, pose, 3 * sizeof(float));
   P.log_odds_free = h->log_odds_free;
   P.log_odds_occ = h->log_odds_occ;
-  HsbUpdateLevelDev& d = P.lv[0];
-  fill_update_level(h, level, d);
-  d.pt_scale = 1.0f;
-  d.pts = reinterpret_cast<const float2*>(scan_points(h->d_upd_pts));
-  d.n = n;
-  d.origo_x = origo ? origo[0] : 0.f;
-  d.origo_y = origo ? origo[1] : 0.f;
-  d.active = n > 0;
-  if (d.active && (s = next_stamp_base(h, level, &d.stamp_base, h->stream)) != HSB_OK) return s;
-  if ((s = run_update(h, P, n)) != HSB_OK) return s;
+  int max_n = 0;
+  if ((s = fill_update_level(h, level, 1.0f, reinterpret_cast<const float2*>(scan_points(h->d_upd_pts)), n, nullptr, origo,
+                             st, P.lv[0], &max_n)) != HSB_OK)
+    return s;
+  if ((s = run_update(h, P, max_n)) != HSB_OK) return s;
   HSB_CUDA(h, cudaStreamSynchronize(st));
   return HSB_OK;
 }
@@ -2252,7 +2305,7 @@ static int get_dirty(hsb_handle* h, int level, int which, int rect[4], int reset
   HandleScope guard(h);
   Level& L = h->lv[level];
   int* src = L.dirty + 4 * which;
-  int* pin = reinterpret_cast<int*>(h->h_pin + 60);
+  int* pin = h->h_pin->rect;
   HSB_CUDA(h, cudaMemcpyAsync(pin, src, 4 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   if (reset) {
     static const int clean[4] = {INT_MAX, INT_MAX, -1, -1};
@@ -2535,7 +2588,8 @@ int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
 // group's stream, whatever M is: the match kernel with one 8-warp CTA per session (the shape hsb_slam_update uses, so
 // every session's pose, Hessian and gate decision are the single call's bits) and the gate of each session in its
 // epilogue, then mark and apply over (session, level).  The per-step handle state the single call keeps on the host
-// (stamp bases, writer slots, the last match's container size and origo) is advanced here exactly as it advances there.
+// (stamp bases, writer slots, the last match's container size and origo) advances through the functions the single
+// call uses: step_session, record_match, fill_update_levels and step_results.
 
 struct hsb_group {
   std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create(_mixed) was given them
@@ -2712,18 +2766,6 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
       return _code;                                                                                          \
     }                                                                                                        \
   } while (0)
-  // the gate state a member's first SLAM step would create (lastMapUpdatePose = FLT_MAX, HectorSlamProcessor.h:117)
-  for (hsb_handle* h : g->m) {
-    if (h->d_gate.p) continue;
-    HandleScope scope(h);
-    const int s = reset_gate(h);
-    if (s != HSB_OK) {
-      group_fail(h0, s, "%s: %s", fn, h->err.c_str());
-      hsb_group_destroy(g);
-      return s;
-    }
-    HSB_GROUP_CUDA(cudaStreamSynchronize(h->stream));
-  }
   HSB_GROUP_CUDA(cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
   HSB_GROUP_CUDA(cudaEventCreateWithFlags(&g->ev, cudaEventDisableTiming));
   {
@@ -2905,46 +2947,29 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
     hsb_handle* h = g->m[members[k]];
     const int n = offsets[k + 1] - offsets[k];   // a cloud's size / a scan's beams: an upper bound of the endpoints kept
     const bool matched = !(map_without_matching && map_without_matching[k]);
-    float og[2] = {0.f, 0.f};
+    const double* T = nullptr;
     if (tf) {
-      const double* T = in.transforms ? in.transforms + 12 * (size_t)k : h->cfmt.laser_transform;
+      T = in.transforms ? in.transforms + 12 * (size_t)k : h->cfmt.laser_transform;
       memcpy(s_tf + 12 * (size_t)k, T, 12 * sizeof(double));
-      cloud_origo(h, T, og);
-    } else if (in.origo) {   // (a LaserScan's origo is zero, HectorMappingRos.cpp:491)
-      og[0] = in.origo[2 * k];
-      og[1] = in.origo[2 * k + 1];
     }
-    s_gin[3 * k] = h->min_dist;
-    s_gin[3 * k + 1] = h->min_angle;
-    s_gin[3 * k + 2] = matched ? 0.f : 1.f;
+    StepSession ss;
+    if ((s = step_session(h, in.kind, n, T, in.origo ? in.origo + 2 * k : nullptr, matched, kept_dev + k, kept_mapped + k,
+                          ss)) != HSB_OK)
+      return s;
+    memcpy(s_gin + 3 * k, ss.gate_in, sizeof(ss.gate_in));
     s_lo[k] = make_float2(h->log_odds_free, h->log_odds_occ);
-    HsbGroupSessionDev& ss = s_sess[k];
-    memset(&ss, 0, sizeof(ss));
-    ss.gate_state = static_cast<float*>(h->d_gate.p);
-    ss.member = members[k];
-    if (matched) {   // this scan becomes the last match's container (without matching the old one stays, :77-81)
-      if ((s = ensure_scan_buf(h, h->d_last_pts, n)) != HSB_OK) return s;
-      if (!conv) ss.last_pts = reinterpret_cast<float2*>(scan_points(h->d_last_pts));
-      h->last_n = n;
-      h->last_origo[0] = og[0];
-      h->last_origo[1] = og[1];
-    }
-    // where level 0 reads this scan, and (converted) where the writer finds its endpoint count
-    const float2* pts0 = nullptr;
-    const int* n_dev = nullptr;
-    if (conv) {   // converted into the buffer the single fused step converts into
-      DevBuf& pbuf = matched ? h->d_last_pts : h->d_upd_pts;
-      if ((s = ensure_scan_buf(h, pbuf, n)) != HSB_OK) return s;
-      fill_conv(h, in.kind, ss.conv);
-      ss.conv.out_pts = reinterpret_cast<float2*>(scan_points(pbuf));
-      ss.conv.out_n = kept_dev + k;
-      ss.conv.out_n_host = kept_mapped + k;
-      pts0 = ss.conv.out_pts;
-      n_dev = kept_dev + k;
-    } else {
-      pts0 = reinterpret_cast<const float2*>(d_in) + offsets[k];
-    }
-    if ((s = fill_update_levels(h, s_upd + (size_t)k * levels, pts0, n, n_dev, og, matched, st, &max_upd)) != HSB_OK) return s;
+    HsbGroupSessionDev& gs = s_sess[k];
+    memset(&gs, 0, sizeof(gs));
+    gs.gate_state = h->d_gate;
+    gs.member = members[k];
+    gs.conv = ss.conv;
+    if (matched && !conv) gs.last_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));   // the match copies the scan there
+    if (matched) record_match(h, n, ss.origo);
+    // level 0 reads the staged endpoints, or a converted scan where it was converted to, with its count on the device
+    const float2* pts0 = conv ? ss.conv.out_pts : reinterpret_cast<const float2*>(d_in) + offsets[k];
+    if ((s = fill_update_levels(h, s_upd + (size_t)k * levels, pts0, n, ss.conv.out_n, ss.origo, matched, st, &max_upd)) !=
+        HSB_OK)
+      return s;
   }
   HSB_CUDA(h0, cudaMemcpyAsync(g->d_stage.p, hs, bytes, cudaMemcpyHostToDevice, st));
 
@@ -2975,38 +3000,17 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
             : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP>(h0, P, max_n, st, 1);
   if (s != HSB_OK) return s;
 
-  // K2: mark and apply over (session, level), behind the match with programmatic dependent launch; the single step's
-  // one-wave grids are shared out among the sessions (a cloud's size or a scan's beam count bounds its endpoints: the
-  // grids are sized by it).  Mark is order-free and apply has one owner per cell, so the bits do not depend on the grid.
+  // K2: mark and apply over (session, level), behind the match with programmatic dependent launch, in the single
+  // write's grids shared out among the sessions (a cloud's size or a scan's beam count bounds its endpoints: the grids
+  // are sized by it)
   HsbGroupUpdateParams U;
   U.lv = reinterpret_cast<const HsbUpdateLevelDev*>(ds + o_upd);
   U.log_odds = reinterpret_cast<const float2*>(ds + o_lo);
   U.res = g->d_res;
   U.levels = levels;
-  constexpr int TEAM = 2;
-  const int slots = K * levels;
-  const int blocks = std::max(1, std::min((max_upd * TEAM + 7) / 8, (h0->sm_count * 6 + slots - 1) / slots));
-  static int apply_ctas_per_sm = 0;
-  if (!apply_ctas_per_sm) {
-    int nb = 0;
-    HSB_CUDA(h0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hsb::update_apply_group_kernel, 256, 0));
-    apply_ctas_per_sm = nb > 0 ? nb : 4;
-  }
-  const int sweep = std::max(1, (h0->sm_count * apply_ctas_per_sm + slots - 1) / slots);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(256);
-  cfg.stream = st;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cfg.gridDim = dim3(blocks, levels, K);
-  HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_mark_group_kernel<TEAM>, U));
-  cfg.gridDim = dim3(sweep, levels, K);
-  HSB_CUDA(h0, cudaLaunchKernelEx(&cfg, hsb::update_apply_group_kernel, U));
-  h0->launches += 2;
-  HSB_CUDA(h0, cudaGetLastError());
+  s = launch_map_write<hsb::update_mark_group_kernel<kMarkTeam>, hsb::update_apply_group_kernel>(h0, st, U, levels, K,
+                                                                                                 max_upd, true);
+  if (s != HSB_OK) return s;
   HSB_CUDA(h0, cudaEventRecord(g->ev, st));
   // every later operation of a stepped member waits for this step (HandleScope).  A member left out keeps its own
   // group_ev: a map write still pending from an earlier nowait step of this group is waited for through the event,
@@ -3025,17 +3029,10 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   }
   const int* kept_host = reinterpret_cast<const int*>(g->h_res + 13 * (size_t)M + 4);
   for (int k = 0; k < K; ++k) {
-    const float* r = g->h_res + 4 * (size_t)k;
-    memcpy(out_poses + 3 * (size_t)k, r, 3 * sizeof(float));
-    if (map_updated) map_updated[k] = r[3] != 0.f;
     const bool matched = !(map_without_matching && map_without_matching[k]);
-    const int n = conv ? kept_host[k] : offsets[k + 1] - offsets[k];   // the endpoints the session had
-    if (conv) {
-      if (out_kept) out_kept[k] = n;
-      if (matched) g->m[members[k]]->last_n = n;   // the last match's container holds exactly these (as the single fused step)
-    }
-    if (cov_inout && matched && n > 0)
-      memcpy(cov_inout + 9 * (size_t)k, g->h_res + 4 * (size_t)M + 9 * (size_t)k, 9 * sizeof(float));
+    step_results(g->m[members[k]], matched, conv ? kept_host[k] : offsets[k + 1] - offsets[k], g->h_res + 4 * (size_t)k,
+                 g->h_res + 4 * (size_t)M + 9 * (size_t)k, out_poses + 3 * (size_t)k, map_updated ? map_updated + k : nullptr,
+                 cov_inout ? cov_inout + 9 * (size_t)k : nullptr, out_kept ? out_kept + k : nullptr);
   }
   return HSB_OK;
 }

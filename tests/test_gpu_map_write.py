@@ -311,6 +311,46 @@ def test_fused_cloud_step_counts_on_device(hsb_lib):
     pair.close()
 
 
+@pytest.mark.parametrize("pdl", [1, 0], ids=["pdl", "no_pdl"])
+def test_single_write_launch_counts(hsb_lib, pdl):
+    """Launches of the single-handle writes, with and without programmatic dependent launch: mark + apply for a write
+    with endpoints on some level and none for a write without, behind one match launch for a matched step, the gate
+    kernel for a map_without_matching step of endpoints, and conversion, gate and count publication for one of a
+    cloud."""
+    sx, sy, levels, res = 256, 256, 3, 0.05
+    pair = Pair(res, sx, sy, levels)
+    rng = np.random.default_rng(71)
+    L0 = pair.lv[0]
+    pose, scan = scan_for(L0, (sx // 2, sy // 2), 0.3, rng)
+    xyz = np.zeros((scan.shape[0], 3), np.float32)
+    xyz[:, :2] = scan * np.float32(res)
+    none = np.zeros((0, 2), np.float32)
+    steps = [
+        ("update_by_scan, no endpoints, no container", 0, lambda r: r.updateByScan(none, pose)),
+        ("update_level_by_scan, no endpoints", 0, lambda r: r.update_level_by_scan(1, none, pose)),
+        ("update_level_by_scan", 2, lambda r: r.update_level_by_scan(1, scan * np.float32(0.5), pose)),
+        ("update_by_scan", 2, lambda r: r.updateByScan(scan, pose)),
+        ("slam_update map_without_matching", 3, lambda r: r.slam_update(pose, scan, map_without_matching=True)),
+        ("slam_update", 3, lambda r: r.slam_update(pose, scan)),
+        ("update_by_scan, no endpoints, matched container", 2, lambda r: r.updateByScan(none, pose)),
+        ("slam_update, no endpoints", 1, lambda r: r.slam_update(pose, none)),
+        ("update_by_scan, no endpoints, empty container", 0, lambda r: r.updateByScan(none, pose)),
+        ("slam_update_cloud map_without_matching", 5,
+         lambda r: r.slam_update_cloud(pose, xyz, map_without_matching=True)),
+        ("slam_update_cloud", 3, lambda r: r.slam_update_cloud(pose, xyz)),
+    ]
+    for rep in pair.reps:
+        rep.set_tuning(pdl=pdl)
+        rep.setMapUpdateMinDistDiff(0.0)
+        rep.setMapUpdateMinAngleDiff(0.0)
+        rep.set_cloud_format(np.float64([1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0]), 0.0, 1e6, -1.0, 1.0)
+        for name, want, fn in steps:
+            n0 = rep.launch_count
+            fn(rep)
+            assert rep.launch_count - n0 == want, (name, rep.gather_mode, rep.launch_count - n0)
+    pair.close()
+
+
 def test_group_step_odd_width(hsb_lib):
     """hsb_group_slam_update on a 243 x 200 geometry (level widths 243, 121: the scalar apply path), members with
     different update factors, one of them map_without_matching (its coarse levels keep the last matched container)."""
