@@ -47,7 +47,7 @@ EXPORTED = [
     "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
     "hsb_group_match_batch", "hsb_group_match_batch_subset",
     "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
-    "hsb_group_create_mixed",
+    "hsb_group_create_mixed", "hsb_group_reset", "hsb_group_reset_subset",
 ]
 
 
@@ -220,6 +220,8 @@ def load_library() -> C.CDLL:
     sig("hsb_group_pack_dirty_device", i, vp, vp, C.c_size_t, i, vp)
     sig("hsb_group_pack_dirty_device_subset", i, vp, i, vp, vp, C.c_size_t, i, vp)
     sig("hsb_group_unpack_dirty_device", i, vp, vp, C.c_size_t, vp)
+    sig("hsb_group_reset", i, vp)
+    sig("hsb_group_reset_subset", i, vp, i, vp)
     _lib = L
     return L
 
@@ -1087,6 +1089,17 @@ class SlamGroup:
         (hsb_group_unpack_dirty_device).  Deferred blocks count on their member's replication_overflows(), a buffer that
         does not fit this group on reps[0]'s.  Asynchronous on `stream`."""
         self._check(self.lib.hsb_group_unpack_dirty_device(self.g, d_buf, int(capacity), stream))
+
+    def reset(self, members=None):
+        """MapRepB200.reset() for the members in one launch (hsb_group_reset): each is left as reset() leaves it, except
+        that its replication rectangles are clean with the cleared flags set, so the next pack ships a clear record and
+        the cells written since instead of whole levels.  members as in slam_update (hsb_group_reset_subset).  Returns
+        once queued; every later call on a reset member runs after it."""
+        K, mem = self._sessions(members)
+        if mem is None:
+            self._check(self.lib.hsb_group_reset(self.g))
+        else:
+            self._check(self.lib.hsb_group_reset_subset(self.g, K, _ptr(mem)))
 
     def get_dist(self, level: int, begin_world, end_world, members=None):
         """DistanceMeasurementProvider::getDist for the members' rays in one pass (hsb_group_get_dist): begin_world and

@@ -35,8 +35,8 @@ struct Level {
   cudaSurfaceObject_t surf = 0;
   int evals = 0;
   int* dirty = nullptr;  // device: two rectangles {xmin, ymin, xmax, ymax} of cells written since their last reset —
-                         // [0..3] for replication (hsb_get_dirty_rect), [4..7] for host mirrors (hsb_get_mirror_dirty_rect);
-                         // points into hsb_handle::d_dirty_all
+                         // [0..3] for replication (hsb_get_dirty_rect), [4..7] for host mirrors (hsb_get_mirror_dirty_rect)
+                         // — and the cleared flag [8] (HSB_DIRTY_WORDS); points into hsb_handle::d_dirty_all
 };
 
 struct DevBuf {
@@ -68,7 +68,7 @@ struct PinnedSlots {
   int conv_kept;       // the stand-alone conversions' kept-endpoint count
   float hessian[12];   // hsb_hessian_derivs: H row-major, then dTr
   float gate[4];       // the gate state on its way to or from the device: lastMapUpdatePose, write flag
-  int rect[4];         // a dirty rectangle on its way to the host
+  int dirty[HSB_DIRTY_WORDS];   // a level's rectangles and cleared flag on their way to the host
 };
 
 // The single-scan calls' device block (hsb_handle::d_scratch)
@@ -124,7 +124,7 @@ struct hsb_handle {
   int tune_time_update = 0;
   BatchSet bset[2];             // device staging of the host-buffer batch calls, alternating between calls
   int next_set = 0;
-  int* d_dirty_all = nullptr;   // HSB_MAX_LEVELS x 8 ints, see Level::dirty
+  int* d_dirty_all = nullptr;   // HSB_MAX_LEVELS x HSB_DIRTY_WORDS ints (see Level::dirty), then kOverflowWord's 4
   uint64_t d2h_bytes = 0;       // bytes the plane / rectangle download entry points copied to the host (diagnostic)
   cudaEvent_t ev_sync[4] = {nullptr, nullptr, nullptr, nullptr};   // ordering of caller streams against the handle's own
   float* d_gate = nullptr;   // SLAM steps: lastMapUpdatePose[3], write-the-map flag
@@ -149,6 +149,9 @@ struct hsb_handle {
 };
 
 namespace {
+
+// hsb_handle::d_dirty_all: the replication overflow counter (hsb_get_replication_overflows) behind the levels' words
+constexpr int kOverflowWord = HSB_MAX_LEVELS * HSB_DIRTY_WORDS;
 
 int fail(hsb_handle* h, int code, const char* fmt, ...) {
   if (h) {
@@ -289,11 +292,12 @@ int check_rect(hsb_handle* h, const Level& L, const int rect[4]) {
   return HSB_OK;
 }
 
-// both dirty rectangles of a level := the whole level (after a reset or an upload every cell may differ)
+// both dirty rectangles of a level := the whole level (after a reset or an upload every cell may differ), cleared flag 0:
+// the next pack ships the whole level's rows
 int mark_level_dirty(hsb_handle* h, int level, cudaStream_t st) {
   Level& L = h->lv[level];
   if (!L.dirty) return HSB_OK;
-  const int full[8] = {0, 0, L.sx - 1, L.sy - 1, 0, 0, L.sx - 1, L.sy - 1};
+  const int full[HSB_DIRTY_WORDS] = {0, 0, L.sx - 1, L.sy - 1, 0, 0, L.sx - 1, L.sy - 1, 0};
   HSB_CUDA(h, cudaMemcpyAsync(L.dirty, full, sizeof(full), cudaMemcpyHostToDevice, st));
   return HSB_OK;
 }
@@ -727,8 +731,8 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
     for (int i = 0; i < 8; ++i) HSB_CUDA_C(cudaEventCreateWithFlags(&h->bset[k].chunk_ready[i], cudaEventDisableTiming));
   }
   for (int i = 0; i < 2; ++i) HSB_CUDA_C(cudaEventCreate(&h->ev_time[i]));
-  HSB_CUDA_C(cudaMalloc(&h->d_dirty_all, (HSB_MAX_LEVELS * 8 + 4) * sizeof(int)));   // + the replication error counter
-  HSB_CUDA_C(cudaMemset(h->d_dirty_all, 0, (HSB_MAX_LEVELS * 8 + 4) * sizeof(int)));
+  HSB_CUDA_C(cudaMalloc(&h->d_dirty_all, (kOverflowWord + 4) * sizeof(int)));
+  HSB_CUDA_C(cudaMemset(h->d_dirty_all, 0, (kOverflowWord + 4) * sizeof(int)));
   HSB_CUDA_C(cudaHostAlloc(&h->h_pin, sizeof(PinnedSlots), cudaHostAllocMapped));
   HSB_CUDA_C(cudaHostGetDevicePointer(&h->h_pin_dev, h->h_pin, 0));
   // pinned memory comes back from earlier allocations with their contents: a nowait step polls step_seq for its
@@ -785,7 +789,7 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
     HSB_CUDA_C(cudaMalloc(&L.logodds, n * sizeof(float)));
     HSB_CUDA_C(cudaMalloc(&L.prob, n * sizeof(float)));
     HSB_CUDA_C(cudaMalloc(&L.stamp, n * sizeof(uint32_t)));
-    L.dirty = h->d_dirty_all + 8 * l;
+    L.dirty = h->d_dirty_all + HSB_DIRTY_WORDS * l;
     HSB_CUDA_C(cudaMalloc(&L.scratch, 16 * sizeof(int)));
     {
       const int clean[16] = {0, INT_MAX, INT_MAX, -1, -1, 0, 0, 0, 0, INT_MAX, INT_MAX, -1, -1, 0, 0, 0};
@@ -814,8 +818,11 @@ int hsb_create(const hsb_config* cfg, hsb_handle** out) {
     res *= 2.0f;  // :68
   }
   {
-    int clean[HSB_MAX_LEVELS * 8];
-    for (int i = 0; i < HSB_MAX_LEVELS * 8; ++i) clean[i] = (i & 2) ? -1 : INT_MAX;
+    int clean[kOverflowWord];
+    for (int i = 0; i < kOverflowWord; ++i) {
+      const int w = i % HSB_DIRTY_WORDS;
+      clean[i] = w == HSB_DIRTY_CLEARED ? 0 : (w & 2) ? -1 : INT_MAX;
+    }
     HSB_CUDA_C(cudaMemcpyAsync(h->d_dirty_all, clean, sizeof(clean), cudaMemcpyHostToDevice, h->stream));
   }
   HSB_TRY(reset_gate(h));
@@ -2300,19 +2307,32 @@ int hsb_covariance_batch(hsb_handle* h, int level, int B, const float* poses, co
   return single_score(h, SCORE_COVARIANCE, level, B, poses, pts, offsets, n_shared, nullptr, out_cov_map, out_cov_world);
 }
 
+// A level's replication rectangle as a host reader sees it: the whole level while the cleared flag is set (the level
+// was cleared by hsb_group_reset and not shipped since), so the two-step protocol ships what it ships after hsb_reset.
+static void replication_rect(const Level& L, const int* words, int* rect) {
+  if (words[HSB_DIRTY_CLEARED]) {
+    const int full[4] = {0, 0, L.sx - 1, L.sy - 1};
+    memcpy(rect, full, sizeof(full));
+  } else {
+    memcpy(rect, words, 4 * sizeof(int));
+  }
+}
+
 static int get_dirty(hsb_handle* h, int level, int which, int rect[4], int reset) {
   if (!h || level < 0 || level >= h->levels || !rect) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
   Level& L = h->lv[level];
   int* src = L.dirty + 4 * which;
-  int* pin = h->h_pin->rect;
-  HSB_CUDA(h, cudaMemcpyAsync(pin, src, 4 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  int* pin = h->h_pin->dirty;
+  HSB_CUDA(h, cudaMemcpyAsync(pin, L.dirty, HSB_DIRTY_WORDS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   if (reset) {
     static const int clean[4] = {INT_MAX, INT_MAX, -1, -1};
     HSB_CUDA(h, cudaMemcpyAsync(src, clean, sizeof(clean), cudaMemcpyHostToDevice, h->stream));
+    if (which == 0) HSB_CUDA(h, cudaMemsetAsync(L.dirty + HSB_DIRTY_CLEARED, 0, sizeof(int), h->stream));
   }
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
-  memcpy(rect, pin, 4 * sizeof(int));
+  if (which == 0) replication_rect(L, pin, rect);
+  else memcpy(rect, pin + 4, 4 * sizeof(int));
   return HSB_OK;
 }
 int hsb_get_dirty_rect(hsb_handle* h, int level, int rect[4], int reset) { return get_dirty(h, level, 0, rect, reset); }
@@ -2322,14 +2342,16 @@ int hsb_get_mirror_dirty_rect(hsb_handle* h, int level, int rect[4], int reset) 
 int hsb_get_dirty_rects(hsb_handle* h, int* rects, int reset) {
   if (!h || !rects) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  int all[HSB_MAX_LEVELS * 8];
+  int all[kOverflowWord];
   HSB_CUDA(h, cudaMemcpyAsync(all, h->d_dirty_all, sizeof(all), cudaMemcpyDeviceToHost, h->stream));
   HSB_CUDA(h, cudaStreamSynchronize(h->stream));
-  for (int l = 0; l < h->levels; ++l) memcpy(rects + 4 * l, all + 8 * l, 4 * sizeof(int));
+  for (int l = 0; l < h->levels; ++l) replication_rect(h->lv[l], all + HSB_DIRTY_WORDS * l, rects + 4 * l);
   if (reset) {
     for (int l = 0; l < h->levels; ++l) {
-      all[8 * l + 0] = all[8 * l + 1] = INT_MAX;
-      all[8 * l + 2] = all[8 * l + 3] = -1;
+      int* w = all + HSB_DIRTY_WORDS * l;
+      w[0] = w[1] = INT_MAX;
+      w[2] = w[3] = -1;
+      w[HSB_DIRTY_CLEARED] = 0;
     }
     HSB_CUDA(h, cudaMemcpyAsync(h->d_dirty_all, all, sizeof(all), cudaMemcpyHostToDevice, h->stream));
     HSB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -2407,7 +2429,7 @@ static void fill_tile_params(hsb_handle* h, HsbTileParams& T, float* d_buf, size
   }
   T.buf = d_buf;
   T.capacity_words = std::min<size_t>(capacity_bytes / 4, 0xffffffffu);
-  T.error_count = h->d_dirty_all + HSB_MAX_LEVELS * 8;
+  T.error_count = h->d_dirty_all + kOverflowWord;
   T.K = 1;
   T.M = 1;
 }
@@ -2443,7 +2465,7 @@ int hsb_unpack_dirty_device(hsb_handle* h, const float* d_buf, size_t capacity_b
 int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset) {
   if (!h || !count) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  int* d = h->d_dirty_all + HSB_MAX_LEVELS * 8;
+  int* d = h->d_dirty_all + kOverflowWord;
   HSB_CUDA(h, cudaDeviceSynchronize());
   HSB_CUDA(h, cudaMemcpy(count, d, sizeof(int), cudaMemcpyDeviceToHost));
   if (reset) HSB_CUDA(h, cudaMemset(d, 0, sizeof(int)));
@@ -2638,6 +2660,8 @@ struct hsb_group {
   HsbTileLevelDev* d_tile_lv = nullptr;
   int** d_tile_counters = nullptr;
   cudaEvent_t ev_tile[2] = {nullptr, nullptr};
+  // map reset (hsb_group_reset): per member its stamp planes and gate state, next to its row of d_tile_lv
+  HsbResetMemberDev* d_reset = nullptr;
 };
 
 namespace {
@@ -2684,6 +2708,7 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->d_best) cudaFree(g->d_best);
   if (g->d_tile_lv) cudaFree(g->d_tile_lv);
   if (g->d_tile_counters) cudaFree(g->d_tile_counters);
+  if (g->d_reset) cudaFree(g->d_reset);
   for (cudaEvent_t e : g->ev_tile)
     if (e) cudaEventDestroy(e);
   if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
@@ -2799,6 +2824,14 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
     HSB_GROUP_CUDA(cudaMemcpy(g->d_tile_lv, tile.data(), tile.size() * sizeof(HsbTileLevelDev), cudaMemcpyHostToDevice));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_tile_counters, counters.size() * sizeof(int*)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_tile_counters, counters.data(), counters.size() * sizeof(int*), cudaMemcpyHostToDevice));
+    std::vector<HsbResetMemberDev> reset(M);
+    memset(reset.data(), 0, reset.size() * sizeof(HsbResetMemberDev));
+    for (int s = 0; s < M; ++s) {
+      reset[s].gate = g->m[s]->d_gate;
+      for (int l = 0; l < g->levels; ++l) reset[s].stamp[l] = g->m[s]->lv[l].stamp;
+    }
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_reset, reset.size() * sizeof(HsbResetMemberDev)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_reset, reset.data(), reset.size() * sizeof(HsbResetMemberDev), cudaMemcpyHostToDevice));
     for (cudaEvent_t& e : g->ev_tile) HSB_GROUP_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
@@ -3588,7 +3621,7 @@ void fill_group_tile_params(hsb_group* g, HsbTileParams& T, float* d_buf, size_t
   T.levels = g->levels;
   T.buf = d_buf;
   T.capacity_words = std::min<size_t>(capacity_bytes / 4, 0xffffffffu);
-  T.error_count = g->m[0]->d_dirty_all + HSB_MAX_LEVELS * 8;
+  T.error_count = g->m[0]->d_dirty_all + kOverflowWord;
   T.table = g->d_tile_lv;
   T.counters = g->d_tile_counters;
   T.K = K;
@@ -3673,6 +3706,76 @@ int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capac
   h0->launches++;
   HSB_CUDA(h0, cudaGetLastError());
   return tile_order_after(g, user, M, nullptr, true);
+}
+
+}  // extern "C"
+
+// ---- group map reset: hsb_reset for K members in one launch, replicated as a clear record ---------------------------
+namespace {
+
+// hsb_reset for the K members members[k] (members == g->all: every member, no list in the launch) with one launch on
+// the group's stream and no synchronise; the replication rectangles are left clean with the cleared flags set.
+int group_reset(hsb_group* g, const char* fn, int K, const int* members) {
+  hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is listed
+  const bool all = members == g->all.data();
+  int s = check_members(g, fn, K, members);
+  if (s != HSB_OK || K == 0) return s;
+  if (!all && K > kTileSubsetMax)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: K is %d, a subset reset lists at most %d sessions", fn, K, kTileSubsetMax);
+  DeviceGuard guard(g->device);
+  cudaStream_t st = g->stream;
+  if ((s = order_members(g, K, members)) != HSB_OK) return s;
+  HsbResetParams P;
+  P.table = g->d_tile_lv;
+  P.mem = g->d_reset;
+  P.levels = g->levels;
+  P.K = K;
+  // blockIdx.y: session; blockIdx.x: about four waves of the device's CTAs over all sessions, no more than a level-0
+  // plane has 256-cell stretches
+  size_t max_cells = 0;
+  for (int k = 0; k < K; ++k) {
+    const Level& L0 = g->m[members[k]]->lv[0];
+    max_cells = std::max(max_cells, (size_t)L0.sx * L0.sy);
+  }
+  const size_t want = ((size_t)h0->sm_count * 32 + K - 1) / K;
+  const dim3 grid((unsigned)std::max<size_t>(1, std::min(want, (max_cells + 255) / 256)), (unsigned)std::min(K, 65535));
+  if (all) {
+    hsb::group_reset_kernel<<<grid, 256, 0, st>>>(P);
+  } else if (K <= kTileSubsetSmall) {
+    hsb::TileMembers<kTileSubsetSmall> S;
+    memcpy(S.idx, members, (size_t)K * sizeof(int));
+    hsb::group_reset_subset_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S);
+  } else {
+    std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
+    memcpy(S->idx, members, (size_t)K * sizeof(int));
+    hsb::group_reset_subset_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S);
+  }
+  h0->launches++;
+  HSB_CUDA(h0, cudaGetLastError());
+  HSB_CUDA(h0, cudaEventRecord(g->ev, st));
+  // every later call on a reset member runs after the reset (HandleScope; a match on a copy stream through
+  // map_write_pending), as after a nowait step; clear_level's host part
+  for (int k = 0; k < K; ++k) {
+    hsb_handle* h = g->m[members[k]];
+    for (int l = 0; l < h->levels; ++l) h->lv[l].stamp_base = 0;
+    h->group_ev = g->ev;
+    h->map_write_pending = true;
+  }
+  return HSB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hsb_group_reset(hsb_group* g) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_reset(g, "hsb_group_reset", (int)g->m.size(), g->all.data());
+}
+
+int hsb_group_reset_subset(hsb_group* g, int K, const int* members) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_reset(g, "hsb_group_reset_subset", K, members);
 }
 
 }  // extern "C"

@@ -169,11 +169,21 @@ struct HsbUpdateLevelDev {
   int slot;
 };
 
+// A level's replication words in device memory (hsb_handle::d_dirty_all, one run of HSB_DIRTY_WORDS per level):
+// [0..3] replication rectangle {xmin, ymin, xmax, ymax} (hsb_get_dirty_rect), [4..7] host-mirror rectangle
+// (hsb_get_mirror_dirty_rect), [8] cleared flag: hsb_group_reset cleared the level since its last shipped pack, so a
+// pack ships the clear record plus the replication rectangle (written since the clear) instead of the whole level.
+#define HSB_DIRTY_WORDS 9
+#define HSB_DIRTY_CLEARED 8
+
 // One-shot, host-free tile transport (hsb_pack_dirty_device / hsb_unpack_dirty_device): buffer layout in 4-byte words —
 // [0] magic, [1] levels, [2] overflow (1 = the dirty area did not fit, nothing packed), [3] total cells,
-// [4 + 4 l ..] rectangle {x0, y0, x1, y1} of level l (x1 < x0: clean), [HSB_TILE_HEADER_WORDS ..] the log-odds rows of
-// level 0's rectangle, then level 1's, ...
+// [4 + 4 l ..] rectangle {x0, y0, x1, y1} of level l (x1 < x0: clean), [HSB_TILE_CLEARED_WORD] the clear record: bit l
+// set = level l was cleared (hsb_group_reset) before the cells of its rectangle were written, so a replica clears the
+// level outside the rectangle (0 when nothing was cleared; every pack writes it), [HSB_TILE_HEADER_WORDS ..] the
+// log-odds rows of level 0's rectangle, then level 1's, ...
 #define HSB_TILE_HEADER_WORDS 64
+#define HSB_TILE_CLEARED_WORD (4 + 4 * HSB_MAX_LEVELS)
 #define HSB_TILE_MAGIC 0x48534254
 // A group's buffer (hsb_group_pack_dirty_device / hsb_group_unpack_dirty_device): a group header of G words —
 // [0] HSB_TILE_GROUP_MAGIC, [1] K, [2] levels, [3] deferred blocks, [4] words used (G + 64 K + shipped cells),
@@ -191,7 +201,19 @@ struct HsbTileLevelDev {
   float* prob;
   cudaSurfaceObject_t surf;
   int sx, sy;
-  int* dirty;   // [0..3] replication rectangle, [4..7] host-mirror rectangle
+  int* dirty;   // the level's HSB_DIRTY_WORDS: [0..3] replication rectangle, [4..7] host-mirror rectangle, [8] cleared flag
+};
+// What a group reset (hsb_group_reset) clears beyond a member's tile descriptors: its stamp planes and its gate state
+// (hsb_handle::d_gate: lastMapUpdatePose[3], write flag).  One entry per member (hsb_group::d_reset).
+struct HsbResetMemberDev {
+  float* gate;
+  uint32_t* stamp[HSB_MAX_LEVELS];
+};
+// A group reset: session k (blockIdx.y) clears every level of member S.member(k).
+struct HsbResetParams {
+  const HsbTileLevelDev* table;     // M x levels, member-major (hsb_group::d_tile_lv)
+  const HsbResetMemberDev* mem;     // M (hsb_group::d_reset)
+  int levels, K;
 };
 struct HsbTileParams {
   HsbTileLevelDev lv[HSB_MAX_LEVELS];   // a single handle's levels (table == nullptr)

@@ -25,6 +25,7 @@
 #ifndef HSB_UPDATE_KERNEL_CUH
 #define HSB_UPDATE_KERNEL_CUH
 
+#include <cfloat>
 #include <climits>
 
 #include "hsb_internal.h"
@@ -53,18 +54,24 @@ __global__ void refresh_prob_kernel(const float* __restrict__ logodds, float* __
   }
 }
 
-// LogOddsCell::resetGridCell for a whole level (GridMapBase.h:71-82): l = 0, P(0) = 0.5, stamps 0.
+// LogOddsCell::resetGridCell (GridMapBase.h:71-82) of cell i of a level sx cells wide: l = 0, P(0) = 0.5 and the
+// texture twin.
+__device__ __forceinline__ void clear_cell(float* logodds, float* prob, cudaSurfaceObject_t surf, int sx, size_t i) {
+  logodds[i] = 0.0f;
+  prob[i] = 0.5f;
+  if (surf) {
+    const int y = (int)(i / (size_t)sx), x = (int)(i - (size_t)y * sx);
+    surf2Dwrite(0.5f, surf, x * (int)sizeof(float), y);
+  }
+}
+
+// resetGridCell for a whole level, stamps 0 too (hsb_reset, one level per launch).
 __global__ void clear_level_kernel(float* __restrict__ logodds, float* __restrict__ prob, uint32_t* __restrict__ stamp,
                                    cudaSurfaceObject_t surf, int sx, int sy) {
   const size_t n = (size_t)sx * (size_t)sy;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    logodds[i] = 0.0f;
-    prob[i] = 0.5f;
+    clear_cell(logodds, prob, surf, sx, i);
     stamp[i] = 0u;
-    if (surf) {
-      const int y = (int)(i / (size_t)sx), x = (int)(i - (size_t)y * sx);
-      surf2Dwrite(0.5f, surf, x * (int)sizeof(float), y);
-    }
   }
 }
 
@@ -583,6 +590,7 @@ struct TileChunk {
   unsigned row0[kTileChunk + 1];           // shipped rows of the chunk before the block's; row0[n]: all of them
   int member[kTileChunk];
   int ship[kTileChunk];                    // 1: rows shipped, 0: deferred
+  unsigned cleared[kTileChunk];            // the block's clear record (HSB_TILE_CLEARED_WORD; unpack: shipped blocks only)
 };
 
 __device__ __forceinline__ bool tile_dirty(int4 r) { return r.z >= r.x && r.w >= r.y; }
@@ -698,15 +706,17 @@ __device__ __forceinline__ void pack_dirty_body(const HsbTileParams& P, const Se
       const int m = S.member(k0 + j);
       const HsbTileLevelDev* lv = tile_levels(P, m);
       unsigned long long cells = 0;
-      unsigned rows = 0;
+      unsigned rows = 0, cleared = 0;
       for (int l = 0; l < levels; ++l) {
         const int* d = lv[l].dirty;
         const int4 q = make_int4(d[0], d[1], d[2], d[3]);
         c.rect[j][l] = q;
         cells += (unsigned long long)(tile_w(q) * tile_h(q));
         rows += (unsigned)tile_h(q);
+        if (d[HSB_DIRTY_CLEARED]) cleared |= 1u << l;
       }
       c.member[j] = m;
+      c.cleared[j] = cleared;
       c.cells[j] = cells;
       c.row0[j + 1] = rows;
     }
@@ -754,6 +764,7 @@ __device__ __forceinline__ void pack_dirty_body(const HsbTileParams& P, const Se
         const int4 q = c.rect[j][l];
         hdr[4 + 4 * l] = q.x; hdr[5 + 4 * l] = q.y; hdr[6 + 4 * l] = q.z; hdr[7 + 4 * l] = q.w;
       }
+      hdr[HSB_TILE_CLEARED_WORD] = (int)c.cleared[j];
       if (group) {
         int* gh = reinterpret_cast<int*>(P.buf);
         gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * (k0 + j)] = c.member[j];
@@ -783,8 +794,9 @@ __global__ void __launch_bounds__(256) pack_dirty_subset_kernel(const __grid_con
   pack_dirty_body(P, S);
 }
 
-// after pack (stream order): the shipped blocks' rectangles are forgotten, a deferred block's are kept.  One thread per
-// (block, level, coordinate); the block's member and start come from the group header (a single handle: member 0, 0).
+// after pack (stream order): the shipped blocks' rectangles and cleared flags are forgotten, a deferred block's are kept.
+// One thread per (block, level, coordinate); the block's member and start come from the group header (a single handle:
+// member 0, 0).
 __global__ void reset_dirty_kernel(const __grid_constant__ HsbTileParams P) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int per = 4 * P.levels, k = i / per;
@@ -794,7 +806,52 @@ __global__ void reset_dirty_kernel(const __grid_constant__ HsbTileParams P) {
   const unsigned long long start = P.table ? (unsigned)gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k + 1] : 0u;
   if (reinterpret_cast<const int*>(P.buf + start)[2] != 0) return;
   const int l = (i - k * per) >> 2, q = i & 3;
-  tile_levels(P, member)[l].dirty[q] = (q < 2) ? INT_MAX : -1;
+  int* d = tile_levels(P, member)[l].dirty;
+  d[q] = (q < 2) ? INT_MAX : -1;
+  if (q == 0) d[HSB_DIRTY_CLEARED] = 0;
+}
+
+// hsb_group_reset: hsb_reset's end state for every level of K members in one launch — log-odds 0, P 0.5, texture twin
+// 0.5 and stamps 0 over every plane (blockIdx.y = session; blockIdx.x strides over each of the member's levels in turn,
+// so every CTA of the launch clears the same share of a member and none idles while a level-0 plane finishes), then, by
+// thread l of the session's first CTA, level l's mirror rectangle := the whole level, its replication rectangle clean and
+// its cleared flag set (the next pack ships the clear record instead of the whole level), and by thread 0 the gate
+// state := lastMapUpdatePose FLT_MAX^3, write flag 0 (HectorSlamProcessor.h:117).
+template <class Sessions>
+__device__ __forceinline__ void group_reset_body(const HsbResetParams& P, const Sessions& S) {
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthreads = (size_t)gridDim.x * blockDim.x;
+  for (int k = blockIdx.y; k < P.K; k += gridDim.y) {
+    const int m = S.member(k);
+    const HsbTileLevelDev* lv = P.table + (size_t)m * P.levels;
+    for (int l = 0; l < P.levels; ++l) {
+      const HsbTileLevelDev L = lv[l];
+      uint32_t* stamp = P.mem[m].stamp[l];
+      const size_t n = (size_t)L.sx * (size_t)L.sy;
+      for (size_t i = tid; i < n; i += nthreads) {
+        clear_cell(L.logodds, L.prob, L.surf, L.sx, i);
+        stamp[i] = 0u;
+      }
+    }
+    if (blockIdx.x == 0 && threadIdx.x < P.levels) {
+      const HsbTileLevelDev L = lv[threadIdx.x];
+      int* d = L.dirty;
+      d[0] = INT_MAX; d[1] = INT_MAX; d[2] = -1; d[3] = -1;
+      d[4] = 0; d[5] = 0; d[6] = L.sx - 1; d[7] = L.sy - 1;
+      d[HSB_DIRTY_CLEARED] = 1;
+      if (threadIdx.x == 0) {
+        float* g = P.mem[m].gate;
+        g[0] = FLT_MAX; g[1] = FLT_MAX; g[2] = FLT_MAX; g[3] = 0.0f;
+      }
+    }
+  }
+}
+__global__ void __launch_bounds__(256) group_reset_kernel(const __grid_constant__ HsbResetParams P) {
+  group_reset_body(P, TileAll());
+}
+template <int N>
+__global__ void __launch_bounds__(256) group_reset_subset_kernel(const __grid_constant__ HsbResetParams P,
+                                                                 const __grid_constant__ TileMembers<N> S) {
+  group_reset_body(P, S);
 }
 
 // Unpack, pass 1: the buffer fits the replica (group header and every block's header inside the capacity, every shipped
@@ -816,6 +873,8 @@ __device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChun
   const int* hdr = reinterpret_cast<const int*>(P.buf + start);
   if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != P.levels) return false;
   const bool ship = hdr[2] == 0;
+  const unsigned cleared = (unsigned)hdr[HSB_TILE_CLEARED_WORD];
+  if (cleared >> P.levels) return false;   // a cleared level the replica does not have
   const HsbTileLevelDev* lv = tile_levels(P, member);
   unsigned long long cells = 0;
   unsigned rows = 0;
@@ -834,8 +893,33 @@ __device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChun
   c.cells[j] = cells;
   c.member[j] = member;
   c.ship[j] = ship ? 1 : 0;
+  c.cleared[j] = ship ? cleared : 0u;
   c.row0[j + 1] = ship ? rows : 0u;
   return true;
+}
+
+// Unpack's clear record: every cell of a cleared level outside the block's shipped rectangle is reset (log-odds 0, P
+// 0.5, texture twin 0.5), grid-stride over the plane.  Disjoint from the cells tile_rows writes, so both run in the one
+// unpack launch in any order.
+__device__ __forceinline__ void tile_clear(const HsbTileParams& P, const TileChunk& c, int n) {
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nthreads = (size_t)gridDim.x * blockDim.x;
+  for (int j = 0; j < n; ++j) {
+    const unsigned cleared = c.cleared[j];
+    if (!cleared) continue;
+    const HsbTileLevelDev* lv = tile_levels(P, c.member[j]);
+    for (int l = 0; l < P.levels; ++l) {
+      if (!((cleared >> l) & 1u)) continue;
+      const HsbTileLevelDev L = lv[l];
+      const int4 q = c.rect[j][l];
+      const bool inside_any = tile_dirty(q);
+      const size_t cells = (size_t)L.sx * (size_t)L.sy;
+      for (size_t i = tid; i < cells; i += nthreads) {
+        const int y = (int)(i / (size_t)L.sx), x = (int)(i - (size_t)y * L.sx);
+        if (inside_any && x >= q.x && x <= q.z && y >= q.y && y <= q.w) continue;
+        clear_cell(L.logodds, L.prob, L.surf, L.sx, i);
+      }
+    }
+  }
 }
 
 __global__ void __launch_bounds__(256) unpack_dirty_kernel(const __grid_constant__ HsbTileParams P) {
@@ -863,17 +947,17 @@ __global__ void __launch_bounds__(256) unpack_dirty_kernel(const __grid_constant
   for (int k0 = 0; k0 < K; k0 += kTileChunk) {
     const int j = threadIdx.x, n = min(kTileChunk, K - k0);
     if (j < n) tile_read_block(P, c, k0 + j, j);
-    __syncthreads();
+    const bool any_cleared = __syncthreads_or(j < n && c.cleared[j] != 0u);
     if (threadIdx.x < 32) tile_row_prefix(c, n);
     if (blockIdx.x == 0 && j < n) {
       const int m = c.member[j];
       if (!c.ship[j]) {   // a deferred block: counted once on its member's counter
         int* cnt = tile_counter(P, m);
         if (cnt) atomicAdd(cnt, 1);
-      } else {            // the replica's host mirror has to follow
+      } else {            // the replica's host mirror has to follow (a cleared level: all of it)
         const HsbTileLevelDev* lv = tile_levels(P, m);
         for (int l = 0; l < P.levels; ++l) {
-          const int4 q = c.rect[j][l];
+          const int4 q = (c.cleared[j] >> l) & 1u ? make_int4(0, 0, lv[l].sx - 1, lv[l].sy - 1) : c.rect[j][l];
           if (!tile_dirty(q)) continue;
           int* md = lv[l].dirty + 4;
           atomicMin(md + 0, q.x); atomicMin(md + 1, q.y);
@@ -883,6 +967,7 @@ __global__ void __launch_bounds__(256) unpack_dirty_kernel(const __grid_constant
     }
     __syncthreads();
     tile_rows<false>(P, c, n);
+    if (any_cleared) tile_clear(P, c, n);
     __syncthreads();
   }
 }

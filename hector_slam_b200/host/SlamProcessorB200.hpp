@@ -255,6 +255,21 @@ class SlamProcessor {
     check(hsb_reset(h_));
   }
 
+  // reset() for the processors ps[members[0..K)] of ps[0..M) in one launch (hsb_group_reset_subset, through the group
+  // updateMany keeps; members null: all M, hsb_group_reset, and K is not read): the node's reset_map service or "reset"
+  // system message for a fleet.  restart_mapping_with_new_pose for K robots is resetMany() followed by their next step
+  // with the new poses as hints.  Returns once the reset is queued; every later call on a reset processor runs after it.
+  static void resetMany(SlamProcessor* const* ps, int M, const int* members = 0, int K = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "resetMany");
+    hsb_group* g = owner.groupFor(ps, M);
+    owner.check(members ? hsb_group_reset_subset(g, K, members) : hsb_group_reset(g));
+    for (int k = 0; k < (members ? K : M); ++k) {
+      SlamProcessor& p = *ps[members ? members[k] : k];
+      p.lastMapUpdatePose_ = Pose{FLT_MAX, FLT_MAX, FLT_MAX};   // as reset()
+      p.lastScanMatchPose_ = Pose{0.f, 0.f, 0.f};
+    }
+  }
+
   const Pose& getLastScanMatchPose() const { return lastScanMatchPose_; }
   const float* getLastScanMatchCovariance() const { return lastScanMatchCov_; }
   float getScaleToMap() const { return hsb_get_scale_to_map(h_); }

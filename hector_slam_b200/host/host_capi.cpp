@@ -411,6 +411,16 @@ int hsbp_reset(void* p) {
   }
   return 0;
 }
+int hsbp_reset_many(void* const* ps, int M, const int* members, int K) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  try {
+    hsb200::SlamProcessor::resetMany(procs.data(), M, members, K);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 void hsbp_set_update_factors(void* p, float ffree, float focc) {
   static_cast<hsb200::SlamProcessor*>(p)->setUpdateFactorFree(ffree);
   static_cast<hsb200::SlamProcessor*>(p)->setUpdateFactorOccupied(focc);

@@ -678,7 +678,8 @@ int hsb_get_dirty_rects(hsb_handle* h, int* rects, int reset);
 /* Ordering: `stream` may be any stream of the caller.  pack waits for the map writes the handle has queued and the
  * handle's next map write waits for pack; unpack waits for everything the handle has queued (matches still reading
  * the planes) and everything the handle queues afterwards waits for unpack — no synchronisation is needed around
- * them.  After hsb_reset / hsb_upload_level the dirty rectangle is the whole level. */
+ * them.  After hsb_reset / hsb_upload_level the dirty rectangle is the whole level; after hsb_group_reset it reads as the
+ * whole level until a reset consumes it (the cleared flag, see hsb_group_reset). */
 int hsb_pack_rect_device(hsb_handle* h, int level, const int rect[4], float* d_buf, void* stream);
 int hsb_unpack_rect_device(hsb_handle* h, int level, const int rect[4], const float* d_buf, void* stream);
 
@@ -728,6 +729,36 @@ int hsb_group_pack_dirty_device(hsb_group* g, float* d_buf, size_t capacity_byte
 int hsb_group_pack_dirty_device_subset(hsb_group* g, int K, const int* members, float* d_buf, size_t capacity_bytes,
                                        int reset, void* stream);
 int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capacity_bytes, void* stream);
+/* MapRepresentationInterface::reset (MapRepMultiMap.h:83-90) for K of the group's members in one launch: the node's
+ * reset_map service, a "reset" system message, and restart_mapping_with_new_pose (reset, then pass the new pose as the
+ * member's next step hint) for many robots.  Session k resets member members[k] (hsb_group_reset: every member).
+ * End state: each listed member is left in the state hsb_reset leaves — every level's log-odds 0 and probability 0.5,
+ * texture twin 0.5, stamps 0, lastMapUpdatePose FLT_MAX^3 and write flag 0, mirror rectangle (hsb_get_mirror_dirty_rect)
+ * the whole level; its last match's container, formats, update factors and gate thresholds stay as they are — with one
+ * difference in the replication state: each level's replication rectangle is left clean and the level's cleared flag
+ * is set; the map writer grows the rectangle from clean as usual.  The tile transport ships the clear record instead of
+ * the whole level: every block hsb_pack_dirty_device / hsb_group_pack_dirty_device(_subset) writes carries in header
+ * word 36 the mask of its member's levels cleared since their last shipped pack (0: none), its rows are only the cells
+ * written since the reset (a reset with nothing written after it ships a 256-byte header), and first fit counts only
+ * those cells; `reset` clears a shipped block's flags with its rectangles, a deferred block keeps both.  Unpack (single
+ * or group) applies a shipped block with bit l set by resetting every cell of level l outside the shipped rectangle
+ * (log-odds 0, probability 0.5, texture twin 0.5) and writing the shipped rows inside it, in its one launch; the
+ * replica's mirror rectangle of level l becomes the whole level and its replication rectangle and flags stay clean.  A
+ * block with a mask bit >= levels makes the buffer one that does not fit (counted once on handles[0], nothing applied).
+ * hsb_get_dirty_rect and hsb_get_dirty_rects report the whole level while its flag is set, and their `reset` clears the
+ * flag with the rectangle, so the two-step protocol ships what it ships after hsb_reset.  hsb_reset and
+ * hsb_upload_level leave the flag clear (whole-level rectangles, as before).
+ * A member not listed is neither read nor changed.
+ * Ordering: the reset runs on the group's stream after everything queued on the listed members (their own work and a
+ * pending step of any group they belong to) and returns once queued, without a synchronise; every later call on a
+ * listed member runs after it.
+ * Cost: one launch, counted on handles[0], whatever K is; the member list travels in the launch parameters (no
+ * host-to-device copy), at most 4096 sessions in a subset.
+ * Rejected with HSB_ERR_INVALID_ARG before anything is queued: K < 0 or K > M; members == NULL with K > 0; an index
+ * outside [0, M) or listed twice (the message names the session); a subset of more than 4096 sessions.  K = 0 returns
+ * HSB_OK and queues nothing. */
+int hsb_group_reset(hsb_group* g);
+int hsb_group_reset_subset(hsb_group* g, int K, const int* members);
 
 /* ---- after the path: what the node does with the results -------------------------------------*/
 /* nav_msgs/OccupancyGrid cell values of one level, as HectorMappingRos::publishMap derives them
