@@ -2159,32 +2159,46 @@ int hsb_best_hypothesis_device(hsb_handle* h, int level, int B, const float* d_p
 
 namespace {
 
-// What a pose-scoring call computes for every pose (likelihood, covariance) or session (best hypothesis).
-enum ScoreKind { SCORE_LIKELIHOOD, SCORE_COVARIANCE, SCORE_BEST };
+// What a pose query computes for every pose (likelihood, covariance, the group match's pose and Hessian from a hint) or
+// session (best hypothesis).
+enum ScoreKind { SCORE_LIKELIHOOD, SCORE_COVARIANCE, SCORE_BEST, SCORE_MATCH };
 constexpr size_t kScoreChunk = 1 << 20;   // most bytes of points score_query stages in its pinned copy
 
-// Every host-buffer pose-scoring body (hsb_likelihood_batch, hsb_covariance_batch and the group calls): Q poses of K
-// sessions, session k's poses [pose_offsets[k], pose_offsets[k+1]) scored on member sess[k].member's map of `level`,
-// whose descriptor is lv[member * levels + level] — or, with lv NULL, h's own level, staged with the poses as a one-entry
-// table.  sessions(sess, pose_offsets, staged) writes the K session descriptors and K + 1 pose offsets into the staging;
-// `staged` is where the n_pts points of `pts` will lie on the device, so a session's scan is a slice of them or any
-// other device scan the caller knows of.  One host-to-device copy from the pinned staging hs (points past kScoreChunk
-// bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K arg-max accumulators are
-// `best`), one device-to-host copy of the asked-for results and one synchronise.  The launches and any error are
-// counted on h.  sessions() also gives each session its member's cell length of `level` (the covariance's world matrix).
+// The group match's part of a score_query (SCORE_MATCH): the launch shape group_match chose, W warps per scan and
+// max_n, the longest scan of a session with hints (launch_match_t sizes its staging by it), and where the results go.
+struct MatchQuery {
+  int W, max_n;
+  float* out_poses;   // Q x 3
+  float* out_cov;     // Q x 9 Hessians, or NULL
+};
+
+// Every host-buffer pose-query body (hsb_likelihood_batch, hsb_covariance_batch, the group scoring calls and the group
+// match): Q poses of K sessions, session k's poses [pose_offsets[k], pose_offsets[k+1]) scored on member
+// sess[k].member's map of `level`, whose descriptor is lv[member * levels + level] — or, with lv NULL, h's own level,
+// staged with the poses as a one-entry table.  For SCORE_MATCH the poses are hints, each matched over every level of
+// its member's row of lv.  sessions(sess, pose_offsets, staged) writes the K session descriptors and K + 1 pose
+// offsets into the staging; `staged` is where the n_pts points of `pts` will lie on the device, so a session's scan is
+// a slice of them or any other device scan the caller knows of.  One host-to-device copy from the pinned staging hs
+// (points past kScoreChunk bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K
+// arg-max accumulators are `best`; the match's in match->W), one device-to-host copy of the asked-for results and one
+// synchronise.  The launches, the match's launch shape and any error are counted on h.  sessions() also gives each
+// session its member's cell length of `level` (the covariance's world matrix).
 template <typename Sessions>
 int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage, const HsbLevelDev* lv,
                 int levels, int level, ScoreKind kind, int K, int Q, const float* poses, const float* pts, size_t n_pts,
                 const Sessions& sessions, unsigned long long* best, float* out_lh, float* out_map, float* out_world,
-                float* out_best4, int* out_best_index) {
+                float* out_best4, int* out_best_index, const MatchQuery* match = nullptr) {
   // staging: sessions | pose offsets | (level descriptor) | poses | scans, then the results: likelihoods | best4 | best
-  // index, or covariance (map) | covariance (world), each only if asked for
+  // index, or covariance (map) | covariance (world), or poses | Hessians, each only if asked for
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
   const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_lv = al(o_off + (size_t)(K + 1) * 4);
   const size_t o_poses = lv ? o_lv : al(o_lv + sizeof(HsbLevelDev));
   const size_t o_pts = al(o_poses + (size_t)Q * 12), in_end = o_pts + n_pts * 8, o_out = al(in_end);
-  size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, out_end = o_out;
-  if (kind == SCORE_COVARIANCE) {
+  size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, o_cov = o_out, out_end = o_out;
+  if (kind == SCORE_MATCH) {
+    o_cov = o_out + (size_t)Q * 12;
+    out_end = o_cov + (match->out_cov ? (size_t)Q * 36 : 0);
+  } else if (kind == SCORE_COVARIANCE) {
     o_world = o_map + (out_map ? (size_t)Q * 36 : 0);
     out_end = o_world + (out_world ? (size_t)Q * 36 : 0);
   } else {
@@ -2223,7 +2237,30 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   P.K = K;
   P.Q = Q;
   const bool tex = h->gather_mode == HSB_GATHER_TEX;
-  if (kind == SCORE_COVARIANCE) {
+  if (kind == SCORE_MATCH) {
+    HsbMatchParams M;
+    fill_match_params(h, M);   // (lv[] is unused: every hint reads its member's row of the group's table)
+    M.B = Q;
+    M.hints = P.poses;
+    M.kind = HSB_IN_ENDPOINTS;
+    M.out_poses = reinterpret_cast<float*>(ds + o_out);
+    M.out_cov = match->out_cov ? reinterpret_cast<float*>(ds + o_cov) : nullptr;
+    M.group_lv = lv;
+    M.match_sess = P.sess;
+    M.match_offsets = P.pose_offsets;
+    M.match_K = K;
+    s = HSB_ERR_UNSUPPORTED;
+#define HSB_GM_CASE(w)                                                                                                 \
+  if (match->W == w)                                                                                                   \
+    s = tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h, M, match->max_n, st, 1)          \
+            : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h, M, match->max_n, st, 1);
+    HSB_GM_CASE(1);
+    HSB_GM_CASE(2);
+    HSB_GM_CASE(4);
+    HSB_GM_CASE(8);
+#undef HSB_GM_CASE
+    if (s != HSB_OK) return s;
+  } else if (kind == SCORE_COVARIANCE) {
     P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
     P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
     const int blocks = std::min(Q, h->sm_count * 8);
@@ -2250,7 +2287,10 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   HSB_CUDA(h, cudaGetLastError());
   HSB_CUDA(h, cudaMemcpyAsync(hs + o_out, ds + o_out, out_end - o_out, cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
-  if (kind == SCORE_COVARIANCE) {
+  if (kind == SCORE_MATCH) {
+    memcpy(match->out_poses, hs + o_out, (size_t)Q * 12);
+    if (match->out_cov) memcpy(match->out_cov, hs + o_cov, (size_t)Q * 36);
+  } else if (kind == SCORE_COVARIANCE) {
     if (out_map) memcpy(out_map, hs + o_map, (size_t)Q * 36);
     if (out_world) memcpy(out_world, hs + o_world, (size_t)Q * 36);
   } else {
@@ -2879,9 +2919,6 @@ struct GroupInput {
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
 constexpr int kGroupW = 8;
 
-// One group step of any input kind over K of the group's members: session k steps member members[k] (a step of every
-// member passes K = M and g->all).  Members not listed are neither read nor changed.  Everything that can reject the
-// step is checked before any member's state moves.
 // The member list of a group call over K sessions: 0 <= K <= M, and with K > 0 a list of distinct indices in [0, M).
 int check_members(hsb_group* g, const char* fn, int K, const int* members) {
   hsb_handle* h0 = g->m[0];
@@ -2897,6 +2934,17 @@ int check_members(hsb_group* g, const char* fn, int K, const int* members) {
     if (g->listed[j]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is listed twice", fn, k, j);
     g->listed[j] = 1;
   }
+  return HSB_OK;
+}
+
+// The K + 1 offsets `name` of a group call's sessions: given, starting at 0, never decreasing.
+int check_offsets(hsb_handle* h0, const char* fn, const char* name, int K, const int* offsets) {
+  if (!offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", fn, name);
+  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s[0] is %d, must be 0", fn, name, offsets[0]);
+  for (int k = 0; k < K; ++k)
+    if (offsets[k + 1] < offsets[k])
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s decrease at session %d (%d -> %d)", fn, name, k, offsets[k],
+                  offsets[k + 1]);
   return HSB_OK;
 }
 
@@ -2916,6 +2964,9 @@ int order_members(hsb_group* g, int K, const int* members) {
   return HSB_OK;
 }
 
+// One group step of any input kind over K of the group's members: session k steps member members[k] (a step of every
+// member passes K = M and g->all).  Members not listed are neither read nor changed.  Everything that can reject the
+// step is checked before any member's state moves.
 int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, const int* map_without_matching,
                int nowait, float* out_poses, float* cov_inout, int* map_updated, int* out_kept) {
   hsb_handle* h0 = g->m[0];   // launches and errors are accounted on handles[0], whether or not it is stepped
@@ -2928,15 +2979,9 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   const int* offsets = in.offsets;
   if (!in.hints || !offsets || !out_poses)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints, offsets and out_poses must not be NULL", in.fn);
-  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", in.fn, offsets[0]);
+  if ((s = check_offsets(h0, in.fn, "offsets", K, offsets)) != HSB_OK) return s;
   int max_n = 0;
-  for (int k = 0; k < K; ++k) {
-    const int n = offsets[k + 1] - offsets[k];
-    if (n < 0)
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets decrease at session %d (%d -> %d)", in.fn, k, offsets[k],
-                  offsets[k + 1]);
-    max_n = std::max(max_n, n);
-  }
+  for (int k = 0; k < K; ++k) max_n = std::max(max_n, offsets[k + 1] - offsets[k]);
   const int total = offsets[K];
   if (total > 0 && !in.pts)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", in.fn, cloud ? "points_xyz" : conv ? "ranges" : "points_xy");
@@ -3196,12 +3241,7 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
   if (s != HSB_OK || K == 0) return s;
   if (level < 0 || level >= g->levels)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
-  if (!offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets is NULL", fn);
-  if (offsets[0] != 0) return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets[0] is %d, must be 0", fn, offsets[0]);
-  for (int k = 0; k < K; ++k)
-    if (offsets[k + 1] < offsets[k])
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: offsets decrease at session %d (%d -> %d)", fn, k, offsets[k],
-                  offsets[k + 1]);
+  if ((s = check_offsets(h0, fn, "offsets", K, offsets)) != HSB_OK) return s;
   const int Q = offsets[K];
   if (Q == 0) return HSB_OK;
   if (!begin || !end || !out_dist)
@@ -3213,10 +3253,41 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
                    world, K, members, offsets, begin, end, out_dist, out_hit, out_found);
 }
 
+// The scans of a group pose query (scoring or match): session k's is pts[scan_offsets[k] .. scan_offsets[k+1]), staged
+// with the call, or, with pts and scan_offsets both NULL, its member's last-match container as it is on the device when
+// the call runs.
+int check_scans(hsb_handle* h0, const char* fn, int K, const float* pts, const int* scan_offsets) {
+  if (!pts != !scan_offsets)
+    return fail(h0, HSB_ERR_INVALID_ARG, "%s: points_xy and scan_offsets must both be given or both be NULL", fn);
+  return pts ? check_offsets(h0, fn, "scan_offsets", K, scan_offsets) : HSB_OK;
+}
+
+// The length of session k's scan on member h by check_scans' rule (a member that never matched has no container: 0).
+int scan_length(const hsb_handle* h, const int* scan_offsets, int k) {
+  if (scan_offsets) return scan_offsets[k + 1] - scan_offsets[k];
+  return h->d_last_pts.p ? h->last_n : 0;
+}
+
+// score_query's `sessions` for a group pose query: session k is member members[k] with its scan by check_scans' rule
+// (`staged`: where score_query puts the scans sent with the call) and the k-th of the K + 1 `offsets` of its poses or
+// hints; its cell length is its member's of `level`.
+auto group_sessions(hsb_group* g, int K, const int* members, int level, const int* offsets, const int* scan_offsets) {
+  return [=](HsbScoreSessionDev* sess, int* staged_offsets, const float2* staged) {
+    for (int k = 0; k < K; ++k) {
+      hsb_handle* h = g->m[members[k]];
+      if (scan_offsets) sess[k].pts = staged + scan_offsets[k];
+      else sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
+      sess[k].n = scan_length(h, scan_offsets, k);
+      sess[k].member = members[k];
+      sess[k].cell_length = h->lv[level].cell_length;
+    }
+    memcpy(staged_offsets, offsets, (size_t)(K + 1) * 4);
+  };
+}
+
 // hsb_likelihood_batch / hsb_covariance_batch / hsb_best_hypothesis_device for K members in one pass: session k's poses
 // [pose_offsets[k], pose_offsets[k+1]) scored on member members[k]'s map of `level` against the session's scan
-// (pts[scan_offsets[k] ..), or, with pts and scan_offsets NULL, the member's last-match container as it is on the device
-// when the call runs).  Behind the members' queued work, through the group's pinned query staging and descriptor table
+// (check_scans).  Behind the members' queued work, through the group's pinned query staging and descriptor table
 // (score_query: one copy each way, one launch, two for the best hypothesis, and one synchronise, whatever K is).  No
 // member's state changes.
 int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* members, int level, const int* pose_offsets,
@@ -3227,24 +3298,8 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
   if (s != HSB_OK || K == 0) return s;
   if (level < 0 || level >= g->levels)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
-  if (!pose_offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets is NULL", fn);
-  if (pose_offsets[0] != 0)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets[0] is %d, must be 0", fn, pose_offsets[0]);
-  for (int k = 0; k < K; ++k)
-    if (pose_offsets[k + 1] < pose_offsets[k])
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: pose_offsets decrease at session %d (%d -> %d)", fn, k, pose_offsets[k],
-                  pose_offsets[k + 1]);
-  if (!pts != !scan_offsets)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: points_xy and scan_offsets must both be given or both be NULL", fn);
-  const bool last = !pts;   // every session's scan is its member's last-match container
-  if (!last) {
-    if (scan_offsets[0] != 0)
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets[0] is %d, must be 0", fn, scan_offsets[0]);
-    for (int k = 0; k < K; ++k)
-      if (scan_offsets[k + 1] < scan_offsets[k])
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets decrease at session %d (%d -> %d)", fn, k, scan_offsets[k],
-                    scan_offsets[k + 1]);
-  }
+  if ((s = check_offsets(h0, fn, "pose_offsets", K, pose_offsets)) != HSB_OK) return s;
+  if ((s = check_scans(h0, fn, K, pts, scan_offsets)) != HSB_OK) return s;
   const int Q = pose_offsets[K];
   if (Q == 0) {   // nothing to score: every session's best hypothesis is the empty batch's
     for (int k = 0; kind == SCORE_BEST && out_best4 && k < K; ++k) {
@@ -3261,56 +3316,26 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
   if (kind == SCORE_BEST && !out_best4) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_best4 is NULL", fn);
   DeviceGuard guard(g->device);
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-  auto sessions = [&](HsbScoreSessionDev* sess, int* offsets, const float2* staged) {
-    for (int k = 0; k < K; ++k) {
-      hsb_handle* h = g->m[members[k]];
-      sess[k].member = members[k];
-      sess[k].cell_length = h->lv[level].cell_length;
-      if (last) {   // (a member that never matched has no container: n = 0)
-        sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
-        sess[k].n = h->d_last_pts.p ? h->last_n : 0;
-      } else {
-        sess[k].pts = staged + scan_offsets[k];
-        sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
-      }
-    }
-    memcpy(offsets, pose_offsets, (size_t)(K + 1) * 4);
-  };
   // (h0's gather mode is every member's: hsb_group_create(_mixed) checked)
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, level, kind,
-                     K, Q, poses, pts, last ? 0 : (size_t)scan_offsets[K], sessions, g->d_best, out_lh, out_map,
+                     K, Q, poses, pts, pts ? (size_t)scan_offsets[K] : 0,
+                     group_sessions(g, K, members, level, pose_offsets, scan_offsets), g->d_best, out_lh, out_map,
                      out_world, out_best4, out_best_index);
 }
 
 // hsb_match_batch in shared-scan mode for K members in one pass: session k's hints [hint_offsets[k], hint_offsets[k+1])
-// each matched over all levels on member members[k]'s maps with the session's one scan (pts[scan_offsets[k] ..), or,
-// with pts and scan_offsets NULL, the member's last-match container as it is on the device when the call runs).  One
-// match-kernel launch (GRP_MATCH: one hint per scan) in the shape hsb_match_batch would take for Q hints, behind the
-// members' queued work, through the group's pinned query staging: one copy each way and one synchronise, whatever K is.
-// No member's state changes.
+// each matched over all levels on member members[k]'s maps with the session's one scan (check_scans).  One match-kernel
+// launch (GRP_MATCH: one hint per scan) in the shape hsb_match_batch would take for Q hints, behind the members' queued
+// work, through the group's pinned query staging (score_query: one copy each way and one synchronise, whatever K is).
+// The launch shape is chosen, and a tuning without a group match kernel rejected, before anything is queued.  No
+// member's state changes.
 int group_match(hsb_group* g, const char* fn, int K, const int* members, const int* hint_offsets, const float* hints,
                 const float* pts, const int* scan_offsets, float* out_poses, float* out_cov) {
   hsb_handle* h0 = g->m[0];   // launches, launch shape and errors are accounted on handles[0], whether or not it is listed
   int s = check_members(g, fn, K, members);
   if (s != HSB_OK || K == 0) return s;
-  if (!hint_offsets) return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets is NULL", fn);
-  if (hint_offsets[0] != 0)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets[0] is %d, must be 0", fn, hint_offsets[0]);
-  for (int k = 0; k < K; ++k)
-    if (hint_offsets[k + 1] < hint_offsets[k])
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: hint_offsets decrease at session %d (%d -> %d)", fn, k, hint_offsets[k],
-                  hint_offsets[k + 1]);
-  if (!pts != !scan_offsets)
-    return fail(h0, HSB_ERR_INVALID_ARG, "%s: points_xy and scan_offsets must both be given or both be NULL", fn);
-  const bool last = !pts;   // every session's scan is its member's last-match container
-  if (!last) {
-    if (scan_offsets[0] != 0)
-      return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets[0] is %d, must be 0", fn, scan_offsets[0]);
-    for (int k = 0; k < K; ++k)
-      if (scan_offsets[k + 1] < scan_offsets[k])
-        return fail(h0, HSB_ERR_INVALID_ARG, "%s: scan_offsets decrease at session %d (%d -> %d)", fn, k, scan_offsets[k],
-                    scan_offsets[k + 1]);
-  }
+  if ((s = check_offsets(h0, fn, "hint_offsets", K, hint_offsets)) != HSB_OK) return s;
+  if ((s = check_scans(h0, fn, K, pts, scan_offsets)) != HSB_OK) return s;
   const int Q = hint_offsets[K];
   if (Q == 0) return HSB_OK;
   if (!hints) return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints_world is NULL", fn);
@@ -3324,70 +3349,18 @@ int group_match(hsb_group* g, const char* fn, int K, const int* members, const i
   if (!has_projected_kernel(h0, W, G, U))   // (the same set of shapes)
     return fail(h0, HSB_ERR_UNSUPPORTED, "%s: no group match kernel for tuning warps_per_scan=%d scans_per_block=%d "
                 "unroll=%d packed=%d", fn, W, G, U, h0->tune_packed);
+  MatchQuery mq = {W, 0, out_poses, out_cov};
+  // (only a session with hints launches work: an unused long scan must not shrink the staging of the others)
+  for (int k = 0; k < K; ++k)
+    if (hint_offsets[k + 1] > hint_offsets[k])
+      mq.max_n = std::max(mq.max_n, scan_length(g->m[members[k]], scan_offsets, k));
   DeviceGuard guard(g->device);
-  cudaStream_t st = g->stream;
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-
-  // staging: sessions | hint offsets | hints | scans, then the results: poses | covariances
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t n_pts = last ? 0 : (size_t)scan_offsets[K];
-  const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_hints = al(o_off + (size_t)(K + 1) * 4);
-  const size_t o_pts = al(o_hints + (size_t)Q * 12), in_end = o_pts + n_pts * 8, o_poses = al(in_end);
-  const size_t o_cov = o_poses + (size_t)Q * 12, out_end = o_cov + (out_cov ? (size_t)Q * 36 : 0);
-  if ((s = ensure_pinned(h0, g->h_ray_stage, g->h_ray_stage_bytes, out_end)) != HSB_OK) return s;
-  if ((s = ensure(h0, g->d_ray_stage, out_end)) != HSB_OK) return s;
-  char* hs = reinterpret_cast<char*>(g->h_ray_stage);
-  char* ds = static_cast<char*>(g->d_ray_stage.p);
-  HsbScoreSessionDev* sess = reinterpret_cast<HsbScoreSessionDev*>(hs);
-  const float2* staged = reinterpret_cast<const float2*>(ds + o_pts);
-  int max_n = 0;
-  for (int k = 0; k < K; ++k) {
-    hsb_handle* h = g->m[members[k]];
-    sess[k].member = members[k];
-    sess[k].cell_length = 0.0f;   // (unused by the match)
-    if (last) {   // (a member that never matched has no container: n = 0)
-      sess[k].pts = h->d_last_pts.p ? reinterpret_cast<const float2*>(scan_points(h->d_last_pts)) : nullptr;
-      sess[k].n = h->d_last_pts.p ? h->last_n : 0;
-    } else {
-      sess[k].pts = staged + scan_offsets[k];
-      sess[k].n = scan_offsets[k + 1] - scan_offsets[k];
-    }
-    // (only a session with hints launches work: an unused long scan must not shrink the staging of the others)
-    if (hint_offsets[k + 1] > hint_offsets[k]) max_n = std::max(max_n, sess[k].n);
-  }
-  memcpy(hs + o_off, hint_offsets, (size_t)(K + 1) * 4);
-  memcpy(hs + o_hints, hints, (size_t)Q * 12);
-  if (n_pts > 0) memcpy(hs + o_pts, pts, n_pts * 8);
-  HSB_CUDA(h0, cudaMemcpyAsync(ds, hs, in_end, cudaMemcpyHostToDevice, st));
-
-  HsbMatchParams P;
-  fill_match_params(h0, P);   // (lv[] is unused: every hint reads its member's row of the group's table)
-  P.B = Q;
-  P.hints = reinterpret_cast<const float*>(ds + o_hints);
-  P.kind = HSB_IN_ENDPOINTS;
-  P.out_poses = reinterpret_cast<float*>(ds + o_poses);
-  P.out_cov = out_cov ? reinterpret_cast<float*>(ds + o_cov) : nullptr;
-  P.group_lv = g->d_lv;
-  P.match_sess = reinterpret_cast<const HsbScoreSessionDev*>(ds);
-  P.match_offsets = reinterpret_cast<const int*>(ds + o_off);
-  P.match_K = K;
-  const bool tex = h0->gather_mode == HSB_GATHER_TEX;   // (every member's: hsb_group_create(_mixed) checked)
-  s = HSB_ERR_UNSUPPORTED;
-#define HSB_GM_CASE(w)                                                                                                 \
-  if (W == w)                                                                                                          \
-    s = tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h0, P, max_n, st, 1)                \
-            : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h0, P, max_n, st, 1);
-  HSB_GM_CASE(1);
-  HSB_GM_CASE(2);
-  HSB_GM_CASE(4);
-  HSB_GM_CASE(8);
-#undef HSB_GM_CASE
-  if (s != HSB_OK) return s;
-  HSB_CUDA(h0, cudaMemcpyAsync(hs + o_poses, ds + o_poses, out_end - o_poses, cudaMemcpyDeviceToHost, st));
-  HSB_CUDA(h0, cudaStreamSynchronize(st));
-  memcpy(out_poses, hs + o_poses, (size_t)Q * 12);
-  if (out_cov) memcpy(out_cov, hs + o_cov, (size_t)Q * 36);
-  return HSB_OK;
+  // (the match reads no cell length: the sessions carry level 0's)
+  return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, 0,
+                     SCORE_MATCH, K, Q, hints, pts, pts ? (size_t)scan_offsets[K] : 0,
+                     group_sessions(g, K, members, 0, hint_offsets, scan_offsets), nullptr, nullptr, nullptr, nullptr,
+                     nullptr, nullptr, &mq);
 }
 
 }  // namespace

@@ -92,7 +92,9 @@ def test_against_single_calls(hsb_lib, geom, mode):
     sessions map_without_matching); after every tick a group match over a permuted subset with ragged sessions (0 to
     hundreds of hints, NaN and infinite hints, angles past 120 rad), the scans sent with the call.  The first four ticks
     size the call so that the default tuning takes 8, 4, 2 and 1 warps per scan; the last four force each through
-    handles[0]'s tuning.  Everything equals hsb_match_batch on the members in bits."""
+    handles[0]'s tuning.  Then one call over every member whose scans hold more than 1 MB of endpoints in all (more than
+    131 072 points: past what the call stages in pinned memory), one session without hints.  Everything equals
+    hsb_match_batch on the members in bits."""
     M, ticks = 3 + GEOMS.index(geom) + (1 if mode == 1 else 0), 8
     reps, g = fleet(geom, M, mode)
     track = Tracker(geom, M, mode)
@@ -118,6 +120,13 @@ def test_against_single_calls(hsb_lib, geom, mode):
         h = np.concatenate(hints)
         ok = np.all(np.isfinite(h), axis=1)
         moved += int((np.abs(poses[ok, :2] - h[ok, :2]).max(axis=1) > 1e-3).sum())
+    sel = [int(j) for j in rng.permutation(M)]
+    counts = [(7, 0, 33, 1)[k % 4] for k in range(M)]
+    hints = [hypotheses(rng, track.pose[j], c) for j, c in zip(sel, counts)]
+    lengths = [48000 + 2000 * k for k in range(M)]
+    scans = [(np.resize(track.scan(j), (n, 2)) + rng.normal(0.0, 0.25, (n, 2))).astype(F32) for j, n in zip(sel, lengths)]
+    assert sum(s.shape[0] for s in scans) > 131072
+    assert_match(g, reps, sel, hints, scans, scans, ("past 1 MB",))
     assert seen == {1, 2, 4, 8}
     assert moved > 100    # the hints were matched, not passed through
     close_all(g, reps, track)
