@@ -47,7 +47,7 @@ EXPORTED = [
     "hsb_group_best_hypothesis", "hsb_group_best_hypothesis_subset",
     "hsb_group_match_batch", "hsb_group_match_batch_subset",
     "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
-    "hsb_group_create_mixed", "hsb_group_reset", "hsb_group_reset_subset",
+    "hsb_group_create_mixed", "hsb_group_create_heterogeneous", "hsb_group_reset", "hsb_group_reset_subset",
 ]
 
 
@@ -194,6 +194,7 @@ def load_library() -> C.CDLL:
     sig("hsb_unpack_rect_device", i, vp, i, vp, vp, vp)
     sig("hsb_group_create", i, vp, i, C.POINTER(vp))
     sig("hsb_group_create_mixed", i, vp, i, C.POINTER(vp))
+    sig("hsb_group_create_heterogeneous", i, vp, i, C.POINTER(vp))
     sig("hsb_group_destroy", i, vp)
     sig("hsb_group_slam_update", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp)
     sig("hsb_group_slam_update_cloud", i, vp, vp, vp, vp, vp, vp, i, vp, vp, vp, vp)
@@ -937,15 +938,19 @@ class SlamGroup:
     (hsb_group_slam_update).  Each session's results and its handle's state equal a slam_update() on that handle bit for
     bit.  The group does not own the handles: close() it before closing any of them.
     mixed=True (hsb_group_create_mixed): the handles may differ in map size, resolution and start; every call then takes
-    each member's own sizes (grids, cell units, world-to-map transforms)."""
+    each member's own sizes (grids, cell units, world-to-map transforms).
+    heterogeneous=True (hsb_group_create_heterogeneous): the handles may also differ in level count, per-level
+    max_iterations and gather mode; every call runs each member's own levels, and a call at a `level` rejects a listed
+    member that does not have it."""
 
-    def __init__(self, reps, mixed: bool = False):
+    def __init__(self, reps, mixed: bool = False, heterogeneous: bool = False):
         self.lib = load_library()
         self.reps = list(reps)
         self.M = len(self.reps)
         arr = (C.c_void_p * max(1, self.M))(*[None if r is None else r.h for r in self.reps])
         g = C.c_void_p()
-        create = self.lib.hsb_group_create_mixed if mixed else self.lib.hsb_group_create
+        create = (self.lib.hsb_group_create_heterogeneous if heterogeneous
+                  else self.lib.hsb_group_create_mixed if mixed else self.lib.hsb_group_create)
         st = create(C.cast(arr, C.c_void_p), self.M, C.byref(g))
         if st != 0:
             raise HsbError(st, (self.lib.hsb_last_error(None) or b"").decode())

@@ -2182,12 +2182,30 @@ struct MatchQuery {
 // (points past kScoreChunk bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K
 // arg-max accumulators are `best`; the match's in match->W), one device-to-host copy of the asked-for results and one
 // synchronise.  The launches, the match's launch shape and any error are counted on h.  sessions() also gives each
-// session its member's cell length of `level` (the covariance's world matrix).
+// session its member's cell length of `level` (the covariance's world matrix) and its level count.  A heterogeneous
+// group's call passes `ragged` (its members differ in level count: the match runs each hint over its member's own
+// levels, GRP_MATCH_HET) and `any_mode` (they differ in gather mode: every kernel takes each level's own path,
+// MODE_ANY); otherwise h's gather mode is every session's, and a ragged group's match runs in it.
+// The group match's launch at W warps per scan: GRP_MATCH when the members share their level count and gather mode,
+// GRP_MATCH_HET otherwise (het), in the members' one gather mode (MODE_TEX / MODE_LDG) or, when they hold both,
+// MODE_ANY.
+template <int W>
+int launch_group_match(hsb_handle* h, HsbMatchParams& M, int max_n, cudaStream_t st, bool het, int mode) {
+  if (!het)
+    return mode == hsb::MODE_TEX ? launch_match_t<W, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1)
+                                 : launch_match_t<W, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1);
+  if (mode == hsb::MODE_ANY)
+    return launch_match_t<W, 1, hsb::MODE_ANY, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1);
+  return mode == hsb::MODE_TEX ? launch_match_t<W, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1)
+                               : launch_match_t<W, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1);
+}
+
 template <typename Sessions>
 int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage, const HsbLevelDev* lv,
                 int levels, int level, ScoreKind kind, int K, int Q, const float* poses, const float* pts, size_t n_pts,
                 const Sessions& sessions, unsigned long long* best, float* out_lh, float* out_map, float* out_world,
-                float* out_best4, int* out_best_index, const MatchQuery* match = nullptr) {
+                float* out_best4, int* out_best_index, const MatchQuery* match = nullptr, bool ragged = false,
+                bool any_mode = false) {
   // staging: sessions | pose offsets | (level descriptor) | poses | scans, then the results: likelihoods | best4 | best
   // index, or covariance (map) | covariance (world), or poses | Hessians, each only if asked for
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
@@ -2240,6 +2258,7 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   if (kind == SCORE_MATCH) {
     HsbMatchParams M;
     fill_match_params(h, M);   // (lv[] is unused: every hint reads its member's row of the group's table)
+    M.levels = levels;         // (the table's stride)
     M.B = Q;
     M.hints = P.poses;
     M.kind = HSB_IN_ENDPOINTS;
@@ -2250,10 +2269,9 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     M.match_offsets = P.pose_offsets;
     M.match_K = K;
     s = HSB_ERR_UNSUPPORTED;
-#define HSB_GM_CASE(w)                                                                                                 \
-  if (match->W == w)                                                                                                   \
-    s = tex ? launch_match_t<w, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h, M, match->max_n, st, 1)          \
-            : launch_match_t<w, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h, M, match->max_n, st, 1);
+    const int mode = any_mode ? hsb::MODE_ANY : tex ? hsb::MODE_TEX : hsb::MODE_LDG;
+#define HSB_GM_CASE(w) \
+  if (match->W == w) s = launch_group_match<w>(h, M, match->max_n, st, ragged || any_mode, mode);
     HSB_GM_CASE(1);
     HSB_GM_CASE(2);
     HSB_GM_CASE(4);
@@ -2264,7 +2282,8 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
     P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
     const int blocks = std::min(Q, h->sm_count * 8);
-    if (tex) hsb::covariance_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
+    if (any_mode) hsb::covariance_kernel<hsb::MODE_ANY><<<blocks, 224, 0, st>>>(P);
+    else if (tex) hsb::covariance_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
     else hsb::covariance_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(P);
     h->launches++;
   } else {
@@ -2275,7 +2294,8 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
       P.out_best_index = reinterpret_cast<int*>(ds + o_index);
     }
     const int blocks = std::min((Q + 3) / 4, h->sm_count * 16);
-    if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
+    if (any_mode) hsb::likelihood_group_kernel<hsb::MODE_ANY><<<blocks, 128, 0, st>>>(P);
+    else if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
     else hsb::likelihood_group_kernel<hsb::MODE_LDG><<<blocks, 128, 0, st>>>(P);
     h->launches++;
     if (kind == SCORE_BEST) {
@@ -2654,11 +2674,17 @@ int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
 // call uses: step_session, record_match, fill_update_levels and step_results.
 
 struct hsb_group {
-  std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create(_mixed) was given them
+  std::vector<hsb_handle*> m;      // the members, in the order hsb_group_create(_mixed / _heterogeneous) was given them
   std::vector<int> all;            // 0 .. M-1: the member list of a step of every member
   std::vector<unsigned char> listed;   // scratch of a step's member-list check, M flags
   int device = 0;
+  // the largest level count of the members (the stride of every member-major table); every member's but in a
+  // heterogeneous group, whose members may each have their own (ragged) and their own gather mode (any_mode: both
+  // occur, so the kernels take the gather path from each level descriptor, MODE_ANY).  Both stay false in groups of
+  // the other two constructors, which require the members to agree.
   int levels = 0;
+  bool ragged = false, any_mode = false;
+  int* d_member_levels = nullptr;  // ragged: the members' level counts (the *_ragged tile and reset kernels)
   cudaStream_t stream = nullptr;   // every step of the group runs here
   cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
   // M x levels match-kernel level descriptors, member-major (a handle's planes never move); a session reads its
@@ -2749,6 +2775,7 @@ int hsb_group_destroy(hsb_group* g) {
   if (g->d_tile_lv) cudaFree(g->d_tile_lv);
   if (g->d_tile_counters) cudaFree(g->d_tile_counters);
   if (g->d_reset) cudaFree(g->d_reset);
+  if (g->d_member_levels) cudaFree(g->d_member_levels);
   for (cudaEvent_t e : g->ev_tile)
     if (e) cudaEventDestroy(e);
   if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
@@ -2767,10 +2794,15 @@ int hsb_group_destroy(hsb_group* g) {
 
 namespace {
 
-// hsb_group_create (mixed = false: every member has handles[0]'s geometry) and hsb_group_create_mixed (members may
-// differ in map size, resolution and start; everything a group launch shares must still agree).  fn names the entry
-// point in the error messages.
-int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed, const char* fn) {
+// What a group's members may differ in: nothing but their maps' contents (hsb_group_create), their map size, resolution
+// and start (hsb_group_create_mixed), or also their level count, per-level iteration counts and gather mode
+// (hsb_group_create_heterogeneous).
+enum GroupKind { GROUP_SAME, GROUP_MIXED, GROUP_HETERO };
+
+// hsb_group_create, hsb_group_create_mixed and hsb_group_create_heterogeneous (see GroupKind).  fn names the entry point
+// in the error messages.
+int group_create(hsb_handle* const* handles, int M, hsb_group** out, GroupKind kind, const char* fn) {
+  const bool mixed = kind == GROUP_MIXED;
   if (!out) return group_fail(nullptr, HSB_ERR_INVALID_ARG, "%s: out is NULL", fn);
   *out = nullptr;
   hsb_handle* h0 = (handles && M > 0) ? handles[0] : nullptr;
@@ -2788,6 +2820,7 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
     if (h->device != h0->device)
       return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: handle %d is on device %d, handle 0 on device %d", fn, s,
                         h->device, h0->device);
+    if (kind == GROUP_HETERO) continue;   // each member runs its own levels, iterations and gather path
     if (mixed) {   // what every group launch shares: the level count, the per-level iteration counts, the gather mode
       if (h->levels != h0->levels)
         return group_fail(h0, HSB_ERR_INVALID_ARG, "%s: handle %d has %d levels, handle 0 has %d", fn, s, h->levels,
@@ -2821,6 +2854,11 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
   g->listed.assign(M, 0);
   g->device = h0->device;
   g->levels = h0->levels;
+  for (int s = 1; s < M; ++s) {
+    g->levels = std::max(g->levels, handles[s]->levels);
+    g->ragged |= handles[s]->levels != h0->levels;
+    g->any_mode |= handles[s]->gather_mode != h0->gather_mode;
+  }
 #define HSB_GROUP_CUDA(expr)                                                                                 \
   do {                                                                                                       \
     cudaError_t _e = (expr);                                                                                 \
@@ -2836,18 +2874,18 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
   {
     std::vector<HsbLevelDev> lv((size_t)M * g->levels);
     memset(lv.data(), 0, lv.size() * sizeof(HsbLevelDev));
-    for (int s = 0; s < M; ++s)
-      for (int l = 0; l < g->levels; ++l) fill_level_dev(g->m[s], l, lv[(size_t)s * g->levels + l]);
+    for (int s = 0; s < M; ++s)   // (a member's rows past its own levels stay zero: nothing reads them)
+      for (int l = 0; l < g->m[s]->levels; ++l) fill_level_dev(g->m[s], l, lv[(size_t)s * g->levels + l]);
     HSB_GROUP_CUDA(cudaMalloc(&g->d_lv, lv.size() * sizeof(HsbLevelDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_lv, lv.data(), lv.size() * sizeof(HsbLevelDev), cudaMemcpyHostToDevice));
     std::vector<int*> mirror((size_t)M * g->levels);
     for (int s = 0; s < M; ++s)
-      for (int l = 0; l < g->levels; ++l) mirror[(size_t)s * g->levels + l] = g->m[s]->lv[l].dirty + 4;
+      for (int l = 0; l < g->m[s]->levels; ++l) mirror[(size_t)s * g->levels + l] = g->m[s]->lv[l].dirty + 4;
     HSB_GROUP_CUDA(cudaMalloc(&g->d_mirror, mirror.size() * sizeof(int*)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_mirror, mirror.data(), mirror.size() * sizeof(int*), cudaMemcpyHostToDevice));
     std::vector<HsbRayLevelDev> ray((size_t)M * g->levels);
     for (int s = 0; s < M; ++s)
-      for (int l = 0; l < g->levels; ++l) fill_ray_level(g->m[s], l, ray[(size_t)s * g->levels + l]);
+      for (int l = 0; l < g->m[s]->levels; ++l) fill_ray_level(g->m[s], l, ray[(size_t)s * g->levels + l]);
     HSB_GROUP_CUDA(cudaMalloc(&g->d_ray_lv, ray.size() * sizeof(HsbRayLevelDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_ray_lv, ray.data(), ray.size() * sizeof(HsbRayLevelDev), cudaMemcpyHostToDevice));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_best, (size_t)M * sizeof(unsigned long long)));
@@ -2857,7 +2895,7 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
     for (int s = 0; s < M; ++s) {
       HsbTileParams T;
       fill_tile_params(g->m[s], T, nullptr, 0);
-      for (int l = 0; l < g->levels; ++l) tile[(size_t)s * g->levels + l] = T.lv[l];
+      for (int l = 0; l < g->m[s]->levels; ++l) tile[(size_t)s * g->levels + l] = T.lv[l];
       counters[s] = T.error_count;
     }
     HSB_GROUP_CUDA(cudaMalloc(&g->d_tile_lv, tile.size() * sizeof(HsbTileLevelDev)));
@@ -2868,10 +2906,16 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
     memset(reset.data(), 0, reset.size() * sizeof(HsbResetMemberDev));
     for (int s = 0; s < M; ++s) {
       reset[s].gate = g->m[s]->d_gate;
-      for (int l = 0; l < g->levels; ++l) reset[s].stamp[l] = g->m[s]->lv[l].stamp;
+      for (int l = 0; l < g->m[s]->levels; ++l) reset[s].stamp[l] = g->m[s]->lv[l].stamp;
     }
     HSB_GROUP_CUDA(cudaMalloc(&g->d_reset, reset.size() * sizeof(HsbResetMemberDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_reset, reset.data(), reset.size() * sizeof(HsbResetMemberDev), cudaMemcpyHostToDevice));
+    if (g->ragged) {
+      std::vector<int> nl(M);
+      for (int s = 0; s < M; ++s) nl[s] = g->m[s]->levels;
+      HSB_GROUP_CUDA(cudaMalloc(&g->d_member_levels, nl.size() * sizeof(int)));
+      HSB_GROUP_CUDA(cudaMemcpy(g->d_member_levels, nl.data(), nl.size() * sizeof(int), cudaMemcpyHostToDevice));
+    }
     for (cudaEvent_t& e : g->ev_tile) HSB_GROUP_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
@@ -2891,11 +2935,15 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, bool mixed,
 extern "C" {
 
 int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out) {
-  return group_create(handles, M, out, false, "hsb_group_create");
+  return group_create(handles, M, out, GROUP_SAME, "hsb_group_create");
 }
 
 int hsb_group_create_mixed(hsb_handle* const* handles, int M, hsb_group** out) {
-  return group_create(handles, M, out, true, "hsb_group_create_mixed");
+  return group_create(handles, M, out, GROUP_MIXED, "hsb_group_create_mixed");
+}
+
+int hsb_group_create_heterogeneous(hsb_handle* const* handles, int M, hsb_group** out) {
+  return group_create(handles, M, out, GROUP_HETERO, "hsb_group_create_heterogeneous");
 }
 
 }  // extern "C"
@@ -2919,6 +2967,18 @@ struct GroupInput {
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
 constexpr int kGroupW = 8;
 
+// The group step's match launch in gather mode `mode`; MODE_ANY only with GRP_STEP_HET (a heterogeneous group holding
+// both gather modes).
+template <int GRP, bool PROJ>
+int launch_group_step(hsb_handle* h0, HsbMatchParams& P, int max_n, cudaStream_t st, int mode) {
+  if constexpr (GRP == hsb::GRP_STEP_HET) {
+    if (mode == hsb::MODE_ANY)
+      return launch_match_t<kGroupW, 1, hsb::MODE_ANY, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1);
+  }
+  return mode == hsb::MODE_TEX ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1)
+                               : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1);
+}
+
 // The member list of a group call over K sessions: 0 <= K <= M, and with K > 0 a list of distinct indices in [0, M).
 int check_members(hsb_group* g, const char* fn, int K, const int* members) {
   hsb_handle* h0 = g->m[0];
@@ -2933,6 +2993,20 @@ int check_members(hsb_group* g, const char* fn, int K, const int* members) {
       return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is outside [0, %d)", fn, k, j, M);
     if (g->listed[j]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: member %d is listed twice", fn, k, j);
     g->listed[j] = 1;
+  }
+  return HSB_OK;
+}
+
+// The level rule of a heterogeneous group's level-taking calls: every listed member has level `level` (members not
+// listed are not checked).  Checked before anything is queued.  In a group whose members share their level count the
+// group's own range check (level < hsb_group::levels) is the whole rule.
+int check_member_level(hsb_group* g, const char* fn, int K, const int* members, int level) {
+  if (!g->ragged) return HSB_OK;
+  for (int k = 0; k < K; ++k) {
+    const hsb_handle* h = g->m[members[k]];
+    if (level >= h->levels)
+      return fail(g->m[0], HSB_ERR_INVALID_ARG, "%s: session %d: member %d has %d levels, level %d is not one of them",
+                  fn, k, members[k], h->levels, level);
   }
   return HSB_OK;
 }
@@ -3040,6 +3114,7 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
     memset(&gs, 0, sizeof(gs));
     gs.gate_state = h->d_gate;
     gs.member = members[k];
+    gs.levels = h->levels;
     gs.conv = ss.conv;
     if (matched && !conv) gs.last_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));   // the match copies the scan there
     if (matched) record_match(h, n, ss.origo);
@@ -3048,12 +3123,16 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
     if ((s = fill_update_levels(h, s_upd + (size_t)k * levels, pts0, n, ss.conv.out_n, ss.origo, matched, st, &max_upd)) !=
         HSB_OK)
       return s;
+    // a member with fewer levels than the group: its writer slots past them are inactive
+    if (h->levels < levels)
+      memset(s_upd + (size_t)k * levels + h->levels, 0, (size_t)(levels - h->levels) * sizeof(HsbUpdateLevelDev));
   }
   HSB_CUDA(h0, cudaMemcpyAsync(g->d_stage.p, hs, bytes, cudaMemcpyHostToDevice, st));
 
   // K1: (conversion +) match + gate, one session per CTA; the last session to finish publishes the step's sequence number
   HsbMatchParams P;
   fill_match_params(h0, P);
+  P.levels = levels;   // the stride of group_lv (the sessions' own level counts: GRP_STEP_HET)
   P.B = K;
   P.hints = reinterpret_cast<const float*>(ds);
   // (a converted session converts with its own descriptor, HsbGroupSessionDev::conv)
@@ -3068,14 +3147,18 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   P.group_lv = g->d_lv;
   P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
-  if (in.kind == HSB_IN_PROJECTED)
-    s = h0->gather_mode == HSB_GATHER_TEX
-            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_STEP, true>(h0, P, max_n, st, 1)
-            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP, true>(h0, P, max_n, st, 1);
-  else
-    s = h0->gather_mode == HSB_GATHER_TEX
-            ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_STEP>(h0, P, max_n, st, 1)
-            : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP>(h0, P, max_n, st, 1);
+  {
+    // each session on its member's levels (GRP_STEP_HET) when the members differ in level count or gather mode, in the
+    // members' one gather mode, or MODE_ANY when they hold both
+    const int mode = g->any_mode ? hsb::MODE_ANY : h0->gather_mode == HSB_GATHER_TEX ? hsb::MODE_TEX : hsb::MODE_LDG;
+    const bool proj = in.kind == HSB_IN_PROJECTED;
+    if (g->ragged || g->any_mode)
+      s = proj ? launch_group_step<hsb::GRP_STEP_HET, true>(h0, P, max_n, st, mode)
+               : launch_group_step<hsb::GRP_STEP_HET, false>(h0, P, max_n, st, mode);
+    else
+      s = proj ? launch_group_step<hsb::GRP_STEP, true>(h0, P, max_n, st, mode)
+               : launch_group_step<hsb::GRP_STEP, false>(h0, P, max_n, st, mode);
+  }
   if (s != HSB_OK) return s;
 
   // K2: mark and apply over (session, level), behind the match with programmatic dependent launch, in the single
@@ -3131,6 +3214,7 @@ int group_sync_occupancy(hsb_group* g, const char* fn, int K, const int* members
   if (s != HSB_OK || K == 0) return s;
   if (level < 0 || level >= g->levels)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if ((s = check_member_level(g, fn, K, members, level)) != HSB_OK) return s;
   if (!grids) return fail(h0, HSB_ERR_INVALID_ARG, "%s: grids is NULL", fn);
   for (int k = 0; k < K; ++k)
     if (!grids[k]) return fail(h0, HSB_ERR_INVALID_ARG, "%s: session %d: grid is NULL", fn, k);
@@ -3241,6 +3325,7 @@ int group_rays(hsb_group* g, const char* fn, bool world, int K, const int* membe
   if (s != HSB_OK || K == 0) return s;
   if (level < 0 || level >= g->levels)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if ((s = check_member_level(g, fn, K, members, level)) != HSB_OK) return s;
   if ((s = check_offsets(h0, fn, "offsets", K, offsets)) != HSB_OK) return s;
   const int Q = offsets[K];
   if (Q == 0) return HSB_OK;
@@ -3280,6 +3365,7 @@ auto group_sessions(hsb_group* g, int K, const int* members, int level, const in
       sess[k].n = scan_length(h, scan_offsets, k);
       sess[k].member = members[k];
       sess[k].cell_length = h->lv[level].cell_length;
+      sess[k].levels = h->levels;
     }
     memcpy(staged_offsets, offsets, (size_t)(K + 1) * 4);
   };
@@ -3298,6 +3384,7 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
   if (s != HSB_OK || K == 0) return s;
   if (level < 0 || level >= g->levels)
     return fail(h0, HSB_ERR_INVALID_ARG, "%s: level %d is outside [0, %d)", fn, level, g->levels);
+  if ((s = check_member_level(g, fn, K, members, level)) != HSB_OK) return s;
   if ((s = check_offsets(h0, fn, "pose_offsets", K, pose_offsets)) != HSB_OK) return s;
   if ((s = check_scans(h0, fn, K, pts, scan_offsets)) != HSB_OK) return s;
   const int Q = pose_offsets[K];
@@ -3316,11 +3403,11 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
   if (kind == SCORE_BEST && !out_best4) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_best4 is NULL", fn);
   DeviceGuard guard(g->device);
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-  // (h0's gather mode is every member's: hsb_group_create(_mixed) checked)
+  // (h0's gather mode is every member's unless the group is heterogeneous and holds both: any_mode)
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, level, kind,
                      K, Q, poses, pts, pts ? (size_t)scan_offsets[K] : 0,
                      group_sessions(g, K, members, level, pose_offsets, scan_offsets), g->d_best, out_lh, out_map,
-                     out_world, out_best4, out_best_index);
+                     out_world, out_best4, out_best_index, nullptr, g->ragged, g->any_mode);
 }
 
 // hsb_match_batch in shared-scan mode for K members in one pass: session k's hints [hint_offsets[k], hint_offsets[k+1])
@@ -3360,7 +3447,7 @@ int group_match(hsb_group* g, const char* fn, int K, const int* members, const i
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, 0,
                      SCORE_MATCH, K, Q, hints, pts, pts ? (size_t)scan_offsets[K] : 0,
                      group_sessions(g, K, members, 0, hint_offsets, scan_offsets), nullptr, nullptr, nullptr, nullptr,
-                     nullptr, nullptr, &mq);
+                     nullptr, nullptr, &mq, g->ragged, g->any_mode);
 }
 
 }  // namespace
@@ -3622,20 +3709,25 @@ int group_pack_dirty(hsb_group* g, const char* fn, int K, const int* members, fl
   fill_group_tile_params(g, T, d_buf, capacity_bytes, K);
   T.reset = reset;
   const int blocks = h0->sm_count * 4;
+  const int* nl = g->d_member_levels;   // a ragged group's blocks each carry their member's level count
   if (!members) {
-    hsb::pack_dirty_group_kernel<<<blocks, 256, 0, user>>>(T);
+    if (nl) hsb::pack_dirty_group_ragged_kernel<<<blocks, 256, 0, user>>>(T, nl);
+    else hsb::pack_dirty_group_kernel<<<blocks, 256, 0, user>>>(T);
   } else if (K <= kTileSubsetSmall) {
     hsb::TileMembers<kTileSubsetSmall> S;
     memcpy(S.idx, members, (size_t)K * sizeof(int));
-    hsb::pack_dirty_subset_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S);
+    if (nl) hsb::pack_dirty_subset_ragged_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S, nl);
+    else hsb::pack_dirty_subset_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S);
   } else {
     std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
     memcpy(S->idx, members, (size_t)K * sizeof(int));
-    hsb::pack_dirty_subset_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S);
+    if (nl) hsb::pack_dirty_subset_ragged_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S, nl);
+    else hsb::pack_dirty_subset_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S);
   }
   if (reset) {
     const int threads = K * 4 * g->levels;
-    hsb::reset_dirty_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T);
+    if (nl) hsb::reset_dirty_ragged_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T, nl);
+    else hsb::reset_dirty_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T);
   }
   h0->launches += reset ? 2 : 1;
   HSB_CUDA(h0, cudaGetLastError());
@@ -3675,7 +3767,8 @@ int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capac
   if ((s = tile_order_before(g, user, M, nullptr, true, true)) != HSB_OK) return s;
   HsbTileParams T;
   fill_group_tile_params(g, T, const_cast<float*>(d_buf), capacity_bytes, 0);
-  hsb::unpack_dirty_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T);
+  if (g->d_member_levels) hsb::unpack_dirty_ragged_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T, g->d_member_levels);
+  else hsb::unpack_dirty_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T);
   h0->launches++;
   HSB_CUDA(h0, cudaGetLastError());
   return tile_order_after(g, user, M, nullptr, true);
@@ -3712,16 +3805,20 @@ int group_reset(hsb_group* g, const char* fn, int K, const int* members) {
   }
   const size_t want = ((size_t)h0->sm_count * 32 + K - 1) / K;
   const dim3 grid((unsigned)std::max<size_t>(1, std::min(want, (max_cells + 255) / 256)), (unsigned)std::min(K, 65535));
+  const int* nl = g->d_member_levels;   // a ragged group: each member's own levels
   if (all) {
-    hsb::group_reset_kernel<<<grid, 256, 0, st>>>(P);
+    if (nl) hsb::group_reset_ragged_kernel<<<grid, 256, 0, st>>>(P, nl);
+    else hsb::group_reset_kernel<<<grid, 256, 0, st>>>(P);
   } else if (K <= kTileSubsetSmall) {
     hsb::TileMembers<kTileSubsetSmall> S;
     memcpy(S.idx, members, (size_t)K * sizeof(int));
-    hsb::group_reset_subset_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S);
+    if (nl) hsb::group_reset_subset_ragged_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S, nl);
+    else hsb::group_reset_subset_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S);
   } else {
     std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
     memcpy(S->idx, members, (size_t)K * sizeof(int));
-    hsb::group_reset_subset_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S);
+    if (nl) hsb::group_reset_subset_ragged_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S, nl);
+    else hsb::group_reset_subset_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S);
   }
   h0->launches++;
   HSB_CUDA(h0, cudaGetLastError());

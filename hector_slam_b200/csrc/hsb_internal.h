@@ -59,6 +59,9 @@ struct HsbGroupSessionDev {
   // the member's position in the group (its row of HsbMatchParams::group_lv).  Kept here rather than in HsbMatchParams
   // so that the parameter block, and with it every other instantiation of the match kernel, is unchanged.
   int member;
+  // the member's level count: a heterogeneous group's step (GRP_STEP_HET) starts the session at its member's coarsest
+  // level; its rows of group_lv past that are never read.  (Fills the descriptor's tail padding: its size is unchanged.)
+  int levels;
 };
 
 // One session of a pose-scoring call or of a group batch match: the scan its poses are scored against (its hints are
@@ -68,6 +71,7 @@ struct HsbScoreSessionDev {
   int n;
   int member;
   float cell_length;   // of the member's level of a scoring call (covariance: the world matrix); unused by the match
+  int levels;          // the member's level count: a heterogeneous group's match (GRP_MATCH_HET) starts at its coarsest
 };
 
 struct HsbMatchParams {
@@ -121,7 +125,8 @@ struct HsbMatchParams {
   float* record;
   int record_floats;
   // group SLAM step (match_kernel<..., GRP = GRP_STEP>): scan b is session b of the step, which steps member
-  // group_sess[b].member of the group.  Its level descriptors are group_lv[member * levels ..] (built once per group)
+  // group_sess[b].member of the group.  Its level descriptors are group_lv[member * levels ..] (built once per group;
+  // `levels` is then the group's largest level count, and a GRP_STEP_HET / GRP_MATCH_HET scan runs its own member's)
   // instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done

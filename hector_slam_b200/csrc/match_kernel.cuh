@@ -23,7 +23,10 @@
 
 namespace hsb {
 
-enum { MODE_LDG = 1, MODE_TEX = 2 };
+// MODE_ANY: the gather path is decided per level descriptor at run time — tex2Dgather where the level has a texture
+// twin (tex != 0), four loads otherwise — each branch exactly its own mode's arithmetic.  Only the kernels a
+// heterogeneous group holding both modes launches are instantiated with it.
+enum { MODE_LDG = 1, MODE_TEX = 2, MODE_ANY = 3 };
 
 struct Acc {
   float h00, h11, h22, h01, h02, h12, d0, d1, d2;
@@ -359,6 +362,18 @@ __device__ __forceinline__ void eval_points(const LevelRegs& L, PtsPtr pts, int 
     for (int u = 0; u < U; ++u) v[u] = point_fetch<MODE>(L, pre[u]);
 #pragma unroll
     for (int u = 0; u < U; ++u) point_accumulate(pre[u], v[u], a);
+  }
+}
+
+// eval_points in the level's gather mode: MODE_ANY picks it from the level descriptor (uniform across the group).
+template <int MODE, int U, typename PtsPtr>
+__device__ __forceinline__ void eval_level(const LevelRegs& L, PtsPtr pts, int first, int stride, int n, float cs, float ss,
+                                           float x, float y, Acc& a) {
+  if constexpr (MODE == MODE_ANY) {
+    if (L.tex) eval_points<MODE_TEX, U>(L, pts, first, stride, n, cs, ss, x, y, a);
+    else eval_points<MODE_LDG, U>(L, pts, first, stride, n, cs, ss, x, y, a);
+  } else {
+    eval_points<MODE, U>(L, pts, first, stride, n, cs, ss, x, y, a);
   }
 }
 
@@ -743,16 +758,26 @@ struct InlineScan<true> {
   float2 pts[HSB_INLINE_MAX_POINTS];
 };
 
-// one-warp scans grouped into CTAs: ask for the registers of 28 warps per SM like the G = 1 shape has
-template <int W, int G>
+// one-warp scans grouped into CTAs: ask for the registers of 28 warps per SM like the G = 1 shape has.  A one-warp
+// MODE_ANY kernel (a heterogeneous group's match) carries both gather paths: at 24 warps per SM its registers hold them
+// without spilling.
+template <int W, int G, int MODE = MODE_TEX>
 struct MatchBounds {
-  static constexpr int kMinBlocks = (W == 1 && 28 % G == 0) ? 28 / G : 1;
+  static constexpr int kMinBlocks = (W == 1 && 28 % G == 0) ? (MODE == MODE_ANY && G == 1 ? 24 : 28 / G) : 1;
 };
 
 // Which group a match kernel serves (its GRP template value): none (one handle's map for the whole batch), the group
 // SLAM step (one session per scan, hsb_group_slam_update) or the group batch match (one hint per scan,
-// hsb_group_match_batch).
-enum { GRP_NONE = 0, GRP_STEP = 1, GRP_MATCH = 2 };
+// hsb_group_match_batch).  The _HET forms serve a heterogeneous group whose members differ in their level count: each
+// scan runs its own member's levels (HsbGroupSessionDev::levels, HsbScoreSessionDev::levels), coarsest first, instead
+// of HsbMatchParams::levels, which is then only the stride of group_lv.
+enum { GRP_NONE = 0, GRP_STEP = 1, GRP_MATCH = 2, GRP_STEP_HET = 3, GRP_MATCH_HET = 4 };
+template <int GRP>
+constexpr bool kGrpStep = GRP == GRP_STEP || GRP == GRP_STEP_HET;
+template <int GRP>
+constexpr bool kGrpMatch = GRP == GRP_MATCH || GRP == GRP_MATCH_HET;
+template <int GRP>
+constexpr bool kGrpHet = GRP == GRP_STEP_HET || GRP == GRP_MATCH_HET;
 
 // The session of hint q of a group batch match or of pose q of a scoring call: the last session whose hints / poses
 // start at or before q (empty sessions are passed over), as ray_kernel finds a ray's.
@@ -771,15 +796,15 @@ __device__ __forceinline__ int session_of(const int* __restrict__ offsets, int K
 // session's member (`member`: the group batch match's, looked up once per scan).
 template <int GRP>
 __device__ __forceinline__ const HsbLevelDev& level_desc(const HsbMatchParams& P, int scan, int member, int lvl) {
-  if constexpr (GRP == GRP_STEP) return P.group_lv[(size_t)P.group_sess[scan].member * P.levels + lvl];
-  else if constexpr (GRP == GRP_MATCH) return P.group_lv[(size_t)member * P.levels + lvl];
+  if constexpr (kGrpStep<GRP>) return P.group_lv[(size_t)P.group_sess[scan].member * P.levels + lvl];
+  else if constexpr (kGrpMatch<GRP>) return P.group_lv[(size_t)member * P.levels + lvl];
   else return P.lv[lvl];
 }
 
 // Conversion descriptor of scan `scan`: the kernel parameters' (one handle), or the session's (group SLAM step).
 template <int GRP>
 __device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, int scan) {
-  if constexpr (GRP == GRP_STEP) return P.group_sess[scan].conv;
+  if constexpr (kGrpStep<GRP>) return P.group_sess[scan].conv;
   else return P.conv;
 }
 
@@ -789,7 +814,7 @@ __device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, 
 // the instantiations the projected SLAM steps and batch matches launch carry that branch (hsb_api.cu
 // launch_match_projected).
 template <int W, int G, int MODE, int U, bool PACK, bool INL = false, int GRP = GRP_NONE, bool PROJ = false>
-__global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
+__global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlocks)
     match_kernel(const __grid_constant__ HsbMatchParams P, const __grid_constant__ InlineScan<INL> S) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* mbars = reinterpret_cast<uint64_t*>(smem_raw);
@@ -812,7 +837,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
 
   // fused SLAM step: let the map writer's CTAs (launched with programmatic stream serialisation, update_kernel.cuh)
   // become resident on the idle SMs while this single-scan match runs; they wait for this grid's completion
-  if (GRP == GRP_STEP || P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (kGrpStep<GRP> || P.gate_state) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (t == 0) mbar_init(mbar, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   // Pacing (G > 1, P.pace_slack > 0).  The per-scan timeline (tuning key trace) shows that the warps of an SM do NOT
@@ -854,17 +879,20 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       n = P.n_shared;
       beg = P.kind == HSB_IN_ENDPOINTS ? 0 : (size_t)scan * n;
     }
-    if constexpr (GRP == GRP_STEP) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
+    if constexpr (kGrpStep<GRP>) {   // map_without_matching (HectorSlamProcessor.h:80): the hint passes through the gate unmatched
       if (P.kind == HSB_IN_ENDPOINTS && P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // (a conversion runs first, below)
     }
     const float2* __restrict__ gpts = P.pts + beg;
     int member = 0;
-    if constexpr (GRP == GRP_MATCH) {   // group batch match: the scan, its length and the map are the hint's session's
+    int levels = 0;   // a heterogeneous group's scan: its member's level count (every other scan runs P.levels)
+    if constexpr (kGrpMatch<GRP>) {   // group batch match: the scan, its length and the map are the hint's session's
       const HsbScoreSessionDev& s = P.match_sess[session_of(P.match_offsets, P.match_K, scan)];
       gpts = s.pts;
       n = s.n;
       member = s.member;
+      if constexpr (GRP == GRP_MATCH_HET) levels = s.levels;
     }
+    if constexpr (GRP == GRP_STEP_HET) levels = P.group_sess[scan].levels;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
     bool staged = false;
     int ns = 0;                      // points [0, ns) are read from shared memory, [ns, n) from global memory
@@ -880,7 +908,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       group_sync<W>(g);
       ns = n;
       staged = true;
-    } else if (GRP != GRP_MATCH && P.kind != HSB_IN_ENDPOINTS) {
+    } else if (!kGrpMatch<GRP> && P.kind != HSB_IN_ENDPOINTS) {
       // a fused conversion: convert + compact straight into shared memory (host guarantees cap >= the input's size)
       const HsbConvDev& C = conv_desc<GRP>(P, scan);
       const double* T = P.cloud_tf ? P.cloud_tf + 12 * (size_t)scan : P.cloud_tf0;
@@ -913,7 +941,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
           if (C.out_n_host) *C.out_n_host = n;
         }
       }
-      if constexpr (GRP == GRP_STEP) {
+      if constexpr (kGrpStep<GRP>) {
         if (P.gate_in[3 * scan + 2] != 0.0f) n = 0;   // map_without_matching: converted for the writer, not matched
       }
       ns = n;
@@ -971,7 +999,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
     const bool recording = P.record && t == 0;
     int evals_ran = 0;   // evaluations this scan actually ran (trace slot 5)
     if (n > 0) {
-      for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
+      for (int lvl = (kGrpHet<GRP> ? levels : P.levels) - 1; lvl >= 0; --lvl) {
         const HsbLevelDev& L = level_desc<GRP>(P, scan, member, lvl);
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
@@ -997,10 +1025,10 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
           if (PACK && staged)
             eval_pairs<(U + 1) / 2>(LR, reinterpret_cast<const float4*>(spts), t, GT, npairs, cs, ss, ex, ey, a);
           else if (staged) {
-            eval_points<MODE, U>(LR, spts_scan, t, GT, ns, cs, ss, ex, ey, a);
-            if (ns < n) eval_points<MODE, U>(LR, gpts, ns + t, GT, n, cs, ss, ex, ey, a);
+            eval_level<MODE, U>(LR, spts_scan, t, GT, ns, cs, ss, ex, ey, a);
+            if (ns < n) eval_level<MODE, U>(LR, gpts, ns + t, GT, n, cs, ss, ex, ey, a);
           } else
-            eval_points<MODE, U>(LR, gpts, t, GT, n, cs, ss, ex, ey, a);
+            eval_level<MODE, U>(LR, gpts, t, GT, n, cs, ss, ex, ey, a);
           warp_reduce(a);
           if (W > 1) {
             // second stage: the W per-warp sums of each of the 9 values sit transposed in shared
@@ -1117,7 +1145,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       P.trace[8 * (size_t)scan + 6] = warp_id();
       P.trace[8 * (size_t)scan + 7] = sm_id();
     }
-    if (GRP == GRP_STEP && t == 0) {
+    if (kGrpStep<GRP> && t == 0) {
       // group SLAM step: the session's gate, against its own handle's state and thresholds
       slam_gate(P.group_sess[scan].gate_state, P.gate_in + 3 * scan, wx, wy, wpsi, P.out_poses + 4 * scan,
                 P.gate_out_host + 4 * scan);
@@ -1142,7 +1170,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
         c[6] = last.h02; c[7] = last.h12; c[8] = last.h22;
       }
     }
-    if (GRP == GRP_STEP && t == 0) {
+    if (kGrpStep<GRP> && t == 0) {
       // group SLAM step: the LAST session to finish publishes the sequence number — every session's results (each made
       // visible system-wide before its count) are then in host memory
       __threadfence_system();
@@ -1155,7 +1183,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G>::kMinBlocks)
       __threadfence_system();
       *reinterpret_cast<volatile unsigned*>(P.seq_host) = P.seq_value;
     }
-    if constexpr (GRP == GRP_STEP) {
+    if constexpr (kGrpStep<GRP>) {
       // a matched scan becomes the member's "containers of the last match" (MapRepMultiMap.h:127): the coarse levels of
       // its later map writes without matching read it (after the pose is out: only the map writers wait for this).
       // A converted scan is already there (the conversion's sink, above).
@@ -1199,6 +1227,10 @@ __global__ void __launch_bounds__(256)
 template <int MODE>
 __device__ __forceinline__ float warp_likelihood(const LevelRegs& LR, float pt_scale, const float2* __restrict__ pts, int n, float ex,
                                                  float ey, float psi, int lane) {
+  if constexpr (MODE == MODE_ANY) {   // the level's own gather path (uniform across the warp)
+    return LR.tex ? warp_likelihood<MODE_TEX>(LR, pt_scale, pts, n, ex, ey, psi, lane)
+                  : warp_likelihood<MODE_LDG>(LR, pt_scale, pts, n, ex, ey, psi, lane);
+  }
   const float cs = cosf_glibc(psi) * pt_scale, ss = sinf_glibc(psi) * pt_scale;
   float residual = 0.0f;
   for (int i = lane; i < n; i += 32) {

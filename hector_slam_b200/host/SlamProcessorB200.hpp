@@ -29,7 +29,7 @@ class SlamProcessor {
   // HectorSlamProcessor.h:54
   SlamProcessor(float mapResolution, int mapSizeX, int mapSizeY, float startX, float startY, int multi_res_size,
                 int device = 0)
-      : h_(0), group_(0), groupOwner_(0) {
+      : h_(0), group_(0), groupOwner_(0), heterogeneous_(false) {
     hsb_config cfg = hsb_config();
     cfg.map_resolution = mapResolution;
     cfg.map_size_x = mapSizeX;
@@ -254,6 +254,17 @@ class SlamProcessor {
     lastScanMatchPose_ = Pose{0.f, 0.f, 0.f};
     check(hsb_reset(h_));
   }
+
+  // Opt-in, on the processor that is ps[0] of the …Many calls: its cached group of ps[0..M) is made with
+  // hsb_group_create_heterogeneous, so the processors may differ in map size, resolution, start, level count
+  // (map_multi_res_levels), per-level iteration counts and gather mode.  Off (the default), the group is made with
+  // hsb_group_create and the …Many calls throw for processors that differ.  Changing it drops the cached group.
+  void setHeterogeneousGroups(bool on) {
+    if (on == heterogeneous_) return;
+    dropGroup();
+    heterogeneous_ = on;
+  }
+  bool heterogeneousGroups() const { return heterogeneous_; }
 
   // reset() for the processors ps[members[0..K)] of ps[0..M) in one launch (hsb_group_reset_subset, through the group
   // updateMany keeps; members null: all M, hsb_group_reset, and K is not read): the node's reset_map service or "reset"
@@ -499,7 +510,8 @@ class SlamProcessor {
       hs[s] = ps[s]->h_;
     }
     hsb_group* g = 0;
-    if (hsb_group_create(hs.data(), M, &g) != HSB_OK)
+    const int st = heterogeneous_ ? hsb_group_create_heterogeneous(hs.data(), M, &g) : hsb_group_create(hs.data(), M, &g);
+    if (st != HSB_OK)
       throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(0));
     group_ = g;
     groupMembers_.assign(ps, ps + M);
@@ -518,6 +530,7 @@ class SlamProcessor {
   hsb_group* group_;                           // updateMany's group, when this processor is its ps[0]
   std::vector<SlamProcessor*> groupMembers_;
   SlamProcessor* groupOwner_;                  // the processor whose cached group contains this one
+  bool heterogeneous_;                         // setHeterogeneousGroups
   Pose lastMapUpdatePose_, lastScanMatchPose_;
   float lastScanMatchCov_[9];
   float minDist_, minAngle_;

@@ -411,6 +411,9 @@ int hsbp_reset(void* p) {
   }
   return 0;
 }
+void hsbp_set_heterogeneous_groups(void* p, int on) {
+  static_cast<hsb200::SlamProcessor*>(p)->setHeterogeneousGroups(on != 0);
+}
 int hsbp_reset_many(void* const* ps, int M, const int* members, int K) {
   std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
   for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);

@@ -404,6 +404,23 @@ int hsb_group_create(hsb_handle* const* handles, int M, hsb_group** out);
  * treats a shipped block whose rectangle on any level lies outside that level of the member it lands on as a buffer
  * that does not fit the group: counted once on handles[0], nothing of it applied. */
 int hsb_group_create_mixed(hsb_handle* const* handles, int M, hsb_group** out);
+/* hsb_group_create for members that differ in everything a robot's node sets per robot: members may differ in all that
+ * hsb_group_create_mixed allows, and also in the level count (1 .. HSB_MAX_LEVELS), the resolved max_iterations of
+ * every level and the resolved gather mode (TEX or LDG).  They must still sit on one device.  NULL, duplicate and
+ * other-device handles are rejected as hsb_group_create_mixed rejects them.  Every group call keeps the contract
+ * documented for it: each session's results and each member's end state are bit-identical to the single-handle call on
+ * that member — its own levels, its own iteration counts, its own gather path — and a step is still one host-to-device
+ * copy and three launches counted on handles[0].
+ * Level rule: a call that takes a `level` (hsb_group_sync_occupancy, hsb_group_get_dist, hsb_group_raycast,
+ * hsb_group_likelihood, hsb_group_covariance, hsb_group_best_hypothesis and their _subset forms) accepts any level below
+ * the largest level count of the members, and rejects with HSB_ERR_INVALID_ARG, before anything is queued, cleared or
+ * written, a listed member that does not have that level; the message names the session and the member's level count.
+ * Members that are not listed are not checked.  hsb_group_match_batch runs each hint over its member's own levels with
+ * its member's iteration counts (W chosen from handles[0] as for every group).  Tile replication: each block is exactly
+ * the member's hsb_pack_dirty_device buffer, its own level count in block word 1; group-header word 2 is the largest
+ * level count; on unpack a block whose level count differs from the member it lands on makes the buffer not fit the
+ * group (counted once on handles[0], nothing of it applied).  hsb_group_reset clears each member's own levels. */
+int hsb_group_create_heterogeneous(hsb_handle* const* handles, int M, hsb_group** out);
 int hsb_group_destroy(hsb_group* g);
 /* HectorSlamProcessor::update for every member at once. Session s is handles[s] with hint hints[3s..], the scan
  * points_xy[offsets[s] .. offsets[s+1]) (level-0 cells, DataContainer layout), origo[2s..] (NULL = 0,0) and
@@ -516,6 +533,8 @@ int hsb_group_slam_update_projected_subset(hsb_group* g, int K, const int* membe
  * Rejected with HSB_ERR_INVALID_ARG before anything is queued or cleared: K < 0 or K > M; members == NULL with K > 0;
  * an index outside [0, M) or listed twice; level outside [0, levels); grids == NULL or a NULL grids[k] (the message
  * names the session).  K = 0 returns HSB_OK, reads no other argument and queues nothing. */
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued, cleared or written; the message names the session and the member's level count. */
 int hsb_group_sync_occupancy(hsb_group* g, int level, int8_t* const* grids, int* out_rects, int reset);
 int hsb_group_sync_occupancy_subset(hsb_group* g, int K, const int* members, int level, int8_t* const* grids,
                                     int* out_rects, int reset);
@@ -537,11 +556,15 @@ int hsb_group_sync_occupancy_subset(hsb_group* g, int K, const int* members, int
  * outside [0, M) or listed twice (the message names the session); level outside [0, levels); offsets == NULL,
  * offsets[0] != 0 or decreasing offsets (the message names the session); begin, end or out_dist NULL with Q > 0.
  * K = 0 returns HSB_OK and reads no other argument; Q = 0 returns HSB_OK and queues nothing. */
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued; the message names the session and the member's level count. */
 int hsb_group_get_dist(hsb_group* g, int level, const int* offsets, const float* begin_world, const float* end_world,
                        float* out_dist, float* out_hit_world, int* out_found);
 int hsb_group_get_dist_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
                               const float* begin_world, const float* end_world, float* out_dist, float* out_hit_world,
                               int* out_found);
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued; the message names the session and the member's level count. */
 int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,
                       float* out_dist, int* out_hit);
 int hsb_group_raycast_subset(hsb_group* g, int K, const int* members, int level, const int* offsets,
@@ -585,16 +608,22 @@ int hsb_group_raycast_subset(hsb_group* g, int K, const int* members, int level,
  * scan_offsets[0] != 0 or decreasing; poses_world, out_likelihood (likelihood), both covariance outputs or out_best4
  * NULL with Q > 0.  K = 0 returns HSB_OK and reads no other argument; Q = 0 returns HSB_OK and queues nothing (the best
  * hypothesis of every session is then the empty session's, written if out_best4 is given). */
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued; the message names the session and the member's level count. */
 int hsb_group_likelihood(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
                          const float* points_xy, const int* scan_offsets, float* out_likelihood);
 int hsb_group_likelihood_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
                                 const float* poses_world, const float* points_xy, const int* scan_offsets,
                                 float* out_likelihood);
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued; the message names the session and the member's level count. */
 int hsb_group_covariance(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
                          const float* points_xy, const int* scan_offsets, float* out_cov_map, float* out_cov_world);
 int hsb_group_covariance_subset(hsb_group* g, int K, const int* members, int level, const int* pose_offsets,
                                 const float* poses_world, const float* points_xy, const int* scan_offsets,
                                 float* out_cov_map, float* out_cov_world);
+/* Level rule (a group from hsb_group_create_heterogeneous): a listed member without `level` is rejected with
+ * HSB_ERR_INVALID_ARG before anything is queued; the message names the session and the member's level count. */
 int hsb_group_best_hypothesis(hsb_group* g, int level, const int* pose_offsets, const float* poses_world,
                               const float* points_xy, const int* scan_offsets, float* out_likelihood, float* out_best4,
                               int* out_best_index);
