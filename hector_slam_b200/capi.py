@@ -48,6 +48,7 @@ EXPORTED = [
     "hsb_group_match_batch", "hsb_group_match_batch_subset",
     "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
     "hsb_group_create_mixed", "hsb_group_create_heterogeneous", "hsb_group_reset", "hsb_group_reset_subset",
+    "hsb_get_level_evals", "hsb_set_step_record", "hsb_get_step_record", "hsb_get_last_match_scan",
 ]
 
 
@@ -223,6 +224,10 @@ def load_library() -> C.CDLL:
     sig("hsb_group_unpack_dirty_device", i, vp, vp, C.c_size_t, vp)
     sig("hsb_group_reset", i, vp)
     sig("hsb_group_reset_subset", i, vp, i, vp)
+    sig("hsb_get_level_evals", i, vp, i)
+    sig("hsb_set_step_record", i, vp, i)
+    sig("hsb_get_step_record", i, vp, vp, vp)
+    sig("hsb_get_last_match_scan", i, vp, vp, i, vp, vp)
     _lib = L
     return L
 
@@ -420,9 +425,36 @@ class MapRepB200:
         """Gauss-Newton evaluations per level, level 0 first (maxIterations + 1, the defaults 5 / 3 for a zero entry)"""
         out = []
         for l in range(self.levels):
-            mi = int(self.cfg.max_iterations[l]) or (5 if l == 0 else 3)
-            out.append(max(mi, 0) + 1)
+            e = int(self.lib.hsb_get_level_evals(self.h, l))
+            if e < 0:
+                self._check(e)
+            out.append(e)
         return out
+
+    # -- the fused steps' record (hsb_set_step_record) ---------------------------------------------
+    def set_step_record(self, on: bool = True):
+        """Every matched fused SLAM step of this handle (single or group) records its match from now on."""
+        self._check(self.lib.hsb_set_step_record(self.h, int(bool(on))))
+
+    def step_record(self, raw: bool = False):
+        """The record of the handle's last fused step: split_record() of it (raw=True: the (R,) float32 array), or None
+        when that step ran no match (map_without_matching, or no step since recording was turned on)."""
+        rec = np.zeros(self.record_floats, np.float32)
+        matched = C.c_int(0)
+        self._check(self.lib.hsb_get_step_record(self.h, rec.ctypes.data, C.byref(matched)))
+        if not matched.value:
+            return None
+        return rec if raw else self.split_record(rec)
+
+    def last_match_scan(self):
+        """-> (endpoints (n, 2) in level-0 cells, origo (2,)): the container of the handle's last matched scan."""
+        n, origo = C.c_int(0), np.zeros(2, np.float32)
+        st = self.lib.hsb_get_last_match_scan(self.h, None, 0, C.byref(n), origo.ctypes.data)
+        if st != 0 and n.value == 0:
+            self._check(st)
+        pts = np.zeros((max(n.value, 1), 2), np.float32)
+        self._check(self.lib.hsb_get_last_match_scan(self.h, pts.ctypes.data, pts.shape[0], C.byref(n), origo.ctypes.data))
+        return pts[:n.value].copy(), origo
 
     def split_record(self, rec) -> list[dict]:
         """(..., R) float32 records -> one dict per level, INDEXED BY LEVEL (0 = finest):

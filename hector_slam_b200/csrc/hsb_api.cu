@@ -143,6 +143,13 @@ struct hsb_handle {
   bool queued = false;
   unsigned step_seq = 0;   // sequence number of the fused SLAM steps (host polling, hsb_slam_update_nowait)
   int trace_scans = 0;
+  // step record (hsb_set_step_record): R floats of mapped pinned memory the match of every fused step writes the
+  // record into while the switch is on, published with the step's pose.  step_rec_matched: the last fused step ran a
+  // match with the switch on (its record is in h_step_rec); stepped: a fused step has run on the handle
+  float* h_step_rec = nullptr;
+  float* h_step_rec_dev = nullptr;   // device alias of h_step_rec
+  bool step_rec_on = false, step_rec_matched = false, stepped = false;
+  bool have_last_match = false;   // the last-match container holds a scan (hsb_get_last_match_scan)
   int last_shape[6] = {0, 0, 0, 0, 0, 0};  // W, G, U, staged points per scan (0 = none), grid, resident CTAs / SM
   uint64_t launches = 0;
   std::string err;
@@ -325,6 +332,8 @@ void fill_level_dev(const hsb_handle* h, int l, HsbLevelDev& d) {
   memcpy(d.wtm, L.wtm, sizeof(d.wtm));
   d.evals = L.evals;
   d.pt_scale = (float)(1.0 / pow(2.0, (double)l));  // MapRepMultiMap.h:127
+  d.rec_off = 0;   // the record holds the levels coarsest first
+  for (int k = h->levels - 1; k > l; --k) d.rec_off += 3 + 15 * h->lv[k].evals;
 }
 
 // ---- match launch -----------------------------------------------------------------------------
@@ -598,11 +607,6 @@ void fill_match_params(const hsb_handle* h, HsbMatchParams& P) {
   memset(&P, 0, sizeof(P));
   P.levels = h->levels;
   for (int l = 0; l < h->levels; ++l) fill_level_dev(h, l, P.lv[l]);
-  int off = 0;   // the record holds the levels coarsest first
-  for (int l = h->levels - 1; l >= 0; --l) {
-    P.lv[l].rec_off = off;
-    off += 3 + 15 * P.lv[l].evals;
-  }
 }
 
 int destroy_level(hsb_handle* h, Level& L) {
@@ -861,6 +865,7 @@ int hsb_destroy(hsb_handle* h) {
   for (int i = 0; i < 4; ++i)
     if (h->ev_sync[i]) cudaEventDestroy(h->ev_sync[i]);
   if (h->h_pin) cudaFreeHost(h->h_pin);
+  if (h->h_step_rec) cudaFreeHost(h->h_step_rec);
   if (h->h_stage) cudaFreeHost(h->h_stage);
   for (int i = 0; i < 4; ++i)
     if (h->ev[i]) cudaEventDestroy(h->ev[i]);
@@ -1025,6 +1030,7 @@ void fill_conv(const hsb_handle* h, HsbInputKind kind, HsbConvDev& c) {
 // (NULL = 0, 0) is the last match's container now (MapRepMultiMap::matchData, MapRepMultiMap.h:127): a later
 // updateByScan draws the coarse levels from it (:143).
 void record_match(hsb_handle* h, int n, const float origo[2]) {
+  h->have_last_match = true;
   h->last_n = n;
   h->last_origo[0] = origo ? origo[0] : 0.f;
   h->last_origo[1] = origo ? origo[1] : 0.f;
@@ -1206,6 +1212,56 @@ int hsb_match_data_record(hsb_handle* h, const float hint[3], const float* pts, 
                           float out_pose[3], float cov_inout[9], float* record_out) {
   if (!record_out) return HSB_ERR_INVALID_ARG;
   return match_data_impl(h, hint, pts, n, origo, out_pose, cov_inout, record_out);
+}
+
+int hsb_get_level_evals(const hsb_handle* h, int level) {
+  if (!h || level < 0 || level >= h->levels) return HSB_ERR_INVALID_ARG;
+  return h->lv[level].evals;
+}
+
+int hsb_set_step_record(hsb_handle* h, int on) {
+  if (!h) return HSB_ERR_INVALID_ARG;
+  if (on && !h->h_step_rec) {
+    DeviceGuard dev(h->device);
+    const size_t bytes = (size_t)record_floats(h) * sizeof(float);
+    HSB_CUDA(h, cudaHostAlloc(reinterpret_cast<void**>(&h->h_step_rec), bytes, cudaHostAllocMapped));
+    memset(h->h_step_rec, 0, bytes);
+    HSB_CUDA(h, cudaHostGetDevicePointer(reinterpret_cast<void**>(&h->h_step_rec_dev), h->h_step_rec, 0));
+  }
+  if (on && !h->step_rec_on) h->step_rec_matched = false;   // no step since the switch was turned on
+  h->step_rec_on = on != 0;
+  return HSB_OK;
+}
+
+int hsb_get_step_record(hsb_handle* h, float* record_out, int* matched) {
+  if (!h) return HSB_ERR_INVALID_ARG;
+  if (!record_out || !matched)
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_step_record: %s is NULL", record_out ? "matched" : "record_out");
+  if (!h->stepped) return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_step_record: the handle has taken no fused SLAM step");
+  *matched = h->step_rec_matched ? 1 : 0;
+  // (every step returns after its match has finished: a nowait step's record is published with its pose)
+  if (h->step_rec_matched) memcpy(record_out, h->h_step_rec, (size_t)record_floats(h) * sizeof(float));
+  return HSB_OK;
+}
+
+int hsb_get_last_match_scan(hsb_handle* h, float* points_xy_out, int capacity, int* n_out, float origo_out[2]) {
+  if (!h) return HSB_ERR_INVALID_ARG;
+  if (!n_out || !origo_out)
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_last_match_scan: %s is NULL", n_out ? "origo_out" : "n_out");
+  if (!h->have_last_match) return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_last_match_scan: the handle has matched no scan");
+  const int n = h->last_n;
+  *n_out = n;
+  if (capacity < n)
+    return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_last_match_scan: capacity %d is below the container's %d endpoints",
+                capacity, n);
+  if (n > 0 && !points_xy_out) return fail(h, HSB_ERR_INVALID_ARG, "hsb_get_last_match_scan: points_xy_out is NULL");
+  origo_out[0] = h->last_origo[0];
+  origo_out[1] = h->last_origo[1];
+  if (n == 0) return HSB_OK;
+  HandleScope guard(h);   // behind the step that filled the container (a group step runs on its group's stream)
+  HSB_CUDA(h, cudaMemcpyAsync(points_xy_out, scan_points(h->d_last_pts), (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
+  HSB_CUDA(h, cudaStreamSynchronize(h->stream));
+  return HSB_OK;
 }
 
 int hsb_hessian_derivs(hsb_handle* h, int level, const float pose_map[3], const float* pts, int n, float H_out[9],
@@ -1876,6 +1932,8 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     dev = {in.kind, d_c + kHdr + kTf, nullptr, n, n, in.tf ? reinterpret_cast<const double*>(d_c + kHdr) : nullptr};
   }
   float2* d_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));
+  h->stepped = true;
+  h->step_rec_matched = h->step_rec_on && matched;
   if (matched) {
     // :78 match, and :83-89 the gate in the same kernel's epilogue (an empty scan still passes through it: pose = hint)
     HsbMatchParams P;
@@ -1891,6 +1949,9 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     P.gate_out_host = host_out ? h_res->pose : nullptr;
     P.seq_host = poll ? seq_dev : nullptr;
     P.seq_value = seq_value;
+    // the step record: stored by the match before the sequence number (or the synchronise) releases the pose
+    P.record = h->step_rec_on ? h->h_step_rec_dev : nullptr;
+    P.record_floats = record_floats(h);
     // (a projected step takes the single step's default shape: hsb_slam_update_projected checked the tuning)
     s = launch_match_single(h, P, inl, header, 6, in.in);
     // (endpoints: the scan is in the container since the staging copy, whether or not the match launched)
@@ -3116,6 +3177,9 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
     gs.member = members[k];
     gs.levels = h->levels;
     gs.conv = ss.conv;
+    h->stepped = true;
+    h->step_rec_matched = h->step_rec_on && matched;
+    gs.record = h->step_rec_matched ? h->h_step_rec_dev : nullptr;
     if (matched && !conv) gs.last_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));   // the match copies the scan there
     if (matched) record_match(h, n, ss.origo);
     // level 0 reads the staged endpoints, or a converted scan where it was converted to, with its count on the device

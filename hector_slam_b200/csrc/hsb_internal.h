@@ -62,6 +62,9 @@ struct HsbGroupSessionDev {
   // the member's level count: a heterogeneous group's step (GRP_STEP_HET) starts the session at its member's coarsest
   // level; its rows of group_lv past that are never read.  (Fills the descriptor's tail padding: its size is unchanged.)
   int levels;
+  // the member's per-evaluation record of this step's match (HsbMatchParams::record's layout for the member's own levels:
+  // group_lv's rec_off), in the member's mapped host buffer (hsb_set_step_record); null: the session records nothing
+  float* record;
 };
 
 // One session of a pose-scoring call or of a group batch match: the scan its poses are scored against (its hints are
@@ -121,7 +124,8 @@ struct HsbMatchParams {
   //   then for every evaluation e = 0 .. evals-1, 15 floats:
   //   [9]  H row-major, [3] dTr, [3] the estimate after e's step in the level's map cells, angle not normalised
   //        (equal to the estimate before it when the H(0,0) != 0 && H(1,1) != 0 gate skipped the step)
-  // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.
+  // An empty scan writes the level start poses (all the hint) and zeros in every evaluation slot.  A group SLAM step
+  // leaves this null: each session records into its own HsbGroupSessionDev::record.
   float* record;
   int record_floats;
   // group SLAM step (match_kernel<..., GRP = GRP_STEP>): scan b is session b of the step, which steps member

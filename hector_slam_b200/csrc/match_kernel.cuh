@@ -808,6 +808,14 @@ __device__ __forceinline__ const HsbConvDev& conv_desc(const HsbMatchParams& P, 
   else return P.conv;
 }
 
+// Where scan `scan`'s per-evaluation record starts: its row of P.record, or — group SLAM step — the session's own buffer
+// (HsbGroupSessionDev::record; its members' records differ in length).  Loaded again at each store (see match_kernel).
+template <int GRP>
+__device__ __forceinline__ float* record_base(const HsbMatchParams& P, int scan) {
+  if constexpr (kGrpStep<GRP>) return P.group_sess[scan].record;
+  else return P.record + (size_t)scan * P.record_floats;
+}
+
 // GRP: GRP_STEP, the group SLAM step (hsb_group_slam_update), one session per scan — see HsbMatchParams::group_lv;
 // GRP_MATCH, the group batch match (hsb_group_match_batch), one hint per scan — see HsbMatchParams::match_sess.
 // PROJ: converted input is HSB_IN_PROJECTED (laser_geometry's projection and the cloud rule, stage_from_projected); only
@@ -995,8 +1003,11 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
     acc_zero(last);
     // per-evaluation record (hsb_internal.h HsbMatchParams::record): thread 0 stores what the group holds anyway.  The
     // address is formed from the kernel parameters at each store (level offsets precomputed on the host), so that the
-    // evaluation loop carries no extra live register for it
-    const bool recording = P.record && t == 0;
+    // evaluation loop carries no extra live register for it.  A group step's session records into its own buffer, set
+    // only for a recording member's matched session
+    bool recording;
+    if constexpr (kGrpStep<GRP>) recording = t == 0 && P.group_sess[scan].record;
+    else recording = P.record && t == 0;
     int evals_ran = 0;   // evaluations this scan actually ran (trace slot 5)
     if (n > 0) {
       for (int lvl = (kGrpHet<GRP> ? levels : P.levels) - 1; lvl >= 0; --lvl) {
@@ -1004,7 +1015,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
         if (recording) {
-          float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off;
+          float* rec = record_base<GRP>(P, scan) + L.rec_off;
           rec[0] = wx; rec[1] = wy; rec[2] = wpsi;
         }
         affine_apply_exact(L.mtw, wx, wy, ex, ey);  // ScanMatcher.h:70 getMapCoordsPose
@@ -1088,7 +1099,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
             epsi = npsi;
           }
           if (recording) {
-            float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off + 3 + 15 * e;
+            float* rec = record_base<GRP>(P, scan) + L.rec_off + 3 + 15 * e;
             rec[0] = a.h00; rec[1] = a.h01; rec[2] = a.h02;
             rec[3] = a.h01; rec[4] = a.h11; rec[5] = a.h12;
             rec[6] = a.h02; rec[7] = a.h12; rec[8] = a.h22;
@@ -1109,7 +1120,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
           // the skipped evaluations: `last` and the pose already are what each of them would leave
           if (recording) {
             for (int e = ran; e < L.evals; ++e) {
-              float* rec = P.record + (size_t)scan * P.record_floats + L.rec_off + 3 + 15 * e;
+              float* rec = record_base<GRP>(P, scan) + L.rec_off + 3 + 15 * e;
               rec[0] = last.h00; rec[1] = last.h01; rec[2] = last.h02;
               rec[3] = last.h01; rec[4] = last.h11; rec[5] = last.h12;
               rec[6] = last.h02; rec[7] = last.h12; rec[8] = last.h22;
@@ -1129,10 +1140,12 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
         if (HSB_DIAG && P.trace && t == 0) P.trace[8 * (size_t)scan + (P.levels - lvl)] = global_timer_ns();
       }
     } else if (recording) {   // nothing evaluated: every level starts from the hint, the evaluation slots are zero
-      for (int lvl = P.levels - 1; lvl >= 0; --lvl) {
-        float* rec = P.record + (size_t)scan * P.record_floats + P.lv[lvl].rec_off;
+      // (a group step's session: its member's own levels, in its member's layout)
+      for (int lvl = (GRP == GRP_STEP_HET ? levels : P.levels) - 1; lvl >= 0; --lvl) {
+        const HsbLevelDev& L = kGrpStep<GRP> ? level_desc<GRP>(P, scan, member, lvl) : P.lv[lvl];
+        float* rec = record_base<GRP>(P, scan) + L.rec_off;
         rec[0] = wx; rec[1] = wy; rec[2] = wpsi;
-        for (int i = 3; i < 3 + 15 * P.lv[lvl].evals; ++i) rec[i] = 0.0f;
+        for (int i = 3; i < 3 + 15 * L.evals; ++i) rec[i] = 0.0f;
       }
     }
     if (pace && n <= 0) {   // nothing evaluated: account for the evaluations the others wait for

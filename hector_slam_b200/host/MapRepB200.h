@@ -26,6 +26,7 @@
 
 #include "slam_main/HectorSlamProcessor.h"  // pulls map/, matcher/, scan/, util/ in the right order
 
+#include "MatchHooksB200.h"
 #include "hector_slam_b200.h"
 
 namespace hectorslam {
@@ -34,7 +35,7 @@ class MapRepB200 : public MapRepresentationInterface {
  public:
   // Arguments as MapRepMultiMap's (MapRepMultiMap.h:48); `device` selects the GPU.
   // The two hooks are what MapRepMultiMap hands every level's ScanMatcher (MapRepMultiMap.h:63); matchData replays the
-  // matcher's calls on them from the device's per-evaluation record (see replay_hooks).
+  // matcher's calls on them from the device's per-evaluation record (replayMatchHooks, MatchHooksB200.h).
   MapRepB200(float mapResolution, int mapSizeX, int mapSizeY, unsigned int numDepth, const Eigen::Vector2f& startCoords,
              DrawInterface* drawInterfaceIn = 0, HectorDebugInfoInterface* debugInterfaceIn = 0, int device = 0)
       : handle_(0), draw_(drawInterfaceIn), debug_(debugInterfaceIn) {
@@ -52,19 +53,13 @@ class MapRepB200 : public MapRepresentationInterface {
       throw std::runtime_error(std::string("hsb_create failed: ") + hsb_last_error(0));
     }
     // host mirrors with the reference's own geometry (MapRepMultiMap.h:51-69)
-    Eigen::Vector2i resolution(mapSizeX, mapSizeY);
-    float totalMapSizeX = mapResolution * static_cast<float>(mapSizeX);
-    float mid_offset_x = totalMapSizeX * startCoords.x();
-    float totalMapSizeY = mapResolution * static_cast<float>(mapSizeY);
-    float mid_offset_y = totalMapSizeY * startCoords.y();
-    for (unsigned int i = 0; i < numDepth; ++i) {
-      mirrors_.push_back(new GridMap(mapResolution, resolution, Eigen::Vector2f(mid_offset_x, mid_offset_y)));
-      stale_.push_back(false);
-      pending_updates_.push_back(0);
-      mutexes_.push_back(0);
-      resolution /= 2;
-      mapResolution *= 2.0f;
-    }
+    forEachMapLevel(mapResolution, mapSizeX, mapSizeY, numDepth, startCoords,
+                    [this](unsigned int, float cellLength, const Eigen::Vector2i& cells, const Eigen::Vector2f& offset) {
+                      mirrors_.push_back(new GridMap(cellLength, cells, offset));
+                      stale_.push_back(false);
+                      pending_updates_.push_back(0);
+                      mutexes_.push_back(0);
+                    });
   }
 
   virtual ~MapRepB200() {
@@ -143,7 +138,7 @@ class MapRepB200 : public MapRepresentationInterface {
     if (draw_ || debug_) {
       record_.resize(static_cast<size_t>(hsb_get_match_record_floats(handle_)));
       check(hsb_match_data_record(handle_, hint, pts, n, og, pose, cov, record_.data()));
-      replay_hooks(dataContainer);
+      replayMatchHooks(handle_, record_.data(), dataContainer, mirrors_.data(), draw_, debug_, scaled_);
     } else {
       check(hsb_match_data(handle_, hint, pts, n, og, pose, cov));
     }
@@ -191,67 +186,6 @@ class MapRepB200 : public MapRepresentationInterface {
   // path can fail; a CUDA failure here is unrecoverable for the caller, so it is raised.
   void check(int st) const {
     if (st != HSB_OK) throw std::runtime_error(std::string("hector_slam_b200: ") + hsb_last_error(handle_));
-  }
-
-  // ScanMatcher::matchData's hook calls (matcher/ScanMatcher.h:56-115) for every level, coarsest first, replayed from
-  // the record of the match that just ran (include/hector_slam_b200.h, hsb_match_data_record).  The world-space
-  // conversions are the reference's own code on the host mirrors' geometry, the drawn scan is the level's container
-  // as MapRepMultiMap.h:127 scales it: the same arithmetic as the CPU matcher, on the device's estimates.
-  void replay_hooks(const DataContainer& dataContainer) {
-    const int levels = static_cast<int>(mirrors_.size());
-    const int n = dataContainer.getSize();
-    const float* r = record_.data();
-    for (int index = levels - 1; index >= 0; --index) {
-      const int numIter = index == 0 ? 5 : 3;  // MapRepMultiMap.h:125,128 (hsb_create's defaults for a zero entry)
-      const GridMap& map = *mirrors_[index];
-      const DataContainer* dc = &dataContainer;
-      if (index > 0) {
-        scaled_.setFrom(dataContainer, static_cast<float>(1.0 / pow(2.0, static_cast<double>(index))));
-        dc = &scaled_;
-      }
-      const Eigen::Vector3f begin(r[0], r[1], r[2]);
-      const float* ev = r + 3;  // 15 floats per evaluation: H (9), dTr (3), estimate after the step (3)
-      if (draw_) {
-        draw_->setScale(0.05f);
-        draw_->setColor(0.0f, 1.0f, 0.0f);
-        draw_->drawArrow(begin);
-        drawScan(map.getMapCoordsPose(begin), map, *dc);
-        draw_->setColor(1.0, 0.0, 0.0);
-      }
-      if (n != 0) {
-        for (int i = 0; i < numIter; ++i) {
-          const float* e = ev + 15 * (i + 1);  // evaluation 0 (before the loop) is not reported
-          if (draw_) {
-            float invNumIterf = 1.0f / static_cast<float>(numIter);
-            draw_->setColor(static_cast<float>(i) * invNumIterf, 0.0f, 0.0f);
-            draw_->drawArrow(map.getWorldCoordsPose(Eigen::Vector3f(e[12], e[13], e[14])));
-          }
-          if (debug_) {
-            Eigen::Matrix3f H;
-            for (int a = 0; a < 3; ++a)
-              for (int b = 0; b < 3; ++b) H(a, b) = e[3 * a + b];
-            debug_->addHessianMatrix(H);
-          }
-        }
-        if (draw_) {
-          const float* e = ev + 15 * numIter;
-          draw_->setColor(0.0, 0.0, 1.0);
-          drawScan(Eigen::Vector3f(e[12], e[13], e[14]), map, *dc);
-        }
-      }
-      r += 3 + 15 * (numIter + 1);
-    }
-  }
-  // ScanMatcher::drawScan (ScanMatcher.h:228-239): OccGridMapUtil::getTransformForState (OccGridMapUtil.h:349-352) and
-  // getWorldCoordsPoint (:62) restated on the mirror, which carries the level's geometry
-  void drawScan(const Eigen::Vector3f& pose, const GridMap& map, const DataContainer& dataContainer) {
-    draw_->setScale(0.02);
-    Eigen::Affine2f transform(Eigen::Translation2f(pose[0], pose[1]) * Eigen::Rotation2Df(pose[2]));
-    int size = dataContainer.getSize();
-    for (int i = 0; i < size; ++i) {
-      const Eigen::Vector2f& currPoint(dataContainer.getVecEntry(i));
-      draw_->drawPoint(map.getWorldCoords(transform * currPoint));
-    }
   }
 
   hsb_handle* handle_;

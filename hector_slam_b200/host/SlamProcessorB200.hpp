@@ -281,6 +281,28 @@ class SlamProcessor {
     }
   }
 
+  // The node's pub_drawings / pub_debug_output for the fused and group steps (hsb_set_step_record): on, every matched
+  // update*() and this processor's session of every updateMany*() records its match; the results are unchanged.
+  // stepRecord() fetches the record of the last step (false: that step ran no match, the reference calls no hook);
+  // lastMatchScan() the level-0 container it matched (n endpoints, 2n floats, and origo).  With the reference's headers,
+  // replayMatchHooks (MatchHooksB200.h) turns the two into the matcher's hook calls.
+  void setStepRecord(bool on) { check(hsb_set_step_record(h_, on ? 1 : 0)); }
+  bool stepRecord(std::vector<float>& record) const {
+    const int R = hsb_get_match_record_floats(h_);
+    if (R < 0) check(R);
+    record.resize((size_t)R);
+    int matched = 0;
+    check(hsb_get_step_record(h_, record.data(), &matched));
+    return matched != 0;
+  }
+  int lastMatchScan(std::vector<float>& pointsXY, float origo[2]) const {
+    int n = 0;
+    if (hsb_get_last_match_scan(h_, 0, 0, &n, origo) != HSB_OK && n == 0) check(HSB_ERR_INVALID_ARG);
+    pointsXY.resize(2 * (size_t)n);
+    check(hsb_get_last_match_scan(h_, pointsXY.data(), n, &n, origo));
+    return n;
+  }
+
   const Pose& getLastScanMatchPose() const { return lastScanMatchPose_; }
   const float* getLastScanMatchCovariance() const { return lastScanMatchCov_; }
   float getScaleToMap() const { return hsb_get_scale_to_map(h_); }

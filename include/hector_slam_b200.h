@@ -160,6 +160,27 @@ int hsb_match_data_record(hsb_handle* h, const float begin_estimate_world[3], co
 int hsb_match_batch_record_device(hsb_handle* h, int B, const float* d_hints_world, const float* d_points_xy,
                                   const int* d_offsets, int n_shared, int max_points_per_scan, float* d_out_poses_world,
                                   float* d_out_cov, float* d_record, void* stream);
+/* Gauss-Newton evaluations of one level's match: maxIterations + 1 (the defaults 5 / 3 for a zero entry of
+ * hsb_config::max_iterations).  Returns the count, or HSB_ERR_INVALID_ARG for a level the handle does not have. */
+int hsb_get_level_evals(const hsb_handle* h, int level);
+
+/* The record of the fused SLAM steps, for the node's pub_drawings / pub_debug_output hooks without leaving the fused
+ * or group step.  on != 0: every matched fused SLAM step of this handle writes the per-evaluation record of its match
+ * (the layout above, R = hsb_get_match_record_floats floats).  This covers hsb_slam_update* and the handle's session in
+ * any hsb_group_slam_update*, full or subset, waiting or nowait.  Recording changes no result and adds no launch,
+ * copy or synchronise: the match kernel stores the record into mapped pinned host memory owned by the handle before
+ * the step's pose is published, so a nowait step's record is complete when the step returns.  The handle's next
+ * fused step overwrites it.  Turning the switch on allocates that memory (once). */
+int hsb_set_step_record(hsb_handle* h, int on);
+/* the record of the handle's last fused step (R floats).  *matched = 0 when that step ran no match
+ * (map_without_matching, or no step since the switch was turned on; record_out is then left untouched): the reference
+ * calls no hook then.  Rejected with a message: a NULL record_out or matched, a handle that took no fused step. */
+int hsb_get_step_record(hsb_handle* h, float* record_out, int* matched);
+/* the level-0 container of the handle's last matched scan (endpoints in level-0 cells, and origo): what drawScan
+ * draws, needed after a converted step (cloud, ranges, projected), whose endpoints exist only on the device.  *n_out
+ * receives the count even when `capacity` is below it (then HSB_ERR_INVALID_ARG).  Rejected with a message: a NULL
+ * n_out or origo_out, a NULL points_xy_out for a non-empty container, a handle that has matched no scan. */
+int hsb_get_last_match_scan(hsb_handle* h, float* points_xy_out, int capacity, int* n_out, float origo_out[2]);
 
 /* ---- raw laser ranges in (the step before the path: scan -> DataContainer) ---------------------*/
 /* The sensor_msgs/LaserScan fields HectorMappingRos::rosLaserScanToDataContainer reads
