@@ -2,6 +2,8 @@
 
   hector_slam_b200/lib/libhsb200.so        CUDA kernels + C-ABI (include/hector_slam_b200.h), sm_90a only
   hector_slam_b200/lib/libhsb200_host.so   C wrapper around the C++ host façade (host/), links libhsb200.so
+  hector_slam_b200/lib/libhsb200_probe.so  the kernels' scalar device functions one by one (tests/device/hsb_probe.cu),
+                                           for the tests only: nothing in the package loads it
 
 nvcc cross-compiles without a GPU, so this runs on a CPU-only build machine; the .so files are
 git-ignored build products.
@@ -20,6 +22,8 @@ HOST = os.path.join(PKG, "host")
 LIBDIR = os.path.join(PKG, "lib")
 LIB = os.path.join(LIBDIR, "libhsb200.so")
 HOST_LIB = os.path.join(LIBDIR, "libhsb200_host.so")
+PROBE_SRC = os.path.join(ROOT, "tests", "device", "hsb_probe.cu")
+PROBE_LIB = os.path.join(LIBDIR, "libhsb200_probe.so")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -84,9 +88,31 @@ def build_host(force: bool = False) -> str | None:
     return HOST_LIB
 
 
+def probe_command() -> list[str]:
+    """nvcc command of the probe library: the product library's NVCC_FLAGS unchanged, so the probed functions are
+    compiled as the kernels compile them (-fmad=false above all)"""
+    return [_nvcc()] + NVCC_FLAGS + ["-I", CSRC, "-o", PROBE_LIB, PROBE_SRC]
+
+
+def build_probe(force: bool = False) -> str | None:
+    if not os.path.exists(PROBE_SRC):
+        return None
+    srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "hector_slam_b200.h"), PROBE_SRC]
+    if not force and _newer(PROBE_LIB, srcs):
+        return PROBE_LIB
+    os.makedirs(LIBDIR, exist_ok=True)
+    cmd = probe_command()
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode != 0:
+        sys.stderr.write(r.stdout + r.stderr)
+        raise RuntimeError("nvcc failed: " + " ".join(cmd))
+    return PROBE_LIB
+
+
 def build_all(force: bool = False, verbose: bool = False):
     build_cuda(force, verbose)
     build_host(force)
+    build_probe(force)
 
 
 if __name__ == "__main__":

@@ -45,7 +45,8 @@ __device__ __forceinline__ void affine_apply_exact(const float* m, float vx, flo
 // util::normalize_angle, UtilFunctions.h:37-49:  a = fmod(fmod(angle, 2pi) + 2pi, 2pi); if (a > pi) a -= 2pi,
 // in double because M_PI is a double, narrowed to float where the reference narrows.  Both fmods are
 // exact operations; for |angle| < 2pi the first is the identity and the second is one exact
-// subtraction (Sterbenz), so the common case needs no fmod at all — bit-identical either way.
+// subtraction (Sterbenz), so the common case needs no fmod at all — bit-identical either way (on every fp32 argument:
+// tests/test_gpu_scalar_functions.py).
 __device__ __forceinline__ float normalize_angle(float angle) {
   const double two_pi = 2.0 * 3.14159265358979323846;
   double r = (double)angle;
@@ -1272,10 +1273,11 @@ __device__ __forceinline__ float pose_likelihood(const HsbLevelDev& L, const Lev
 
 // arg-max over a batch (relocalisation: the most likely hypothesis): (score, index) packed so that one 64-bit atomicMax
 // keeps the highest score and, among equals, the LOWEST index; a non-finite pose scores -1, and so does a NaN
-// likelihood (an empty scan: 1 - 0/0), whose bits would otherwise pack above every score
+// likelihood (an empty scan: 1 - 0/0), whose bits would otherwise pack above every score.  Every finite pose keeps its
+// score, FLT_MAX included (hsb_reset stores FLT_MAX as a pose); only +-inf and NaN are non-finite.
 __device__ __forceinline__ unsigned long long best_pack(float lh, const float* __restrict__ pose_world, unsigned index) {
   const float px = pose_world[0], py = pose_world[1], pp = pose_world[2];
-  const bool finite = fabsf(px) <= 3.4e38f && fabsf(py) <= 3.4e38f && fabsf(pp) <= 3.4e38f;
+  const bool finite = isfinite(px) && isfinite(py) && isfinite(pp);
   const float sc = (finite && lh == lh) ? lh : -1.0f;
   unsigned u = __float_as_uint(sc);
   u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);

@@ -12,7 +12,8 @@
 // FMA-enabled build (transcribed from the disassembly of __sinf_fma / __cosf_fma in
 // libm.so.6 2.39-0ubuntu8.5, which every AVX2+FMA host selects through ifunc), constants read
 // from that library's __sincosf_table.  tests/test_sincosf_glibc.py checks the host build of
-// this header against the running libm bit for bit over tens of millions of arguments.
+// this header against the running libm bit for bit on every fp32 argument, and
+// tests/test_gpu_scalar_functions.py the device build.
 //
 // Provenance / licence: this header is a restatement of the GNU C Library's single-precision
 // sin/cos algorithm (glibc 2.39, sysdeps/ieee754/flt-32/{s_sinf.c,s_cosf.c,sincosf.h,
@@ -250,7 +251,8 @@ HSB_HD void sincosf_glibc(float y, float* sp, float* cp) {
 //   s = asdouble(T[ki % 32] + (ki << 47)); z = fma(r, C0, C1); r2 = r * r; y = fma(r, C2, 1); y = fma(z, r2, y); return (float)(y * s)
 // constants and the 2^(i/32) table read from that library's __exp2f_data.  Out-of-range arguments as glibc handles them:
 // NaN / +inf -> x + x, x > 0x1.62e42ep6 -> +inf, x < -0x1.9fe368p6 -> +0, x < -0x1.9d1d9ep6 -> 0x1.4p-75f squared (= 2^-149).
-// tests/test_sincosf_glibc.py checks the host build against the running libm bit for bit.
+// tests/test_sincosf_glibc.py checks the host build against the running libm bit for bit on every fp32 argument,
+// tests/test_gpu_scalar_functions.py the device build.
 #define HSB_EXPF_SHIFT 0x1.8p+52
 #define HSB_EXPF_INVLN2N 0x1.71547652b82fep+5
 #define HSB_EXPF_C0 0x1.c6af84b912394p-20

@@ -458,6 +458,10 @@ void hso_pose_difference_larger_than(const float* p1, const float* p2, const flo
                                      int* out) {
   for (int i = 0; i < n; ++i) out[i] = pose_difference_larger_than(p1 + 3 * i, p2 + 3 * i, dist[i], ang[i]);
 }
+/* the Gauss-Newton step's `H.inverse() * dTr` on its own, n at a time: m n x 9 (row-major 3x3), v n x 3, out n x 3 */
+void hso_inverse3_times(const float* m, const float* v, int n, float* out) {
+  for (int i = 0; i < n; ++i) inverse3_times(m + 9 * i, v + 3 * i, out + 3 * i);
+}
 
 /* MapRepMultiMap.h:134-147 updateByScan (coarse levels use the containers left by matchData) */
 static void maprep_update_by_scan(hso_t* h, const container_t* dc, const float pose[3]) {

@@ -456,6 +456,57 @@ def test_best_hypothesis_edge_cases(M, mode):
     assert np.array_equal(bits(b_lo2), bits(b_lo))
 
 
+@pytest.mark.parametrize("mode", MODES)
+def test_best_hypothesis_largest_finite_poses(M, mode):
+    """A finite pose keeps its score however large its coordinates: FLT_MAX (what hsb_reset stores as a pose), the
+    largest negative value and the rest of (3.4e38, FLT_MAX] are finite.  Through hsb_best_hypothesis_device,
+    hsb_group_best_hypothesis and its _subset form."""
+    from hector_slam_b200 import capi
+
+    S = M["sq"]
+    rep = S.reps[mode]
+    lv = S.levels[0]
+    fmax = np.finfo(F32).max
+    big = np.nextafter(F32(3.4e38), F32(np.inf))
+    rng = np.random.default_rng(77)
+    g = capi.SlamGroup([rep])
+    try:
+        def all_calls(poses, scan, what):
+            """(best4, index) of the three entry points, which must agree bit for bit"""
+            best4, out = best_on_device(rep, 0, poses, scan, None, n_shared=len(scan), want_out=True)
+            lh = rep.likelihood_batch(0, poses, scan)
+            assert np.array_equal(bits(out), bits(lh)), what
+            check_winner(best4, lh, poses, what)
+            k = int(np.flatnonzero(np.all(bits(poses) == bits(best4[1:]), axis=1))[0])
+            for members in (None, [0]):
+                out_g, b4, idx = g.best_hypothesis(0, [poses], [scan], members=members)
+                assert np.array_equal(bits(out_g), bits(lh)), (what, members)
+                assert np.array_equal(bits(b4[0]), bits(best4)) and idx[0] == k, (what, members, b4[0], idx[0], best4, k)
+            return best4, k, lh
+
+        # (FLT_MAX, 0, 0), then a far-off finite pose: every endpoint of both is out of the map, both score exactly 0,
+        # and the lower index wins the tie
+        pose_map = S.random_pose(lv, rng)
+        scan = lv.scan(300, rng, pose_map)
+        poses = F32([[fmax, 0.0, 0.0], [1e6, -1e6, 0.5]])
+        best4, k, lh = all_calls(poses, scan, f"mode{mode} FLT_MAX then far off")
+        assert np.all(bits(lh) == 0) and k == 0, (lh, best4)
+        # poses made only of largest-finite coordinates: x, y far out of the map score 0; a psi of FLT_MAX, -FLT_MAX or
+        # just above 3.4e38 with x, y on the map scores a real likelihood, pinned to the float64 reference
+        xy = pose_map[:2] * F32(lv.cell)
+        psis = F32([fmax, -fmax, big, -big])
+        poses = np.concatenate([F32([[fmax, fmax, fmax], [-fmax, big, 0.0]]),
+                                np.stack([np.full(4, xy[0]), np.full(4, xy[1]), psis], 1)]).astype(F32)
+        scan = lv.scan(500, rng, F32([pose_map[0], pose_map[1], fmax]))
+        best4, k, lh = all_calls(poses, scan, f"mode{mode} largest finite coordinates")
+        assert np.all(bits(lh[:2]) == 0)
+        for j in range(2, poses.shape[0]):
+            Ref(lv, scan, F32([pose_map[0], pose_map[1], poses[j, 2]])).check(lh[j], f"mode{mode} psi {poses[j, 2]}")
+        assert k >= 2 and best4[0] > 0, (k, best4)
+    finally:
+        g.close()
+
+
 # ---- 3. covariance -------------------------------------------------------------------------------------------------
 def sigma_world(r):
     sp = likelihood64.sigma_points(r.pose_map)

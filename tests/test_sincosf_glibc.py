@@ -1,11 +1,17 @@
 """CPU: hector_slam_b200/csrc/sincosf_glibc.h (the sinf/cosf the kernels use for the pose angle)
 against the running libm, bit for bit.  The header transcribes glibc 2.39's FMA build, which libm
 selects through ifunc on every AVX2+FMA host; on a host without FMA libm takes another code path
-and the comparison is skipped."""
+and the comparison is skipped.
+
+The sampled cases below aim at the reductions' edges; test_*_every_argument then compares the host build with libm on
+all 2^32 bit patterns (tests/libm_sweep.py), so the transcription is right everywhere and the device sweep
+(test_gpu_scalar_functions.py) only has to show that nvcc compiles it to the same bits.  Cost: the two exhaustive
+tests take about 45-60 s of wall time on an 8-thread x86-64 CPU (the sweep uses every CPU the process may run on)."""
 import os
 import shutil
 import subprocess
 
+import numpy as np
 import pytest
 
 from conftest import ROOT
@@ -175,3 +181,47 @@ def test_expf_matches_libm(tmp_path):
     out = subprocess.run([str(exe)], capture_output=True, text=True)
     n, bad = (int(v) for v in out.stdout.split())
     assert bad == 0 and n > 16000000, out.stdout
+
+
+# ---- every fp32 argument ---------------------------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def sweep(tmp_path_factory):
+    import libm_sweep
+
+    why = libm_sweep.skip_reason()
+    if why:
+        pytest.skip(why)
+    return libm_sweep.build(tmp_path_factory.mktemp("libm_sweep"))
+
+
+def _exhaustive(run, names):
+    import libm_sweep
+
+    total, counts, first_bad, n = None, np.zeros(len(names), np.int64), [[] for _ in names], 0
+    for first, size in libm_sweep.chunks(1 << 26):
+        c, bad = run(first, size)
+        for k in range(len(names)):
+            first_bad[k] += bad[k][:max(0, min(int(c[k]), libm_sweep.MAX_BAD) - len(first_bad[k]))].tolist()
+        counts += c
+        n += size
+    bad = np.array([(b + [0] * libm_sweep.MAX_BAD)[:libm_sweep.MAX_BAD] for b in first_bad], np.uint32)
+    return n, counts, bad
+
+
+def test_sincosf_every_argument(sweep):
+    """sinf_glibc, cosf_glibc and both outputs of sincosf_glibc (host build) equal libm on all 2^32 arguments"""
+    import libm_sweep
+
+    names = ["sinf_glibc", "cosf_glibc", "sincosf_glibc sin", "sincosf_glibc cos"]
+    n, counts, bad = _exhaustive(sweep.host_trig, names)
+    print(f"sincosf: {n} arguments, mismatches {dict(zip(names, counts.tolist()))}")
+    assert n == libm_sweep.ALL and not counts.any(), libm_sweep.report_bad(names, counts, bad)
+
+
+def test_expf_every_argument(sweep):
+    """expf_glibc (host build) equals libm expf on all 2^32 arguments"""
+    import libm_sweep
+
+    n, counts, bad = _exhaustive(sweep.host_exp, ["expf_glibc"])
+    print(f"expf: {n} arguments, {int(counts[0])} mismatches")
+    assert n == libm_sweep.ALL and not counts.any(), libm_sweep.report_bad(["expf_glibc"], counts, bad)
