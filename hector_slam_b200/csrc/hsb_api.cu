@@ -554,6 +554,26 @@ int launch_match(hsb_handle* h, HsbMatchParams& P, int max_n, cudaStream_t st) {
   return launch_match_mode<hsb::MODE_LDG>(h, P, max_n, st, W, G, U, Gr);
 }
 
+// Whether a converted scan of n inputs fits whole in the shared memory of the shape launch_match gives one scan of h
+// (W from the tuning or auto_warps_per_scan, every one of the tuning's G groups reserved), the limit launch_match_t
+// applies.  The header of MatchSmem<W, G> depends on W only through W > 1.  A shape that is not compiled passes here:
+// the launcher refuses its tuning.
+bool single_scan_fits(const hsb_handle* h, int n) {
+  const int W = h->tune_warps_per_scan > 0 ? h->tune_warps_per_scan : auto_warps_per_scan(h, 1);
+  const int G = h->tune_scans_per_block > 0 ? h->tune_scans_per_block : 1;
+  const int slots = whole_scan_slots(n);
+#define HSB_FITS(g) \
+  if (G == g) return W > 1 ? staging_fits<2, g>(slots, g) : staging_fits<1, g>(slots, g);
+  HSB_FITS(1);
+  HSB_FITS(2);
+  HSB_FITS(7);
+  HSB_FITS(14);
+  HSB_FITS(28);
+  HSB_FITS(32);
+#undef HSB_FITS
+  return true;
+}
+
 // Whether a single scan of n endpoints (hsb_match_data, hsb_slam_update) travels INSIDE the kernel parameters
 // (match_kernel.cuh InlineScan): tuning "inline_scan", and a tuning that leaves the single scan its usual shape.
 bool inline_scan_applies(const hsb_handle* h, int n) {
@@ -1890,6 +1910,9 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
   const int n = in.n_shared;   // converted: a cloud's points or a scan's beams, an upper bound of the endpoints kept
   const bool conv = in.kind != HSB_IN_ENDPOINTS;
   const bool matched = !map_without_matching;
+  // a matched converted scan is staged whole in the match's shared memory: refused here, before the session below
+  // regrows the last match's container (its endpoints would be lost) and marks the handle stepped
+  if (conv && matched && !single_scan_fits(h, n)) return fail_fused_too_long(h, n);
   PoseResult* d_res = &h->d_scratch->step;
   int* n_dev = conv ? &h->d_scratch->step_kept : nullptr;
   cudaStream_t st = h->stream;

@@ -77,3 +77,21 @@ def test_scan_to_points_port_equals_node_source(pyoracle, oracle_kinds):
                                     kind="reference")
         assert a.shape == b.shape and np.array_equal(a, b)
         assert np.allclose(a, synth.ranges_to_points(r, 20.0), rtol=1e-6, atol=1e-5)  # numpy cos is not glibc cosf
+
+
+@pytest.mark.parametrize("angle_min,angle_increment", [(-3.14159, 1.0e-6), (0.5, 3.0e-6),
+                                                       (-3.1415927, float(np.float32(2 * np.pi / (1 << 20)))),
+                                                       (1.0e3, 1.0e-6)])
+def test_scan_to_points_port_equals_node_source_on_long_formats(pyoracle, oracle_kinds, angle_min, angle_increment):
+    """2^20 beams (the longest scan format the library accepts) with increments down to 1e-6 rad: both accumulate the
+    beam angle in fp32 (`angle += angle_increment`), so the port equals the node's converter bit for bit, endpoints
+    at the far end of the accumulation included."""
+    if "reference" not in oracle_kinds:
+        pytest.skip("oracle/_ref not built here")
+    rng = np.random.default_rng(7)
+    r = rng.uniform(0.05, 32.0, 1 << 20).astype(np.float32)
+    r[::11] = np.nan
+    a = pyoracle.scan_to_points(r, angle_min, angle_increment, 0.1, 30.0, 20.0)
+    b = pyoracle.scan_to_points(r, angle_min, angle_increment, 0.1, 30.0, 20.0, kind="reference")
+    assert a.shape == b.shape and a.shape[0] > (1 << 19)
+    assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
