@@ -49,6 +49,9 @@ EXPORTED = [
     "hsb_group_pack_dirty_device", "hsb_group_pack_dirty_device_subset", "hsb_group_unpack_dirty_device",
     "hsb_group_create_mixed", "hsb_group_create_heterogeneous", "hsb_group_reset", "hsb_group_reset_subset",
     "hsb_get_level_evals", "hsb_set_step_record", "hsb_get_step_record", "hsb_get_last_match_scan",
+    "hsb_group_match_batch_ranges", "hsb_group_match_batch_cloud", "hsb_group_match_batch_projected",
+    "hsb_group_match_batch_ranges_subset", "hsb_group_match_batch_cloud_subset",
+    "hsb_group_match_batch_projected_subset",
 ]
 
 
@@ -219,6 +222,12 @@ def load_library() -> C.CDLL:
     sig("hsb_group_best_hypothesis_subset", i, vp, i, vp, i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_match_batch", i, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_match_batch_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_ranges", i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_cloud", i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_projected", i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_ranges_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_cloud_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
+    sig("hsb_group_match_batch_projected_subset", i, vp, i, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp)
     sig("hsb_group_pack_dirty_device", i, vp, vp, C.c_size_t, i, vp)
     sig("hsb_group_pack_dirty_device_subset", i, vp, i, vp, vp, C.c_size_t, i, vp)
     sig("hsb_group_unpack_dirty_device", i, vp, vp, C.c_size_t, vp)
@@ -1258,6 +1267,58 @@ class SlamGroup:
             self._check(self.lib.hsb_group_match_batch_subset(self.g, K, _ptr(mem), *args))
         del keep
         return poses, None if cov is None else cov.reshape(Q, 3, 3)
+
+    def match_batch_ranges(self, hints, scans, transforms=None, members=None, want_cov: bool = True,
+                           score: bool = False):
+        """match_batch from each session's new raw LaserScan ranges, converted on the device with its member's scan
+        format (hsb_group_match_batch_ranges): hints as in match_batch; scans is one (n_beams_s,) array per session, or a
+        tuple (ranges (N,), offsets (K + 1,)).  transforms is unused (the ranges kind has none).  members as in
+        slam_update (hsb_group_match_batch_ranges_subset).  score: also each matched pose's level-0 likelihood and each
+        session's best hypothesis (best_hypothesis on the returned poses with the converted scan).
+        -> (poses (Q, 3), cov (Q, 3, 3) | None, kept (K,) int[, likelihood (Q,), best4 (K, 4), index (K,)])"""
+        assert transforms is None, "LaserScan ranges have no laser transform"
+        return self._match_raw("ranges", 1, hints, scans, None, members, want_cov, score)
+
+    def match_batch_cloud(self, hints, scans, transforms=None, members=None, want_cov: bool = True,
+                          score: bool = False):
+        """The same from each session's Point32 cloud in the laser frame (hsb_group_match_batch_cloud): scans is one
+        (n_s, 3) array per session, or a tuple (points (N, 3), offsets (K + 1,)); transforms (K, 12) float64, None = each
+        member's cloud format.  Arguments and results as in match_batch_ranges."""
+        return self._match_raw("cloud", 3, hints, scans, transforms, members, want_cov, score)
+
+    def match_batch_projected(self, hints, scans, transforms=None, members=None, want_cov: bool = True,
+                              score: bool = False):
+        """The same from each session's LaserScan ranges as a default-configured node projects them
+        (hsb_group_match_batch_projected): each member projects with its laser projection and converts with its cloud
+        format.  Arguments and results as in match_batch_cloud, scans as in match_batch_ranges."""
+        return self._match_raw("projected", 1, hints, scans, transforms, members, want_cov, score)
+
+    def _match_raw(self, kind, width, hints, scans, transforms, members, want_cov, score):
+        K, mem = self._sessions(members)
+        h, hint_off = self._pack(hints, 3, K)
+        x, scan_off = self._pack(scans, width, K)
+        T = None if transforms is None else np.ascontiguousarray(transforms, dtype=np.float64).reshape(K, 12)
+        Q = h.shape[0]
+        poses = np.zeros((Q, 3), np.float32)
+        cov = np.zeros((Q, 9), np.float32) if want_cov else None
+        kept = np.zeros(max(1, K), np.int32)
+        lh = np.zeros(max(1, Q), np.float32) if score else None
+        best4 = np.zeros((max(1, K), 4), np.float32) if score else None
+        index = np.zeros(max(1, K), np.int32) if score else None
+        args = [hint_off.ctypes.data, _ptr(h if Q else None), _ptr(x if x.size else None), scan_off.ctypes.data]
+        if kind != "ranges":
+            args.append(_ptr(T))
+        args += [_ptr(poses if Q else None), _ptr(cov if Q else None), _ptr(lh), _ptr(best4), _ptr(index),
+                 kept.ctypes.data]
+        fn = "hsb_group_match_batch_" + kind
+        if mem is None:
+            self._check(getattr(self.lib, fn)(self.g, *args))
+        else:
+            self._check(getattr(self.lib, fn + "_subset")(self.g, K, _ptr(mem), *args))
+        out = (poses, None if cov is None else cov.reshape(Q, 3, 3), kept[:K].astype(int))
+        if score:
+            out += (lh[:Q], best4[:K], index[:K])
+        return out
 
     def _sessions(self, members):
         """-> (sessions of the step, the member list as int32, or None for a step of every member)"""

@@ -106,7 +106,7 @@ struct hsb_handle {
   bool fmt_set = false;
   hsb_cloud_format cfmt = hsb_cloud_format();
   bool cfmt_set = false;
-  DevBuf d_conv_in, d_cloud_tf;   // the stand-alone conversions' input (ranges or cloud) and laser transform
+  DevBuf d_conv_in, d_conv_tab;   // the stand-alone conversions' input (ranges or cloud), one-entry table and transform
   DevBuf d_proj_unit;   // laser_geometry's unit vectors, n_beams x double (cos, sin)
   hsb_laser_projection proj = hsb_laser_projection();
   bool proj_set = false;
@@ -864,7 +864,7 @@ int hsb_destroy(hsb_handle* h) {
   for (int l = 0; l < HSB_MAX_LEVELS; ++l) destroy_level(h, h->lv[l]);
   DevBuf* bufs[] = {&h->d_pts, &h->d_last_pts, &h->d_upd_pts,
                     &h->d_beam_cs, &h->d_occ, &h->d_trace, &h->d_best, &h->d_record,
-                    &h->d_conv_in, &h->d_cloud_tf, &h->d_fused_in, &h->d_proj_unit};
+                    &h->d_conv_in, &h->d_conv_tab, &h->d_fused_in, &h->d_proj_unit};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int k = 0; k < 2; ++k) {
@@ -1427,12 +1427,11 @@ int fixed_beams(const hsb_handle* h, HsbInputKind kind) {
   return 0;
 }
 
-// The stand-alone conversion of n_in inputs of `kind` at d_in (laser transform d_T) into c's sink.
-int launch_conversion(hsb_handle* h, HsbInputKind kind, const float* d_in, int n_in, const double* d_T, const HsbConvDev& c,
-                      cudaStream_t st) {
-  if (kind == HSB_IN_RANGES) hsb::conv_to_points_kernel<HSB_IN_RANGES><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
-  else if (kind == HSB_IN_CLOUD) hsb::conv_to_points_kernel<HSB_IN_CLOUD><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
-  else hsb::conv_to_points_kernel<HSB_IN_PROJECTED><<<1, 256, 0, st>>>(d_in, n_in, d_T, c);
+// The stand-alone conversion of the K scans of the device table d_tab, all of `kind`: one CTA of 8 warps per scan.
+int launch_conversion(hsb_handle* h, HsbInputKind kind, const HsbConvScanDev* d_tab, int K, cudaStream_t st) {
+  if (kind == HSB_IN_RANGES) hsb::conv_to_points_kernel<HSB_IN_RANGES><<<K, 256, 0, st>>>(d_tab);
+  else if (kind == HSB_IN_CLOUD) hsb::conv_to_points_kernel<HSB_IN_CLOUD><<<K, 256, 0, st>>>(d_tab);
+  else hsb::conv_to_points_kernel<HSB_IN_PROJECTED><<<K, 256, 0, st>>>(d_tab);
   h->launches++;
   HSB_CUDA(h, cudaGetLastError());
   return HSB_OK;
@@ -1444,21 +1443,31 @@ int to_points(hsb_handle* h, HsbInputKind kind, const float* in, int n, const do
               float out_origo[2]) {
   HandleScope guard(h);
   const size_t in_bytes = (size_t)n * (kind == HSB_IN_CLOUD ? 12 : 4);
+  // the conversion's one-entry table, then the laser transform: one copy (the call synchronises before it returns)
+  struct {
+    HsbConvScanDev e;
+    double T[12];
+  } tab;
   int s;
   if ((s = ensure(h, h->d_conv_in, in_bytes > 0 ? in_bytes : 12)) != HSB_OK) return s;
   if ((s = ensure(h, h->d_pts, (size_t)(n > 0 ? n : 1) * 8 + 16)) != HSB_OK) return s;
-  if (T && (s = ensure(h, h->d_cloud_tf, 12 * sizeof(double))) != HSB_OK) return s;
+  if ((s = ensure(h, h->d_conv_tab, sizeof(tab))) != HSB_OK) return s;
   cudaStream_t st = h->stream;
   if (n > 0) HSB_CUDA(h, cudaMemcpyAsync(h->d_conv_in.p, in, in_bytes, cudaMemcpyHostToDevice, st));
-  if (T) HSB_CUDA(h, cudaMemcpyAsync(h->d_cloud_tf.p, T, 12 * sizeof(double), cudaMemcpyHostToDevice, st));
-  HsbConvDev c;
-  fill_conv(h, kind, c);
-  c.out_pts = static_cast<float2*>(h->d_pts.p);
-  c.out_n = &h->d_scratch->conv_kept;
-  if ((s = launch_conversion(h, kind, static_cast<const float*>(h->d_conv_in.p), n,
-                             T ? static_cast<const double*>(h->d_cloud_tf.p) : nullptr, c, st)) != HSB_OK)
-    return s;
-  HSB_CUDA(h, cudaMemcpyAsync(&h->h_pin->conv_kept, c.out_n, sizeof(int), cudaMemcpyDeviceToHost, st));
+  const HsbConvScanDev* d_tab = static_cast<const HsbConvScanDev*>(h->d_conv_tab.p);
+  memset(&tab, 0, sizeof(tab));
+  fill_conv(h, kind, tab.e.conv);
+  tab.e.conv.out_pts = static_cast<float2*>(h->d_pts.p);
+  tab.e.conv.out_n = &h->d_scratch->conv_kept;
+  tab.e.in = static_cast<const float*>(h->d_conv_in.p);
+  tab.e.n_in = n;
+  if (T) {
+    memcpy(tab.T, T, sizeof(tab.T));
+    tab.e.T = reinterpret_cast<const double*>(reinterpret_cast<const char*>(d_tab) + offsetof(decltype(tab), T));
+  }
+  HSB_CUDA(h, cudaMemcpyAsync(h->d_conv_tab.p, &tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+  if ((s = launch_conversion(h, kind, d_tab, 1, st)) != HSB_OK) return s;
+  HSB_CUDA(h, cudaMemcpyAsync(&h->h_pin->conv_kept, tab.e.conv.out_n, sizeof(int), cudaMemcpyDeviceToHost, st));
   HSB_CUDA(h, cudaStreamSynchronize(st));
   const int kept = h->h_pin->conv_kept;
   if (kept > 0) HSB_CUDA(h, cudaMemcpy(out_xy, h->d_pts.p, (size_t)kept * 8, cudaMemcpyDeviceToHost));
@@ -1932,6 +1941,7 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
   const bool inl = !conv && matched && inline_scan_applies(h, n);   // header + scan travel in the match launch
   const float* d_hdr;   // the header on the device: [0..2] hint, [3..5] minDist / minAngle / force
   ScanIn dev;           // the scan on the device
+  const HsbConvScanDev* d_tab = nullptr;   // converted without matching: the conversion's table on the device
   if (!conv) {
     // staging, endpoints: header + points straight into the container the map writer reads
     if (!inl && (s = upload_scan(h, *ss.sink, header, 6, in.in, n, st)) != HSB_OK) return s;
@@ -1939,9 +1949,12 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     dev = {HSB_IN_ENDPOINTS, scan_points(*ss.sink), nullptr, n, n, nullptr};
   } else {
     // staging, converted input (floats): [0..15] header; cloud / projected: [16..39] the laser transform (12 doubles),
-    // [40..] the cloud or the ranges; ranges: [16..] the ranges.  The conversion writes the endpoints into the sink.
+    // [40..] the cloud or the ranges; ranges: [16..] the ranges; without matching, then the stand-alone conversion's
+    // one-entry table.  The conversion writes the endpoints into the sink.
     const size_t kHdr = 16, kTf = in.tf ? 24 : 0, per_pt = in.kind == HSB_IN_CLOUD ? 3 : 1;
-    const size_t bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
+    const size_t in_bytes = (kHdr + kTf + (size_t)n * per_pt) * sizeof(float);
+    const size_t o_tab = (in_bytes + 15) & ~(size_t)15;
+    const size_t bytes = matched ? in_bytes : o_tab + sizeof(HsbConvScanDev);
     if ((s = ensure(h, h->d_fused_in, bytes + 16)) != HSB_OK) return s;
     if ((s = ensure_pinned(h, h->h_stage, h->h_stage_bytes, bytes)) != HSB_OK) return s;
     float* hs = h->h_stage;
@@ -1949,10 +1962,15 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     memcpy(hs, header, sizeof(header));
     if (in.tf) memcpy(hs + kHdr, in.tf, 12 * sizeof(double));
     if (n > 0) memcpy(hs + kHdr + kTf, in.in, (size_t)n * per_pt * sizeof(float));
-    HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
     const float* d_c = static_cast<const float*>(h->d_fused_in.p);
     d_hdr = d_c;
     dev = {in.kind, d_c + kHdr + kTf, nullptr, n, n, in.tf ? reinterpret_cast<const double*>(d_c + kHdr) : nullptr};
+    if (!matched) {
+      const HsbConvScanDev e = {ss.conv, dev.in, dev.tf, n};
+      memcpy(reinterpret_cast<char*>(hs) + o_tab, &e, sizeof(e));
+      d_tab = reinterpret_cast<const HsbConvScanDev*>(reinterpret_cast<const char*>(d_c) + o_tab);
+    }
+    HSB_CUDA(h, cudaMemcpyAsync(h->d_fused_in.p, hs, bytes, cudaMemcpyHostToDevice, st));
   }
   float2* d_pts = reinterpret_cast<float2*>(scan_points(*ss.sink));
   h->stepped = true;
@@ -1988,7 +2006,7 @@ static int slam_step(hsb_handle* h, const float hint[3], const ScanIn& in, const
     HSB_CUDA(h, cudaGetLastError());
   } else {
     // without matching, converted input: the stand-alone conversion kernel, the gate, then the kept count's publication
-    if ((s = launch_conversion(h, in.kind, dev.in, n, dev.tf, ss.conv, st)) != HSB_OK) return s;
+    if ((s = launch_conversion(h, in.kind, d_tab, 1, st)) != HSB_OK) return s;
     hsb::slam_gate_kernel<<<1, 32, 0, st>>>(h->d_gate, d_hdr + 3, d_hdr, d_res->pose, h_res->pose, nullptr, 0);
     hsb::publish_int_kernel<<<1, 32, 0, st>>>(n_dev, kept_dev, poll ? seq_dev : nullptr, seq_value);
     h->launches += 2;
@@ -2254,6 +2272,16 @@ struct MatchQuery {
   int W, max_n;
   float* out_poses;   // Q x 3
   float* out_cov;     // Q x 9 Hessians, or NULL
+  // Raw scans (kind other than HSB_IN_ENDPOINTS): the staged inputs are the sessions' scans of that kind, converted
+  // before the match by one conv_to_points_kernel launch, session k with conv[k] (its member's conversion) and, cloud and
+  // projected, the laser transform tf + 12 k (host), into `scratch` (device, room for every input): a session's
+  // endpoints start at its input offset, and their count replaces its descriptor's n on the device and goes to out_kept
+  // (K, or NULL).
+  HsbInputKind kind = HSB_IN_ENDPOINTS;
+  const HsbConvDev* conv = nullptr;
+  const double* tf = nullptr;
+  float2* scratch = nullptr;
+  int* out_kept = nullptr;
 };
 
 // Every host-buffer pose-query body (hsb_likelihood_batch, hsb_covariance_batch, the group scoring calls and the group
@@ -2270,6 +2298,9 @@ struct MatchQuery {
 // group's call passes `ragged` (its members differ in level count: the match runs each hint over its member's own
 // levels, GRP_MATCH_HET) and `any_mode` (they differ in gather mode: every kernel takes each level's own path,
 // MODE_ANY); otherwise h's gather mode is every session's, and a ragged group's match runs in it.
+// A match from raw scans (match->kind) stages their conversion table and transforms, and converts before it matches
+// (one launch more); a match given out_lh, out_best4 or out_best_index scores its poses at `level` where they lie on the
+// device, as SCORE_LIKELIHOOD / SCORE_BEST would (one or two launches more).
 // The group match's launch at W warps per scan: GRP_MATCH when the members share their level count and gather mode,
 // GRP_MATCH_HET otherwise (het), in the members' one gather mode (MODE_TEX / MODE_LDG) or, when they hold both,
 // MODE_ANY.
@@ -2290,16 +2321,40 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
                 const Sessions& sessions, unsigned long long* best, float* out_lh, float* out_map, float* out_world,
                 float* out_best4, int* out_best_index, const MatchQuery* match = nullptr, bool ragged = false,
                 bool any_mode = false) {
-  // staging: sessions | pose offsets | (level descriptor) | poses | scans, then the results: likelihoods | best4 | best
-  // index, or covariance (map) | covariance (world), or poses | Hessians, each only if asked for
+  // staging: sessions | pose offsets | (level descriptor) | poses | (raw scans: conversion table | laser transforms) |
+  // scans, then the results: likelihoods | best4 | best index, or covariance (map) | covariance (world), or poses |
+  // Hessians (| raw scans: kept counts) (| likelihoods | best4 | best index), each only if asked for
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+  const bool conv = kind == SCORE_MATCH && match->kind != HSB_IN_ENDPOINTS;
+  const bool tf = conv && match->kind != HSB_IN_RANGES;
+  const size_t pt_bytes = !conv ? 8 : match->kind == HSB_IN_CLOUD ? 12 : 4;
   const size_t o_off = (size_t)K * sizeof(HsbScoreSessionDev), o_lv = al(o_off + (size_t)(K + 1) * 4);
   const size_t o_poses = lv ? o_lv : al(o_lv + sizeof(HsbLevelDev));
-  const size_t o_pts = al(o_poses + (size_t)Q * 12), in_end = o_pts + n_pts * 8, o_out = al(in_end);
+  const size_t o_tab = al(o_poses + (size_t)Q * 12);
+  const size_t o_tf = conv ? al(o_tab + (size_t)K * sizeof(HsbConvScanDev)) : o_tab;
+  const size_t o_pts = al(o_tf + (tf ? (size_t)K * 12 * sizeof(double) : 0)), in_end = o_pts + n_pts * pt_bytes;
+  const size_t o_out = al(in_end);
+  // the group match's scoring of its poses: likelihoods, and the best hypothesis when best4 or its index is asked for
+  const bool pick = kind == SCORE_MATCH && (out_best4 || out_best_index);
+  const bool match_score = kind == SCORE_MATCH && (out_lh || pick);
   size_t o_lh = o_out, o_best4 = o_out, o_index = o_out, o_map = o_out, o_world = o_out, o_cov = o_out, out_end = o_out;
+  size_t o_kept = o_out;
   if (kind == SCORE_MATCH) {
     o_cov = o_out + (size_t)Q * 12;
     out_end = o_cov + (match->out_cov ? (size_t)Q * 36 : 0);
+    if (conv) {
+      o_kept = out_end;
+      out_end = o_kept + (size_t)K * 4;
+    }
+    if (match_score) {
+      o_lh = al(out_end);
+      out_end = o_lh + (size_t)Q * 4;
+    }
+    if (pick) {
+      o_best4 = al(out_end);
+      o_index = o_best4 + (size_t)K * 16;
+      out_end = o_index + (size_t)K * 4;
+    }
   } else if (kind == SCORE_COVARIANCE) {
     o_world = o_map + (out_map ? (size_t)Q * 36 : 0);
     out_end = o_world + (out_world ? (size_t)Q * 36 : 0);
@@ -2313,20 +2368,40 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   if ((s = ensure(h, d_stage, out_end)) != HSB_OK) return s;
   char* hs = reinterpret_cast<char*>(hs_buf);
   char* ds = static_cast<char*>(d_stage.p);
-  sessions(reinterpret_cast<HsbScoreSessionDev*>(hs), reinterpret_cast<int*>(hs + o_off),
-           reinterpret_cast<const float2*>(ds + o_pts));
+  // (raw scans: a session's scan is matched where its conversion leaves it)
+  HsbScoreSessionDev* hsess = reinterpret_cast<HsbScoreSessionDev*>(hs);
+  sessions(hsess, reinterpret_cast<int*>(hs + o_off), conv ? match->scratch : reinterpret_cast<const float2*>(ds + o_pts));
   if (!lv) {
     HsbLevelDev L = {};
     fill_level_dev(h, level, L);
     memcpy(hs + o_lv, &L, sizeof(L));
   }
   memcpy(hs + o_poses, poses, (size_t)Q * 12);
+  if (conv) {
+    // session k's conversion: its inputs at the input offset of its slice of the scratch, its n (the input length until
+    // the conversion replaces it by the kept count), its member's descriptor and its laser transform
+    HsbConvScanDev* tab = reinterpret_cast<HsbConvScanDev*>(hs + o_tab);
+    const size_t per_in = match->kind == HSB_IN_CLOUD ? 3 : 1;
+    for (int k = 0; k < K; ++k) {
+      const size_t off = (size_t)(hsess[k].pts - match->scratch);
+      tab[k].conv = match->conv[k];
+      tab[k].conv.out_pts = match->scratch + off;
+      tab[k].conv.out_n = &reinterpret_cast<HsbScoreSessionDev*>(ds)[k].n;
+      tab[k].conv.out_n_host = reinterpret_cast<int*>(ds + o_kept) + k;
+      tab[k].in = reinterpret_cast<const float*>(ds + o_pts) + off * per_in;
+      tab[k].T = tf ? reinterpret_cast<const double*>(ds + o_tf) + 12 * (size_t)k : nullptr;
+      tab[k].n_in = hsess[k].n;
+    }
+    if (tf) memcpy(hs + o_tf, match->tf, (size_t)K * 12 * sizeof(double));
+  }
   // More points than kScoreChunk bytes go straight from the caller's memory: the driver overlaps its host staging of a
   // pageable copy with the transfer, where staging megabytes here first would serialise the two.
-  const bool inline_pts = n_pts * 8 <= kScoreChunk;
-  if (inline_pts && n_pts > 0) memcpy(hs + o_pts, pts, n_pts * 8);
+  const bool inline_pts = n_pts * pt_bytes <= kScoreChunk;
+  if (inline_pts && n_pts > 0) memcpy(hs + o_pts, pts, n_pts * pt_bytes);
   HSB_CUDA(h, cudaMemcpyAsync(ds, hs, inline_pts ? in_end : o_pts, cudaMemcpyHostToDevice, st));
-  if (!inline_pts) HSB_CUDA(h, cudaMemcpyAsync(ds + o_pts, pts, n_pts * 8, cudaMemcpyHostToDevice, st));
+  if (!inline_pts) HSB_CUDA(h, cudaMemcpyAsync(ds + o_pts, pts, n_pts * pt_bytes, cudaMemcpyHostToDevice, st));
+  if (conv && (s = launch_conversion(h, match->kind, reinterpret_cast<const HsbConvScanDev*>(ds + o_tab), K, st)) != HSB_OK)
+    return s;
 
   HsbScoreParams P;
   memset(&P, 0, sizeof(P));
@@ -2362,6 +2437,8 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     HSB_GM_CASE(8);
 #undef HSB_GM_CASE
     if (s != HSB_OK) return s;
+    HSB_CUDA(h, cudaGetLastError());
+    P.poses = M.out_poses;   // (scored below, where the match leaves them)
   } else if (kind == SCORE_COVARIANCE) {
     P.out_map = out_map ? reinterpret_cast<float*>(ds + o_map) : nullptr;
     P.out_world = out_world ? reinterpret_cast<float*>(ds + o_world) : nullptr;
@@ -2370,9 +2447,11 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     else if (tex) hsb::covariance_kernel<hsb::MODE_TEX><<<blocks, 224, 0, st>>>(P);
     else hsb::covariance_kernel<hsb::MODE_LDG><<<blocks, 224, 0, st>>>(P);
     h->launches++;
-  } else {
+  }
+  if (kind == SCORE_LIKELIHOOD || kind == SCORE_BEST || match_score) {
     P.out = reinterpret_cast<float*>(ds + o_lh);
-    if (kind == SCORE_BEST) {
+    const bool best_pick = kind == SCORE_BEST || pick;
+    if (best_pick) {
       P.best = best;
       P.out_best4 = reinterpret_cast<float*>(ds + o_best4);
       P.out_best_index = reinterpret_cast<int*>(ds + o_index);
@@ -2382,7 +2461,7 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     else if (tex) hsb::likelihood_group_kernel<hsb::MODE_TEX><<<blocks, 128, 0, st>>>(P);
     else hsb::likelihood_group_kernel<hsb::MODE_LDG><<<blocks, 128, 0, st>>>(P);
     h->launches++;
-    if (kind == SCORE_BEST) {
+    if (best_pick) {
       HSB_CUDA(h, cudaGetLastError());
       hsb::best_group_finish_kernel<<<(K + 127) / 128, 128, 0, st>>>(P);
       h->launches++;
@@ -2394,6 +2473,10 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
   if (kind == SCORE_MATCH) {
     memcpy(match->out_poses, hs + o_out, (size_t)Q * 12);
     if (match->out_cov) memcpy(match->out_cov, hs + o_cov, (size_t)Q * 36);
+    if (conv && match->out_kept) memcpy(match->out_kept, hs + o_kept, (size_t)K * 4);
+    if (match_score && out_lh) memcpy(out_lh, hs + o_lh, (size_t)Q * 4);
+    if (pick && out_best4) memcpy(out_best4, hs + o_best4, (size_t)K * 16);
+    if (pick && out_best_index) memcpy(out_best_index, hs + o_index, (size_t)K * 4);
   } else if (kind == SCORE_COVARIANCE) {
     if (out_map) memcpy(out_map, hs + o_map, (size_t)Q * 36);
     if (out_world) memcpy(out_world, hs + o_world, (size_t)Q * 36);
@@ -2804,6 +2887,9 @@ struct hsb_group {
   // staging above (every call that fills it returns synchronised); M arg-max accumulators of the best hypothesis,
   // zeroed once (every call re-arms the ones it used)
   unsigned long long* d_best = nullptr;
+  // the group match from raw scans (hsb_group_match_batch_ranges / _cloud / _projected): the converted endpoints, a
+  // session's at its input offset; grown to the largest call's input count, never shrunk
+  DevBuf d_conv_pts;
   // map replication (hsb_group_pack_dirty_device, hsb_group_unpack_dirty_device): M x levels tile descriptors,
   // member-major like d_lv, and the members' replication-overflow counters; two events ordering the caller's stream
   // against the group's
@@ -2863,6 +2949,7 @@ int hsb_group_destroy(hsb_group* g) {
   for (cudaEvent_t e : g->ev_tile)
     if (e) cudaEventDestroy(e);
   if (g->d_ray_stage.p) cudaFree(g->d_ray_stage.p);
+  if (g->d_conv_pts.p) cudaFree(g->d_conv_pts.p);
   if (g->h_ray_stage) cudaFreeHost(g->h_ray_stage);
   if (g->d_res) cudaFree(g->d_res);
   if (g->d_stage.p) cudaFree(g->d_stage.p);
@@ -3498,20 +3585,44 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
 }
 
 // hsb_match_batch in shared-scan mode for K members in one pass: session k's hints [hint_offsets[k], hint_offsets[k+1])
-// each matched over all levels on member members[k]'s maps with the session's one scan (check_scans).  One match-kernel
-// launch (GRP_MATCH: one hint per scan) in the shape hsb_match_batch would take for Q hints, behind the members' queued
-// work, through the group's pinned query staging (score_query: one copy each way and one synchronise, whatever K is).
-// The launch shape is chosen, and a tuning without a group match kernel rejected, before anything is queued.  No
-// member's state changes.
-int group_match(hsb_group* g, const char* fn, int K, const int* members, const int* hint_offsets, const float* hints,
-                const float* pts, const int* scan_offsets, float* out_poses, float* out_cov) {
+// each matched over all levels on member members[k]'s maps with the session's one scan.  One match-kernel launch
+// (GRP_MATCH: one hint per scan) in the shape hsb_match_batch would take for Q hints, behind the members' queued work,
+// through the group's pinned query staging (score_query: one copy each way and one synchronise, whatever K is).
+// Endpoint input (HSB_IN_ENDPOINTS): the scan by check_scans' rule.  Raw input (ranges, cloud, projected): session k's
+// scan is in[scan_offsets[k] .. scan_offsets[k+1]) (cloud: Point32 triples), converted first by its member's formats
+// with laser transform transforms + 12 k (NULL: the member's cloud format's), all sessions in one conversion launch,
+// into the group's endpoint scratch; out_kept (K, or NULL) gets each conversion's kept count.  out_lh (Q), out_best4
+// (K x 4) and out_best_index (K), each may be NULL: the matched poses scored at level 0 against the session's scan, and
+// each session's best hypothesis (a launch for the likelihoods, one more for the pick).  The launch shape is chosen,
+// and a tuning without a group match kernel rejected, before anything is queued.  No member's state changes.
+int group_match(hsb_group* g, const char* fn, HsbInputKind kind, int K, const int* members, const int* hint_offsets,
+                const float* hints, const float* in, const int* scan_offsets, const double* transforms, float* out_poses,
+                float* out_cov, float* out_lh, float* out_best4, int* out_best_index, int* out_kept) {
   hsb_handle* h0 = g->m[0];   // launches, launch shape and errors are accounted on handles[0], whether or not it is listed
   int s = check_members(g, fn, K, members);
   if (s != HSB_OK || K == 0) return s;
   if ((s = check_offsets(h0, fn, "hint_offsets", K, hint_offsets)) != HSB_OK) return s;
-  if ((s = check_scans(h0, fn, K, pts, scan_offsets)) != HSB_OK) return s;
+  const bool raw = kind != HSB_IN_ENDPOINTS;
+  if (!raw && (s = check_scans(h0, fn, K, in, scan_offsets)) != HSB_OK) return s;
+  if (raw) {
+    if ((s = check_offsets(h0, fn, "scan_offsets", K, scan_offsets)) != HSB_OK) return s;
+    if (scan_offsets[K] > 0 && !in)
+      return fail(h0, HSB_ERR_INVALID_ARG, "%s: %s is NULL", fn, kind == HSB_IN_CLOUD ? "points_xyz" : "ranges");
+    for (int k = 0; k < K; ++k)
+      if ((s = check_input(g->m[members[k]], h0, kind, fn, k, scan_offsets[k + 1] - scan_offsets[k], false)) != HSB_OK)
+        return s;
+  }
   const int Q = hint_offsets[K];
-  if (Q == 0) return HSB_OK;
+  if (Q == 0) {   // nothing to match: every session's best hypothesis is the empty batch's
+    for (int k = 0; k < K; ++k) {
+      if (out_best4) {
+        out_best4[4 * k] = -1.0f;
+        out_best4[4 * k + 1] = out_best4[4 * k + 2] = out_best4[4 * k + 3] = 0.0f;
+      }
+      if (out_best_index) out_best_index[k] = -1;
+    }
+    return HSB_OK;
+  }
   if (!hints) return fail(h0, HSB_ERR_INVALID_ARG, "%s: hints_world is NULL", fn);
   if (!out_poses) return fail(h0, HSB_ERR_INVALID_ARG, "%s: out_poses_world is NULL", fn);
   // the launch shape: hsb_match_batch's for Q hints (launch_match), among the shapes the group match is compiled for —
@@ -3524,17 +3635,38 @@ int group_match(hsb_group* g, const char* fn, int K, const int* members, const i
     return fail(h0, HSB_ERR_UNSUPPORTED, "%s: no group match kernel for tuning warps_per_scan=%d scans_per_block=%d "
                 "unroll=%d packed=%d", fn, W, G, U, h0->tune_packed);
   MatchQuery mq = {W, 0, out_poses, out_cov};
-  // (only a session with hints launches work: an unused long scan must not shrink the staging of the others)
+  // (only a session with hints launches work: an unused long scan must not shrink the staging of the others; a raw
+  // scan's input length bounds its kept endpoints)
   for (int k = 0; k < K; ++k)
     if (hint_offsets[k + 1] > hint_offsets[k])
       mq.max_n = std::max(mq.max_n, scan_length(g->m[members[k]], scan_offsets, k));
+  const size_t n_in = in ? (size_t)scan_offsets[K] : 0;
+  std::vector<HsbConvDev> conv;
+  std::vector<double> tf;
   DeviceGuard guard(g->device);
+  if (raw) {
+    // the members' conversions as they are at the call, and the endpoint scratch: room for every input
+    if ((s = ensure(h0, g->d_conv_pts, std::max<size_t>(n_in, 1) * 8)) != HSB_OK) return s;
+    conv.resize(K);
+    if (kind != HSB_IN_RANGES) tf.resize((size_t)K * 12);
+    for (int k = 0; k < K; ++k) {
+      const hsb_handle* h = g->m[members[k]];
+      fill_conv(h, kind, conv[k]);
+      if (kind != HSB_IN_RANGES)
+        memcpy(tf.data() + 12 * (size_t)k, transforms ? transforms + 12 * (size_t)k : h->cfmt.laser_transform,
+               12 * sizeof(double));
+    }
+    mq.kind = kind;
+    mq.conv = conv.data();
+    mq.tf = tf.empty() ? nullptr : tf.data();
+    mq.scratch = static_cast<float2*>(g->d_conv_pts.p);
+    mq.out_kept = out_kept;
+  }
   if ((s = order_members(g, K, members)) != HSB_OK) return s;
-  // (the match reads no cell length: the sessions carry level 0's)
+  // (the match reads no cell length: the sessions carry level 0's, which the scoring takes)
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, 0,
-                     SCORE_MATCH, K, Q, hints, pts, pts ? (size_t)scan_offsets[K] : 0,
-                     group_sessions(g, K, members, 0, hint_offsets, scan_offsets), nullptr, nullptr, nullptr, nullptr,
-                     nullptr, nullptr, &mq, g->ragged, g->any_mode);
+                     SCORE_MATCH, K, Q, hints, in, n_in, group_sessions(g, K, members, 0, hint_offsets, scan_offsets),
+                     g->d_best, out_lh, nullptr, nullptr, out_best4, out_best_index, &mq, g->ragged, g->any_mode);
 }
 
 }  // namespace
@@ -3590,16 +3722,76 @@ int hsb_group_best_hypothesis_subset(hsb_group* g, int K, const int* members, in
 int hsb_group_match_batch(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* points_xy,
                           const int* scan_offsets, float* out_poses_world, float* out_cov) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  return group_match(g, "hsb_group_match_batch", (int)g->m.size(), g->all.data(), hint_offsets, hints_world, points_xy,
-                     scan_offsets, out_poses_world, out_cov);
+  return group_match(g, "hsb_group_match_batch", HSB_IN_ENDPOINTS, (int)g->m.size(), g->all.data(), hint_offsets,
+                     hints_world, points_xy, scan_offsets, nullptr, out_poses_world, out_cov, nullptr, nullptr, nullptr,
+                     nullptr);
 }
 
 int hsb_group_match_batch_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
                                  const float* hints_world, const float* points_xy, const int* scan_offsets,
                                  float* out_poses_world, float* out_cov) {
   if (!g) return HSB_ERR_INVALID_ARG;
-  return group_match(g, "hsb_group_match_batch_subset", K, members, hint_offsets, hints_world, points_xy, scan_offsets,
-                     out_poses_world, out_cov);
+  return group_match(g, "hsb_group_match_batch_subset", HSB_IN_ENDPOINTS, K, members, hint_offsets, hints_world,
+                     points_xy, scan_offsets, nullptr, out_poses_world, out_cov, nullptr, nullptr, nullptr, nullptr);
+}
+
+int hsb_group_match_batch_ranges(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* ranges,
+                                 const int* scan_offsets, float* out_poses_world, float* out_cov, float* out_likelihood,
+                                 float* out_best4, int* out_best_index, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_ranges", HSB_IN_RANGES, (int)g->m.size(), g->all.data(), hint_offsets,
+                     hints_world, ranges, scan_offsets, nullptr, out_poses_world, out_cov, out_likelihood, out_best4,
+                     out_best_index, out_kept);
+}
+
+int hsb_group_match_batch_cloud(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* points_xyz,
+                                const int* scan_offsets, const double* transforms, float* out_poses_world, float* out_cov,
+                                float* out_likelihood, float* out_best4, int* out_best_index, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_cloud", HSB_IN_CLOUD, (int)g->m.size(), g->all.data(), hint_offsets,
+                     hints_world, points_xyz, scan_offsets, transforms, out_poses_world, out_cov, out_likelihood,
+                     out_best4, out_best_index, out_kept);
+}
+
+int hsb_group_match_batch_projected(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* ranges,
+                                    const int* scan_offsets, const double* transforms, float* out_poses_world,
+                                    float* out_cov, float* out_likelihood, float* out_best4, int* out_best_index,
+                                    int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_projected", HSB_IN_PROJECTED, (int)g->m.size(), g->all.data(),
+                     hint_offsets, hints_world, ranges, scan_offsets, transforms, out_poses_world, out_cov,
+                     out_likelihood, out_best4, out_best_index, out_kept);
+}
+
+int hsb_group_match_batch_ranges_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                        const float* hints_world, const float* ranges, const int* scan_offsets,
+                                        float* out_poses_world, float* out_cov, float* out_likelihood, float* out_best4,
+                                        int* out_best_index, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_ranges_subset", HSB_IN_RANGES, K, members, hint_offsets, hints_world,
+                     ranges, scan_offsets, nullptr, out_poses_world, out_cov, out_likelihood, out_best4,
+                     out_best_index, out_kept);
+}
+
+int hsb_group_match_batch_cloud_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                       const float* hints_world, const float* points_xyz, const int* scan_offsets,
+                                       const double* transforms, float* out_poses_world, float* out_cov,
+                                       float* out_likelihood, float* out_best4, int* out_best_index, int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_cloud_subset", HSB_IN_CLOUD, K, members, hint_offsets, hints_world,
+                     points_xyz, scan_offsets, transforms, out_poses_world, out_cov, out_likelihood, out_best4,
+                     out_best_index, out_kept);
+}
+
+int hsb_group_match_batch_projected_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                           const float* hints_world, const float* ranges, const int* scan_offsets,
+                                           const double* transforms, float* out_poses_world, float* out_cov,
+                                           float* out_likelihood, float* out_best4, int* out_best_index,
+                                           int* out_kept) {
+  if (!g) return HSB_ERR_INVALID_ARG;
+  return group_match(g, "hsb_group_match_batch_projected_subset", HSB_IN_PROJECTED, K, members, hint_offsets,
+                     hints_world, ranges, scan_offsets, transforms, out_poses_world, out_cov, out_likelihood,
+                     out_best4, out_best_index, out_kept);
 }
 
 int hsb_group_raycast(hsb_group* g, int level, const int* offsets, const int* begin_cells, const int* end_cells,

@@ -41,11 +41,21 @@ struct HsbConvDev {
   float sqr_min_dist, sqr_max_dist, z_min, z_max;
   float scale_to_map;
   // the sink (SLAM steps and the stand-alone conversion; null for batch matches): the compacted endpoints go to
-  // out_pts, their number to device memory (out_n, the map writer's n_dev) and, if set, to mapped host memory
-  // (out_n_host, written before the step's sequence number is published)
+  // out_pts, their number to device memory (out_n, the map writer's n_dev) and, if set, to a second place (out_n_host:
+  // a step's mapped host memory, written before the step's sequence number is published; a group match's result block)
   float2* out_pts;
   int* out_n;
   int* out_n_host;
+};
+
+// One scan of a stand-alone conversion (conv_to_points_kernel, one CTA per entry): n_in inputs of the launch's kind at
+// `in` (ranges: one float per beam; cloud: Point32 triples), laser transform T (cloud and projected: 12 doubles, rows
+// of [R | t]), converted by conv into conv's sink.
+struct HsbConvScanDev {
+  HsbConvDev conv;
+  const float* in;
+  const double* T;
+  int n_in;
 };
 
 // One session of a group SLAM step (hsb_group_slam_update / _cloud / _ranges / _projected and their _subset forms): the

@@ -1211,28 +1211,33 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
   if (pace && t == 0) prog[g] = 0x7fffffff;   // this group is done: nobody waits for it any more
 }
 
-// The conversion alone (one scan of n_in ranges or cloud points, laser transform T; one CTA of 8 warps) into C's sink:
-// the stand-alone conversion calls and the SLAM steps without matching.
+// The conversion alone, one CTA of 8 warps per scan of the table (table[blockIdx.x]: its input, length, laser transform
+// and descriptor) into each scan's sink: the stand-alone conversion calls (a table of one) and the group batch match
+// from raw scans (one entry per session).  Each scan's kept count goes to its out_n and, if set, out_n_host.
 template <int KIND>
-__global__ void __launch_bounds__(256)
-    conv_to_points_kernel(const float* __restrict__ in, int n_in, const double* __restrict__ T, const HsbConvDev C) {
+__global__ void __launch_bounds__(256) conv_to_points_kernel(const HsbConvScanDev* __restrict__ table) {
   __shared__ int warp_cnt[32];
+  const HsbConvScanDev& S = table[blockIdx.x];
+  const HsbConvDev& C = S.conv;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int n;
   if constexpr (KIND == HSB_IN_RANGES) {
-    n = stage_from_ranges<8>(in, C.beam_cs, n_in, C.range_min, C.range_max_c, C.scale_to_map, C.out_pts, warp_cnt, 0, w,
-                             lane);
+    n = stage_from_ranges<8>(S.in, C.beam_cs, S.n_in, C.range_min, C.range_max_c, C.scale_to_map, C.out_pts, warp_cnt, 0,
+                             w, lane);
   } else if constexpr (KIND == HSB_IN_CLOUD) {
-    n = stage_from_cloud<8>(in, n_in, T, C.sqr_min_dist, C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map, C.out_pts,
-                            warp_cnt, 0, w, lane);
+    n = stage_from_cloud<8>(S.in, S.n_in, S.T, C.sqr_min_dist, C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map,
+                            C.out_pts, warp_cnt, 0, w, lane);
   } else {
     double Tr[12];   // the transform read once (left to ptxas, the per-point reloads spill at its 32-register choice)
 #pragma unroll
-    for (int k = 0; k < 12; ++k) Tr[k] = T[k];
-    n = stage_from_projected<8>(in, C.proj_unit, n_in, C.range_min, C.range_cutoff, Tr, C.sqr_min_dist, C.sqr_max_dist,
-                                C.z_min, C.z_max, C.scale_to_map, C.out_pts, warp_cnt, 0, w, lane);
+    for (int k = 0; k < 12; ++k) Tr[k] = S.T[k];
+    n = stage_from_projected<8>(S.in, C.proj_unit, S.n_in, C.range_min, C.range_cutoff, Tr, C.sqr_min_dist,
+                                C.sqr_max_dist, C.z_min, C.z_max, C.scale_to_map, C.out_pts, warp_cnt, 0, w, lane);
   }
-  if (threadIdx.x == 0) *C.out_n = n;
+  if (threadIdx.x == 0) {
+    *C.out_n = n;
+    if (C.out_n_host) *C.out_n_host = n;
+  }
 }
 
 // N3: OccGridMapUtil::getLikelihoodForState (OccGridMapUtil.h:189-221) for one state (map coordinates of the level),

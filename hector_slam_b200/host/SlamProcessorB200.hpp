@@ -463,6 +463,68 @@ class SlamProcessor {
     owner.check(hsb_group_match_batch_subset(owner.groupFor(ps, M), K, members, hintOffsets, hintsWorld, pointsXY,
                                              scanOffsets, posesWorld, cov));
   }
+
+  // matchMany() from each processor's new LaserScan ranges[scanOffsets[s] .. scanOffsets[s+1]), converted on the device
+  // with its scan format, followed by the pick (hsb_group_match_batch_ranges): relocalising lost robots from the scans
+  // they just sent, before anything writes them into a map.  likelihood (one per hint), best4 ({likelihood, x, y, psi}
+  // per processor), bestIndex (per processor) and kept (endpoints each conversion kept, per processor) may be null; the
+  // scoring runs only when one of the first three is given.  No processor's state changes.
+  static void matchManyRanges(SlamProcessor* const* ps, int M, const int* hintOffsets, const float* hintsWorld,
+                              const float* ranges, const int* scanOffsets, float* posesWorld, float* cov = 0,
+                              float* likelihood = 0, float* best4 = 0, int* bestIndex = 0, int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyRanges");
+    owner.check(hsb_group_match_batch_ranges(owner.groupFor(ps, M), hintOffsets, hintsWorld, ranges, scanOffsets,
+                                             posesWorld, cov, likelihood, best4, bestIndex, kept));
+  }
+  // matchManyRanges() for the processors ps[members[0..K)] (hsb_group_match_batch_ranges_subset).
+  static void matchManyRanges(SlamProcessor* const* ps, int M, const int* members, int K, const int* hintOffsets,
+                              const float* hintsWorld, const float* ranges, const int* scanOffsets, float* posesWorld,
+                              float* cov = 0, float* likelihood = 0, float* best4 = 0, int* bestIndex = 0,
+                              int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyRanges");
+    owner.check(hsb_group_match_batch_ranges_subset(owner.groupFor(ps, M), K, members, hintOffsets, hintsWorld, ranges,
+                                                    scanOffsets, posesWorld, cov, likelihood, best4, bestIndex, kept));
+  }
+  // matchManyRanges() from Point32 clouds in the laser frame, pointsXYZ[scanOffsets[s] .. scanOffsets[s+1]) with laser
+  // transforms (12 doubles per processor, null: each processor's cloud format), each converted with its cloud format
+  // (hsb_group_match_batch_cloud).
+  static void matchManyCloud(SlamProcessor* const* ps, int M, const int* hintOffsets, const float* hintsWorld,
+                             const float* pointsXYZ, const int* scanOffsets, const double* transforms, float* posesWorld,
+                             float* cov = 0, float* likelihood = 0, float* best4 = 0, int* bestIndex = 0, int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyCloud");
+    owner.check(hsb_group_match_batch_cloud(owner.groupFor(ps, M), hintOffsets, hintsWorld, pointsXYZ, scanOffsets,
+                                            transforms, posesWorld, cov, likelihood, best4, bestIndex, kept));
+  }
+  // matchManyCloud() for the processors ps[members[0..K)] (hsb_group_match_batch_cloud_subset).
+  static void matchManyCloud(SlamProcessor* const* ps, int M, const int* members, int K, const int* hintOffsets,
+                             const float* hintsWorld, const float* pointsXYZ, const int* scanOffsets,
+                             const double* transforms, float* posesWorld, float* cov = 0, float* likelihood = 0,
+                             float* best4 = 0, int* bestIndex = 0, int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyCloud");
+    owner.check(hsb_group_match_batch_cloud_subset(owner.groupFor(ps, M), K, members, hintOffsets, hintsWorld, pointsXYZ,
+                                                   scanOffsets, transforms, posesWorld, cov, likelihood, best4,
+                                                   bestIndex, kept));
+  }
+  // matchManyRanges() from the LaserScans of default-configured nodes: each processor projects its ranges with its laser
+  // projection and converts them with its cloud format; transforms as in matchManyCloud (hsb_group_match_batch_projected).
+  static void matchManyProjected(SlamProcessor* const* ps, int M, const int* hintOffsets, const float* hintsWorld,
+                                 const float* ranges, const int* scanOffsets, const double* transforms,
+                                 float* posesWorld, float* cov = 0, float* likelihood = 0, float* best4 = 0,
+                                 int* bestIndex = 0, int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyProjected");
+    owner.check(hsb_group_match_batch_projected(owner.groupFor(ps, M), hintOffsets, hintsWorld, ranges, scanOffsets,
+                                                transforms, posesWorld, cov, likelihood, best4, bestIndex, kept));
+  }
+  // matchManyProjected() for the processors ps[members[0..K)] (hsb_group_match_batch_projected_subset).
+  static void matchManyProjected(SlamProcessor* const* ps, int M, const int* members, int K, const int* hintOffsets,
+                                 const float* hintsWorld, const float* ranges, const int* scanOffsets,
+                                 const double* transforms, float* posesWorld, float* cov = 0, float* likelihood = 0,
+                                 float* best4 = 0, int* bestIndex = 0, int* kept = 0) {
+    SlamProcessor& owner = groupOwnerOf(ps, M, "matchManyProjected");
+    owner.check(hsb_group_match_batch_projected_subset(owner.groupFor(ps, M), K, members, hintOffsets, hintsWorld,
+                                                       ranges, scanOffsets, transforms, posesWorld, cov, likelihood,
+                                                       best4, bestIndex, kept));
+  }
   hsb_handle* handle() { return h_; }
 
   // util::poseDifferenceLargerThan, util/UtilFunctions.h:73-92 (float norm, double pi arithmetic)

@@ -394,6 +394,39 @@ int hsbp_match_many_subset(void* const* ps, int M, const int* members, int K, co
   }
   return 0;
 }
+// matchManyRanges / matchManyCloud / matchManyProjected (kind 0 / 1 / 2), over ps[members[0..K)] or, with members
+// NULL, all M processors; `in` is the ranges or the Point32 triples, transforms is ignored for ranges
+int hsbp_match_many_scans(void* const* ps, int M, int kind, const int* members, int K, const int* hint_offsets,
+                          const float* hints_world, const float* in, const int* scan_offsets, const double* transforms,
+                          float* out_poses_world, float* out_cov, float* likelihood, float* best4, int* best_index,
+                          int* kept) {
+  std::vector<hsb200::SlamProcessor*> procs(M > 0 ? M : 0);
+  for (int s = 0; s < M; ++s) procs[s] = static_cast<hsb200::SlamProcessor*>(ps[s]);
+  using P = hsb200::SlamProcessor;
+  try {
+    if (kind == 0 && !members)
+      P::matchManyRanges(procs.data(), M, hint_offsets, hints_world, in, scan_offsets, out_poses_world, out_cov,
+                         likelihood, best4, best_index, kept);
+    else if (kind == 0)
+      P::matchManyRanges(procs.data(), M, members, K, hint_offsets, hints_world, in, scan_offsets, out_poses_world,
+                         out_cov, likelihood, best4, best_index, kept);
+    else if (kind == 1 && !members)
+      P::matchManyCloud(procs.data(), M, hint_offsets, hints_world, in, scan_offsets, transforms, out_poses_world,
+                        out_cov, likelihood, best4, best_index, kept);
+    else if (kind == 1)
+      P::matchManyCloud(procs.data(), M, members, K, hint_offsets, hints_world, in, scan_offsets, transforms,
+                        out_poses_world, out_cov, likelihood, best4, best_index, kept);
+    else if (!members)
+      P::matchManyProjected(procs.data(), M, hint_offsets, hints_world, in, scan_offsets, transforms, out_poses_world,
+                            out_cov, likelihood, best4, best_index, kept);
+    else
+      P::matchManyProjected(procs.data(), M, members, K, hint_offsets, hints_world, in, scan_offsets, transforms,
+                            out_poses_world, out_cov, likelihood, best4, best_index, kept);
+  } catch (const std::exception&) {
+    return -1;
+  }
+  return 0;
+}
 int hsbp_get_pose_and_cov(void* p, float out_pose[3], float out_cov[9]) {
   hsb200::SlamProcessor* s = static_cast<hsb200::SlamProcessor*>(p);
   const hsb200::Pose& q = s->getLastScanMatchPose();

@@ -689,6 +689,63 @@ int hsb_group_match_batch(hsb_group* g, const int* hint_offsets, const float* hi
 int hsb_group_match_batch_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
                                  const float* hints_world, const float* points_xy, const int* scan_offsets,
                                  float* out_poses_world, float* out_cov);
+/* hsb_group_match_batch from each session's new raw scan, with the pick: the relocalisation round of a lost robot from
+ * what a node receives (LaserScan ranges, a Point32 cloud, or LaserScan ranges the default node projects), in one pass.
+ * Sessions and hints are hsb_group_match_batch's.  Session k's ONE scan is [scan_offsets[k], scan_offsets[k+1]) of
+ * `ranges` (one float per beam: _ranges, _projected) or of `points_xyz` (Point32 triples: _cloud); transforms holds 12
+ * doubles per session, rows of [R | t] (NULL: each member's hsb_set_cloud_format transform, as in the group steps).
+ * The scan is converted once with its member's scan format, cloud format or laser projection as they are at the call
+ * (members may differ in all of these, and in map geometry and pyramid), then each hint runs the full coarse-to-fine
+ * matchData with it on the member's own levels.
+ * Outputs: out_poses_world Q x 3, out_cov Q x 9 (may be NULL) and out_likelihood Q, in hint order; out_kept K: the
+ * endpoints each conversion kept (may be NULL).  Scoring runs only when asked for: out_likelihood scores every matched
+ * pose at level 0 against the session's converted scan; out_best4 K x 4 {likelihood, x, y, psi} and out_best_index K
+ * pick each session's winner by hsb_group_best_hypothesis's rule (any of the three may be NULL; all NULL: no scoring
+ * launch).
+ * Bits: out_kept[k] equals hsb_scan_to_points / hsb_cloud_to_points / hsb_projected_scan_to_points on member members[k]
+ * with the same input and transform; every pose and Hessian equals hsb_group_match_batch(_subset) on the same hints with
+ * points_xy set to those endpoints, in the same launch shape (W from Q and handles[0]'s tuning, reported by
+ * hsb_get_last_launch_shape(handles[0])); every likelihood, best4 and index equals hsb_group_best_hypothesis(_subset) at
+ * level 0 on the returned poses with those endpoints (NaN likelihoods and non-finite poses score -1; an empty session
+ * gives {-1, 0, 0, 0} and index -1; an all-dropped scan returns its hints and all-zero Hessians).
+ * No member's state changes: planes, texture twin, stamps, dirty rectangles and gate pose stay, and the new scan does
+ * not replace the last-match container.  A member not listed is neither read nor waited for.  Ordering is
+ * hsb_group_match_batch's.
+ * Cost, whatever K is: one host-to-device copy from the group's pinned query staging of the sessions' descriptors,
+ * offsets, hints, conversion table, transforms and raw scans (scans past the staging chunk: a second copy straight from
+ * the caller's memory); one conversion launch (one CTA of 8 warps per session, into a group-owned device scratch of
+ * one endpoint slot per input), one match launch, and one (likelihood) or two (best hypothesis) scoring launches on the
+ * matched poses where they lie on the device, all counted on handles[0]; one device-to-host copy of one result block;
+ * one synchronise.  No endpoint crosses the bus.
+ * Rejected before anything is queued, no output byte written: every rejection of hsb_group_match_batch(_subset)
+ * (HSB_ERR_UNSUPPORTED tuning rule included); scan_offsets NULL, not starting at 0 or decreasing; a NULL ranges /
+ * points_xyz with scan_offsets[K] > 0; a listed member without the format its kind needs (the message names the
+ * session); ranges / projected scan offsets that disagree with a member's n_beams.  K = 0 returns HSB_OK and reads no
+ * other argument; Q = 0 returns HSB_OK and queues nothing (out_best4 / out_best_index get the empty session's values
+ * if given, out_kept is not written).  No scan-length limit beyond the group match's. */
+int hsb_group_match_batch_ranges(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* ranges,
+                                 const int* scan_offsets, float* out_poses_world, float* out_cov, float* out_likelihood,
+                                 float* out_best4, int* out_best_index, int* out_kept);
+int hsb_group_match_batch_cloud(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* points_xyz,
+                                const int* scan_offsets, const double* transforms, float* out_poses_world, float* out_cov,
+                                float* out_likelihood, float* out_best4, int* out_best_index, int* out_kept);
+int hsb_group_match_batch_projected(hsb_group* g, const int* hint_offsets, const float* hints_world, const float* ranges,
+                                    const int* scan_offsets, const double* transforms, float* out_poses_world,
+                                    float* out_cov, float* out_likelihood, float* out_best4, int* out_best_index,
+                                    int* out_kept);
+int hsb_group_match_batch_ranges_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                        const float* hints_world, const float* ranges, const int* scan_offsets,
+                                        float* out_poses_world, float* out_cov, float* out_likelihood, float* out_best4,
+                                        int* out_best_index, int* out_kept);
+int hsb_group_match_batch_cloud_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                       const float* hints_world, const float* points_xyz, const int* scan_offsets,
+                                       const double* transforms, float* out_poses_world, float* out_cov,
+                                       float* out_likelihood, float* out_best4, int* out_best_index, int* out_kept);
+int hsb_group_match_batch_projected_subset(hsb_group* g, int K, const int* members, const int* hint_offsets,
+                                           const float* hints_world, const float* ranges, const int* scan_offsets,
+                                           const double* transforms, float* out_poses_world, float* out_cov,
+                                           float* out_likelihood, float* out_best4, int* out_best_index,
+                                           int* out_kept);
 /* lastMapUpdatePose of the fused step (HectorSlamProcessor.h:151) */
 int hsb_get_last_map_update_pose(hsb_handle* h, float out[3]);
 /* ... and its setter, for a host that wrote the map itself (hsb_update_by_scan) between fused steps: the gate of the
