@@ -2294,33 +2294,27 @@ struct MatchQuery {
 // (points past kScoreChunk bytes: a second one from `pts`), one launch on `st` (two for the best hypothesis, whose K
 // arg-max accumulators are `best`; the match's in match->W), one device-to-host copy of the asked-for results and one
 // synchronise.  The launches, the match's launch shape and any error are counted on h.  sessions() also gives each
-// session its member's cell length of `level` (the covariance's world matrix) and its level count.  A heterogeneous
-// group's call passes `ragged` (its members differ in level count: the match runs each hint over its member's own
-// levels, GRP_MATCH_HET) and `any_mode` (they differ in gather mode: every kernel takes each level's own path,
-// MODE_ANY); otherwise h's gather mode is every session's, and a ragged group's match runs in it.
+// session its member's cell length of `level` (the covariance's world matrix) and its level count, over which the match
+// runs each hint.  A heterogeneous group whose members differ in gather mode passes `any_mode` (every kernel takes each
+// level's own path, MODE_ANY); otherwise h's gather mode is every session's.
 // A match from raw scans (match->kind) stages their conversion table and transforms, and converts before it matches
 // (one launch more); a match given out_lh, out_best4 or out_best_index scores its poses at `level` where they lie on the
 // device, as SCORE_LIKELIHOOD / SCORE_BEST would (one or two launches more).
-// The group match's launch at W warps per scan: GRP_MATCH when the members share their level count and gather mode,
-// GRP_MATCH_HET otherwise (het), in the members' one gather mode (MODE_TEX / MODE_LDG) or, when they hold both,
-// MODE_ANY.
+// The group match's launch at W warps per scan, in the members' one gather mode (MODE_TEX / MODE_LDG) or, when they
+// hold both, MODE_ANY.
 template <int W>
-int launch_group_match(hsb_handle* h, HsbMatchParams& M, int max_n, cudaStream_t st, bool het, int mode) {
-  if (!het)
-    return mode == hsb::MODE_TEX ? launch_match_t<W, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1)
-                                 : launch_match_t<W, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1);
+int launch_group_match(hsb_handle* h, HsbMatchParams& M, int max_n, cudaStream_t st, int mode) {
   if (mode == hsb::MODE_ANY)
-    return launch_match_t<W, 1, hsb::MODE_ANY, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1);
-  return mode == hsb::MODE_TEX ? launch_match_t<W, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1)
-                               : launch_match_t<W, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH_HET>(h, M, max_n, st, 1);
+    return launch_match_t<W, 1, hsb::MODE_ANY, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1);
+  return mode == hsb::MODE_TEX ? launch_match_t<W, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1)
+                               : launch_match_t<W, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_MATCH>(h, M, max_n, st, 1);
 }
 
 template <typename Sessions>
 int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes, DevBuf& d_stage, const HsbLevelDev* lv,
                 int levels, int level, ScoreKind kind, int K, int Q, const float* poses, const float* pts, size_t n_pts,
                 const Sessions& sessions, unsigned long long* best, float* out_lh, float* out_map, float* out_world,
-                float* out_best4, int* out_best_index, const MatchQuery* match = nullptr, bool ragged = false,
-                bool any_mode = false) {
+                float* out_best4, int* out_best_index, const MatchQuery* match = nullptr, bool any_mode = false) {
   // staging: sessions | pose offsets | (level descriptor) | poses | (raw scans: conversion table | laser transforms) |
   // scans, then the results: likelihoods | best4 | best index, or covariance (map) | covariance (world), or poses |
   // Hessians (| raw scans: kept counts) (| likelihoods | best4 | best index), each only if asked for
@@ -2430,7 +2424,7 @@ int score_query(hsb_handle* h, cudaStream_t st, float*& hs_buf, size_t& hs_bytes
     s = HSB_ERR_UNSUPPORTED;
     const int mode = any_mode ? hsb::MODE_ANY : tex ? hsb::MODE_TEX : hsb::MODE_LDG;
 #define HSB_GM_CASE(w) \
-  if (match->W == w) s = launch_group_match<w>(h, M, match->max_n, st, ragged || any_mode, mode);
+  if (match->W == w) s = launch_group_match<w>(h, M, match->max_n, st, mode);
     HSB_GM_CASE(1);
     HSB_GM_CASE(2);
     HSB_GM_CASE(4);
@@ -2846,12 +2840,12 @@ struct hsb_group {
   std::vector<unsigned char> listed;   // scratch of a step's member-list check, M flags
   int device = 0;
   // the largest level count of the members (the stride of every member-major table); every member's but in a
-  // heterogeneous group, whose members may each have their own (ragged) and their own gather mode (any_mode: both
-  // occur, so the kernels take the gather path from each level descriptor, MODE_ANY).  Both stay false in groups of
-  // the other two constructors, which require the members to agree.
+  // heterogeneous group, whose members may each have their own, and their own gather mode (any_mode: both occur, so the
+  // kernels take the gather path from each level descriptor, MODE_ANY).  any_mode stays false in groups of the other
+  // two constructors, which require the members to agree.
   int levels = 0;
-  bool ragged = false, any_mode = false;
-  int* d_member_levels = nullptr;  // ragged: the members' level counts (the *_ragged tile and reset kernels)
+  bool any_mode = false;
+  int* d_member_levels = nullptr;  // the members' level counts, M ints (the group tile and reset kernels)
   cudaStream_t stream = nullptr;   // every step of the group runs here
   cudaEvent_t ev = nullptr;        // recorded behind every step; members wait on it lazily (HandleScope)
   // M x levels match-kernel level descriptors, member-major (a handle's planes never move); a session reads its
@@ -3027,7 +3021,6 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, GroupKind k
   g->levels = h0->levels;
   for (int s = 1; s < M; ++s) {
     g->levels = std::max(g->levels, handles[s]->levels);
-    g->ragged |= handles[s]->levels != h0->levels;
     g->any_mode |= handles[s]->gather_mode != h0->gather_mode;
   }
 #define HSB_GROUP_CUDA(expr)                                                                                 \
@@ -3081,12 +3074,10 @@ int group_create(hsb_handle* const* handles, int M, hsb_group** out, GroupKind k
     }
     HSB_GROUP_CUDA(cudaMalloc(&g->d_reset, reset.size() * sizeof(HsbResetMemberDev)));
     HSB_GROUP_CUDA(cudaMemcpy(g->d_reset, reset.data(), reset.size() * sizeof(HsbResetMemberDev), cudaMemcpyHostToDevice));
-    if (g->ragged) {
-      std::vector<int> nl(M);
-      for (int s = 0; s < M; ++s) nl[s] = g->m[s]->levels;
-      HSB_GROUP_CUDA(cudaMalloc(&g->d_member_levels, nl.size() * sizeof(int)));
-      HSB_GROUP_CUDA(cudaMemcpy(g->d_member_levels, nl.data(), nl.size() * sizeof(int), cudaMemcpyHostToDevice));
-    }
+    std::vector<int> nl(M);
+    for (int s = 0; s < M; ++s) nl[s] = g->m[s]->levels;
+    HSB_GROUP_CUDA(cudaMalloc(&g->d_member_levels, nl.size() * sizeof(int)));
+    HSB_GROUP_CUDA(cudaMemcpy(g->d_member_levels, nl.data(), nl.size() * sizeof(int), cudaMemcpyHostToDevice));
     for (cudaEvent_t& e : g->ev_tile) HSB_GROUP_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     HSB_GROUP_CUDA(cudaMalloc(&g->d_occ_meta, OccMeta(M).bytes));
     HSB_GROUP_CUDA(cudaMallocHost(reinterpret_cast<void**>(&g->h_occ_meta), OccMeta(M).bytes));
@@ -3138,16 +3129,15 @@ struct GroupInput {
 // warps per session of the group match kernel: the shape the single SLAM steps take, so results are theirs bit for bit
 constexpr int kGroupW = 8;
 
-// The group step's match launch in gather mode `mode`; MODE_ANY only with GRP_STEP_HET (a heterogeneous group holding
-// both gather modes).
-template <int GRP, bool PROJ>
+// The group step's match launch in the members' one gather mode (MODE_TEX / MODE_LDG) or, when they hold both (a
+// heterogeneous group), MODE_ANY.
+template <bool PROJ>
 int launch_group_step(hsb_handle* h0, HsbMatchParams& P, int max_n, cudaStream_t st, int mode) {
-  if constexpr (GRP == hsb::GRP_STEP_HET) {
-    if (mode == hsb::MODE_ANY)
-      return launch_match_t<kGroupW, 1, hsb::MODE_ANY, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1);
-  }
-  return mode == hsb::MODE_TEX ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1)
-                               : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, GRP, PROJ>(h0, P, max_n, st, 1);
+  if (mode == hsb::MODE_ANY)
+    return launch_match_t<kGroupW, 1, hsb::MODE_ANY, 4, false, false, hsb::GRP_STEP, PROJ>(h0, P, max_n, st, 1);
+  return mode == hsb::MODE_TEX
+             ? launch_match_t<kGroupW, 1, hsb::MODE_TEX, 4, false, false, hsb::GRP_STEP, PROJ>(h0, P, max_n, st, 1)
+             : launch_match_t<kGroupW, 1, hsb::MODE_LDG, 4, false, false, hsb::GRP_STEP, PROJ>(h0, P, max_n, st, 1);
 }
 
 // The member list of a group call over K sessions: 0 <= K <= M, and with K > 0 a list of distinct indices in [0, M).
@@ -3168,11 +3158,10 @@ int check_members(hsb_group* g, const char* fn, int K, const int* members) {
   return HSB_OK;
 }
 
-// The level rule of a heterogeneous group's level-taking calls: every listed member has level `level` (members not
-// listed are not checked).  Checked before anything is queued.  In a group whose members share their level count the
-// group's own range check (level < hsb_group::levels) is the whole rule.
+// The level rule of a group's level-taking calls: every listed member has level `level` (members not listed are not
+// checked).  Checked before anything is queued.  In a group whose members share their level count it follows from the
+// group's own range check (level < hsb_group::levels).
 int check_member_level(hsb_group* g, const char* fn, int K, const int* members, int level) {
-  if (!g->ragged) return HSB_OK;
   for (int k = 0; k < K; ++k) {
     const hsb_handle* h = g->m[members[k]];
     if (level >= h->levels)
@@ -3306,7 +3295,7 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   // K1: (conversion +) match + gate, one session per CTA; the last session to finish publishes the step's sequence number
   HsbMatchParams P;
   fill_match_params(h0, P);
-  P.levels = levels;   // the stride of group_lv (the sessions' own level counts: GRP_STEP_HET)
+  P.levels = levels;   // the stride of group_lv (each session runs its member's own level count)
   P.B = K;
   P.hints = reinterpret_cast<const float*>(ds);
   // (a converted session converts with its own descriptor, HsbGroupSessionDev::conv)
@@ -3322,16 +3311,9 @@ int group_step(hsb_group* g, const GroupInput& in, int K, const int* members, co
   P.group_sess = reinterpret_cast<const HsbGroupSessionDev*>(ds + o_sess);
   P.group_done = reinterpret_cast<unsigned*>(g->d_res + 4 * (size_t)M);
   {
-    // each session on its member's levels (GRP_STEP_HET) when the members differ in level count or gather mode, in the
-    // members' one gather mode, or MODE_ANY when they hold both
     const int mode = g->any_mode ? hsb::MODE_ANY : h0->gather_mode == HSB_GATHER_TEX ? hsb::MODE_TEX : hsb::MODE_LDG;
-    const bool proj = in.kind == HSB_IN_PROJECTED;
-    if (g->ragged || g->any_mode)
-      s = proj ? launch_group_step<hsb::GRP_STEP_HET, true>(h0, P, max_n, st, mode)
-               : launch_group_step<hsb::GRP_STEP_HET, false>(h0, P, max_n, st, mode);
-    else
-      s = proj ? launch_group_step<hsb::GRP_STEP, true>(h0, P, max_n, st, mode)
-               : launch_group_step<hsb::GRP_STEP, false>(h0, P, max_n, st, mode);
+    s = in.kind == HSB_IN_PROJECTED ? launch_group_step<true>(h0, P, max_n, st, mode)
+                                    : launch_group_step<false>(h0, P, max_n, st, mode);
   }
   if (s != HSB_OK) return s;
 
@@ -3581,7 +3563,7 @@ int group_score(hsb_group* g, const char* fn, ScoreKind kind, int K, const int* 
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, level, kind,
                      K, Q, poses, pts, pts ? (size_t)scan_offsets[K] : 0,
                      group_sessions(g, K, members, level, pose_offsets, scan_offsets), g->d_best, out_lh, out_map,
-                     out_world, out_best4, out_best_index, nullptr, g->ragged, g->any_mode);
+                     out_world, out_best4, out_best_index, nullptr, g->any_mode);
 }
 
 // hsb_match_batch in shared-scan mode for K members in one pass: session k's hints [hint_offsets[k], hint_offsets[k+1])
@@ -3666,7 +3648,7 @@ int group_match(hsb_group* g, const char* fn, HsbInputKind kind, int K, const in
   // (the match reads no cell length: the sessions carry level 0's, which the scoring takes)
   return score_query(h0, g->stream, g->h_ray_stage, g->h_ray_stage_bytes, g->d_ray_stage, g->d_lv, g->levels, 0,
                      SCORE_MATCH, K, Q, hints, in, n_in, group_sessions(g, K, members, 0, hint_offsets, scan_offsets),
-                     g->d_best, out_lh, nullptr, nullptr, out_best4, out_best_index, &mq, g->ragged, g->any_mode);
+                     g->d_best, out_lh, nullptr, nullptr, out_best4, out_best_index, &mq, g->any_mode);
 }
 
 }  // namespace
@@ -3988,25 +3970,21 @@ int group_pack_dirty(hsb_group* g, const char* fn, int K, const int* members, fl
   fill_group_tile_params(g, T, d_buf, capacity_bytes, K);
   T.reset = reset;
   const int blocks = h0->sm_count * 4;
-  const int* nl = g->d_member_levels;   // a ragged group's blocks each carry their member's level count
+  const int* nl = g->d_member_levels;   // each block carries its member's level count
   if (!members) {
-    if (nl) hsb::pack_dirty_group_ragged_kernel<<<blocks, 256, 0, user>>>(T, nl);
-    else hsb::pack_dirty_group_kernel<<<blocks, 256, 0, user>>>(T);
+    hsb::pack_dirty_group_kernel<<<blocks, 256, 0, user>>>(T, nl);
   } else if (K <= kTileSubsetSmall) {
     hsb::TileMembers<kTileSubsetSmall> S;
     memcpy(S.idx, members, (size_t)K * sizeof(int));
-    if (nl) hsb::pack_dirty_subset_ragged_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S, nl);
-    else hsb::pack_dirty_subset_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S);
+    hsb::pack_dirty_subset_kernel<kTileSubsetSmall><<<blocks, 256, 0, user>>>(T, S, nl);
   } else {
     std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
     memcpy(S->idx, members, (size_t)K * sizeof(int));
-    if (nl) hsb::pack_dirty_subset_ragged_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S, nl);
-    else hsb::pack_dirty_subset_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S);
+    hsb::pack_dirty_subset_kernel<kTileSubsetMax><<<blocks, 256, 0, user>>>(T, *S, nl);
   }
   if (reset) {
     const int threads = K * 4 * g->levels;
-    if (nl) hsb::reset_dirty_ragged_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T, nl);
-    else hsb::reset_dirty_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T);
+    hsb::reset_dirty_group_kernel<<<(threads + 255) / 256, 256, 0, user>>>(T, nl);
   }
   h0->launches += reset ? 2 : 1;
   HSB_CUDA(h0, cudaGetLastError());
@@ -4046,8 +4024,7 @@ int hsb_group_unpack_dirty_device(hsb_group* g, const float* d_buf, size_t capac
   if ((s = tile_order_before(g, user, M, nullptr, true, true)) != HSB_OK) return s;
   HsbTileParams T;
   fill_group_tile_params(g, T, const_cast<float*>(d_buf), capacity_bytes, 0);
-  if (g->d_member_levels) hsb::unpack_dirty_ragged_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T, g->d_member_levels);
-  else hsb::unpack_dirty_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T);
+  hsb::unpack_dirty_group_kernel<<<h0->sm_count * 4, 256, 0, user>>>(T, g->d_member_levels);
   h0->launches++;
   HSB_CUDA(h0, cudaGetLastError());
   return tile_order_after(g, user, M, nullptr, true);
@@ -4084,20 +4061,17 @@ int group_reset(hsb_group* g, const char* fn, int K, const int* members) {
   }
   const size_t want = ((size_t)h0->sm_count * 32 + K - 1) / K;
   const dim3 grid((unsigned)std::max<size_t>(1, std::min(want, (max_cells + 255) / 256)), (unsigned)std::min(K, 65535));
-  const int* nl = g->d_member_levels;   // a ragged group: each member's own levels
+  const int* nl = g->d_member_levels;   // each member's own levels
   if (all) {
-    if (nl) hsb::group_reset_ragged_kernel<<<grid, 256, 0, st>>>(P, nl);
-    else hsb::group_reset_kernel<<<grid, 256, 0, st>>>(P);
+    hsb::group_reset_kernel<<<grid, 256, 0, st>>>(P, nl);
   } else if (K <= kTileSubsetSmall) {
     hsb::TileMembers<kTileSubsetSmall> S;
     memcpy(S.idx, members, (size_t)K * sizeof(int));
-    if (nl) hsb::group_reset_subset_ragged_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S, nl);
-    else hsb::group_reset_subset_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S);
+    hsb::group_reset_subset_kernel<kTileSubsetSmall><<<grid, 256, 0, st>>>(P, S, nl);
   } else {
     std::unique_ptr<hsb::TileMembers<kTileSubsetMax>> S(new hsb::TileMembers<kTileSubsetMax>());   // 16 KB: not on the stack
     memcpy(S->idx, members, (size_t)K * sizeof(int));
-    if (nl) hsb::group_reset_subset_ragged_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S, nl);
-    else hsb::group_reset_subset_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S);
+    hsb::group_reset_subset_kernel<kTileSubsetMax><<<grid, 256, 0, st>>>(P, *S, nl);
   }
   h0->launches++;
   HSB_CUDA(h0, cudaGetLastError());

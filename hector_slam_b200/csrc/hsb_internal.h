@@ -69,8 +69,8 @@ struct HsbGroupSessionDev {
   // the member's position in the group (its row of HsbMatchParams::group_lv).  Kept here rather than in HsbMatchParams
   // so that the parameter block, and with it every other instantiation of the match kernel, is unchanged.
   int member;
-  // the member's level count: a heterogeneous group's step (GRP_STEP_HET) starts the session at its member's coarsest
-  // level; its rows of group_lv past that are never read.  (Fills the descriptor's tail padding: its size is unchanged.)
+  // the member's level count: the step starts the session at its member's coarsest level; its rows of group_lv past
+  // that are never read.  (Fills the descriptor's tail padding: its size is unchanged.)
   int levels;
   // the member's per-evaluation record of this step's match (HsbMatchParams::record's layout for the member's own levels:
   // group_lv's rec_off), in the member's mapped host buffer (hsb_set_step_record); null: the session records nothing
@@ -84,7 +84,7 @@ struct HsbScoreSessionDev {
   int n;
   int member;
   float cell_length;   // of the member's level of a scoring call (covariance: the world matrix); unused by the match
-  int levels;          // the member's level count: a heterogeneous group's match (GRP_MATCH_HET) starts at its coarsest
+  int levels;          // the member's level count: a group match starts the session's hints at its coarsest
 };
 
 struct HsbMatchParams {
@@ -140,7 +140,7 @@ struct HsbMatchParams {
   int record_floats;
   // group SLAM step (match_kernel<..., GRP = GRP_STEP>): scan b is session b of the step, which steps member
   // group_sess[b].member of the group.  Its level descriptors are group_lv[member * levels ..] (built once per group;
-  // `levels` is then the group's largest level count, and a GRP_STEP_HET / GRP_MATCH_HET scan runs its own member's)
+  // `levels` is then the group's largest level count, and each scan runs its own member's)
   // instead of lv[], its gate thresholds and map_without_matching flag
   // gate_in[3b ..] (a set flag skips the match: the hint passes through the gate), its gate state and last-match
   // container group_sess[b]; out_poses and gate_out_host hold 4 floats per session (pose, write flag).  group_done

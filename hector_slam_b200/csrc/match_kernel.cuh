@@ -769,16 +769,13 @@ struct MatchBounds {
 
 // Which group a match kernel serves (its GRP template value): none (one handle's map for the whole batch), the group
 // SLAM step (one session per scan, hsb_group_slam_update) or the group batch match (one hint per scan,
-// hsb_group_match_batch).  The _HET forms serve a heterogeneous group whose members differ in their level count: each
-// scan runs its own member's levels (HsbGroupSessionDev::levels, HsbScoreSessionDev::levels), coarsest first, instead
-// of HsbMatchParams::levels, which is then only the stride of group_lv.
-enum { GRP_NONE = 0, GRP_STEP = 1, GRP_MATCH = 2, GRP_STEP_HET = 3, GRP_MATCH_HET = 4 };
+// hsb_group_match_batch).  A group's scan runs its own member's levels (HsbGroupSessionDev::levels,
+// HsbScoreSessionDev::levels), coarsest first; HsbMatchParams::levels is then only the stride of group_lv.
+enum { GRP_NONE = 0, GRP_STEP = 1, GRP_MATCH = 2 };
 template <int GRP>
-constexpr bool kGrpStep = GRP == GRP_STEP || GRP == GRP_STEP_HET;
+constexpr bool kGrpStep = GRP == GRP_STEP;
 template <int GRP>
-constexpr bool kGrpMatch = GRP == GRP_MATCH || GRP == GRP_MATCH_HET;
-template <int GRP>
-constexpr bool kGrpHet = GRP == GRP_STEP_HET || GRP == GRP_MATCH_HET;
+constexpr bool kGrpMatch = GRP == GRP_MATCH;
 
 // The session of hint q of a group batch match or of pose q of a scoring call: the last session whose hints / poses
 // start at or before q (empty sessions are passed over), as ray_kernel finds a ray's.
@@ -893,15 +890,15 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
     }
     const float2* __restrict__ gpts = P.pts + beg;
     int member = 0;
-    int levels = 0;   // a heterogeneous group's scan: its member's level count (every other scan runs P.levels)
+    int levels = 0;   // a group's scan: its member's level count (a GRP_NONE scan runs P.levels)
     if constexpr (kGrpMatch<GRP>) {   // group batch match: the scan, its length and the map are the hint's session's
       const HsbScoreSessionDev& s = P.match_sess[session_of(P.match_offsets, P.match_K, scan)];
       gpts = s.pts;
       n = s.n;
       member = s.member;
-      if constexpr (GRP == GRP_MATCH_HET) levels = s.levels;
+      levels = s.levels;
     }
-    if constexpr (GRP == GRP_STEP_HET) levels = P.group_sess[scan].levels;
+    if constexpr (kGrpStep<GRP>) levels = P.group_sess[scan].levels;
     const float2* spts_scan = spts;  // shared-memory copy of the scan's first `ns` points (valid when staged)
     bool staged = false;
     int ns = 0;                      // points [0, ns) are read from shared memory, [ns, n) from global memory
@@ -1011,7 +1008,7 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
     else recording = P.record && t == 0;
     int evals_ran = 0;   // evaluations this scan actually ran (trace slot 5)
     if (n > 0) {
-      for (int lvl = (kGrpHet<GRP> ? levels : P.levels) - 1; lvl >= 0; --lvl) {
+      for (int lvl = (GRP == GRP_NONE ? P.levels : levels) - 1; lvl >= 0; --lvl) {
         const HsbLevelDev& L = level_desc<GRP>(P, scan, member, lvl);
         const LevelRegs LR = level_regs(L);
         float ex, ey, epsi = wpsi;
@@ -1141,8 +1138,8 @@ __global__ void __launch_bounds__(W * G * 32, MatchBounds<W, G, MODE>::kMinBlock
         if (HSB_DIAG && P.trace && t == 0) P.trace[8 * (size_t)scan + (P.levels - lvl)] = global_timer_ns();
       }
     } else if (recording) {   // nothing evaluated: every level starts from the hint, the evaluation slots are zero
-      // (a group step's session: its member's own levels, in its member's layout)
-      for (int lvl = (GRP == GRP_STEP_HET ? levels : P.levels) - 1; lvl >= 0; --lvl) {
+      // (a group step's session: its member's own levels, in its member's layout; a group match records nothing)
+      for (int lvl = (kGrpStep<GRP> ? levels : P.levels) - 1; lvl >= 0; --lvl) {
         const HsbLevelDev& L = kGrpStep<GRP> ? level_desc<GRP>(P, scan, member, lvl) : P.lv[lvl];
         float* rec = record_base<GRP>(P, scan) + L.rec_off;
         rec[0] = wx; rec[1] = wy; rec[2] = wpsi;

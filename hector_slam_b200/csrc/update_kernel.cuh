@@ -601,19 +601,19 @@ __device__ __forceinline__ long long tile_h(int4 r) { return tile_dirty(r) ? (lo
 __device__ __forceinline__ const HsbTileLevelDev* tile_levels(const HsbTileParams& P, int member) {
   return P.table ? P.table + (size_t)member * P.levels : P.lv;
 }
-// How many levels a block's member has: the launch's (a single handle, or a group whose members share their level
-// count), or each member its own (a heterogeneous group whose members differ in it: hsb_group::d_member_levels, read
-// through the *_ragged kernels).  A member's rows of the group's table past its own levels are never read.
-struct TileLevelsUniform {};
-struct TileLevelsRagged {
+// How many levels a block's member has: the launch's (P.levels: a single handle), or — a group, whose members may each
+// have their own — its entry of hsb_group::d_member_levels.  A member's rows of the group's table past its own levels
+// are never read.
+struct TileLevelsSingle {};
+struct TileLevelsMember {
   const int* n;
 };
-// member m's level count; `uniform` is the launch's (P.levels, or a copy of it the body already holds)
-__device__ __forceinline__ int tile_member_levels(TileLevelsUniform, int uniform, int) { return uniform; }
-__device__ __forceinline__ int tile_member_levels(const TileLevelsRagged& LV, int, int m) { return LV.n[m]; }
-// whether level l lies past member m's levels (never, where every member has the launch's levels)
-__device__ __forceinline__ bool tile_level_past(TileLevelsUniform, int, int) { return false; }
-__device__ __forceinline__ bool tile_level_past(const TileLevelsRagged& LV, int m, int l) { return l >= LV.n[m]; }
+// member m's level count; `single` is the launch's (P.levels, or a copy of it the body already holds)
+__device__ __forceinline__ int tile_member_levels(TileLevelsSingle, int single, int) { return single; }
+__device__ __forceinline__ int tile_member_levels(const TileLevelsMember& LV, int, int m) { return LV.n[m]; }
+// whether level l lies past member m's levels (never, for a single handle)
+__device__ __forceinline__ bool tile_level_past(TileLevelsSingle, int, int) { return false; }
+__device__ __forceinline__ bool tile_level_past(const TileLevelsMember& LV, int m, int l) { return l >= LV.n[m]; }
 
 // where a block's deferral is counted: its member's overflow counter (a single handle: its own)
 __device__ __forceinline__ int* tile_counter(const HsbTileParams& P, int member) {
@@ -799,27 +799,19 @@ __device__ __forceinline__ void pack_dirty_body(const HsbTileParams& P, const Se
 }
 
 __global__ void __launch_bounds__(256) pack_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  pack_dirty_body(P, TileSingle(), TileLevelsUniform());
+  pack_dirty_body(P, TileSingle(), TileLevelsSingle());
 }
-__global__ void __launch_bounds__(256) pack_dirty_group_kernel(const __grid_constant__ HsbTileParams P) {
-  pack_dirty_body(P, TileAll(), TileLevelsUniform());
+// a group: every block carries its member's own levels (header word 1, exactly hsb_pack_dirty_device's block), the
+// group header the group's largest count (P.levels)
+__global__ void __launch_bounds__(256) pack_dirty_group_kernel(const __grid_constant__ HsbTileParams P,
+                                                               const int* __restrict__ member_levels) {
+  pack_dirty_body(P, TileAll(), TileLevelsMember{member_levels});
 }
 template <int N>
 __global__ void __launch_bounds__(256) pack_dirty_subset_kernel(const __grid_constant__ HsbTileParams P,
-                                                                const __grid_constant__ TileMembers<N> S) {
-  pack_dirty_body(P, S, TileLevelsUniform());
-}
-// a heterogeneous group whose members differ in level count: every block carries its member's own levels (header word
-// 1, exactly hsb_pack_dirty_device's block), the group header the group's largest count (P.levels)
-__global__ void __launch_bounds__(256) pack_dirty_group_ragged_kernel(const __grid_constant__ HsbTileParams P,
-                                                                      const int* __restrict__ member_levels) {
-  pack_dirty_body(P, TileAll(), TileLevelsRagged{member_levels});
-}
-template <int N>
-__global__ void __launch_bounds__(256) pack_dirty_subset_ragged_kernel(const __grid_constant__ HsbTileParams P,
-                                                                       const __grid_constant__ TileMembers<N> S,
-                                                                       const int* __restrict__ member_levels) {
-  pack_dirty_body(P, S, TileLevelsRagged{member_levels});
+                                                                const __grid_constant__ TileMembers<N> S,
+                                                                const int* __restrict__ member_levels) {
+  pack_dirty_body(P, S, TileLevelsMember{member_levels});
 }
 
 // after pack (stream order): the shipped blocks' rectangles and cleared flags are forgotten, a deferred block's are kept.
@@ -841,10 +833,10 @@ __device__ __forceinline__ void reset_dirty_body(const HsbTileParams& P, const L
   if (q == 0) d[HSB_DIRTY_CLEARED] = 0;
 }
 __global__ void reset_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  reset_dirty_body(P, TileLevelsUniform());
+  reset_dirty_body(P, TileLevelsSingle());
 }
-__global__ void reset_dirty_ragged_kernel(const __grid_constant__ HsbTileParams P, const int* __restrict__ member_levels) {
-  reset_dirty_body(P, TileLevelsRagged{member_levels});
+__global__ void reset_dirty_group_kernel(const __grid_constant__ HsbTileParams P, const int* __restrict__ member_levels) {
+  reset_dirty_body(P, TileLevelsMember{member_levels});
 }
 
 // hsb_group_reset: hsb_reset's end state for every level of K members in one launch — log-odds 0, P 0.5, texture twin
@@ -881,24 +873,16 @@ __device__ __forceinline__ void group_reset_body(const HsbResetParams& P, const 
     }
   }
 }
-__global__ void __launch_bounds__(256) group_reset_kernel(const __grid_constant__ HsbResetParams P) {
-  group_reset_body(P, TileAll(), TileLevelsUniform());
+// each member's own levels only
+__global__ void __launch_bounds__(256) group_reset_kernel(const __grid_constant__ HsbResetParams P,
+                                                          const int* __restrict__ member_levels) {
+  group_reset_body(P, TileAll(), TileLevelsMember{member_levels});
 }
 template <int N>
 __global__ void __launch_bounds__(256) group_reset_subset_kernel(const __grid_constant__ HsbResetParams P,
-                                                                 const __grid_constant__ TileMembers<N> S) {
-  group_reset_body(P, S, TileLevelsUniform());
-}
-// a heterogeneous group whose members differ in level count: each member's own levels only
-__global__ void __launch_bounds__(256) group_reset_ragged_kernel(const __grid_constant__ HsbResetParams P,
+                                                                 const __grid_constant__ TileMembers<N> S,
                                                                  const int* __restrict__ member_levels) {
-  group_reset_body(P, TileAll(), TileLevelsRagged{member_levels});
-}
-template <int N>
-__global__ void __launch_bounds__(256) group_reset_subset_ragged_kernel(const __grid_constant__ HsbResetParams P,
-                                                                        const __grid_constant__ TileMembers<N> S,
-                                                                        const int* __restrict__ member_levels) {
-  group_reset_body(P, S, TileLevelsRagged{member_levels});
+  group_reset_body(P, S, TileLevelsMember{member_levels});
 }
 
 // Unpack, pass 1: the buffer fits the replica (group header and every block's header inside the capacity, every shipped
@@ -907,7 +891,8 @@ __global__ void __launch_bounds__(256) group_reset_subset_ragged_kernel(const __
 // rows: its rectangles may be larger than the whole buffer (that is why it was deferred) and are not checked.  The
 // level-size check keeps a block packed on a member of another size (an owner group listing its handles in another
 // order than a mixed replica group) from growing a mirror rectangle past the plane it lands on.
-__device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChunk& c, int k, int j) {
+template <class Levels>
+__device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, const Levels& LV, TileChunk& c, int k, int j) {
   const int* gh = reinterpret_cast<const int*>(P.buf);
   int member = 0;
   unsigned long long start = 0;
@@ -918,14 +903,14 @@ __device__ __forceinline__ bool tile_read_block(const HsbTileParams& P, TileChun
   }
   if (start + HSB_TILE_HEADER_WORDS > P.capacity_words) return false;
   const int* hdr = reinterpret_cast<const int*>(P.buf + start);
-  if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != P.levels) return false;
+  if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != tile_member_levels(LV, P.levels, member)) return false;
   const bool ship = hdr[2] == 0;
   const unsigned cleared = (unsigned)hdr[HSB_TILE_CLEARED_WORD];
-  if (cleared >> P.levels) return false;   // a cleared level the replica does not have
+  if (cleared >> tile_member_levels(LV, P.levels, member)) return false;   // a cleared level the replica does not have
   const HsbTileLevelDev* lv = tile_levels(P, member);
   unsigned long long cells = 0;
   unsigned rows = 0;
-  for (int l = 0; l < P.levels; ++l) {
+  for (int l = 0; l < tile_member_levels(LV, P.levels, member); ++l) {
     const int4 q = make_int4(hdr[4 + 4 * l], hdr[5 + 4 * l], hdr[6 + 4 * l], hdr[7 + 4 * l]);
     c.rect[j][l] = q;
     if (!ship) continue;
@@ -969,149 +954,65 @@ __device__ __forceinline__ void tile_clear(const HsbTileParams& P, const TileChu
   }
 }
 
+template <class Levels>
+__device__ __forceinline__ void unpack_dirty_body(const HsbTileParams& P, const Levels& LV) {
+  __shared__ TileChunk c;
+  const int* gh = reinterpret_cast<const int*>(P.buf);
+  int K = 1;
+  bool fits = true;
+  if (P.table) {
+    fits = P.capacity_words >= HSB_TILE_GROUP_FIXED_WORDS && gh[0] == HSB_TILE_GROUP_MAGIC && gh[2] == P.levels &&
+           gh[1] >= 0 && gh[1] <= P.M;
+    if (fits) {
+      K = gh[1];
+      fits = hsb_tile_group_header_words(K) <= P.capacity_words;
+    }
+  }
+  for (int k0 = 0; fits && k0 < K; k0 += kTileChunk) {
+    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
+    const bool ok = j >= n || tile_read_block(P, LV, c, k0 + j, j);
+    fits = __syncthreads_and(ok);
+  }
+  if (!fits) {   // nothing from a buffer that does not fit is applied; counted once on handles[0]
+    if (blockIdx.x == 0 && threadIdx.x == 0 && P.error_count) atomicAdd(P.error_count, 1);
+    return;
+  }
+  for (int k0 = 0; k0 < K; k0 += kTileChunk) {
+    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
+    if (j < n) tile_read_block(P, LV, c, k0 + j, j);
+    const bool any_cleared = __syncthreads_or(j < n && c.cleared[j] != 0u);
+    if (threadIdx.x < 32) tile_row_prefix(c, n);
+    if (blockIdx.x == 0 && j < n) {
+      const int m = c.member[j];
+      if (!c.ship[j]) {   // a deferred block: counted once on its member's counter
+        int* cnt = tile_counter(P, m);
+        if (cnt) atomicAdd(cnt, 1);
+      } else {            // the replica's host mirror has to follow (a cleared level: all of it)
+        const HsbTileLevelDev* lv = tile_levels(P, m);
+        for (int l = 0; l < tile_member_levels(LV, P.levels, m); ++l) {
+          const int4 q = (c.cleared[j] >> l) & 1u ? make_int4(0, 0, lv[l].sx - 1, lv[l].sy - 1) : c.rect[j][l];
+          if (!tile_dirty(q)) continue;
+          int* md = lv[l].dirty + 4;
+          atomicMin(md + 0, q.x); atomicMin(md + 1, q.y);
+          atomicMax(md + 2, q.z); atomicMax(md + 3, q.w);
+        }
+      }
+    }
+    __syncthreads();
+    tile_rows<false>(P, c, n);
+    if (any_cleared) tile_clear(P, c, n);
+    __syncthreads();
+  }
+}
+
 __global__ void __launch_bounds__(256) unpack_dirty_kernel(const __grid_constant__ HsbTileParams P) {
-  __shared__ TileChunk c;
-  const int* gh = reinterpret_cast<const int*>(P.buf);
-  int K = 1;
-  bool fits = true;
-  if (P.table) {
-    fits = P.capacity_words >= HSB_TILE_GROUP_FIXED_WORDS && gh[0] == HSB_TILE_GROUP_MAGIC && gh[2] == P.levels &&
-           gh[1] >= 0 && gh[1] <= P.M;
-    if (fits) {
-      K = gh[1];
-      fits = hsb_tile_group_header_words(K) <= P.capacity_words;
-    }
-  }
-  for (int k0 = 0; fits && k0 < K; k0 += kTileChunk) {
-    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
-    const bool ok = j >= n || tile_read_block(P, c, k0 + j, j);
-    fits = __syncthreads_and(ok);
-  }
-  if (!fits) {   // nothing from a buffer that does not fit is applied; counted once on handles[0]
-    if (blockIdx.x == 0 && threadIdx.x == 0 && P.error_count) atomicAdd(P.error_count, 1);
-    return;
-  }
-  for (int k0 = 0; k0 < K; k0 += kTileChunk) {
-    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
-    if (j < n) tile_read_block(P, c, k0 + j, j);
-    const bool any_cleared = __syncthreads_or(j < n && c.cleared[j] != 0u);
-    if (threadIdx.x < 32) tile_row_prefix(c, n);
-    if (blockIdx.x == 0 && j < n) {
-      const int m = c.member[j];
-      if (!c.ship[j]) {   // a deferred block: counted once on its member's counter
-        int* cnt = tile_counter(P, m);
-        if (cnt) atomicAdd(cnt, 1);
-      } else {            // the replica's host mirror has to follow (a cleared level: all of it)
-        const HsbTileLevelDev* lv = tile_levels(P, m);
-        for (int l = 0; l < P.levels; ++l) {
-          const int4 q = (c.cleared[j] >> l) & 1u ? make_int4(0, 0, lv[l].sx - 1, lv[l].sy - 1) : c.rect[j][l];
-          if (!tile_dirty(q)) continue;
-          int* md = lv[l].dirty + 4;
-          atomicMin(md + 0, q.x); atomicMin(md + 1, q.y);
-          atomicMax(md + 2, q.z); atomicMax(md + 3, q.w);
-        }
-      }
-    }
-    __syncthreads();
-    tile_rows<false>(P, c, n);
-    if (any_cleared) tile_clear(P, c, n);
-    __syncthreads();
-  }
+  unpack_dirty_body(P, TileLevelsSingle());
 }
-
-// tile_read_block for a heterogeneous group whose members differ in level count (nl: hsb_group::d_member_levels): a block
-// must carry exactly its member's level count; a block whose count differs does not fit, like a rectangle outside its
-// level.
-__device__ __forceinline__ bool tile_read_block_ragged(const HsbTileParams& P, const int* __restrict__ nl, TileChunk& c,
-                                                       int k, int j) {
-  const int* gh = reinterpret_cast<const int*>(P.buf);
-  int member = 0;
-  unsigned long long start = 0;
-  if (P.table) {
-    member = gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k];
-    start = (unsigned)gh[HSB_TILE_GROUP_FIXED_WORDS + 2 * k + 1];
-    if (member < 0 || member >= P.M) return false;
-  }
-  if (start + HSB_TILE_HEADER_WORDS > P.capacity_words) return false;
-  const int* hdr = reinterpret_cast<const int*>(P.buf + start);
-  if (hdr[0] != HSB_TILE_MAGIC || hdr[1] != nl[member]) return false;
-  const bool ship = hdr[2] == 0;
-  const unsigned cleared = (unsigned)hdr[HSB_TILE_CLEARED_WORD];
-  if (cleared >> nl[member]) return false;   // a cleared level the replica does not have
-  const HsbTileLevelDev* lv = tile_levels(P, member);
-  unsigned long long cells = 0;
-  unsigned rows = 0;
-  for (int l = 0; l < nl[member]; ++l) {
-    const int4 q = make_int4(hdr[4 + 4 * l], hdr[5 + 4 * l], hdr[6 + 4 * l], hdr[7 + 4 * l]);
-    c.rect[j][l] = q;
-    if (!ship) continue;
-    if (tile_dirty(q) && (q.x < 0 || q.y < 0 || q.z >= lv[l].sx || q.w >= lv[l].sy)) return false;
-    const long long w = tile_w(q), h = tile_h(q);
-    if (w > P.capacity_words || h > P.capacity_words) return false;   // (keeps w * h and the sums below in 64 bits)
-    cells += (unsigned long long)(w * h);
-    rows += (unsigned)h;
-  }
-  if (ship && start + HSB_TILE_HEADER_WORDS + cells > P.capacity_words) return false;
-  c.start[j] = start;
-  c.cells[j] = cells;
-  c.member[j] = member;
-  c.ship[j] = ship ? 1 : 0;
-  c.cleared[j] = ship ? cleared : 0u;
-  c.row0[j + 1] = ship ? rows : 0u;
-  return true;
-}
-
-// a heterogeneous group whose members differ in level count: unpack_dirty_kernel with each member's own level count
-// (tile_read_block_ragged)
-__global__ void __launch_bounds__(256) unpack_dirty_ragged_kernel(const __grid_constant__ HsbTileParams P,
-                                                                  const int* __restrict__ nl) {
-  __shared__ TileChunk c;
-  const int* gh = reinterpret_cast<const int*>(P.buf);
-  int K = 1;
-  bool fits = true;
-  if (P.table) {
-    fits = P.capacity_words >= HSB_TILE_GROUP_FIXED_WORDS && gh[0] == HSB_TILE_GROUP_MAGIC && gh[2] == P.levels &&
-           gh[1] >= 0 && gh[1] <= P.M;
-    if (fits) {
-      K = gh[1];
-      fits = hsb_tile_group_header_words(K) <= P.capacity_words;
-    }
-  }
-  for (int k0 = 0; fits && k0 < K; k0 += kTileChunk) {
-    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
-    const bool ok = j >= n || tile_read_block_ragged(P, nl, c, k0 + j, j);
-    fits = __syncthreads_and(ok);
-  }
-  if (!fits) {   // nothing from a buffer that does not fit is applied; counted once on handles[0]
-    if (blockIdx.x == 0 && threadIdx.x == 0 && P.error_count) atomicAdd(P.error_count, 1);
-    return;
-  }
-  for (int k0 = 0; k0 < K; k0 += kTileChunk) {
-    const int j = threadIdx.x, n = min(kTileChunk, K - k0);
-    if (j < n) tile_read_block_ragged(P, nl, c, k0 + j, j);
-    const bool any_cleared = __syncthreads_or(j < n && c.cleared[j] != 0u);
-    if (threadIdx.x < 32) tile_row_prefix(c, n);
-    if (blockIdx.x == 0 && j < n) {
-      const int m = c.member[j];
-      if (!c.ship[j]) {   // a deferred block: counted once on its member's counter
-        int* cnt = tile_counter(P, m);
-        if (cnt) atomicAdd(cnt, 1);
-      } else {            // the replica's host mirror has to follow (a cleared level: all of it)
-        const HsbTileLevelDev* lv = tile_levels(P, m);
-        for (int l = 0; l < nl[m]; ++l) {
-          const int4 q = (c.cleared[j] >> l) & 1u ? make_int4(0, 0, lv[l].sx - 1, lv[l].sy - 1) : c.rect[j][l];
-          if (!tile_dirty(q)) continue;
-          int* md = lv[l].dirty + 4;
-          atomicMin(md + 0, q.x); atomicMin(md + 1, q.y);
-          atomicMax(md + 2, q.z); atomicMax(md + 3, q.w);
-        }
-      }
-    }
-    __syncthreads();
-    tile_rows<false>(P, c, n);
-    if (any_cleared) tile_clear(P, c, n);
-    __syncthreads();
-  }
+// a group: a block must carry exactly its member's level count; a block whose count differs does not fit, like a
+// rectangle outside its level
+__global__ void __launch_bounds__(256) unpack_dirty_group_kernel(const __grid_constant__ HsbTileParams P,
+                                                                 const int* __restrict__ member_levels) {
+  unpack_dirty_body(P, TileLevelsMember{member_levels});
 }
 
 }  // namespace hsb

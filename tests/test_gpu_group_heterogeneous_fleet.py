@@ -10,10 +10,9 @@ lists the handles in the owner's order; every comparison is bit for bit.
     members, the second 128-session pass of the pack and unpack layout, and the first-fit loop over more than 32
     blocks, all with per-member level counts.
   - test_group_kinds: a small group for each way its members may differ on their own — gather mode at one level count
-    (GRP_STEP_HET in MODE_ANY with the uniform tile and reset kernels), level count at one gather mode (TEX and LDG: the
-    heterogeneous kernels in that mode with the ragged tile and reset kernels), and per-level iteration counts only
-    (the existing group kernels, each member's own evaluation counts): steps, the match at W = 1 and 8, scoring, tile
-    replication and a subset reset."""
+    (the group kernels in MODE_ANY), level count at one gather mode (TEX and LDG: the group kernels in that mode, each
+    session, block and reset on its member's own level count), and per-level iteration counts only (each member's own
+    evaluation counts): steps, the match at W = 1 and 8, scoring, tile replication and a subset reset."""
 import numpy as np
 import pytest
 
