@@ -2602,6 +2602,14 @@ static int order_after(hsb_handle* h, cudaStream_t user, bool all_streams) {
     for (int i = 0; i < 2; ++i) HSB_CUDA(h, cudaStreamWaitEvent(h->copy_stream[i], h->ev_sync[3], 0));
   return HSB_OK;
 }
+// order_after of a call that wrote the planes on the caller's stream: the handle's streams wait for it, and so does a
+// later match or likelihood on any other caller stream, through map_write_pending (launch_match, likelihood_device)
+static int order_after_map_write(hsb_handle* h, cudaStream_t user) {
+  const int s = order_after(h, user, true);
+  if (s != HSB_OK) return s;
+  h->map_write_pending = true;
+  return HSB_OK;
+}
 
 int hsb_pack_rect_device(hsb_handle* h, int level, const int rect[4], float* d_buf, void* stream) {
   if (!h || level < 0 || level >= h->levels || !rect || !d_buf) return HSB_ERR_INVALID_ARG;
@@ -2633,7 +2641,7 @@ int hsb_unpack_rect_device(hsb_handle* h, int level, const int rect[4], const fl
                                                                     d_buf, L.dirty + 4);
   h->launches++;
   HSB_CUDA(h, cudaGetLastError());
-  return order_after(h, (cudaStream_t)stream, true);
+  return order_after_map_write(h, (cudaStream_t)stream);
 }
 
 static void fill_tile_params(hsb_handle* h, HsbTileParams& T, float* d_buf, size_t capacity_bytes) {
@@ -2680,7 +2688,7 @@ int hsb_unpack_dirty_device(hsb_handle* h, const float* d_buf, size_t capacity_b
   hsb::unpack_dirty_kernel<<<h->sm_count * 4, 256, 0, (cudaStream_t)stream>>>(T);
   h->launches++;
   HSB_CUDA(h, cudaGetLastError());
-  return order_after(h, (cudaStream_t)stream, true);
+  return order_after_map_write(h, (cudaStream_t)stream);
 }
 
 int hsb_get_replication_overflows(hsb_handle* h, int* count, int reset) {
@@ -2812,16 +2820,21 @@ void* hsb_level_logodds_device_ptr(hsb_handle* h, int level) {
 int hsb_refresh_level(hsb_handle* h, int level, void* stream) {
   if (!h || level < 0 || level >= h->levels) return HSB_ERR_INVALID_ARG;
   HandleScope guard(h);
-  int s = refresh_level(h, level, (cudaStream_t)stream);
+  cudaStream_t user = (cudaStream_t)stream;
+  // ordered as an unpack: after everything the handle has queued (a pending map write, matches still reading the
+  // planes), and everything the handle queues afterwards waits for it
+  int s = order_before(h, user, true);
   if (s != HSB_OK) return s;
+  if ((s = refresh_level(h, level, user)) != HSB_OK) return s;
   // the plane was written from outside (a full-plane broadcast): the host mirror has to re-read the whole level, so the
   // mirror rectangle becomes the level, in order on `stream`.  The replication rectangle is left alone: marking it
   // would make a replica re-ship a whole plane it has only received.
   Level& L = h->lv[level];
-  if (!L.dirty) return HSB_OK;
-  const int full[4] = {0, 0, L.sx - 1, L.sy - 1};
-  HSB_CUDA(h, cudaMemcpyAsync(L.dirty + 4, full, sizeof(full), cudaMemcpyHostToDevice, (cudaStream_t)stream));
-  return HSB_OK;
+  if (L.dirty) {
+    const int full[4] = {0, 0, L.sx - 1, L.sy - 1};
+    HSB_CUDA(h, cudaMemcpyAsync(L.dirty + 4, full, sizeof(full), cudaMemcpyHostToDevice, user));
+  }
+  return order_after_map_write(h, user);
 }
 
 }  // extern "C"
@@ -3899,7 +3912,10 @@ constexpr int kTileSubsetSmall = 128, kTileSubsetMax = 4096;
 
 // The caller's stream behind everything queued on the sessions' members (members == nullptr: all M in order): a pending
 // step of any group they belong to, and, for a member that queued work of its own since, its stream (all_streams: its
-// copy streams too).  group_stream: also behind everything queued on this group's stream.
+// copy streams too).  group_stream: also behind everything queued on this group's stream.  (No call leaves work on the
+// group's stream without leaving its event in every member it touched -- a nowait step, a pack, a reset; the group's
+// queries return once done -- so the member loop below already orders an unpack behind it; the wait keeps the unpack's
+// promise independent of that.)
 int tile_order_before(hsb_group* g, cudaStream_t user, int K, const int* members, bool all_streams, bool group_stream) {
   hsb_handle* h0 = g->m[0];
   if (group_stream) {

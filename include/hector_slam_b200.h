@@ -768,7 +768,11 @@ int hsb_download_prob(hsb_handle* h, int level, float* prob_host_out);
  * recompute of the probability plane and texture twin after such an external write, on `stream`.
  * hsb_refresh_level also sets the level's mirror rectangle (hsb_get_mirror_dirty_rect) to the whole
  * level, in order on `stream`, so that a host mirror re-reads the plane; the replication rectangle
- * (hsb_get_dirty_rect) is left as it is, so a replica does not ship back a plane it only received. */
+ * (hsb_get_dirty_rect) is left as it is, so a replica does not ship back a plane it only received.
+ * Ordering as for hsb_unpack_rect_device: the refresh runs after everything the handle has queued (a pending map write
+ * of a nowait step, single or group, and matches still reading the planes) and everything the handle queues afterwards
+ * waits for it, on any stream.  The external write itself is the caller's: it must be ordered before the refresh on
+ * `stream`, and after whatever the handle queued before it. */
 void* hsb_level_logodds_device_ptr(hsb_handle* h, int level);
 int hsb_refresh_level(hsb_handle* h, int level, void* stream);
 
